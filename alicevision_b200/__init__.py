@@ -1,4 +1,4 @@
-"""alicevision_b200 — Blackwell (sm_100a) engine for AliceVision's descriptor-matching hot path.
+"""alicevision_b200 — H100 (sm_90a) engine for AliceVision's descriptor-matching hot path.
 
 Only what the path needs lives here: ``csrc/`` (CUDA kernels + the C ABI of include/b200match.h),
 ``adaptor/`` (C++ classes deriving from the reference's ArrayMatcher / IRegionsMatcher / IImageCollectionMatcher),

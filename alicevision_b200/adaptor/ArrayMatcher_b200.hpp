@@ -1,4 +1,4 @@
-// Reference-side adaptor, Surface 1: a matching::ArrayMatcher whose search runs on the B200 engine through the C ABI.
+// Reference-side adaptor, Surface 1: a matching::ArrayMatcher whose search runs on the b200match engine (H100) through the C ABI.
 // Header-only; compiled INSIDE an AliceVision build (it derives from the reference's own interface,
 // src/aliceVision/matching/ArrayMatcher.hpp:19-66) and linked against libb200match.so.  Drop-in for
 // ArrayMatcher_bruteForce<Scalar,Metric> (matching/ArrayMatcher_bruteForce.hpp:24-151): same template parameters,

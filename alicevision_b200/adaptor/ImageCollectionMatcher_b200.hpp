@@ -1,4 +1,4 @@
-// Reference-side adaptor, Surface 2: an IImageCollectionMatcher that hands the whole pair list to the B200 engine.
+// Reference-side adaptor, Surface 2: an IImageCollectionMatcher that hands the whole pair list to the b200match engine (H100).
 // Header-only; compiled inside an AliceVision build, derives from the reference's own interface
 // (src/aliceVision/matchingImageCollection/IImageCollectionMatcher.hpp:28-42) and is the drop-in for
 // ImageCollectionMatcher_generic with BRUTE_FORCE_L2 / BRUTE_FORCE_HAMMING (ImageCollectionMatcher_generic.cpp:30-123).

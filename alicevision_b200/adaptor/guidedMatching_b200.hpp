@@ -1,6 +1,6 @@
 // Reference-side adaptor for the step after the path: matching::guidedMatching<Mat3Model, FundamentalEpipolarDistanceError>
 // (matching/guidedMatching.hpp:206-268, called by GeometricFilterMatrix_F_AC.hpp:381-389 / GeometricFilterMatrix_E_AC.hpp:163)
-// on the B200 engine.  Header-only; compiled inside an AliceVision build and linked against libb200match.so.
+// on the b200match engine (H100).  Header-only; compiled inside an AliceVision build and linked against libb200match.so.
 // Cameras with distortion are not handled here (the reference un-distorts the positions first, :220-243): pass
 // camL == camR == nullptr semantics, i.e. call it when the intrinsics have no distortion or the positions are already undistorted.
 #pragma once

@@ -1,6 +1,6 @@
-"""In-tree build of the native engine: nvcc -> alicevision_b200/libb200match.so (sm_100a only).
+"""In-tree build of the native engine: nvcc -> alicevision_b200/libb200match.so (sm_90a only).
 
-The .so is git-ignored but travels to the GPU box with the repo snapshot, so the box never compiles.
+The .so is a build product (git-ignored): build() compiles it next to the sources, and a tree built once is used as is.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ def _deps():
                   + glob.glob(os.path.join(CSRC, "*.h")) + glob.glob(os.path.join(_HERE, "..", "include", "*.h")) + [os.path.abspath(__file__)])
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",   # explicit form: `-arch=sm_100a` also emits compute_100 PTX, which rejects tcgen05
+    "-gencode", "arch=compute_90a,code=sm_90a",   # explicit form: `-arch=sm_90a` also emits compute_90 PTX, which rejects wgmma
     "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
 ]
 
@@ -34,7 +34,7 @@ def _nvcc() -> str:
 def stale() -> bool:
     if not os.path.exists(LIB):
         return True
-    if os.environ.get("B200M_NO_BUILD"):       # GPU box: use the library that travelled with the snapshot, whatever the source timestamps say
+    if os.environ.get("B200M_NO_BUILD"):       # use the library as built, whatever the source timestamps say (e.g. a read-only tree)
         return False
     t = os.path.getmtime(LIB)
     return any(os.path.getmtime(f) > t for f in _deps())
@@ -45,7 +45,7 @@ def build_native(force: bool = False, verbose: bool = False) -> str:
     if not force and not stale():
         return LIB
     env = dict(os.environ)
-    env.pop("CXX", None); env.pop("CC", None)       # the image exports a gcc wrapper without OpenMP specs; nvcc finds /usr/bin/g++
+    env.pop("CXX", None); env.pop("CC", None)       # nvcc picks its host compiler itself; a CXX wrapper without OpenMP specs breaks it
     cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + [os.path.join(CSRC, s) for s in SOURCES] + ["-o", LIB]
     r = subprocess.run(cmd, env=env, capture_output=True, text=True)
     if r.returncode != 0:

@@ -22,8 +22,7 @@ enum : uint32_t {
 
 // One uploaded view (image) resident in HBM.
 struct alignas(128) ViewDev {
-  CUtensorMap tmap128;  // fp16 [m x 128], box {64 x 128 rows}, SWIZZLE_128B (query tiles; only when dim == 128 scalar)
-  CUtensorMap tmap256;  // same tensor, box {64 x 256 rows}: one box = one K-half of a database tile
+  CUtensorMap tmap128;  // fp16 [m x 128], box {64 x 128 rows}, SWIZZLE_128B: one K-block of a query or database tile (only when dim == 128 scalar)
   CUtensorMap tmap_aug; // fp16 [m_pad x 16] half-norm limbs, box {16 x 128 rows}, SWIZZLE_32B (9th K-step of the AUG kernel)
   CUtensorMap tmap_augq; // the same for augq16 (the view as QUERY of the real-valued kernel: its own half-norm limbs as A columns)
   const void* raw;      // descriptors as STORED, row-major m x dim: f32 / u8 / 64-byte binary; `dtype` is the storage type (integer-valued
@@ -54,10 +53,10 @@ struct PairDev {
 enum : uint32_t { PM_TC = 0, PM_EXACT_F32 = 1, PM_EXACT_U8 = 2, PM_HAMMING = 3, PM_SKIP = 4,
                   PM_TC_FUSED = 5 /* tensor-core pair whose kernel also ran the exactness pass: candidates are final */,
                   PM_GENERIC_F32 = 6, PM_GENERIC_U8 = 7 /* scalar descriptors whose length is not 128 (AKAZE float 64, LIOP 144): one warp per query */,
-                  PM_TC_REAL = 8 /* real-valued fp32 pair on the tensor-core FILTER kernel (l2_tc2.cuh MODE_REAL): its candidates are made final by
+                  PM_TC_REAL = 8 /* real-valued fp32 pair on the tensor-core FILTER kernel (l2_tc.cuh MODE_REAL): its candidates are made final by
                                     the exact re-scoring (in-kernel or rescore_real_kernel) and the exact_rows fallback before they are packed */ };
 
-// Work item of the tensor-core kernel: 128 consecutive queries of pair `pair` against the whole database image.
+// Work item of the tensor-core kernel: 128 or 256 (per launch) consecutive queries of pair `pair` against the whole database image.
 struct WorkItem { uint32_t pair, qtile; };
 
 // Candidate produced by a search kernel, one per query that passed the (pre-)ratio test.

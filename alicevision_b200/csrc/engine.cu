@@ -12,7 +12,6 @@
 #include "hamming.cuh"
 #include "l2_exact.cuh"
 #include "l2_tc.cuh"
-#include "l2_tc2.cuh"
 #include "prep.cuh"
 #include "verify.cuh"
 #include "hostconv.hpp"
@@ -257,7 +256,6 @@ struct b200m_ctx {
   std::recursive_mutex api_mu;
   unsigned int* d_err = nullptr;
   long long* d_trace = nullptr;   // optional pipeline trace of CTA 0 (debug)
-  int dbg_ablate = 0;             // debug-only ablation switch of the CTA-pair kernel (results are WRONG when non-zero)
   std::vector<cudaEvent_t> tev;   // search-kernel timing events, reused across calls
   cudaEvent_t ev_start = nullptr, ev_end = nullptr;
   std::unique_ptr<Pool> pool;
@@ -269,8 +267,9 @@ struct b200m_ctx {
   bool real_tc = true;            // real-valued fp32 pairs on the tensor-core filter kernel (B200M_REAL_TC=0: exact CUDA-core kernel as in round 1)
   int first_batch_pairs = 16;     // while uploads are in flight: pairs of the first batch (then 2x per batch): how soon the GPU starts (B200M_FIRST_BATCH)
   long real_fused_rows = 6144;    // average database rows per item from which the real-valued re-scoring runs inside the filter kernel
-  int tc_variant = 4;             // 1 = single-CTA kernel (l2_tc.cuh); CTA-pair kernel (l2_tc2.cuh): 2 = 8 epilogue warps, 3 = 16 epilogue warps,
-                                  // 4 (default) = 8 epilogue warps + half-norms folded into the GEMM (AUG)
+  int tc_variant = 4;             // tensor-core kernel (l2_tc.cuh): 4 (default) = half-norms folded into the GEMM (AUG), 256-query work items;
+                                  // half-norms added in the epilogue: 2 = 256-query items, 3 = 128-query items, 1 = 128-query items and
+                                  // the stand-alone exactness pass (2-4 re-score in the kernel when the database images are long)
   // last-call instrumentation
   double last_gpu_ms = 0, last_search_ms = 0; int last_launches = 0, last_tc_pairs = 0; int64_t last_records = 0;
   int last_real_pairs = 0; int64_t last_fallback_rows = 0;      // real-valued pairs on the tensor-core filter kernel; queries left to the exact_rows fallback
@@ -295,7 +294,7 @@ static int alloc_view_buffers(b200m_ctx* c, ViewHost& v) {
   const size_t esz = v.store_dtype() == DT_F32 ? 4 : 1;
   auto al = [](size_t x) { return (x + 255) / 256 * 256; };
   const bool tcv = v.tc_capable(), pos = !v.xy.empty();
-  if (tcv) v.m_pad = (v.m + tc::BN - 1) / tc::BN * tc::BN;
+  if (tcv) v.m_pad = (v.m + tc::ROW_PAD - 1) / tc::ROW_PAD * tc::ROW_PAD;
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off += al(std::max<size_t>(bytes, 1)); return o; };
   const size_t o_raw = take(std::max<size_t>((size_t)v.m * v.dim * esz, 256));
@@ -330,9 +329,9 @@ static int make_view_dev(b200m_ctx* c, const ViewHost& v, ViewDev& d) {
     const cuuint64_t gdim[2] = {128, (cuuint64_t)v.m};
     const cuuint64_t gstr[1] = {256};
     const cuuint32_t estr[2] = {1, 1};
-    for (int which = 0; which < 2; ++which) {
-      const cuuint32_t box[2] = {64, which ? 256u : 128u};
-      CUresult r = c->encode(which ? &d.tmap256 : &d.tmap128, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)v.h16, gdim, gstr, box, estr,
+    {
+      const cuuint32_t box[2] = {64, 128};
+      CUresult r = c->encode(&d.tmap128, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)v.h16, gdim, gstr, box, estr,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) return fail(B200M_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
@@ -430,12 +429,10 @@ static int ensure_batch_buffers(b200m_ctx* c) {
     CK(cudaEventCreateWithFlags(&b.ev_copy, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&b.ev_tab, cudaEventDisableTiming));
   }
-  CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tc2::l2_top2_tc2_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::Lay<false>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tc2::l2_top2_tc2_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::Lay<true>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tc2::l2_top2_tc2_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::Lay<false>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tc2::l2_top2_tc2_kernel<8, true, tc2::MODE_REAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::Lay<true, true>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tc2::l2_top2_tc2_kernel<8, true, tc2::MODE_KNN>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::Lay<true>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<false>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true, tc::MODE_REAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true, true>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true, tc::MODE_KNN>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(exact_rows_pairs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XP_SMEM));
   CK(cudaFuncSetAttribute(exact_top2_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, EX_SMEM));
   CK(cudaFuncSetAttribute(exact_top2_kernel<uint8_t, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, EX_SMEM));
@@ -527,7 +524,7 @@ int b200m_ctx_create(int device, void* stream, b200m_ctx** out) {
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(B200M_ERR_UNSUPPORTED, "this build contains sm_100a code only (found sm_" + std::to_string(prop.major * 10 + prop.minor) + ")");
+  if (prop.major != 9 || prop.minor != 0) return fail(B200M_ERR_UNSUPPORTED, "this build contains sm_90a code only (found sm_" + std::to_string(prop.major * 10 + prop.minor) + ")");
   std::unique_ptr<b200m_ctx> c(new b200m_ctx());
   c->device = device; c->num_sms = prop.multiProcessorCount;
   if (stream) { c->stream = (cudaStream_t)stream; }
@@ -616,16 +613,15 @@ int b200m_ctx_set_host_threads(b200m_ctx* c, int n) {
   return B200M_OK;
 }
 int b200m_ctx_set_tc_variant(b200m_ctx* c, int variant) {
-  if (!c || variant < 1 || variant > 4) return fail(B200M_ERR_ARG, "tc variant must be 1 (single CTA), 2 (CTA pair), 3 (CTA pair, 16 epilogue warps) or 4 (CTA pair, half-norms folded into the GEMM)");
+  if (!c || variant < 1 || variant > 4) return fail(B200M_ERR_ARG, "tc variant must be 1 (128-query items, stand-alone exactness pass), 2 (256-query items), 3 (128-query items) or 4 (256-query items, half-norms folded into the GEMM)");
   c->tc_variant = variant;
   return B200M_OK;
 }
 // Debug: enable (n>0) / read back the per-tile pipeline trace of CTA 0 of the tensor-core kernel.
-// out receives 4 roles x TRACE_TILES x 4 SM-clock stamps (producer, MMA issuer, epilogue half 0, epilogue half 1).
+// out receives 4 roles x TRACE_TILES x 4 SM-clock stamps: role 0 the TMA producer (slot free, loads issued), roles 1 and 2 the two
+// consumer warpgroups (before / after the tile's wait, MMAs complete, epilogue done); role 3 is unused.
 int b200m_debug_trace(b200m_ctx* c, int enable, long long* out, int n) {
   if (!c) return fail(B200M_ERR_ARG, "ctx is null");
-  c->dbg_ablate = enable >> 8;   // bits 8+: ablation mode of the CTA-pair kernel (debug only)
-  enable &= 0xff;
   CK(cudaSetDevice(c->device));
   const size_t total = 4ull * ptx::TRACE_TILES * 4;
   if (enable && !c->d_trace) { CK(cudaMalloc((void**)&c->d_trace, total * 8)); CK(cudaMemset(c->d_trace, 0, total * 8)); }
@@ -1127,6 +1123,7 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       if (d.mode == PM_TC_REAL) { real_rows += c->views[d.slot_i].m; ++real_n; }
     }
     const bool fused = c->tc_variant >= 2 && tc_n > 0 && tc_rows / tc_n >= 6144;
+    const int tc_ctas_per_item = (c->tc_variant == 2 || c->tc_variant == 4) ? 2 : 1;
     const bool fused_real = real_n > 0 && real_rows / real_n >= c->real_fused_rows;
     bool any_f32 = false, any_u8 = false, any_ham = false, any_gf32 = false, any_gu8 = false; int max_qblk_gen = 0;
     for (int p = 0; p < np; ++p) {
@@ -1136,9 +1133,9 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       const uint32_t dev_mode = (d.mode == PM_TC && fused) ? (uint32_t)PM_TC_FUSED : d.mode;
       bb.h_pairs[p] = PairDev{(uint32_t)d.slot_i, (uint32_t)d.slot_j, (uint32_t)vi.m, (uint32_t)vj.m, cbase, dev_mode, sbase};
       cbase += (uint32_t)vj.m; sbase += (uint32_t)vi.m;
-      const int qrows = c->tc_variant >= 2 ? 2 * tc2::BM : tc::BM;   // queries per work item
+      const int qrows = tc_ctas_per_item * tc::BM;   // queries per work item
       if (d.mode == PM_TC) for (int qt = 0; qt < (vj.m + qrows - 1) / qrows; ++qt) bb.h_items[n_items++] = WorkItem{(uint32_t)p, (uint32_t)qt};
-      if (d.mode == PM_TC_REAL) for (int qt = 0; qt < (vj.m + 2 * tc2::BM - 1) / (2 * tc2::BM); ++qt) bb.h_items_real[n_items_real++] = WorkItem{(uint32_t)p, (uint32_t)qt};
+      if (d.mode == PM_TC_REAL) for (int qt = 0; qt < (vj.m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items_real[n_items_real++] = WorkItem{(uint32_t)p, (uint32_t)qt};
       if (d.mode == PM_EXACT_F32) { any_f32 = true; max_qblk_exact = std::max(max_qblk_exact, (vj.m + EX_TQ - 1) / EX_TQ); }
       if (d.mode == PM_EXACT_U8) { any_u8 = true; max_qblk_exact = std::max(max_qblk_exact, (vj.m + EX_TQ - 1) / EX_TQ); }
       if (d.mode == PM_HAMMING) { any_ham = true; max_qblk_ham = std::max(max_qblk_ham, (vj.m + HM_TQ - 1) / HM_TQ); }
@@ -1157,18 +1154,12 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
     if (c->pipe_streams) { CK(cudaEventRecord(bb.ev_tab, ts)); CK(cudaStreamWaitEvent(c->stream, bb.ev_tab, 0)); }
     cudaEvent_t k0 = timing_event(c, tev_used), k1 = timing_event(c, tev_used);
     CK(cudaEventRecord(k0, c->stream));
-    if (n_items && c->tc_variant >= 2) {
-      const int grid = 2 * std::min(n_items, c->num_sms / 2);     // CTA pairs (cluster of 2), one pair per work item
-      if (c->tc_variant == 3)
-        tc2::l2_top2_tc2_kernel<16, false><<<grid, 128 + 16 * 32, tc2::Lay<false>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->dbg_ablate, c->d_err, (int)fused, nullptr, FbSink{});
-      else if (c->tc_variant == 4)
-        tc2::l2_top2_tc2_kernel<8, true><<<grid, 128 + 8 * 32, tc2::Lay<true>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->dbg_ablate, c->d_err, (int)fused, nullptr, FbSink{});
+    if (n_items) {
+      const int grid = tc_ctas_per_item * std::min(n_items, c->num_sms / tc_ctas_per_item);   // one CTA per SM, whole work items per CTA group
+      if (c->tc_variant == 4)
+        tc::l2_top2_tc_kernel<true><<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<true>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, tc_ctas_per_item, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->d_err, (int)fused, nullptr, FbSink{});
       else
-        tc2::l2_top2_tc2_kernel<8, false><<<grid, 128 + 8 * 32, tc2::Lay<false>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->dbg_ablate, c->d_err, (int)fused, nullptr, FbSink{});
-      ++launches;
-    } else if (n_items) {
-      const int grid = std::min(n_items, c->num_sms);
-      tc::l2_top2_tc_kernel<<<grid, tc::NUM_THREADS, tc::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, bb.d_cands, bb.d_count, ratio_sq, c->d_trace);
+        tc::l2_top2_tc_kernel<false><<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, tc_ctas_per_item, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->d_err, (int)fused, nullptr, FbSink{});
       ++launches;
     }
     if (n_items_real) {
@@ -1176,8 +1167,8 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       // exact search of the few queries the error bound could not decide; after that their candidates are final like everyone else's
       const int grid = 2 * std::min(n_items_real, c->num_sms / 2);
       const FbSink fbs{bb.d_fb_pair, bb.d_fb_pair_cnt, bb.d_fb, bb.d_fb_count, (int)CAND_CAP, bb.d_fb_count + 1};
-      tc2::l2_top2_tc2_kernel<8, true, tc2::MODE_REAL><<<grid, tc2::block_threads<8, tc2::MODE_REAL>(), tc2::Lay<true, true>::SMEM_BYTES, c->stream>>>(
-          c->d_views, bb.d_pairs, bb.d_items_real, n_items_real, bb.d_cands, bb.d_count, ratio_sq, nullptr, 0, c->d_err, (int)fused_real, bb.d_candx, fbs);
+      tc::l2_top2_tc_kernel<true, tc::MODE_REAL><<<grid, tc::block_threads<tc::MODE_REAL>(), tc::Lay<true, true>::SMEM_BYTES, c->stream>>>(
+          c->d_views, bb.d_pairs, bb.d_items_real, n_items_real, 2, bb.d_cands, bb.d_count, ratio_sq, nullptr, c->d_err, (int)fused_real, bb.d_candx, fbs);
       ++launches;
       if (!fused_real) {
         rescore_real_kernel<<<dim3(np, 4), VERIFY_WARPS_REAL * 32, 0, c->stream>>>(c->d_views, bb.d_pairs, bb.d_cands, bb.d_candx, bb.d_count, ratio_sq, c->d_err, fbs);
@@ -1690,7 +1681,7 @@ int b200m_multi_match(b200m_multi* m, int n_views, const uint32_t* view_ids, con
 // ---- Surface 1: ArrayMatcher ------------------------------------------------------------------------------------
 // Build keeps the dataset RESIDENT in the form the tensor-core kernel reads (fp16 copy, half-norm limbs, tensor maps: the same
 // preparation as an uploaded view), so SearchNeighbours with NN = 2 on 128-D integer-valued descriptors - what RegionsMatcher<ArrayMatcherT>
-// ::Match calls, matching/RegionsMatcher.hpp:140-146 - is one query copy, the preparation kernel, the tcgen05 kernel in its MODE_KNN
+// ::Match calls, matching/RegionsMatcher.hpp:140-146 - is one query copy, the preparation kernel, the tensor-core kernel in its MODE_KNN
 // (both neighbours' chunks kept, every query emitted) and knn_finalize_kernel, out of grow-only scratch: no allocation, one synchronisation.
 int b200m_db_create(b200m_ctx* c, const void* data, int rows, int dim, int dtype, int metric, b200m_db** out) {
   if (!c || !out) return fail(B200M_ERR_ARG, "bad arguments");
@@ -1743,7 +1734,7 @@ static int ensure_knn_scratch(b200m_ctx* c, int nq, int dim, size_t esz) {
   if (nq <= k.cap && raw_bytes <= k.raw_bytes) return B200M_OK;
   CK(cudaStreamSynchronize(c->stream));
   const int cap = std::max(nq, k.cap * 2);
-  const int cap_pad = (cap + tc::BN - 1) / tc::BN * tc::BN;
+  const int cap_pad = (cap + tc::ROW_PAD - 1) / tc::ROW_PAD * tc::ROW_PAD;
   const size_t rb = std::max(raw_bytes, (size_t)cap * dim * esz);
   for (void* q : {(void*)k.raw, (void*)k.h16, (void*)k.nbh, (void*)k.nrm, (void*)k.aug16, (void*)k.augq16, (void*)k.err, (void*)k.cands, (void*)k.idx, (void*)k.dist, (void*)k.items}) if (q) cudaFree(q);
   CK(cudaMalloc(&k.raw, rb));
@@ -1786,14 +1777,14 @@ int b200m_knn(b200m_ctx* c, const b200m_db* db, const void* query, int nq, int n
   bool done = false;
   if (nn == 2 && v.tc_ok() && !c->force_exact && c->tc_variant == 4 && v.m <= 16 * 0xFFFF) {
     ViewHost qv;
-    qv.m = nq; qv.dim = v.dim; qv.dtype = v.dtype; qv.m_pad = (nq + tc::BN - 1) / tc::BN * tc::BN;
+    qv.m = nq; qv.dim = v.dim; qv.dtype = v.dtype; qv.m_pad = (nq + tc::ROW_PAD - 1) / tc::ROW_PAD * tc::ROW_PAD;
     qv.raw = k.raw; qv.h16 = k.h16; qv.nbh = k.nbh; qv.nrm = k.nrm; qv.aug16 = k.aug16; qv.augq16 = k.augq16; qv.err = k.err; qv.stats = d_stats;
     ViewDev hv[2];
     hv[0] = db->dev;
     if ((rc = make_view_dev(c, qv, hv[1]))) return rc;
     CK(cudaMemsetAsync(d_flag, 0, 4, st));
     if ((rc = run_prep(c, qv, d_flag, st))) return rc;
-    const int n_items = (nq + 2 * tc2::BM - 1) / (2 * tc2::BM);
+    const int n_items = (nq + 2 * tc::BM - 1) / (2 * tc::BM);
     std::vector<WorkItem> items(n_items);
     for (int t = 0; t < n_items; ++t) items[t] = WorkItem{0u, (uint32_t)t};
     const PairDev hp{0u, 1u, (uint32_t)v.m, (uint32_t)nq, 0u, (uint32_t)PM_TC, 0u};
@@ -1801,8 +1792,8 @@ int b200m_knn(b200m_ctx* c, const b200m_db* db, const void* query, int nq, int n
     CK(cudaMemcpyAsync(d_pair, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(k.items, items.data(), sizeof(WorkItem) * n_items, cudaMemcpyHostToDevice, st));
     const int grid = 2 * std::min(n_items, c->num_sms / 2);
-    tc2::l2_top2_tc2_kernel<8, true, tc2::MODE_KNN><<<grid, 128 + 8 * 32, tc2::Lay<true>::SMEM_BYTES, st>>>(
-        d_views, d_pair, k.items, n_items, k.cands, nullptr, 0.f, nullptr, 0, c->d_err, 0, nullptr, FbSink{});
+    tc::l2_top2_tc_kernel<true, tc::MODE_KNN><<<grid, tc::block_threads<tc::MODE_KNN>(), tc::Lay<true>::SMEM_BYTES, st>>>(
+        d_views, d_pair, k.items, n_items, 2, k.cands, nullptr, 0.f, nullptr, c->d_err, 0, nullptr, FbSink{});
     knn_finalize_kernel<<<(nq + 7) / 8, 256, 0, st>>>(d_views, d_pair, k.cands, k.idx, (float*)k.dist, c->d_err);
     CK(cudaGetLastError());
     uint32_t qflags = 0;

@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk[.tensor]), tcgen05 (MMA / TMEM).
-// Hand-written for this engine; encodings cross-checked against the PTX ISA 8.8 text and the CuTe
-// headers shipped in the image (cute/arch/mma_sm100_desc.hpp, copy_sm90_tma.hpp, copy_sm100.hpp).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk[.tensor]), wgmma (warpgroup MMA from shared memory).
+// Hand-written for this engine; encodings follow the PTX ISA text (wgmma matrix descriptors, "Asynchronous Warpgroup Level
+// Matrix Multiply-Accumulate") and the CuTe headers shipped with CUDA (cute/arch/mma_sm90_desc.hpp, copy_sm90_tma.hpp).
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -9,16 +9,6 @@ namespace b200m {
 namespace ptx {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -44,7 +34,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must surface as a trap (reported as a CUDA error) instead of hanging the box.
+// Bounded wait: a protocol bug must surface as a trap (reported as a CUDA error) instead of hanging the device.
 #ifndef B200M_WAIT_TIMEOUT_NS
 #define B200M_WAIT_TIMEOUT_NS 4000000000ull
 #endif
@@ -81,142 +71,46 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols) : "memory");
+// ---------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor of a K-major operand (cute/arch/mma_sm90_desc.hpp GmmaDescriptor):
+//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major, 1) |
+//   [32,46) stride byte offset >> 4 (distance between 8-row groups) | [62,64) layout: 1 = SWIZZLE_128B, 3 = SWIZZLE_32B
+// 128-byte swizzle: rows of 64 fp16, 8 rows * 128 B = 1024 B between row groups; K advances by +32 B per K16 step.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ void tmem_relinquish() { asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// 32-byte swizzle: rows of 16 fp16 (one K16 step), 8 rows * 32 B = 256 B between row groups.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw32(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)3 << 62);
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (=1, unused for swizzled K-major)
-//   [32,46) stride byte offset >> 4 (8 rows * 128 B = 1024 -> 64) | [46,48) version = 1 | [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// Same for a K-major operand whose rows are 32 bytes (16 fp16) wide with 32-byte swizzle: 8 rows * 32 B = 256 B between
-// row groups, layout = 6 (SWIZZLE_32B).
-__device__ __forceinline__ uint64_t umma_desc_k_sw32(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(256 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)6 << 61;
-  return d;
-}
-// Instruction descriptor, kind::f16, F16 x F16 -> F32, both operands K-major (InstrDescriptor in the same header):
-//   [4,6) c_format = 1 (F32) | [7,10) a_format = 0 (F16) | [10,13) b_format = 0 | [13] a_negate | [14] b_negate
-//   [15] a_major = 0 (K) | [16] b_major = 0 (K) | [17,23) N >> 3 | [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N, bool neg_a, bool neg_b) {
-  return (1u << 4) | ((neg_a ? 1u : 0u) << 13) | ((neg_b ? 1u : 0u) << 14) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 128] (+)= A[64 x 16] * (-B[128 x 16])^T, fp16 inputs from shared memory, fp32 accumulators in registers (the whole warpgroup
+// issues it).  Thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 + {0, 8}, columns 8*j + 2*(t%4) + {0, 1}, j = 0..15:
+// d[4j + 0/1] on the first row, d[4j + 2/3] on the second.  B is negated by the instruction (imm-scale-b = -1).
+__device__ __forceinline__ void wgmma_m64n128k16_f16_negb(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued MMAs of this thread arrive (once) on the mbarrier when they complete.
-// Implies tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---------------------------------------------------------------- 2-CTA (cta_group::2) variants and cluster helpers
-// A CTA pair (cluster of 2 on one TPC) executes one M=256 MMA: each CTA supplies 128 rows of A and 128 rows of B from
-// its own shared memory (same offsets in both CTAs) and receives 128 accumulator rows in its own TMEM.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address -> even (leader) CTA
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}\n"   // default .release.cta: a cluster-scope release costs a full fence per tile
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-// TMA load issued by either CTA of the pair; completion bytes are credited to the LEADER CTA's barrier.
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() { asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Completion of all prior MMAs of this thread arrives on the barrier at this offset in every CTA of `cta_mask`.
-__device__ __forceinline__ void umma_commit_2sm_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive 32-bit columns (thread t gets lane t of the warp's quadrant).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, -1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 3-input float min (sm_100+: one FMNMX3).
-__device__ __forceinline__ float fmin3(float a, float b, float c) {
-  float d;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-
-// Packed fp32x2 add (sm_100+: one FADD2 for two columns): (o0,o1) = (a0,a1) + (b0,b1), round-to-nearest like FADD.
-__device__ __forceinline__ void add_f32x2(float& o0, float& o1, float a0, float a1, float b0, float b1) {
-  uint64_t x, y, z;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(x) : "f"(a0), "f"(a1));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(y) : "f"(b0), "f"(b1));
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(z) : "l"(x), "l"(y));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(o0), "=f"(o1) : "l"(z));
 }
 
 // Optional pipeline trace (debug): SM-clock timestamps of one CTA's roles, written only when `trace` is non-null.

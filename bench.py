@@ -2,7 +2,7 @@
 """bench.py — image-pairs matched/sec on the descriptor-matching hot path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 1|2|3|sweep]
-                    [--features M] [--images I] [--dtype f32|u8|bin] [--data int|real] [--cpu-seconds S]
+                    [--features M] [--images I] [--dtype f32|u8|bin] [--data int|real] [--cpu-seconds S] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over the rank's shard of the pair list.  Default (N=1): BASELINE configs[1],
 100 synthetic images x 8192 SIFT features, exhaustive 4950 pairs.  Printed by rank 0 as ONE JSON line:
@@ -12,7 +12,8 @@ One "step" = one pass of the hot path over the rank's shard of the pair list.  D
                kernels, D2H of the records); max over ranks
   e2e          the same pairs through the reference-facing C-ABI call chain with HOST buffers, wall clock:
                b200m_clear_views + b200m_upload_views_async (H2D inside) + b200m_match_pairs(STAGE_FULL) + result arrays
-  roofline     dominant kernel (tcgen05 distance GEMM + fused top-2): 2*M^2*128 FLOP per pair / its own device time
+  roofline     dominant kernel (wgmma distance GEMM + fused top-2): 2*M^2*128 FLOP per pair / its own device time, against the
+               H100 SXM data-sheet peak (the card's name and power limit are printed under "gpu")
   cpu_baseline the reference's CPU brute force (oracle/_ref, else the port) on a bounded sample of the same pairs
 
 Multi-GPU (torchrun, one rank per GPU): pairs are independent, so the pair list is sharded (2-D blocks of the pair matrix,
@@ -20,6 +21,10 @@ b200m_shard_pairs_2d: a rank uploads only the views its blocks touch) and there 
 torch.distributed is used for the barrier and the max-over-ranks reduction of the timings only.
 --config 1 (default): weak scaling, ~4950 pairs per GPU.  --config 2 / 3 = BASELINE configs[2] / [3]: a FIXED list
 (1000 x 8k SIFT vocabulary-tree style / 500 x 16k AKAZE-MLDB exhaustive) split over the ranks: strong scaling.
+
+--dump-outputs DIR writes what the last timed step returned (rank 0's shard) as .npy files: pairs, offsets and the match fields
+(i, j, distance, ratio; a fixed seeded sample when there are more than fit in 64 MB), so that two builds can be compared output
+for output on identical inputs.
 """
 from __future__ import annotations
 
@@ -55,12 +60,14 @@ def parse():
     ap.add_argument("--dtype", default="f32", choices=["f32", "u8", "bin"])
     ap.add_argument("--data", default="int", choices=["int", "real"], help="real = real-valued fp32 descriptors (not integer-valued)")
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="budget of the cpu_baseline sample")
-    ap.add_argument("--tc-variant", type=int, default=4, choices=[1, 2, 3, 4], help="4 = CTA-pair tcgen05 kernel, half-norms folded into the GEMM (default); 2/3 = CTA pair with epilogue add (8/16 epilogue warps); 1 = single-CTA kernel")
+    ap.add_argument("--tc-variant", type=int, default=4, choices=[1, 2, 3, 4], help="4 = half-norms folded into the GEMM, 256-query work items (default); "
+                    "half-norms added in the epilogue: 2 = 256-query items, 3 = 128-query items, 1 = 128-query items + stand-alone exactness pass")
     ap.add_argument("--pairs", default="", choices=["", "exhaustive", "voctree"],
                     help="voctree = synthetic vocabulary-tree style list, 50 neighbours per image (default for --config 2)")
     ap.add_argument("--sharding", default="2d", choices=["2d", "rows"], help="multi-rank split of the pair list: 2-D blocks (default) or by database image")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed step's results as DIR/<name>.npy")
     a = ap.parse_args()
     if a.config == "3":
         a.dtype = "bin"
@@ -108,7 +115,7 @@ def shard_pairs(pairs: np.ndarray, rank: int, world: int, how: str) -> np.ndarra
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -240,31 +247,44 @@ def cpu_baseline_cascade(views, pairs, budget_s):
                       "reference headers with plain-loop stand-ins for Eigen's MatrixXf/VectorXf (timing baseline, results unpinned)"}
 
 
-def ncu_traffic(kernel_key: str):
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture (profiles/traffic.json), or None."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
+# NVIDIA H100 SXM data sheet (a card allowed 700 W): dense FP16 tensor rate and HBM3 bandwidth.  A card with a lower power limit
+# reaches less; "gpu" in the output names the card and its limit.
+H100_FP16_TFLOPS = 989.4
+H100_HBM_GBS = 3350.0
+PEAK_SOURCE = "NVIDIA H100 SXM data sheet, dense FP16 (700 W); not a measured figure"
+
+
+def gpu_info(index: int) -> dict:
+    """Name, power limit and maximum SM clock of the GPU the numbers were measured on."""
     try:
-        return json.load(open(p)).get(kernel_key)
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        name, plim, smax = [x.strip() for x in r.stdout.strip().splitlines()[0].split(",")[:3]]
+        return {"name": name, "power_limit_w": float(plim), "sm_max_mhz": float(smax)}
     except Exception:
-        return None
+        return {"name": None, "power_limit_w": None, "sm_max_mhz": None}
 
 
-def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1449.7), "measured (MEASURED_PEAKS.json bf16_tflops_sustained: kernel timed inside a long step)"
-    return 1400.0, "fallback (B200_PROFILING.md: ~1.4 PFLOP/s sustained)"
+DUMP_BYTES = 60 * 10**6      # array bytes; with the .npy headers the files stay below 64 MB
 
 
-def burst_peak():
-    """The burst (kernel-timed-alone) bf16 figure of MEASURED_PEAKS.json, reported next to `frac` because the sustained figure was taken at a
-    1372 MHz median clock under random data and this kernel holds a higher clock: a `frac` above 1 is a statement about clocks, not about the pipe."""
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    try:
-        return float(json.load(open(p)).get("bf16_tflops"))
-    except Exception:
-        return None
+def dump_outputs(out_dir: str, result) -> None:
+    """The arrays a caller of the timed path receives (pair list, per-pair offsets, match records), as float64 / float32 .npy files.
+    Past DUMP_BYTES the match records are a fixed seeded sample (match_index.npy holds the sampled record indices)."""
+    pair_ids, offsets, matches = result
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "pairs.npy"), np.asarray(pair_ids, np.float64))
+    np.save(os.path.join(out_dir, "offsets.npy"), np.asarray(offsets, np.float64))
+    n = len(matches)
+    cap = (DUMP_BYTES - 8 * (np.asarray(pair_ids).size + len(offsets))) // (8 + 8 + 8 + 4 + 4)
+    idx = np.arange(n) if n <= cap else np.sort(np.random.default_rng(0).choice(n, cap, replace=False))
+    if n > cap:
+        np.save(os.path.join(out_dir, "match_index.npy"), idx.astype(np.float64))
+    sel = matches[idx]
+    np.save(os.path.join(out_dir, "match_i.npy"), sel["i"].astype(np.float64))
+    np.save(os.path.join(out_dir, "match_j.npy"), sel["j"].astype(np.float64))
+    np.save(os.path.join(out_dir, "match_distance.npy"), sel["dist"].astype(np.float32))
+    np.save(os.path.join(out_dir, "match_ratio.npy"), sel["ratio"].astype(np.float32))
 
 
 def workload_text(args, n_img, n_pairs):
@@ -390,14 +410,20 @@ def main():
     sampler = ClockSampler(local) if rank == 0 else None
     barrier()
     t0w = time.time()
-    gpu_ms = 0.0; search_ms = 0.0; launches = 0; records = 0
-    for _ in range(args.steps):
-        m.match_uploaded(mine, matching.STAGE_FULL)
+    gpu_ms = 0.0; search_ms = 0.0; launches = 0; records = 0; last = None
+    for step in range(args.steps):
+        res = m.match_uploaded(mine, matching.STAGE_FULL)
+        if args.dump_outputs and step == args.steps - 1:
+            last = res
+        del res
         gpu_ms += ctx.last_gpu_ms(); search_ms += ctx.last_search_kernel_ms(); launches += ctx.last_launches(); records += ctx.last_records()
     barrier()
     t1w = time.time()
     clocks = sampler.stop(t0w, t1w) if sampler else None
     tc_pairs = ctx.last_tc_pairs(); errs = ctx.exactness_errors(); real_pairs = ctx.last_real_tc_pairs(); fb_rows = ctx.last_fallback_rows()
+    if last is not None and rank == 0:
+        dump_outputs(args.dump_outputs, last)
+    del last
 
     # ---- e2e: host buffers -> upload -> match -> D2H -> finishing -> result arrays -------------------------------------
     e2e_s = 0.0; h2d = 0; d2h = 0; e2e_steps = 0
@@ -433,7 +459,7 @@ def main():
     if rank == 0:
         M = args.features
         flop_pair = 2.0 * M * M * 128
-        peak, peak_src = peaks()
+        peak, peak_src = H100_FP16_TFLOPS, PEAK_SOURCE
         # the roofline kernel's rate on ONE GPU: the slowest rank's search-kernel time against the largest shard
         achieved = mx[0].item() * flop_pair / (ms_search * 1e-3) / 1e12 if not hamming else None
         out = {
@@ -445,13 +471,13 @@ def main():
             "config": {"workload": workload_text(args, n_img, n_pairs),
                        "pairs_per_gpu": n_pairs / world, "max_pairs_on_a_gpu": mx[0].item(), "views_per_gpu": views_sum / world, "max_views_on_a_gpu": mx[1].item(),
                        "sharding": ("2-D blocks of the pair matrix (b200m_shard_pairs_2d)" if args.sharding == "2d" else "pairs dealt round-robin by database image") + ", no collective on the data path",
-                       "l2_policy": f"inputs larger than L2 ({mx[1].item() * M * (64 if hamming else 256) / 1e6:.0f} MB of resident descriptors per GPU vs 126 MB L2)",
+                       "l2_policy": f"inputs larger than L2 ({mx[1].item() * M * (64 if hamming else 256) / 1e6:.0f} MB of resident descriptors per GPU vs 50 MB L2)",
                        "value_timing": "CUDA events: first enqueue of the step -> last match list landed in pinned host memory (b200m_match_pairs STAGE_FULL on resident views)",
                        "tensor_core_pairs": tc_pairs, "real_valued_tensor_core_pairs": real_pairs,
                        "fallback_rows_per_step": fb_rows, "fallback_rows_fraction_of_queries": (fb_rows / (real_pairs * M)) if real_pairs else 0.0,
                        "exactness_errors": errs, "wall_ms_per_step": ms_wall, "records_per_step": records / args.steps,
                        "host": cores_info(), "numa": numa},
-            "clocks": clocks, "gpu_launches": int(launches),
+            "gpu": gpu_info(local), "clocks": clocks, "gpu_launches": int(launches),
             "e2e": {"value": (n_pairs / (ms_e2e * 1e-3)) if ms_e2e > 0 else None, "unit": "pairs/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                     "steps": e2e_steps,
                     "what": "b200m_clear_views + b200m_upload_views_async (every view the shard references, from pageable host memory; integer-valued fp32 staged as "
@@ -460,22 +486,17 @@ def main():
         }
         if hamming:
             hb = mx[0].item() * 2.0 * M * 64 / (ms_search * 1e-3) / 1e9
-            hp = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 6650.0) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
-            tr = ncu_traffic("hamming_top2_kernel")
-            out["roofline"] = {"bound": "hbm", "achieved": hb, "peak": hp, "unit": "GB/s", "frac": hb / hp, "traffic": tr["dram_bytes_per_launch"] if tr else None,
-                               "traffic_note": tr["note"] if tr else None, "kernel": "hamming_top2_kernel", "kernel_ms_per_step": ms_search,
+            hp = H100_HBM_GBS
+            out["roofline"] = {"bound": "hbm", "achieved": hb, "peak": hp, "unit": "GB/s", "frac": hb / hp, "peak_source": "NVIDIA H100 SXM data sheet, HBM3",
+                               "kernel": "hamming_top2_kernel", "kernel_ms_per_step": ms_search,
                                "note": "integer-ALU bound by construction (M^2 x (16 XOR + 22 LOP3 + 5 POPC) per pair vs 2*M*64 bytes); HBM fraction reported because the north star asks"}
         else:
-            tr = (ncu_traffic("l2_top2_tc2_kernel") if tc_pairs > 0 else ncu_traffic("l2_top2_tc2_kernel_real") if real_pairs > 0 else None) if (args.tc_variant == 4 and M == 8192) else None
-            kern = {1: "tc::l2_top2_tc_kernel", 2: "tc2::l2_top2_tc2_kernel<8,false> (cta_group::2)", 3: "tc2::l2_top2_tc2_kernel<16,false> (cta_group::2)",
-                    4: "tc2::l2_top2_tc2_kernel<8,true> (cta_group::2, K=128+16)"}[args.tc_variant] if tc_pairs > 0 else (
-                        "tc2::l2_top2_tc2_kernel<8,true,MODE_REAL> (cta_group::2, fp16-rounded filter GEMM, K=128+16) + exact re-scoring in the reference's fp32 order + exact_rows fallback"
+            kern = {1: "tc::l2_top2_tc_kernel<false> (128-query items, stand-alone exactness pass)", 2: "tc::l2_top2_tc_kernel<false> (256-query items)",
+                    3: "tc::l2_top2_tc_kernel<false> (128-query items)", 4: "tc::l2_top2_tc_kernel<true> (wgmma, K=128+16)"}[args.tc_variant] if tc_pairs > 0 else (
+                        "tc::l2_top2_tc_kernel<true,MODE_REAL> (wgmma fp16-rounded filter GEMM, K=128+16) + exact re-scoring in the reference's fp32 order + exact_rows fallback"
                         if real_pairs > 0 else "exact_top2_kernel<float> (CUDA cores, reference summation order)")
             out["roofline"] = {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                               "traffic": tr["dram_bytes_per_launch"] if tr else None, "traffic_note": tr["note"] if tr else None,
-                               "kernel": kern, "peak_source": peak_src, "flop_per_pair": flop_pair, "kernel_ms_per_step": ms_search,
-                               "peak_burst": burst_peak(), "frac_of_burst_peak": (achieved / burst_peak()) if burst_peak() else None,
-                               "ncu_tensor_pipe_pct": tr.get("tensor_pipe_pct") if tr else None}
+                               "kernel": kern, "peak_source": peak_src, "flop_per_pair": flop_pair, "kernel_ms_per_step": ms_search}
         if not args.no_cpu and world == 1:      # contract: the CPU baseline is timed on rank 0 at N=1 only
             sub = pairs[np.random.default_rng(0).permutation(len(pairs))] if args.config == "1" else np.array([p for p in pairs if int(p[0]) in views and int(p[1]) in views], np.uint32)
             out["cpu_baseline"] = cpu_baseline(views, sub, hamming, args.cpu_seconds)

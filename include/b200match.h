@@ -1,5 +1,5 @@
 /*
- * b200match — C ABI of the Blackwell (sm_100a) descriptor-matching engine.
+ * b200match — C ABI of the H100 (sm_90a) descriptor-matching engine.
  *
  * Drop-in boundary for the one hot path of AliceVision's featureMatching step.  Every entry point below is what
  * a reference-side adaptor binds (see INTEGRATION.md and alicevision_b200/adaptor/):
@@ -58,8 +58,9 @@ void b200m_ctx_destroy(b200m_ctx* ctx);
 int b200m_ctx_set_host_threads(b200m_ctx* ctx, int n);
 /* force every L2 pair through the exact CUDA-core kernels (testing / A-B comparison); default 0 */
 int b200m_ctx_set_force_exact(b200m_ctx* ctx, int on);
-/* tensor-core kernel variant (A-B comparison): 4 = CTA pair (cta_group::2) with the half-norms folded into the GEMM (default),
- * 2 / 3 = CTA pair with an add in the epilogue (8 / 16 epilogue warps), 1 = single CTA */
+/* tensor-core kernel variant (A-B comparison): 4 = half-norms folded into the GEMM, 256-query work items (default);
+ * half-norms added in the epilogue: 2 = 256-query work items, 3 = 128-query work items, 1 = 128-query work items with the
+ * exactness pass in a separate kernel */
 int b200m_ctx_set_tc_variant(b200m_ctx* ctx, int variant);
 
 /* debug / test hook, host only: the checked fp32 -> uchar conversion the upload staging applies to integer-valued fp32 descriptors
@@ -67,7 +68,8 @@ int b200m_ctx_set_tc_variant(b200m_ctx* ctx, int variant);
  * holds them; 0 = some value is not (dst unspecified); -1 = bad arguments. */
 int b200m_debug_convert_f32_u8(const float* src, uint8_t* dst, size_t n, int which);
 
-/* debug: per-tile SM-clock trace of CTA 0 of the tensor-core kernel (4 roles x 512 tiles x 4 stamps); enable!=0 allocates,
+/* debug: per-tile SM-clock trace of CTA 0 of the tensor-core kernel (4 roles x 512 tiles x 4 stamps: TMA producer, the two
+ * consumer warpgroups, unused); enable!=0 allocates,
  * out (may be NULL) receives up to n values after synchronising */
 int b200m_debug_trace(b200m_ctx* ctx, int enable, long long* out, int n);
 

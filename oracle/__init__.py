@@ -4,11 +4,14 @@ ctypes front-end for the two CPU checkers:
 
 * ``Oracle("ref")``  -> oracle/_ref/libref_oracle.so: the reference's own headers
   (ArrayMatcher_bruteForce.hpp, metric.hpp, Hamming.hpp, filters.hpp, RegionsMatcher.hpp,
-  IndMatch.hpp, IndMatchDecorator.hpp) compiled verbatim from /root/reference/src.
+  IndMatch.hpp, IndMatchDecorator.hpp) compiled verbatim from an AliceVision source tree (``ALICEVISION_SRC``).
 * ``Oracle("port")`` -> oracle/libport_oracle.so: the from-scratch restatement.
 
 Only tests/, ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline / ``--impl reference``
 legs may import this package.  The product (alicevision_b200/) never does.
+
+``reference_output()`` lets a test compare with the compiled reference without it: the reference's outputs are stored
+in tests/golden/reference_outputs.npz and replayed when oracle/_ref is not built.
 """
 from __future__ import annotations
 
@@ -24,15 +27,31 @@ DT_F32, DT_U8, DT_BIN = 0, 1, 2
 MATCH_DTYPE = np.dtype([("i", np.uint32), ("j", np.uint32), ("ratio", np.float32), ("dist", np.float32)])
 
 
+# Where the build machine keeps the (read-only) AliceVision checkout the oracle is compiled against, when ALICEVISION_SRC does not say.
+DEFAULT_REFERENCE_SRC = "/root/reference/src"
+
+
+def reference_src() -> str | None:
+    """The `src` directory of the AliceVision checkout: ALICEVISION_SRC, else DEFAULT_REFERENCE_SRC; None when neither is a readable
+    AliceVision tree (the tests then use the reference's stored outputs)."""
+    for src in (os.environ.get("ALICEVISION_SRC"), DEFAULT_REFERENCE_SRC):
+        if src and os.access(os.path.join(src, "aliceVision", "matching", "ArrayMatcher_bruteForce.hpp"), os.R_OK):
+            return src
+    return None
+
+
 def build(ref: bool | None = None) -> None:
-    """Compile the oracle libraries (port always; ref when /root/reference is present)."""
+    """Compile the oracle libraries (port always; ref and the C++ adaptor test when reference_src() finds an AliceVision tree)."""
+    src = reference_src()
     if ref is None:
-        ref = os.path.isdir("/root/reference/src")
-    targets = ["all"] + (["ref"] if ref else [])
+        ref = src is not None
+    if ref and src is None:
+        raise RuntimeError("the compiled reference needs an AliceVision source tree: set ALICEVISION_SRC to its src directory")
+    targets = ["all"] + (["ref", f"REF={src}"] if ref else [])
     subprocess.run(["make", "-C", _HERE] + targets, check=True, stdout=subprocess.DEVNULL)
     # the C++ adaptor test needs the reference's interface headers AND the built CUDA library
     if ref and os.path.exists(os.path.join(os.path.dirname(_HERE), "alicevision_b200", "libb200match.so")):
-        subprocess.run(["make", "-C", _HERE, "adaptor"], check=True, stdout=subprocess.DEVNULL)
+        subprocess.run(["make", "-C", _HERE, "adaptor", f"REF={src}"], check=True, stdout=subprocess.DEVNULL)
 
 
 def available(kind: str) -> bool:
@@ -262,7 +281,7 @@ class Oracle:
 
 class VoctreeOracle:
     """CPU statement of the vocabulary-tree pair-list producer (oracle/voctree_oracle.cpp): kind "ref" = the reference's own
-    VocabularyTree.hpp / VocabularyTree.cpp compiled from /root/reference, kind "port" = the restatement."""
+    VocabularyTree.hpp / VocabularyTree.cpp compiled from the AliceVision sources, kind "port" = the restatement."""
 
     def __init__(self, kind: str = "port"):
         assert kind in ("ref", "port")
@@ -316,3 +335,197 @@ def best(prefer_ref: bool = True) -> Oracle:
     if prefer_ref and available("ref"):
         return Oracle("ref")
     return Oracle("port")
+
+
+# ---------------------------------------------------------------------------------------------- stored reference outputs
+REFERENCE_OUTPUTS = os.path.join(os.path.dirname(_HERE), "tests", "golden", "reference_outputs.npz")
+_stored: dict | None = None
+
+
+def _flatten(key, v, out):
+    if v is None:
+        out[key + "#none"] = np.array(0)
+    elif isinstance(v, dict):
+        ks = list(v)
+        out[key + "#dict"] = np.array(ks, np.int64).reshape(len(ks), -1) if ks else np.zeros((0, 2), np.int64)
+        for n, k in enumerate(ks):
+            _flatten(f"{key}/{n}", v[k], out)
+    elif isinstance(v, (tuple, list)):
+        out[key + "#tuple"] = np.array(len(v))
+        for n, x in enumerate(v):
+            _flatten(f"{key}/{n}", x, out)
+    else:
+        out[key] = np.asarray(v)
+
+
+def _unflatten(key, z):
+    if key + "#none" in z:
+        return None
+    if key + "#dict" in z:
+        ks = z[key + "#dict"]
+        return {tuple(int(x) for x in k): _unflatten(f"{key}/{n}", z) for n, k in enumerate(ks)}
+    if key + "#tuple" in z:
+        return tuple(_unflatten(f"{key}/{n}", z) for n in range(int(z[key + "#tuple"])))
+    a = z[key]
+    return a.item() if a.ndim == 0 else a
+
+
+def _same(a, b) -> bool:
+    if isinstance(a, dict):
+        return isinstance(b, dict) and a.keys() == b.keys() and all(_same(a[k], b[k]) for k in a)
+    if isinstance(a, (tuple, list)):
+        return isinstance(b, (tuple, list)) and len(a) == len(b) and all(_same(x, y) for x, y in zip(a, b))
+    return np.array_equal(np.asarray(a), np.asarray(b))
+
+
+def _save_flat(path, flat):
+    """All arrays in one byte block + a JSON index (name, dtype, shape, offset): one compressed entry instead of one per array."""
+    import json
+    index, parts, off = [], [], 0
+    for k in sorted(flat):
+        a = np.asarray(flat[k])            # (ascontiguousarray would turn 0-d into 1-d)
+        index.append([k, np.lib.format.dtype_to_descr(a.dtype), list(a.shape), off])
+        parts.append(a.tobytes()); off += a.nbytes
+    np.savez_compressed(path, index=np.array(json.dumps(index)), data=np.frombuffer(b"".join(parts), np.uint8))
+
+
+def _load_flat(path):
+    import json
+    z = np.load(path)
+    data = z["data"].tobytes()
+    out = {}
+    for k, descr, shape, off in json.loads(str(z["index"])):
+        dt = np.lib.format.descr_to_dtype(descr if isinstance(descr, str) else [tuple(f) for f in descr])
+        n = int(np.prod(shape)) * dt.itemsize
+        out[k] = np.frombuffer(data[off:off + n], dt).reshape(tuple(shape)).copy()
+    return out
+
+
+def reference_output(key: str, compute, live: bool):
+    """What the compiled reference returns for test case `key`.  live (the reference is built): compute() it and check it against
+    the stored copy - or, with ORACLE_RECORD_REFERENCE=1, store it (ORACLE_RECORD_REFERENCE=1 python -m pytest tests -m "not gpu"
+    with the reference built rewrites the file).  Otherwise the stored copy, so that the comparison with the reference runs without the
+    reference's sources."""
+    global _stored
+    if _stored is None:
+        _stored = {}
+        if os.path.exists(REFERENCE_OUTPUTS):
+            flat = _load_flat(REFERENCE_OUTPUTS)
+            tops = {k.split("/")[0].split("#")[0] for k in flat}
+            _stored = {t: _unflatten(t, flat) for t in tops}
+    if not live:
+        if key not in _stored:
+            raise KeyError(f"no stored reference output for {key!r}: regenerate {REFERENCE_OUTPUTS} with the reference built")
+        return _stored[key]
+    v = compute()
+    if os.environ.get("ORACLE_RECORD_REFERENCE") == "1":
+        _stored[key] = v
+        out = {}
+        for k, x in _stored.items():
+            _flatten(k, x, out)
+        _save_flat(REFERENCE_OUTPUTS, out)
+    elif key in _stored:
+        assert _same(v, _stored[key]), f"the compiled reference no longer gives the stored output for {key!r}"
+    return v
+
+
+def _digest(h, x):
+    """Feeds a call argument into the hash that names a stored reference output.  A path is named by the content of the file
+    it points to, or by its base name when there is none yet (outputs are written to temporary directories)."""
+    if isinstance(x, (np.ndarray, np.generic)):
+        a = np.ascontiguousarray(x)
+        h.update(f"{a.dtype.str}{a.shape}".encode()); h.update(a.tobytes())
+    elif isinstance(x, (list, tuple)):
+        h.update(f"[{len(x)}".encode())
+        for y in x:
+            _digest(h, y)
+    elif isinstance(x, str):
+        h.update(b"file:" + open(x, "rb").read() if os.path.isfile(x) else b"name:" + os.path.basename(x).encode())
+    elif isinstance(x, (np.dtype, type)):
+        h.update(f"dtype:{np.dtype(x).str}".encode())
+    else:
+        h.update(f"{type(x).__name__}:{x!r}".encode())
+
+
+def _arg_blobs(args, out):
+    """The bytes of every array argument and of every existing file an argument names, in argument order."""
+    for x in args:
+        if isinstance(x, (np.ndarray, np.generic)):
+            out.append(np.ascontiguousarray(x).tobytes())
+        elif isinstance(x, (list, tuple)):
+            _arg_blobs(x, out)
+        elif isinstance(x, str) and os.path.isfile(x):
+            out.append(open(x, "rb").read())
+    return out
+
+
+def _pack(v, blobs):
+    """Stores a large output array that repeats an argument's bytes (a loaded descriptor block, a written descriptor file) as
+    a reference into that argument: ("@in", [arg, offset, bytes], dtype, shape) or ("@around", prefix, [arg], suffix, dtype, shape)."""
+    if isinstance(v, dict):
+        return {k: _pack(x, blobs) for k, x in v.items()}
+    if isinstance(v, (tuple, list)):
+        return tuple(_pack(x, blobs) for x in v)
+    if isinstance(v, np.ndarray) and v.nbytes >= 4096 and v.dtype.fields is None:
+        b = np.ascontiguousarray(v).tobytes()
+        for n, blob in enumerate(blobs):
+            if len(blob) >= 4096 and (o := blob.find(b)) >= 0:
+                return ("@in", np.array([n, o, len(b)]), v.dtype.str, np.array(v.shape))
+            if len(blob) >= 4096 and (o := b.find(blob)) >= 0:
+                u = np.frombuffer(b, np.uint8)
+                return ("@around", u[:o].copy(), np.array([n]), u[o + len(blob):].copy(), v.dtype.str, np.array(v.shape))
+    return v
+
+
+def _unpack(v, blobs):
+    if isinstance(v, dict):
+        return {k: _unpack(x, blobs) for k, x in v.items()}
+    tag = v[0] if isinstance(v, tuple) and v and isinstance(v[0], str) else None
+    if tag == "@in":
+        n, o, ln = (int(x) for x in v[1])
+        return np.frombuffer(blobs[n][o:o + ln], v[2]).reshape(tuple(int(x) for x in v[3])).copy()
+    if tag == "@around":
+        b = np.asarray(v[1], np.uint8).tobytes() + blobs[int(v[2][0])] + np.asarray(v[3], np.uint8).tobytes()
+        return np.frombuffer(b, v[4]).reshape(tuple(int(x) for x in v[5])).copy()
+    if isinstance(v, tuple):
+        return tuple(_unpack(x, blobs) for x in v)
+    return v
+
+
+class ReferenceOracle:
+    """Oracle("ref") behind reference_output(): every call of the compiled reference is checked against (or, with
+    ORACLE_RECORD_REFERENCE=1, stored as) its stored output, and without the compiled reference the stored output is returned.
+    Files a call writes to paths named by its arguments are part of its output and are written again on replay."""
+
+    kind = "ref"
+
+    def __init__(self):
+        self._live = Oracle("ref") if available("ref") else None
+
+    def __getattr__(self, name):
+        if name.startswith("_"):
+            raise AttributeError(name)
+
+        def call(*args, **kw):
+            import hashlib
+            h = hashlib.sha256(name.encode())
+            for x in args + tuple(v for _, v in sorted(kw.items())):
+                _digest(h, x)
+            out_paths = [(n, a) for n, a in enumerate(args) if isinstance(a, str) and not os.path.exists(a)]
+            blobs = _arg_blobs(args, [])
+
+            def compute():
+                ret = getattr(self._live, name)(*args, **kw)
+                return _pack((ret, {(n,): np.frombuffer(open(a, "rb").read(), np.uint8) for n, a in out_paths if os.path.isfile(a)}), blobs)
+            ret, files = _unpack(reference_output(f"ref_{name}_{h.hexdigest()[:20]}", compute, self._live is not None), blobs)
+            if self._live is None:
+                for (n,), data in files.items():
+                    with open(args[n], "wb") as f:
+                        f.write(np.asarray(data, np.uint8).tobytes())
+            return ret
+        return call
+
+
+def reference() -> ReferenceOracle:
+    """The compiled reference's answers, with or without the compiled reference (see ReferenceOracle)."""
+    return ReferenceOracle()

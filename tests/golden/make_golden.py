@@ -1,7 +1,9 @@
-"""Generates tests/golden/*.npz from the REFERENCE itself (oracle/_ref/libref_oracle.so = the reference's own
-headers compiled verbatim from /root/reference/src).  Run in the build container:  python tests/golden/make_golden.py
-The fixtures pin both the port oracle (CPU tests) and the CUDA path (GPU tests) to reference outputs even where
-/root/reference is absent."""
+"""Generates tests/golden/reference_small.npz and the io_* files from the REFERENCE itself (oracle/_ref/libref_oracle.so = the
+reference's own headers compiled verbatim from an AliceVision source tree):
+    python tests/golden/make_golden.py      (ALICEVISION_SRC=<AliceVision>/src when it is not at oracle.DEFAULT_REFERENCE_SRC)
+The fixtures pin both the port oracle (CPU tests) and the CUDA path (GPU tests) to reference outputs even where the
+AliceVision sources are absent.  tests/golden/reference_outputs.npz (the reference's side of the port-vs-reference tests) is
+written by those tests themselves: ORACLE_RECORD_REFERENCE=1 python -m pytest tests -m "not gpu" with the reference built."""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box).  Every comparison goes through the C ABI
+"""GPU parity tests (run with -m gpu on an H100).  Every comparison goes through the C ABI
 (alicevision_b200.matching binds include/b200match.h with ctypes) and checks the CUDA path against the
 oracle: match index pairs bit-exact, distances exact on integer-valued data and exact by construction on
 real-valued data (the exact path follows the reference's summation order; tolerance 1e-4 relative is the
@@ -215,11 +215,11 @@ def test_raw_stage_is_superset_of_full(ora):
 
 def test_cpp_adaptors_against_reference_classes():
     """oracle/_ref/adaptor_test: the header-only C++ adaptors (deriving from the reference's ArrayMatcher /
-    IImageCollectionMatcher) vs the reference classes themselves, compiled together in the build container."""
+    IImageCollectionMatcher) vs the reference classes themselves, compiled together by oracle.build() from an AliceVision source tree."""
     import subprocess
     exe = os.path.join(os.path.dirname(os.path.dirname(__file__)), "oracle", "_ref", "adaptor_test")
     if not os.path.exists(exe):
-        pytest.skip("adaptor_test not built (needs /root/reference at build time)")
+        pytest.skip("adaptor_test not built (oracle.build() needs the AliceVision source tree)")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0 and "ADAPTOR TEST PASSED" in r.stdout, r.stdout + r.stderr
 

@@ -1,5 +1,5 @@
 """File formats on either side of the matching path (include/b200io.h, alicevision_b200/regions_io.py) against the
-reference's own stream code: Regions::Save/Load compiled from /root/reference (oracle/_ref) when available, the restated
+reference's own stream code: Regions::Save/Load compiled from the AliceVision sources (oracle/_ref) when available, the restated
 port otherwise, the reference's IO unit tests (feature/features_test.cpp:38-140), and golden files written by the compiled
 reference (tests/golden/make_golden.py).  Host code only: runs without a GPU."""
 import os
@@ -16,7 +16,7 @@ GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
 
 def kinds():
-    return [k for k in ("ref", "port") if oracle.available(k)]
+    return ["ref", "port"]         # "ref": the compiled reference, or its stored outputs
 
 
 def _feats(n, seed):
@@ -60,7 +60,7 @@ def test_descriptorIO_BINARY(tmp_path, dtype):
 @pytest.mark.parametrize("kind", kinds())
 @pytest.mark.parametrize("what", ["u8", "f32", "bin"])
 def test_regions_files_equal_reference(tmp_path, kind, what):
-    ora = oracle.Oracle(kind)
+    ora = oracle.reference() if kind == "ref" else oracle.Oracle(kind)
     n = 300
     if what == "bin":
         descs, _ = synth.mldb_images(1, n, seed=5)
@@ -83,16 +83,21 @@ def test_regions_files_equal_reference(tmp_path, kind, what):
     assert ora.load_regions(str(tmp_path / "missing.feat"), rd, d.dtype, d.shape[1]) is None
 
 
-@pytest.mark.skipif(not oracle.available("ref"), reason="compiled reference not available")
 def test_desc_type_conversion_equals_reference(tmp_path):
-    """loadDescsFromBinFile<Descriptor<float,128>, Descriptor<uchar,128>> (Descriptor.hpp:221-283)."""
+    """loadDescsFromBinFile<Descriptor<float,128>, Descriptor<uchar,128>> (Descriptor.hpp:221-283); the compiled reference's
+    result, or its stored copy (tests/golden/reference_outputs.npz) without it."""
     descs, _ = synth.sift_images(1, 200, np.uint8, seed=6, pool_factor=1.0)
     path = str(tmp_path / "u8.desc")
     rio.saveDescsToBinFile(path, descs[0])
-    ref = oracle.Oracle("ref")
-    out = np.zeros((200, 128), np.float32)
-    import ctypes as C
-    assert ref.lib.ref_load_desc_u8_as_f32(path.encode(), out.ctypes.data_as(C.c_void_p), C.c_int(200)) == 200
+
+    def load_with_reference():
+        import ctypes as C
+        out = np.zeros((200, 128), np.float32)
+        n = oracle.Oracle("ref").lib.ref_load_desc_u8_as_f32(path.encode(), out.ctypes.data_as(C.c_void_p), C.c_int(200))
+        assert np.array_equal(out, out.astype(np.uint8)), "the reference's floats are not the file's uchar values"
+        return n, out.astype(np.uint8)          # kept as the uchar values the floats hold exactly
+    n, out = oracle.reference_output("io.load_desc_u8_as_f32", load_with_reference, oracle.available("ref"))
+    assert n == 200
     got = rio.loadDescsFromBinFile(path, 128, np.float32, file_dtype=np.uint8)
     assert got.dtype == np.float32 and np.array_equal(got, out) and np.array_equal(got, descs[0].astype(np.float32))
 

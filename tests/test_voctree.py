@@ -1,8 +1,9 @@
 """Vocabulary-tree pair-list producer (include/b200voc.h, alicevision_b200/voctree.py).
 
 CPU: the restated oracle equals the reference's own voctree code (VocabularyTree.hpp quantize/load, VocabularyTree.cpp
-sparseDistance compiled from /root/reference) on words, ranked matches, scores, TF-IDF weights and the pair list; the
-reference's own unit test of the tree file round trip (voctree/vocabularyTree_test.cpp) on the product's loader.
+sparseDistance compiled from the AliceVision sources, or their stored outputs in tests/golden/reference_outputs.npz) on words,
+ranked matches, scores, TF-IDF weights and the pair list; the reference's own unit test of the tree file round trip
+(voctree/vocabularyTree_test.cpp) on the product's loader.
 GPU (-m gpu): the CUDA quantiser and scorer equal the oracle bit for bit."""
 import os
 
@@ -33,16 +34,18 @@ def tree(seed=4, invalid_tail=1):
     return synth.vocabulary_tree(K, L, seed=seed, invalid_tail=invalid_tail)
 
 
-@pytest.mark.skipif(len(kinds()) < 2, reason="needs both the compiled reference and the port")
 @pytest.mark.parametrize("method", ["strongCommonPoints", "commonPoints", "classic", "inversedWeightedCommonPoints"])
 def test_port_equals_reference(method, tmp_path):
-    R, P = oracle.VoctreeOracle("ref"), oracle.VoctreeOracle("port")
+    live = oracle.VoctreeOracle.available("ref")
+    R, P = oracle.VoctreeOracle("ref") if live else None, oracle.VoctreeOracle("port")
+    ref = lambda key, f: oracle.reference_output("voctree." + key, f, live)    # noqa: E731
     c, v = tree()
     d = views()
-    for descs in (d[3], d[5].astype(np.float32), synth.real_valued([d[8 if len(d[8]) else 13]])[0]):
-        assert np.array_equal(R.quantize(K, L, c, v, descs, str(tmp_path / "t.tree")), P.quantize(K, L, c, v, descs))
+    for n, descs in enumerate((d[3], d[5].astype(np.float32), synth.real_valued([d[8 if len(d[8]) else 13]])[0])):
+        assert np.array_equal(ref(f"quantize.{n}", lambda: R.quantize(K, L, c, v, descs, str(tmp_path / "t.tree"))), P.quantize(K, L, c, v, descs))
     for nq, nmax in ((0, 0), (4, 0), (3, 200)):
-        a = R.image_matching(K, L, c, v, d, nmax, nq, method, str(tmp_path / "t.tree")); b = P.image_matching(K, L, c, v, d, nmax, nq, method)
+        a = ref(f"{method}.{nq}.{nmax}", lambda: R.image_matching(K, L, c, v, d, nmax, nq, method, str(tmp_path / "t.tree")))
+        b = P.image_matching(K, L, c, v, d, nmax, nq, method)
         for x, y in zip(a, b):
             assert np.array_equal(x, y)
         assert len(a[4]) > 0 and np.all(a[4][:, 0] != a[4][:, 1])
