@@ -30,7 +30,7 @@ struct alignas(128) ViewDev {
   const __half* h16;    // fp16 copy (scalar, dim == 128) or nullptr
   const float* nbh;     // ||row||^2 / 2, padded to a multiple of 256 rows with 1e30f
   const float* nrm;     // ||row||^2
-  const __half* aug16;  // m_pad x 16: [b0, l0, l1, -0.5, -1, -2048, 0...] with ||row||^2/2 = 0.5*b0 + l0 + 2048*l1; pad rows [0, 0, 2047, ...]
+  const __half* aug16;  // m_pad x 16: [b0, l0, l1, -0.5, -1, -2048, 0...] with ||row||^2/2 = 0.5*b0 + l0 + 2048*l1; pad rows [0, 0, 4096, ...] (prep.cuh)
   const __half* augq16; // m_pad x 16: [-0.5, -1, -2048, b0, l0, l1, 0...] (prep.cuh)
   const float* err;     // m_pad: upper bound of ||row - fp16(row)||_2 (0 for integer-valued rows)
   const uint32_t* stats; // float bits: [0] max err over the view, [1] max ||fp16(row)||^2

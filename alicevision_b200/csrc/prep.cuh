@@ -30,7 +30,7 @@ __device__ __forceinline__ void halfnorm_limbs(float s, bool integer_valued, flo
 // One warp per row; lane handles components lane, lane+32, lane+64, lane+96.
 //   h16   m x 128 fp16 (rounded to nearest)
 //   nrm   ||fp16(row)||^2 (== ||row||^2 for integer-valued rows), nbh = half of it (pad rows 1e30)
-//   aug16 m_pad x 16, the row as DATABASE (B operand):  [b0, l0, l1, -0.5, -1, -2048, 0...]   pad rows [0, 0, 2047, ...]
+//   aug16 m_pad x 16, the row as DATABASE (B operand):  [b0, l0, l1, -0.5, -1, -2048, 0...]   pad rows [0, 0, 4096, ...]
 //   augq16 m_pad x 16, the row as QUERY (A operand):    [-0.5, -1, -2048, b0, l0, l1, 0...]
 //         With B negated by the instruction descriptor the 9th K-step adds  +nb/2 (cols 0-2)  and, in the real-valued kernel whose
 //         A tile is augq16,  +na/2 (cols 3-5): the accumulator is ||a-b||^2 / 2.  The integer kernel's constant A tile has zeros in
@@ -46,10 +46,14 @@ prep_view_kernel(const T* __restrict__ raw, int m, __half* __restrict__ h16, flo
   const int lane = threadIdx.x & 31;
   if (row >= m_pad) return;
   const float cst = lane == 0 ? -0.5f : lane == 1 ? -1.f : lane == 2 ? -2048.f : 0.f;     // the constant limb multipliers
-  if (row >= m) {     // pad rows: a half-norm larger than any real one (2048 * 2047 = 2^22 - 2048)
+  if (row >= m) {
+    // pad rows (zero in h16): their AUG accumulator is 2048 * 4096 = 2^23 (+ ||a||^2/2 in MODE_REAL), exact in fp16 and fp32 and above
+    // every real row's: h = ||b||^2/2 - a.b < 2^21 + 2^22 for signed rows inside the domain, and ||a - b||^2/2 < 2^21 + 2^22 + ||a||^2/2.
+    // So a chunk of padding never wins and never ties with another; it is the second chunk minimum only when m <= 16, and then the
+    // exactness pass re-scores the one real chunk.  (A pad half-norm below 2^21 + 2^22 lost to anti-correlated queries.)
     if (lane == 0) { nbh[row] = 1e30f; err[row] = 0.f; }
     if (lane < 16) {
-      aug16[(size_t)row * 16 + lane] = __float2half_rn(lane == 2 ? 2047.f : (lane >= 3 && lane < 6) ? (lane == 3 ? -0.5f : lane == 4 ? -1.f : -2048.f) : 0.f);
+      aug16[(size_t)row * 16 + lane] = __float2half_rn(lane == 2 ? 4096.f : (lane >= 3 && lane < 6) ? (lane == 3 ? -0.5f : lane == 4 ? -1.f : -2048.f) : 0.f);
       augq16[(size_t)row * 16 + lane] = __float2half_rn(cst);
     }
     return;
