@@ -9,6 +9,7 @@
 #include "common.cuh"
 #include "finish.cuh"
 #include "guided.cuh"
+#include "guided_fast.cuh"
 #include "hamming.cuh"
 #include "l2_exact.cuh"
 #include "l2_tc.cuh"
@@ -16,11 +17,13 @@
 #include "verify.cuh"
 #include "hostconv.hpp"
 
+#include <cub/cub.cuh>
 #include <pthread.h>
 #include <sched.h>
 
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstdlib>
 #include <atomic>
 #include <condition_variable>
@@ -177,7 +180,8 @@ struct ViewHost {
   void* arena = nullptr; void* raw_own = nullptr;     // the one allocation all device buffers of the view live in; a separately owned `raw`
   bool stored_u8 = false;     // dtype == DT_F32 whose values are integers in 0..255: staged and kept on the device as uchar (hostconv.hpp)
   float* d_xy = nullptr; uint32_t* d_yrank = nullptr;   // positions + rank of y on the device (device finishing stage, finish.cuh)
-  bool failed = false;        // its upload job failed: the device buffers were never filled
+  double2* d_geom = nullptr;  // b200m_set_view_geometry: the (undistorted) positions guided matching uses instead of xy; own allocation
+  bool failed = false;       // its upload job failed: the device buffers were never filled
   std::vector<float> xy;      // m x 2 positions (host copy: finishing of views that are not in general position, cross check)
   uint32_t flags = 0; bool flags_known = true;
   uint64_t seq = 0;           // upload order (monotonic per context)
@@ -227,9 +231,22 @@ struct KnnScratch {
   Cand* cands = nullptr; int32_t* idx = nullptr; uint32_t* dist = nullptr; WorkItem* items = nullptr; uint8_t* small = nullptr;
 };
 
+// grow-only scratch of b200m_guided_match_fast_pairs (guided_fast.cuh): one batch of pairs at a time
+struct GuidedFastScratch {
+  struct Buf { void* p = nullptr; size_t bytes = 0; };
+  enum { PAIRS, LBUCKET, BEST, SECOND, BCOUNT, BOFF, CSR, RSTART, RCOUNT, RCOFF, RPAIR, KEEP, KPOS, OUT, PSTART, EXPAND, TEMP, NBUF };
+  Buf d[NBUF];
+  void* h_pairs = nullptr; size_t h_pairs_bytes = 0;      // pinned: FastPair table
+  void* h_meta = nullptr; size_t h_meta_bytes = 0;        // pinned: read-back of the candidate total and the per-pair starts
+  void* h_out = nullptr; size_t h_out_bytes = 0;          // pinned: read-back of the matches
+  cudaEvent_t ev_c0 = nullptr, ev_c1 = nullptr;           // candidate-kernel timing
+};
+
 struct b200m_ctx {
   int device = 0, num_sms = 148;
   KnnScratch knn;
+  GuidedFastScratch gf;
+  long gf_left_cap = 1l << 21;    // left features per internal batch of b200m_guided_match_fast_pairs (B200M_GUIDED_FAST_LEFT_CAP)
   cudaStream_t stream = nullptr, copy_stream = nullptr, up_stream = nullptr, tab_stream = nullptr, pack_stream = nullptr;
   bool pipe_streams = true;       // tables / packing+finishing on their own streams (B200M_PIPE_STREAMS=0: everything on the search stream)
   bool own_stream = false;
@@ -316,7 +333,8 @@ static int alloc_view_buffers(b200m_ctx* c, ViewHost& v) {
 static void free_view_buffers(b200m_ctx* c, ViewHost& v) {
   if (v.arena) cudaFreeAsync(v.arena, c->stream);
   if (v.raw_own) cudaFreeAsync(v.raw_own, c->stream);      // fp32 re-upload of a view whose uchar staging failed late
-  v.arena = nullptr; v.raw_own = nullptr;
+  if (v.d_geom) cudaFreeAsync(v.d_geom, c->stream);        // re-uploading or removing a view drops its geometry positions
+  v.arena = nullptr; v.raw_own = nullptr; v.d_geom = nullptr;
   v.raw = nullptr; v.h16 = nullptr; v.nbh = nullptr; v.nrm = nullptr; v.aug16 = nullptr; v.d_xy = nullptr; v.d_yrank = nullptr;
   v.augq16 = nullptr; v.err = nullptr; v.stats = nullptr;
 }
@@ -557,6 +575,7 @@ int b200m_ctx_create(int device, void* stream, b200m_ctx** out) {
   if (const char* e = getenv("B200M_FIRST_BATCH")) c->first_batch_pairs = std::max(1, atoi(e));
   if (const char* e = getenv("B200M_REAL_TC")) c->real_tc = atoi(e) != 0;
   if (const char* e = getenv("B200M_REAL_FUSED_ROWS")) c->real_fused_rows = std::max(0l, atol(e));
+  if (const char* e = getenv("B200M_GUIDED_FAST_LEFT_CAP")) c->gf_left_cap = std::max(1l, atol(e));
   *out = c.release();
   return B200M_OK;
 }
@@ -600,6 +619,15 @@ void b200m_ctx_destroy(b200m_ctx* c) {
   {
     KnnScratch& k = c->knn;
     for (void* q : {(void*)k.raw, (void*)k.h16, (void*)k.nbh, (void*)k.nrm, (void*)k.aug16, (void*)k.augq16, (void*)k.err, (void*)k.cands, (void*)k.idx, (void*)k.dist, (void*)k.items, (void*)k.small}) if (q) cudaFree(q);
+  }
+  {
+    GuidedFastScratch& g = c->gf;
+    for (auto& b : g.d) if (b.p) cudaFree(b.p);
+    if (g.h_pairs) cudaFreeHost(g.h_pairs);
+    if (g.h_out) cudaFreeHost(g.h_out);
+    if (g.h_meta) cudaFreeHost(g.h_meta);
+    if (g.ev_c0) cudaEventDestroy(g.ev_c0);
+    if (g.ev_c1) cudaEventDestroy(g.ev_c1);
   }
   cudaEventDestroy(c->ev_start); cudaEventDestroy(c->ev_end);
   cudaStreamDestroy(c->copy_stream);
@@ -1421,7 +1449,8 @@ int b200m_guided_match_model(b200m_ctx* c, uint32_t view_left, uint32_t view_rig
   if (usable) {
     if (!((vl.dtype == DT_BIN && vl.dim == 64) || (vl.dtype != DT_BIN && vl.dim == 128)))
       return fail(B200M_ERR_UNSUPPORTED, "guided matching takes 128-component scalar or 64-byte binary descriptors");
-    if (vl.xy.empty() || vr.xy.empty()) return fail(B200M_ERR_ARG, "guided matching needs feature positions for both views");
+    if ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom))
+      return fail(B200M_ERR_ARG, "guided matching needs feature positions (or geometry positions) for both views");
     float* d_xy = nullptr; double2* d_xl = nullptr; double2* d_xr = nullptr; Rec* d_out = nullptr; int* d_cnt = nullptr;
     cudaStream_t st = c->stream;
     CK(cudaMallocAsync((void**)&d_xy, sizeof(float) * 2 * (size_t)std::max(vl.m, vr.m), st));
@@ -1430,11 +1459,18 @@ int b200m_guided_match_model(b200m_ctx* c, uint32_t view_left, uint32_t view_rig
     CK(cudaMallocAsync((void**)&d_out, sizeof(Rec) * (size_t)vl.m, st));
     CK(cudaMallocAsync((void**)&d_cnt, sizeof(int), st));
     CK(cudaMemsetAsync(d_cnt, 0, sizeof(int), st));
-    CK(cudaMemcpyAsync(d_xy, vl.xy.data(), sizeof(float) * 2 * (size_t)vl.m, cudaMemcpyHostToDevice, st));
-    positions_to_double_kernel<<<(vl.m + 255) / 256, 256, 0, st>>>(d_xy, vl.m, d_xl);
-    CK(cudaStreamSynchronize(st));                     // d_xy is reused for the right view
-    CK(cudaMemcpyAsync(d_xy, vr.xy.data(), sizeof(float) * 2 * (size_t)vr.m, cudaMemcpyHostToDevice, st));
-    positions_to_double_kernel<<<(vr.m + 255) / 256, 256, 0, st>>>(d_xy, vr.m, d_xr);
+    // a view's geometry positions (b200m_set_view_geometry) replace its widened float upload positions
+    if (!vl.d_geom) {
+      CK(cudaMemcpyAsync(d_xy, vl.xy.data(), sizeof(float) * 2 * (size_t)vl.m, cudaMemcpyHostToDevice, st));
+      positions_to_double_kernel<<<(vl.m + 255) / 256, 256, 0, st>>>(d_xy, vl.m, d_xl);
+      CK(cudaStreamSynchronize(st));                   // d_xy is reused for the right view
+    }
+    if (!vr.d_geom) {
+      CK(cudaMemcpyAsync(d_xy, vr.xy.data(), sizeof(float) * 2 * (size_t)vr.m, cudaMemcpyHostToDevice, st));
+      positions_to_double_kernel<<<(vr.m + 255) / 256, 256, 0, st>>>(d_xy, vr.m, d_xr);
+    }
+    const double2* xl = vl.d_geom ? vl.d_geom : d_xl;
+    const double2* xr = vr.d_geom ? vr.d_geom : d_xr;
     GuidedParams P;
     P.model = model == B200M_MODEL_HOMOGRAPHY ? GM_HOMOGRAPHY : GM_FUNDAMENTAL;
     for (int k = 0; k < 9; ++k) P.F[k] = F[k];
@@ -1453,9 +1489,9 @@ int b200m_guided_match_model(b200m_ctx* c, uint32_t view_left, uint32_t view_rig
       (vl.stored_u8 ? rawl : rawr) = tmp32;
       kdt = DT_F32;
     }
-    if (kdt == DT_F32) guided_top2_kernel<DT_F32><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, d_xl, d_xr, vl.m, vr.m, P, d_out, d_cnt);
-    else if (kdt == DT_U8) guided_top2_kernel<DT_U8><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, d_xl, d_xr, vl.m, vr.m, P, d_out, d_cnt);
-    else guided_top2_kernel<DT_BIN><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, d_xl, d_xr, vl.m, vr.m, P, d_out, d_cnt);
+    if (kdt == DT_F32) guided_top2_kernel<DT_F32><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, xl, xr, vl.m, vr.m, P, d_out, d_cnt);
+    else if (kdt == DT_U8) guided_top2_kernel<DT_U8><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, xl, xr, vl.m, vr.m, P, d_out, d_cnt);
+    else guided_top2_kernel<DT_BIN><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, xl, xr, vl.m, vr.m, P, d_out, d_cnt);
     if (tmp32) cudaFreeAsync(tmp32, st);
     CK(cudaGetLastError());
     CK(cudaEventRecord(c->ev_end, st));
@@ -1475,6 +1511,250 @@ int b200m_guided_match_model(b200m_ctx* c, uint32_t view_left, uint32_t view_rig
     res->offsets[1] = n;
   } else {
     res->matches = c->recycler->take(1);
+  }
+  *out = res.release();
+  return B200M_OK;
+}
+
+int b200m_set_view_geometry(b200m_ctx* c, uint32_t view_id, const double* xy, int n) {
+  if (!c) return fail(B200M_ERR_ARG, "ctx is null");
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  auto it = c->slot_of.find(view_id);
+  if (it == c->slot_of.end()) return fail(B200M_ERR_ARG, "unknown view id");
+  ViewHost& v = c->views[it->second];
+  CK(cudaSetDevice(c->device));
+  if (xy && n != v.m) return fail(B200M_ERR_ARG, "geometry positions: n = " + std::to_string(n) + " but the view has " + std::to_string(v.m) + " features");
+  if (v.d_geom) { CK(cudaFreeAsync(v.d_geom, c->stream)); v.d_geom = nullptr; }   // stream-ordered: kernels already enqueued still see it
+  if (!xy || n == 0) return B200M_OK;
+  CK(cudaMallocAsync((void**)&v.d_geom, sizeof(double2) * (size_t)n, c->stream));
+  CK(cudaMemcpyAsync(v.d_geom, xy, sizeof(double2) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+  CK(cudaStreamSynchronize(c->stream));    // the caller's array may go once this returns
+  return B200M_OK;
+}
+
+}  // extern "C"
+
+// ---- guided matching from known poses: guidedMatchingFundamentalFast for a list of pairs (guided_fast.cuh) -------------------
+template <class T> static int gf_reserve(GuidedFastScratch& g, int which, size_t count, T** p) {
+  GuidedFastScratch::Buf& b = g.d[which];
+  const size_t bytes = std::max<size_t>(count * sizeof(T), 256);
+  if (b.bytes < bytes) {
+    if (b.p) CK(cudaFree(b.p));      // cudaFree synchronises: nothing enqueued still uses the old buffer
+    b.p = nullptr; b.bytes = 0;
+    const size_t nb = bytes + bytes / 4;
+    CK(cudaMalloc(&b.p, nb));
+    b.bytes = nb;
+  }
+  *p = static_cast<T*>(b.p);
+  return B200M_OK;
+}
+static int gf_reserve_host(void*& p, size_t& have, size_t bytes) {
+  if (have >= bytes) return B200M_OK;
+  if (p) CK(cudaFreeHost(p));
+  p = nullptr; have = 0;
+  const size_t nb = std::max<size_t>(bytes + bytes / 4, 4096);
+  CK(cudaMallocHost(&p, nb));
+  have = nb;
+  return B200M_OK;
+}
+
+template <class T> static int gf_exclusive_scan(b200m_ctx* c, const T* in, T* out, size_t n, cudaStream_t st, int& launches) {
+  size_t tb = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, (int64_t)n, st));
+  void* tmp = nullptr;
+  if (int rc = gf_reserve(c->gf, GuidedFastScratch::TEMP, tb, (char**)&tmp)) return rc;
+  CK(cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, (int64_t)n, st));
+  launches += 2;
+  return B200M_OK;
+}
+
+namespace {
+struct GfPairHost { int index, slot_l, slot_r, kclass; };   // kclass: kernel dtype, or 3 = mixed (uchar-stored view expanded to fp32)
+}
+
+// One batch of pairs of one kernel class.  Appends the pair's matches to per_pair[index].
+static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, const double* F, const double* ep2, const int32_t* wh, double errorTh,
+                        double distRatio, std::vector<std::vector<uint2>>& per_pair, double& gpu_ms, double& cand_ms, int& launches, int64_t& cands) {
+  GuidedFastScratch& g = c->gf;
+  cudaStream_t st = c->stream;
+  const int np = (int)batch.size();
+  const int kclass = batch[0].kclass;
+  // uchar-stored views of mixed pairs: one fp32 expansion each
+  std::map<int, size_t> exp_off; size_t exp_elems = 0;
+  if (kclass == 3)
+    for (const auto& p : batch) {
+      const int s = c->views[p.slot_l].stored_u8 ? p.slot_l : p.slot_r;
+      if (!exp_off.count(s)) { exp_off[s] = exp_elems; exp_elems += (size_t)c->views[s].m * 128; }
+    }
+  int rc;
+  if ((rc = gf_reserve_host(g.h_pairs, g.h_pairs_bytes, sizeof(FastPair) * (size_t)np))) return rc;
+  FastPair* hp = static_cast<FastPair*>(g.h_pairs);
+  float* d_exp = nullptr;
+  if (exp_elems && (rc = gf_reserve(g, GuidedFastScratch::EXPAND, exp_elems, &d_exp))) return rc;
+  long sum_l = 0, sum_r = 0, sum_b = 0; int max_l = 0, max_r = 0;
+  for (int k = 0; k < np; ++k) {
+    const GfPairHost& q = batch[k];
+    const ViewHost& vl = c->views[q.slot_l]; const ViewHost& vr = c->views[q.slot_r];
+    FastPair& P = hp[k];
+    std::memset(&P, 0, sizeof(P));
+    P.rawl = vl.raw; P.rawr = vr.raw;
+    if (kclass == 3) {
+      if (vl.stored_u8) P.rawl = d_exp + exp_off[q.slot_l]; else P.rawr = d_exp + exp_off[q.slot_r];
+    }
+    P.gl = vl.d_geom; P.gr = vr.d_geom; P.fl = (const float2*)vl.d_xy; P.fr = (const float2*)vr.d_xy;
+    // normalise once (guidedMatching.hpp:378-385): F and ep2 negated when ep2(2) > 0, then ep2 / ep2(2)
+    const double* f = F + 9 * (size_t)q.index; const double* e = ep2 + 3 * (size_t)q.index;
+    const bool neg = e[2] > 0.0;
+    for (int t = 0; t < 9; ++t) P.F[t] = neg ? -f[t] : f[t];
+    const double e0 = neg ? -e[0] : e[0], e1 = neg ? -e[1] : e[1], e2 = neg ? -e[2] : e[2];
+    P.e0 = e0 / e2; P.e1 = e1 / e2; P.e2 = e2 / e2;
+    P.ml = vl.m; P.mr = vr.m; P.W = wh[2 * q.index]; P.H = wh[2 * q.index + 1]; P.nb = 2 * (P.W + P.H - 2);
+    P.left_base = (int)sum_l; P.right_base = (int)sum_r; P.bucket_base = (int)sum_b;
+    sum_l += vl.m; sum_r += vr.m; sum_b += P.nb + 1;
+    max_l = std::max(max_l, vl.m); max_r = std::max(max_r, vr.m);
+  }
+  FastPair* d_pairs; int *d_lbucket, *d_bcount, *d_boff, *d_csr, *d_rstart, *d_rpair, *d_keep, *d_kpos, *d_pstart;
+  unsigned long long *d_best, *d_second, *d_rcount, *d_rcoff; uint2* d_out;
+  if ((rc = gf_reserve(g, GuidedFastScratch::PAIRS, np, &d_pairs)) || (rc = gf_reserve(g, GuidedFastScratch::LBUCKET, sum_l, &d_lbucket)) ||
+      (rc = gf_reserve(g, GuidedFastScratch::BEST, sum_l, &d_best)) || (rc = gf_reserve(g, GuidedFastScratch::SECOND, sum_l, &d_second)) ||
+      (rc = gf_reserve(g, GuidedFastScratch::BCOUNT, sum_b, &d_bcount)) || (rc = gf_reserve(g, GuidedFastScratch::BOFF, sum_b, &d_boff)) ||
+      (rc = gf_reserve(g, GuidedFastScratch::CSR, sum_l, &d_csr)) || (rc = gf_reserve(g, GuidedFastScratch::RSTART, sum_r, &d_rstart)) ||
+      (rc = gf_reserve(g, GuidedFastScratch::RCOUNT, sum_r + 1, &d_rcount)) || (rc = gf_reserve(g, GuidedFastScratch::RCOFF, sum_r + 1, &d_rcoff)) ||
+      (rc = gf_reserve(g, GuidedFastScratch::RPAIR, sum_r, &d_rpair)) || (rc = gf_reserve(g, GuidedFastScratch::KEEP, sum_l + 1, &d_keep)) ||
+      (rc = gf_reserve(g, GuidedFastScratch::KPOS, sum_l + 1, &d_kpos)) || (rc = gf_reserve(g, GuidedFastScratch::OUT, sum_l, &d_out)) ||
+      (rc = gf_reserve(g, GuidedFastScratch::PSTART, np + 1, &d_pstart)))
+    return rc;
+  // the temporary storage of the three scans is taken inside gf_exclusive_scan; reserve it for the largest one first so that
+  // no reallocation (a synchronising cudaFree) happens between launches
+  { size_t tb = 0; CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_rcount, d_rcoff, (int64_t)std::max(sum_r + 1, std::max(sum_b, sum_l + 1)), st));
+    char* t; if ((rc = gf_reserve(g, GuidedFastScratch::TEMP, tb, &t))) return rc; }
+  if (!g.ev_c0) { CK(cudaEventCreate(&g.ev_c0)); CK(cudaEventCreate(&g.ev_c1)); }
+  CK(cudaEventRecord(c->ev_start, st));
+  CK(cudaMemcpyAsync(d_pairs, hp, sizeof(FastPair) * (size_t)np, cudaMemcpyHostToDevice, st));
+  for (const auto& x : exp_off) {
+    const ViewHost& vu = c->views[x.first];
+    const size_t ne = (size_t)vu.m * 128;
+    u8_to_f32_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>((const uint8_t*)vu.raw, d_exp + x.second, ne);
+    ++launches;
+  }
+  CK(cudaMemsetAsync(d_bcount, 0, sizeof(int) * (size_t)sum_b, st));
+  CK(cudaMemsetAsync(d_rcount + sum_r, 0, sizeof(unsigned long long), st));
+  CK(cudaMemsetAsync(d_keep + sum_l, 0, sizeof(int), st));
+  const dim3 gl((max_l + GF_THREADS - 1) / GF_THREADS, np), gr((max_r + GF_THREADS - 1) / GF_THREADS, np);
+  guided_fast_left_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, d_lbucket, d_bcount, d_best, d_second);
+  if ((rc = gf_exclusive_scan(c, d_bcount, d_boff, (size_t)sum_b, st, launches))) return rc;
+  CK(cudaMemcpyAsync(d_bcount, d_boff, sizeof(int) * (size_t)sum_b, cudaMemcpyDeviceToDevice, st));   // scatter cursors
+  guided_fast_scatter_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, d_lbucket, d_bcount, d_csr);
+  guided_fast_right_kernel<<<gr, GF_THREADS, 0, st>>>(d_pairs, std::sqrt(errorTh), d_boff, d_rstart, d_rcount, d_rpair);
+  if ((rc = gf_exclusive_scan(c, d_rcount, d_rcoff, (size_t)sum_r + 1, st, launches))) return rc;
+  CK(cudaEventRecord(g.ev_c0, st));
+  const int cgrid = c->num_sms * 8;
+  if (kclass == DT_U8) guided_fast_cand_kernel<DT_U8><<<cgrid, GF_THREADS, 0, st>>>(d_pairs, (int)sum_r, d_rcoff, d_rstart, d_rpair, d_csr, d_best, d_second);
+  else if (kclass == DT_BIN) guided_fast_cand_kernel<DT_BIN><<<cgrid, GF_THREADS, 0, st>>>(d_pairs, (int)sum_r, d_rcoff, d_rstart, d_rpair, d_csr, d_best, d_second);
+  else guided_fast_cand_kernel<DT_F32><<<cgrid, GF_THREADS, 0, st>>>(d_pairs, (int)sum_r, d_rcoff, d_rstart, d_rpair, d_csr, d_best, d_second);
+  CK(cudaEventRecord(g.ev_c1, st));
+  guided_fast_keep_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, distRatio, d_best, d_second, d_keep);
+  if ((rc = gf_exclusive_scan(c, d_keep, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+  guided_fast_emit_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, np, (int)sum_l, d_keep, d_kpos, d_best, d_out, d_pstart);
+  CK(cudaGetLastError());
+  launches += 5;
+  CK(cudaEventRecord(c->ev_end, st));
+  // read-back: the candidate total + per-pair starts, then the matches
+  if ((rc = gf_reserve_host(g.h_meta, g.h_meta_bytes, sizeof(unsigned long long) + sizeof(int) * (size_t)(np + 1)))) return rc;
+  unsigned long long* h_total = static_cast<unsigned long long*>(g.h_meta);
+  int* h_pstart = reinterpret_cast<int*>(h_total + 1);
+  CK(cudaMemcpyAsync(h_pstart, d_pstart, sizeof(int) * (size_t)(np + 1), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h_total, d_rcoff + sum_r, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const int n_out = h_pstart[np];
+  std::vector<int> starts(h_pstart, h_pstart + np + 1);
+  cands += (int64_t)*h_total;
+  float ms = 0.f, cms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
+  CK(cudaEventElapsedTime(&cms, g.ev_c0, g.ev_c1));
+  gpu_ms += ms; cand_ms += cms;
+  if (n_out > 0) {
+    if ((rc = gf_reserve_host(g.h_out, g.h_out_bytes, sizeof(uint2) * (size_t)n_out))) return rc;
+    CK(cudaMemcpyAsync(g.h_out, d_out, sizeof(uint2) * (size_t)n_out, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const uint2* h = static_cast<const uint2*>(g.h_out);
+    for (int k = 0; k < np; ++k) per_pair[batch[k].index].assign(h + starts[k], h + starts[k + 1]);
+  }
+  return B200M_OK;
+}
+
+extern "C" {
+
+int b200m_guided_match_fast_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, const double* F, const double* epipole2, const int32_t* wh,
+                                  double errorTh, double distRatio, b200m_result** out) {
+  if (!c || !out || n_pairs < 0 || (n_pairs > 0 && (!pairs || !F || !epipole2 || !wh))) return fail(B200M_ERR_ARG, "bad arguments");
+  *out = nullptr;
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  CK(cudaSetDevice(c->device));
+  // checks first: nothing runs for a list with a bad entry
+  std::vector<GfPairHost> work;
+  for (int k = 0; k < n_pairs; ++k) {
+    const int W = wh[2 * k], H = wh[2 * k + 1];
+    if (W < 2 || H < 2 || W > (1 << 24) || H > (1 << 24))
+      return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": the right image must be at least 2 x 2 pixels (and at most 2^24 on a side)");
+    auto sl = c->slot_of.find(pairs[2 * k]), sr = c->slot_of.find(pairs[2 * k + 1]);
+    if (sl == c->slot_of.end() || sr == c->slot_of.end()) return fail(B200M_ERR_ARG, "guided matching references a view that was never uploaded");
+    const ViewHost& vl = c->views[sl->second]; const ViewHost& vr = c->views[sr->second];
+    if (!(vl.m > 0 && vr.m > 0 && vl.dtype == vr.dtype && vl.dim == vr.dim)) continue;     // no common descriptor type / empty view: empty list
+    if (!((vl.dtype == DT_BIN && vl.dim == 64) || (vl.dtype != DT_BIN && vl.dim == 128)))
+      return fail(B200M_ERR_UNSUPPORTED, "guided matching takes 128-component scalar or 64-byte binary descriptors");
+    if ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom))
+      return fail(B200M_ERR_ARG, "guided matching needs feature positions (or geometry positions) for both views");
+    work.push_back({k, sl->second, sr->second, 0});
+  }
+  std::vector<std::vector<uint2>> per_pair((size_t)n_pairs);
+  double gpu_ms = 0, cand_ms = 0; int launches = 0; int64_t cands = 0;
+  // Batches: the list is walked once in input order and every pair joins the open batch of its kernel class (uchar, fp32, mixed,
+  // binary); a batch runs when it is full - bounded by left features (a pair larger than the bound runs alone), right features,
+  // buckets and fp32 expansions - and the rest at the end.  Each view is waited for when its first pair is reached.
+  const long pair_cap = 8192, right_cap = std::max(c->gf_left_cap, 1l << 20), bucket_cap = 16l << 20, exp_cap = 64l << 20;
+  struct Open { std::vector<GfPairHost> pairs; long l = 0, r = 0, b = 0, e = 0; std::set<int> exp_views; };
+  Open open[4];
+  auto flush = [&](Open& o) -> int {
+    if (o.pairs.empty()) return B200M_OK;
+    const int rc = gf_run_batch(c, o.pairs, F, epipole2, wh, errorTh, distRatio, per_pair, gpu_ms, cand_ms, launches, cands);
+    o = Open();
+    return rc;
+  };
+  for (GfPairHost p : work) {
+    int rc;
+    if ((rc = ensure_view_ready(c, p.slot_l)) || (rc = ensure_view_ready(c, p.slot_r))) return rc;
+    // the stored type is final once the view is ready (a uchar-staged view that met a non-integer value was re-uploaded as fp32)
+    const ViewHost& vl = c->views[p.slot_l]; const ViewHost& vr = c->views[p.slot_r];
+    p.kclass = vl.store_dtype() == vr.store_dtype() ? vl.store_dtype() : 3;
+    Open& o = open[p.kclass];
+    const int W = wh[2 * p.index], H = wh[2 * p.index + 1];
+    const long nb = 2l * (W + H - 2) + 1;
+    const int su = p.kclass == 3 ? (vl.stored_u8 ? p.slot_l : p.slot_r) : -1;
+    long ne = su >= 0 && !o.exp_views.count(su) ? (long)c->views[su].m * 128 : 0;
+    if (!o.pairs.empty() && ((long)o.pairs.size() + 1 > pair_cap || o.l + vl.m > c->gf_left_cap || o.r + vr.m > right_cap || o.b + nb > bucket_cap ||
+                             o.e + ne > exp_cap)) {
+      if ((rc = flush(o))) return rc;
+      ne = su >= 0 ? (long)c->views[su].m * 128 : 0;
+    }
+    o.pairs.push_back(p);
+    o.l += vl.m; o.r += vr.m; o.b += nb; o.e += ne;
+    if (su >= 0) o.exp_views.insert(su);
+  }
+  for (Open& o : open)
+    if (int rc = flush(o)) return rc;
+  if (int rc = wait_uploads(c)) return rc;
+  c->last_gpu_ms = gpu_ms; c->last_search_ms = cand_ms; c->last_launches = launches; c->last_records = cands; c->last_tc_pairs = 0;
+  // one result pair per input pair, in input order (empty lists included)
+  std::unique_ptr<b200m_result> res(new b200m_result());
+  res->recycler = c->recycler;
+  res->pair_ids.assign(pairs, pairs + 2 * (size_t)n_pairs);
+  res->offsets.assign((size_t)n_pairs + 1, 0);
+  for (int k = 0; k < n_pairs; ++k) res->offsets[k + 1] = res->offsets[k] + (int64_t)per_pair[k].size();
+  res->matches = c->recycler->take((size_t)std::max<int64_t>(res->offsets[n_pairs], 1));
+  for (int k = 0; k < n_pairs; ++k) {
+    b200m_match* m = res->matches.p + res->offsets[k];
+    for (const uint2& x : per_pair[k]) *m++ = b200m_match{x.x, x.y, 0.f, 0.f};     // IndMatch(i, j): ratio and distance 0
   }
   *out = res.release();
   return B200M_OK;

@@ -36,7 +36,7 @@ ABI_SYMBOLS = [
     "b200m_match_pairs", "b200m_result_num_pairs", "b200m_result_get", "b200m_result_free", "b200m_last_gpu_ms",
     "b200m_last_search_kernel_ms", "b200m_last_launches", "b200m_last_tc_pairs", "b200m_exactness_errors", "b200m_last_records", "b200m_last_real_tc_pairs", "b200m_last_fallback_rows",
     "b200m_shard_pairs", "b200m_shard_pairs_2d", "b200m_multi_create", "b200m_multi_destroy", "b200m_multi_num_devices", "b200m_multi_ctx", "b200m_multi_match",
-    "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model",
+    "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model", "b200m_set_view_geometry", "b200m_guided_match_fast_pairs",
 ]
 
 
@@ -151,6 +151,37 @@ class Context:
     def last_records(self) -> int: return self.lib.b200m_last_records(self._h)
     def last_real_tc_pairs(self) -> int: return self.lib.b200m_last_real_tc_pairs(self._h)
     def last_fallback_rows(self) -> int: return self.lib.b200m_last_fallback_rows(self._h)
+
+    def set_view_geometry(self, view_id: int, xy) -> None:
+        """b200m_set_view_geometry: the n x 2 double positions guided matching uses for an uploaded view instead of its float
+        upload positions (typically camera::IntrinsicBase::getUndistortedPixel of every feature); None drops them."""
+        if xy is None:
+            _check(self.lib.b200m_set_view_geometry(self._h, C.c_uint32(view_id), None, C.c_int(0)), "b200m_set_view_geometry")
+            return
+        a = np.ascontiguousarray(xy, np.float64).reshape(-1, 2)
+        _check(self.lib.b200m_set_view_geometry(self._h, C.c_uint32(view_id), a.ctypes.data_as(C.c_void_p), C.c_int(a.shape[0])),
+               "b200m_set_view_geometry")
+
+    def guided_match_fast_pairs(self, pairs, F, epipole2, wh, errorTh: float, distRatio: float) -> dict:
+        """b200m_guided_match_fast_pairs on resident views: guidedMatchingFundamentalFast (matching/guidedMatching.hpp:353-460) for
+        every (L, R) of `pairs`, with per-pair F [n, 3, 3] (x_R^T F x_L = 0), epipole2 [n, 3] (not normalised) and wh [n, 2] =
+        (widthR, heightR); errorTh / distRatio already squared.  Returns {(L, R): matches[MATCH_DTYPE]} in input order, empty lists
+        included; matches in ascending i, not de-duplicated."""
+        p = np.ascontiguousarray(pairs, np.uint32).reshape(-1, 2)
+        n = p.shape[0]
+        Fm = np.ascontiguousarray(F, np.float64).reshape(n, 9)
+        ep = np.ascontiguousarray(epipole2, np.float64).reshape(n, 3)
+        whm = np.ascontiguousarray(wh, np.int32).reshape(n, 2)
+        res = C.c_void_p()
+        _check(self.lib.b200m_guided_match_fast_pairs(self._h, p.ctypes.data_as(C.c_void_p), C.c_int(n), Fm.ctypes.data_as(C.c_void_p),
+                                                      ep.ctypes.data_as(C.c_void_p), whm.ctypes.data_as(C.c_void_p), C.c_double(errorTh),
+                                                      C.c_double(distRatio), C.byref(res)), "b200m_guided_match_fast_pairs")
+        owner = _ResultOwner(self.lib, res)
+        off, mat = C.c_void_p(), C.c_void_p()
+        _check(self.lib.b200m_result_get(res, None, C.byref(off), C.byref(mat)), "b200m_result_get")
+        offsets = _alias(off.value, (n + 1) * 8, np.int64, owner) if n else np.zeros(1, np.int64)
+        matches = _alias(mat.value, int(offsets[-1]) * MATCH_DTYPE.itemsize, MATCH_DTYPE, owner)
+        return {(int(a), int(b)): matches[offsets[k]:offsets[k + 1]].copy() for k, (a, b) in enumerate(p.tolist())}
 
 
 _default_ctx: dict[int, Context] = {}
@@ -448,24 +479,34 @@ PairwiseMatches.__hash__ = None
 MODEL_FUNDAMENTAL, MODEL_HOMOGRAPHY = 0, 1
 
 
+def _upload_pair(ctx: Context, ids, regions, geometry, up: list) -> None:
+    """Uploads two Regions (and their geometry positions, when given) under `ids`; appends each uploaded id to `up`."""
+    lib = ctx.lib
+    for vid, r, xy in zip(ids, regions, geometry):
+        n = r.RegionCount()
+        code = _dtype_code(r.descriptors, r.binary)
+        _check(lib.b200m_upload_view(ctx._h, C.c_uint32(vid), r.descriptors.ctypes.data_as(C.c_void_p) if n else None, C.c_int(n),
+                                     C.c_int(max(r.DescriptorLength(), 1)), C.c_int(code), r.positions.ctypes.data_as(C.c_void_p) if n else None), "b200m_upload_view")
+        up.append(vid)
+        if xy is not None:
+            ctx.set_view_geometry(vid, xy)
+
+
 def guidedMatching(F, regions_left: "Regions", regions_right: "Regions", errorTh: float, distRatio: float, ctx: Context | None = None,
-                   model: int = MODEL_FUNDAMENTAL) -> np.ndarray:
-    """matching::guidedMatching<Mat3Model, FundamentalEpipolarDistanceError> (matching/guidedMatching.hpp:206-268) for cameras
-    without distortion: F = 3x3 fundamental matrix (x_right^T F x_left = 0), errorTh / distRatio already squared as at the
-    call site (GeometricFilterMatrix_F_AC.hpp:387-388).  model = MODEL_HOMOGRAPHY: F is a homography and the error is
-    HomographyAsymmetricError (GeometricFilterMatrix_H_AC.hpp:217-225).  Returns matches[MATCH_DTYPE] with i = left, j = right feature."""
+                   model: int = MODEL_FUNDAMENTAL, xy_left=None, xy_right=None) -> np.ndarray:
+    """matching::guidedMatching<Mat3Model, FundamentalEpipolarDistanceError> (matching/guidedMatching.hpp:206-268): F = 3x3
+    fundamental matrix (x_right^T F x_left = 0), errorTh / distRatio already squared as at the call site
+    (GeometricFilterMatrix_F_AC.hpp:387-388).  model = MODEL_HOMOGRAPHY: F is a homography and the error is
+    HomographyAsymmetricError (GeometricFilterMatrix_H_AC.hpp:217-225).  xy_left / xy_right: optional n x 2 double positions used
+    instead of the regions' positions - the undistorted pixels the reference matches on when the camera is valid (:229-248).
+    Returns matches[MATCH_DTYPE] with i = left, j = right feature."""
     ctx = ctx or default_context()
     lib = ctx.lib
     ids = (_new_view_id(), _new_view_id())
     Fm = np.ascontiguousarray(F, np.float64).reshape(9)
     up = []
     try:
-        for vid, r in zip(ids, (regions_left, regions_right)):
-            n = r.RegionCount()
-            code = _dtype_code(r.descriptors, r.binary)
-            _check(lib.b200m_upload_view(ctx._h, C.c_uint32(vid), r.descriptors.ctypes.data_as(C.c_void_p) if n else None, C.c_int(n),
-                                         C.c_int(max(r.DescriptorLength(), 1)), C.c_int(code), r.positions.ctypes.data_as(C.c_void_p) if n else None), "b200m_upload_view")
-            up.append(vid)
+        _upload_pair(ctx, ids, (regions_left, regions_right), (xy_left, xy_right), up)
         res = C.c_void_p()
         _check(lib.b200m_guided_match_model(ctx._h, C.c_uint32(ids[0]), C.c_uint32(ids[1]), C.c_int(model), Fm.ctypes.data_as(C.c_void_p), C.c_double(errorTh),
                                             C.c_double(distRatio), C.byref(res)), "b200m_guided_match_model")
@@ -477,6 +518,24 @@ def guidedMatching(F, regions_left: "Regions", regions_right: "Regions", errorTh
     finally:
         for vid in up:
             lib.b200m_remove_view(ctx._h, C.c_uint32(vid))
+
+
+def guidedMatchingFundamentalFast(F, epipole2, regions_left: "Regions", regions_right: "Regions", widthR: int, heightR: int, errorTh: float,
+                                  distRatio: float, xy_left=None, xy_right=None, ctx: Context | None = None) -> np.ndarray:
+    """matching::guidedMatchingFundamentalFast<FundamentalEpipolarDistanceError> (matching/guidedMatching.hpp:353-460) for one pair:
+    F (x_right^T F x_left = 0), epipole2 = the left camera centre in the right image, not normalised (epipole_from_P), the right
+    image's size, errorTh / distRatio already squared (StructureEstimationFromKnownPoses.cpp:138-150).  xy_left / xy_right: optional
+    n x 2 double (undistorted) positions used instead of the regions' positions.  Returns matches[MATCH_DTYPE] in ascending i, not
+    de-duplicated.  For lists of pairs over resident views use Context.guided_match_fast_pairs."""
+    ctx = ctx or default_context()
+    ids = (_new_view_id(), _new_view_id())
+    up = []
+    try:
+        _upload_pair(ctx, ids, (regions_left, regions_right), (xy_left, xy_right), up)
+        return ctx.guided_match_fast_pairs([ids], [F], [epipole2], [(widthR, heightR)], errorTh, distRatio)[ids]
+    finally:
+        for vid in up:
+            ctx.lib.b200m_remove_view(ctx._h, C.c_uint32(vid))
 
 
 def createImageCollectionMatcher(matcherType: EMatcherType, distRatio: float, crossMatching: bool, ctx: Context | None = None):

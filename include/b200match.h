@@ -136,6 +136,34 @@ enum { B200M_MODEL_FUNDAMENTAL = 0, B200M_MODEL_HOMOGRAPHY = 1 };
 int b200m_guided_match_model(b200m_ctx* ctx, uint32_t view_left, uint32_t view_right, int model, const double* M, double errorTh, double distRatio,
                              b200m_result** out);
 
+/* Positions guided matching uses for one uploaded view instead of its (float) upload positions: n x 2 doubles, typically
+ * camera::IntrinsicBase::getUndistortedPixel of every feature (matching/guidedMatching.hpp:229-248, :395, :416): the reference
+ * matches on undistorted positions whenever the intrinsic is valid.  b200m_guided_match, b200m_guided_match_model and
+ * b200m_guided_match_fast_pairs use them when they are set; a view with geometry positions needs no upload positions.
+ * n must equal the view's feature count (else B200M_ERR_ARG); xy == NULL drops them; unknown view -> B200M_ERR_ARG.
+ * Re-uploading or removing the view drops them.  The array is copied before the call returns. */
+int b200m_set_view_geometry(b200m_ctx* ctx, uint32_t view_id, const double* xy, int n);
+
+/* matching::guidedMatchingFundamentalFast<FundamentalEpipolarDistanceError> (matching/guidedMatching.hpp:353-460), what
+ * StructureEstimationFromKnownPoses::match (sfm/pipeline/structureFromKnownPoses/StructureEstimationFromKnownPoses.cpp:72-163)
+ * runs for every pair of its list, for every pair (L = pairs[2k], R = pairs[2k+1]) of resident views:
+ *   F         n_pairs x 9 row-major (x_R^T F x_L = 0)
+ *   epipole2  n_pairs x 3, NOT normalised (as epipole_from_P returns it)
+ *   wh        n_pairs x 2 = (widthR, heightR), each >= 2 (else B200M_ERR_ARG)
+ *   errorTh, distRatio already squared, as StructureEstimationFromKnownPoses.cpp:138-150 passes them.
+ * Left features are bucketed by where their epipolar line meets the right image's border; each right feature compares against
+ * every left feature of the bucket range its +-sqrt(errorTh) band reaches (no geometric-error test), keeping the left feature's
+ * best right feature iff best < distRatio * second.  The result holds one pair per input pair, in input order (empty lists
+ * included); matches = IndMatch(i = left feature, j = right feature) in ascending i, ratio and distance 0, NOT de-duplicated
+ * (the reference does not).  Descriptors as for b200m_guided_match; a pair whose views differ in descriptor type, or with an
+ * empty view, gets an empty list.  Waits only for the views the list references; long lists run in internal batches of
+ * bounded size.  Instrumentation: b200m_last_records = candidate (left, right) distances evaluated.
+ * Where the reference is undefined - an epipole at infinity (epipole2[2] == 0) or a right feature exactly at the epipole - it
+ * indexes its buckets with NaN cast to int; here a line with a non-finite coefficient has no end points: the left feature
+ * joins no bucket and the right feature has no candidates. */
+int b200m_guided_match_fast_pairs(b200m_ctx* ctx, const uint32_t* pairs, int n_pairs, const double* F, const double* epipole2,
+                                  const int32_t* wh, double errorTh, double distRatio, b200m_result** out);
+
 /* ---- Surface 2 on several GPUs from one process --------------------------------------------------------------------- */
 /* Which shard (0..n_shards-1) each pair goes to: database images (first id) in ascending order are dealt round-robin over
  * the shards, direction alternating every round; all pairs of one database image stay together (its descriptors are
