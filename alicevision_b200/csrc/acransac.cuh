@@ -1,0 +1,306 @@
+// K10: a-contrario RANSAC fundamental-matrix estimation for a list of pairs (b200m_acransac_fundamental_pairs), sm_90a.
+//
+// One CTA runs one pair's robustEstimation::ACRANSAC loop (robustEstimation/ACRansac.hpp:186-272) iteration by iteration, with the
+// reference's control flow (10 % reserve, strict `<` on minNFA, the switch to sampling among the inliers, the "no model at all"
+// extension, the precision mode and its early exit).  Per iteration thread 0 draws the sample from the pair's own copy of the
+// caller's std::mt19937 (shared memory) and fits the 7-point models (acransac_math.h); then the whole CTA scores each model:
+//   * n residuals (point-to-line error on normalised points);
+//   * certified skip: a shared-memory histogram of the residuals over quarter-binade bins gives, for every k, a lower bound of the
+//     k-th smallest residual (the low edge of its bin), hence of NFA(k), which increases with that residual.  When the least bound
+//     over k is not below the current minNFA (less a 1e-9 relative margin that covers the device log10), the model cannot be
+//     `better` and is not scored exactly.  The loop is sequential, so the bound is compared with the true running minNFA;
+//   * exact score: (residual bits, index) keys sorted by a bitonic network, in shared memory up to kSmemSort keys and in a
+//     per-pair global scratch beyond; every k's NFA; the (NFA, k)-lexicographic argmin (bestNFA keeps the first k reaching the
+//     minimum).  NaN residuals sort after +inf, where std::sort is unspecified.
+// The winner's sorted indices are its inlier list in the reference's order.
+#pragma once
+#include "acransac_math.h"
+
+#include <cfloat>
+#include <cstdint>
+
+namespace acrk {
+
+constexpr int kThreads = 128;
+constexpr int kSmemSort = 1024;    // keys sorted in shared memory; larger pairs sort in global scratch
+constexpr int kBinLo = 1023 - 100; // biased exponent of the first quarter-binade bin (2^-100); bin 0 holds [0, 2^-100)
+constexpr int kBins = 2 + 4 * 128; // ... up to 2^28; the last bin holds everything above, +inf and NaN
+constexpr int kTraceCap = 256;      // `better` events (iteration, new minNFA) kept per pair (b200m_acransac_last_trace)
+
+struct Pair { long long off, sort_off; int n, w1, h1, w2, h2; };
+struct Out {
+  double F[9]; double error_max, min_nfa;
+  long long evaluated, skipped, exact;
+  int valid, n_inl, iterations, n_trace;
+};
+
+__device__ __forceinline__ int bin_of(double r) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(r);
+  const int e = (int)(b >> 52);
+  if (e < kBinLo) return 0;
+  const int q = 1 + (e - kBinLo) * 4 + (int)((b >> 50) & 3);
+  return q < kBins - 1 ? q : kBins - 1;
+}
+__device__ __forceinline__ double bin_low(int b) {
+  if (b == 0) return 0.0;
+  const int q = b - 1;
+  return __longlong_as_double((long long)(((unsigned long long)(kBinLo + q / 4) << 52) | ((unsigned long long)(q & 3) << 50)));
+}
+
+// NFA(k) of bestNFA for the squared residual e of rank k (errorVectorDimension 1)
+__device__ __forceinline__ double nfa_of(double e, int k, double la0, double loge0, const float* lcn, const float* lck) {
+  const double la = acr::add(la0, log10(acr::add(sqrt(e), (double)FLT_EPSILON)));
+  return acr::add(acr::add(acr::add(loge0, acr::mul(la, (double)(k - acr::kSample))), (double)lcn[k]), (double)lck[k]);
+}
+
+__device__ __forceinline__ bool lex_less(double v, int k, double v2, int k2) { return v2 < v || (v2 == v && k2 < k); }
+
+// (value, k) lexicographic minimum over the CTA; every thread gets the result
+__device__ void block_min(double& v, int& k, double* sv, int* sk) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int o = 16; o; o >>= 1) {
+    const double v2 = __shfl_down_sync(0xffffffffu, v, o);
+    const int k2 = __shfl_down_sync(0xffffffffu, k, o);
+    if (lex_less(v, k, v2, k2)) { v = v2; k = k2; }
+  }
+  if (lane == 0) { sv[warp] = v; sk[warp] = k; }
+  __syncthreads();
+  v = sv[0]; k = sk[0];
+  for (int w = 1; w < kThreads / 32; ++w)
+    if (lex_less(v, k, sv[w], sk[w])) { v = sv[w]; k = sk[w]; }
+  __syncthreads();
+}
+
+__device__ int block_sum(int x, int* si) {
+  for (int o = 16; o; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+  if ((threadIdx.x & 31) == 0) si[threadIdx.x >> 5] = x;
+  __syncthreads();
+  int s = 0;
+  for (int w = 0; w < kThreads / 32; ++w) s += si[w];
+  __syncthreads();
+  return s;
+}
+
+__device__ void bitonic(unsigned long long* K, uint32_t* V, int N2) {
+  for (int size = 2; size <= N2; size <<= 1)
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int t = threadIdx.x; t < N2 / 2; t += kThreads) {
+        const int i = 2 * t - (t & (stride - 1)), j = i + stride;
+        const unsigned long long ki = K[i], kj = K[j];
+        const uint32_t vi = V[i], vj = V[j];
+        const bool gt = ki > kj || (ki == kj && vi > vj);
+        if (gt == ((i & size) == 0)) { K[i] = kj; K[j] = ki; V[i] = vj; V[j] = vi; }
+      }
+      __syncthreads();
+    }
+}
+
+__device__ __forceinline__ double residual(const double* F, const double* pts, int i) {
+  const double2 a = reinterpret_cast<const double2*>(pts)[2 * i], b = reinterpret_cast<const double2*>(pts)[2 * i + 1];
+  return acr::epipolar_error(F, a.x, a.y, b.x, b.y);
+}
+
+// corr: per correspondence (xI, yI, xJ, yJ) at the pair's offset; l10[k] = (float)log10((double)k) for k <= the largest n.
+// Scratch at the pair's offset: pts (4 doubles), idx (the sampling list), logc (n + 1 floats each of logc_n and logc_k, at
+// 2 * (off + pair)), gkeys / gvals (pow2(n) at sort_off, pairs above kSmemSort only).  inliers: the result list at the offset.
+__global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __restrict__ pairs, const double* __restrict__ corr,
+                                                             const float* __restrict__ l10, const uint32_t* __restrict__ mt_state,
+                                                             long long max_iter, double precision, int skip_on, double* pts_all,
+                                                             uint32_t* idx_all, float* logc_all, unsigned long long* gkeys,
+                                                             uint32_t* gvals, uint32_t* inliers_all, int* trace_all, double* trace_nfa_all,
+                                                             Out* out_all) {
+  __shared__ acr::Mt19937 g;
+  __shared__ double models[27], bestF[9];
+  __shared__ int hist[kBins];
+  __shared__ unsigned long long skeys[kSmemSort];
+  __shared__ uint32_t svals[kSmemSort];
+  __shared__ double red_v[kThreads / 32];
+  __shared__ int red_k[kThreads / 32];
+  __shared__ long long nIter, nReserve, iter, evaluated, skipped, exact;
+  __shared__ int nb, mode, better, n_inl, n_idx, stop, copy_idx, n_trace;
+  __shared__ double minNFA, errorMax;
+
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const Pair P = pairs[p];
+  const int n = P.n;
+  Out* out = out_all + p;
+  const double inf = __longlong_as_double(0x7ff0000000000000ll);
+  if (n <= acr::kSample) {   // ACRANSAC returns (0, 0) at once
+    if (tid == 0) {
+      for (int t = 0; t < 9; ++t) out->F[t] = 0;
+      out->error_max = 0; out->min_nfa = 0; out->evaluated = out->skipped = out->exact = 0;
+      out->valid = 0; out->n_inl = 0; out->iterations = 0; out->n_trace = 0;
+    }
+    return;
+  }
+  const acr::Norm n1 = acr::precondition(P.w1, P.h1), n2 = acr::precondition(P.w2, P.h2);
+  double* pts = pts_all + 4 * P.off;
+  uint32_t* idx = idx_all + P.off;
+  uint32_t* inl = inliers_all + P.off;
+  float* lcn = logc_all + 2 * (P.off + p);
+  float* lck = lcn + n + 1;
+  const double* c = corr + 4 * P.off;
+  for (int i = tid; i < n; i += kThreads) {
+    pts[4 * i] = acr::norm_x(n1, c[4 * i]); pts[4 * i + 1] = acr::norm_y(n1, c[4 * i + 1]);
+    pts[4 * i + 2] = acr::norm_x(n2, c[4 * i + 2]); pts[4 * i + 3] = acr::norm_y(n2, c[4 * i + 3]);
+    idx[i] = i;
+  }
+  // makelogcombi: logcombi(k, n) is the float sum of the first min(k, n - k) terms l10[n - i + 1] - l10[i] in ascending i, so one
+  // running sum over k <= n / 2 gives every entry with the reference's bits (k >= n and k <= 0 give 0)
+  if (tid == 0) {
+    float r = 0.0f;
+    lcn[0] = 0.0f;
+    for (int k = 1; k <= n / 2; ++k) {
+      r = __fadd_rn(r, __fsub_rn(l10[n - k + 1], l10[k]));
+      lcn[k] = r;
+    }
+  }
+  __syncthreads();
+  for (int k = n / 2 + 1 + tid; k <= n; k += kThreads) lcn[k] = k >= n ? 0.0f : lcn[n - k];
+  for (int k = tid; k <= n; k += kThreads) {   // logcombi(7, k): at most 7 terms
+    float s = 0.0f;
+    if (!(acr::kSample >= k)) {
+      int kk = acr::kSample;
+      if (k - kk < kk) kk = k - kk;
+      for (int i = 1; i <= kk; ++i) s = __fadd_rn(s, __fsub_rn(l10[k - i + 1], l10[i]));
+    }
+    lck[k] = s;
+  }
+  for (int i = tid; i < acr::kMtN; i += kThreads) g.x[i] = mt_state[i];
+  const double la0 = log10(2.0 * sqrt(acr::add(acr::mul((double)P.w2, (double)P.w2), acr::mul((double)P.h2, (double)P.h2)))
+                           / acr::mul((double)P.w2, (double)P.h2) / n2.s);
+  const double loge0 = log10(acr::mul((double)acr::kMaxModels, (double)(n - acr::kSample)));
+  const double maxThr = precision == inf ? inf : acr::mul(acr::mul(acr::mul(precision, precision), n2.s), n2.s);
+  if (tid == 0) {
+    g.p = (int)mt_state[acr::kMtN];
+    nReserve = max_iter / 10; nIter = max_iter - nReserve; iter = 0;
+    evaluated = skipped = exact = 0;
+    mode = precision == inf; minNFA = inf; errorMax = inf; n_inl = 0; n_idx = n; stop = 0; n_trace = 0;
+    for (int t = 0; t < 9; ++t) bestF[t] = 0;
+  }
+  __syncthreads();
+
+  while (true) {
+    if (tid == 0) {
+      if (iter >= nIter) {
+        stop = 1;
+      } else {
+        uint32_t s[acr::kSample];
+        acr::rand_sample7(g, (uint32_t)(mode ? n_idx : n), s);
+        double a[7], b[7], cc[7], d[7];
+        for (int i = 0; i < acr::kSample; ++i) {
+          const uint32_t j = mode ? idx[s[i]] : s[i];
+          a[i] = pts[4 * j]; b[i] = pts[4 * j + 1]; cc[i] = pts[4 * j + 2]; d[i] = pts[4 * j + 3];
+        }
+        nb = acr::fit7(a, b, cc, d, models);
+        better = 0; copy_idx = 0;
+      }
+    }
+    __syncthreads();
+    if (stop) break;
+    for (int m = 0; m < nb; ++m) {
+      const double* F = models + 9 * m;
+      if (!mode) {   // precision mode: a model with more than 2.5 * 7 inliers switches to the a-contrario mode
+        int cnt = 0;
+        for (int i = tid; i < n; i += kThreads) cnt += residual(F, pts, i) <= maxThr;
+        cnt = block_sum(cnt, red_k);
+        if (tid == 0 && cnt > 2.5 * acr::kSample) mode = 1;
+        __syncthreads();
+        if (!mode) continue;
+      }
+      if (tid == 0) ++evaluated;
+      if (skip_on && minNFA < inf) {
+        for (int b = tid; b < kBins; b += kThreads) hist[b] = 0;
+        __syncthreads();
+        for (int i = tid; i < n; i += kThreads) atomicAdd(&hist[bin_of(residual(F, pts, i))], 1);
+        __syncthreads();
+        if (tid < 32) {   // inclusive prefix counts, 17 bins per lane
+          constexpr int per = (kBins + 31) / 32;
+          int s = 0;
+          for (int b = tid * per; b < min(kBins, (tid + 1) * per); ++b) s += hist[b];
+          int incl = s;
+          for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (tid >= o) incl += t; }
+          int run = incl - s;
+          for (int b = tid * per; b < min(kBins, (tid + 1) * per); ++b) { run += hist[b]; hist[b] = run; }
+        }
+        __syncthreads();
+        double lb = inf; int lk = 0;
+        for (int k = acr::kSample + 1 + tid; k <= n; k += kThreads) {
+          int lo = 0, hi = kBins - 1;   // first bin whose prefix count reaches k
+          while (lo < hi) { const int mid = (lo + hi) >> 1; if (hist[mid] >= k) hi = mid; else lo = mid + 1; }
+          const double v = nfa_of(bin_low(lo), k, la0, loge0, lcn, lck);
+          if (v < lb) { lb = v; lk = k; }
+        }
+        block_min(lb, lk, red_v, red_k);
+        if (acr::sub(lb, 1e-9 * fmax(1.0, fabs(lb))) >= minNFA) {
+          if (tid == 0) ++skipped;
+          continue;
+        }
+      }
+      if (tid == 0) ++exact;
+      int N2 = 1;
+      while (N2 < n) N2 <<= 1;
+      unsigned long long* K = N2 <= kSmemSort ? skeys : gkeys + P.sort_off;
+      uint32_t* V = N2 <= kSmemSort ? svals : gvals + P.sort_off;
+      for (int i = tid; i < N2; i += kThreads) {
+        K[i] = i < n ? (unsigned long long)__double_as_longlong(residual(F, pts, i)) : ~0ull;
+        V[i] = i < n ? (uint32_t)i : ~0u;
+      }
+      __syncthreads();
+      bitonic(K, V, N2);
+      double bv = inf; int bk = acr::kSample;
+      for (int k = acr::kSample + 1 + tid; k <= n; k += kThreads) {
+        const double e = __longlong_as_double((long long)K[k - 1]);
+        if (!(e <= maxThr)) continue;   // sorted: the ranks with e <= maxThreshold are a prefix
+        const double v = nfa_of(e, k, la0, loge0, lcn, lck);
+        if (lex_less(bv, bk, v, k)) { bv = v; bk = k; }
+      }
+      block_min(bv, bk, red_v, red_k);
+      if (bv < minNFA) {   // every thread holds the same (bv, bk) and minNFA
+        for (int i = tid; i < bk; i += kThreads) inl[i] = V[i];
+        __syncthreads();
+        if (tid == 0) {
+          better = 1; minNFA = bv; n_inl = bk;
+          errorMax = __longlong_as_double((long long)K[bk - 1]);
+          for (int t = 0; t < 9; ++t) bestF[t] = F[t];
+          if (n_trace < kTraceCap) {
+            trace_all[(long long)p * kTraceCap + n_trace] = (int)iter;
+            trace_nfa_all[(long long)p * kTraceCap + n_trace] = bv;
+          }
+          ++n_trace;
+        }
+      }
+      __syncthreads();
+    }
+    if (tid == 0) {
+      if (!mode && iter > nReserve * 2) stop = 1;
+      else if (mode && ((better && minNFA < 0) || (iter + 1 == nIter && nReserve))) {
+        if (n_inl == 0) { ++nIter; --nReserve; }
+        else {
+          copy_idx = 1; n_idx = n_inl;
+          if (nReserve) { nIter = iter + 1 + nReserve; nReserve = 0; }
+        }
+      }
+      ++iter;
+    }
+    __syncthreads();
+    const bool done = stop, copy = copy_idx;
+    if (done) break;
+    if (copy)
+      for (int i = tid; i < n_idx; i += kThreads) idx[i] = inl[i];
+    __syncthreads();   // every thread has read stop / copy_idx, and the sampling list is complete, before thread 0 draws again
+  }
+  if (tid == 0) {
+    const bool valid = minNFA < 0 && n_inl > 0;
+    double Fo[9];
+    for (int t = 0; t < 9; ++t) Fo[t] = bestF[t];
+    double em = errorMax;
+    if (valid) { acr::unnormalize(n1, n2, Fo); em = sqrt(em) / n2.s; }
+    for (int t = 0; t < 9; ++t) out->F[t] = Fo[t];
+    out->error_max = em; out->min_nfa = minNFA;
+    out->evaluated = evaluated; out->skipped = skipped; out->exact = exact;
+    out->valid = valid; out->n_inl = valid ? n_inl : 0; out->iterations = (int)iter; out->n_trace = n_trace;
+  }
+}
+
+}  // namespace acrk

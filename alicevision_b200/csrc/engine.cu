@@ -9,6 +9,7 @@
 #include "common.cuh"
 #include "finish.cuh"
 #include "guided.cuh"
+#include "acransac.cuh"
 #include "guided_fast.cuh"
 #include "hamming.cuh"
 #include "l2_exact.cuh"
@@ -242,8 +243,18 @@ struct GuidedFastScratch {
   cudaEvent_t ev_c0 = nullptr, ev_c1 = nullptr;           // candidate-kernel timing
 };
 
+// grow-only scratch of b200m_acransac_fundamental_pairs (acransac.cuh)
+struct AcransacScratch {
+  void* d = nullptr; size_t bytes = 0;
+  bool skip = true;                                   // certified skip (b200m_ctx_set_acransac_skip)
+  double last_ms = 0; int64_t stats[4] = {0, 0, 0, 0};
+  std::vector<int32_t> trace; std::vector<double> trace_nfa; std::vector<int32_t> n_trace;   // last call: kTraceCap entries per pair
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+};
+
 struct b200m_ctx {
   int device = 0, num_sms = 148;
+  AcransacScratch acr;
   KnnScratch knn;
   GuidedFastScratch gf;
   long gf_left_cap = 1l << 21;    // left features per internal batch of b200m_guided_match_fast_pairs (B200M_GUIDED_FAST_LEFT_CAP)
@@ -615,6 +626,8 @@ void b200m_ctx_destroy(b200m_ctx* c) {
   cudaStreamDestroy(c->up_stream);
   cudaStreamDestroy(c->tab_stream); cudaStreamDestroy(c->pack_stream);
   if (c->d_trace) cudaFree(c->d_trace);
+  if (c->acr.d) cudaFree(c->acr.d);
+  if (c->acr.ev0) { cudaEventDestroy(c->acr.ev0); cudaEventDestroy(c->acr.ev1); }
   cudaFree(c->d_views); cudaFree(c->d_flags); cudaFree(c->d_err);
   {
     KnnScratch& k = c->knn;
@@ -1757,6 +1770,137 @@ int b200m_guided_match_fast_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pai
     for (const uint2& x : per_pair[k]) *m++ = b200m_match{x.x, x.y, 0.f, 0.f};     // IndMatch(i, j): ratio and distance 0
   }
   *out = res.release();
+  return B200M_OK;
+}
+
+// ---- K10: a-contrario RANSAC fundamental matrix for a pair list (acransac.cuh) ------------------------------------------
+int b200m_acransac_fundamental_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh,
+                                     const uint32_t* mt_state, int64_t max_iteration, double precision, uint8_t* valid,
+                                     int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max, double* min_nfa,
+                                     int32_t* iterations) {
+  if (!c || n_pairs < 0 || max_iteration < 0 || max_iteration > INT32_MAX || !(precision > 0) ||
+      (n_pairs > 0 && (!offsets || !wh || !mt_state || !valid || !n_inliers || !F || !error_max || !min_nfa || !iterations)))
+    return fail(B200M_ERR_ARG, "bad arguments");
+  if (n_pairs > 0 && offsets[0] != 0) return fail(B200M_ERR_ARG, "offsets[0] must be 0");
+  std::vector<acrk::Pair> pairs((size_t)n_pairs);
+  int64_t sort_total = 0; int max_n = 0;
+  for (int k = 0; k < n_pairs; ++k) {
+    const int64_t n = offsets[k + 1] - offsets[k];
+    if (n < 0 || n > (1 << 24)) return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": offsets must ascend, at most 2^24 correspondences a pair");
+    for (int t = 0; t < 4; ++t)
+      if (wh[4 * k + t] < 1) return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": image sizes must be positive");
+    if ((int64_t)wh[4 * k] * wh[4 * k + 1] > INT32_MAX || (int64_t)wh[4 * k + 2] * wh[4 * k + 3] > INT32_MAX)
+      return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": width * height must fit an int, as in the reference");
+    int64_t n2 = 1;
+    while (n2 < n) n2 <<= 1;
+    pairs[k] = acrk::Pair{offsets[k], n2 > acrk::kSmemSort ? sort_total : 0, (int)n, wh[4 * k], wh[4 * k + 1], wh[4 * k + 2], wh[4 * k + 3]};
+    if (n2 > acrk::kSmemSort) sort_total += n2;
+    max_n = std::max(max_n, (int)n);
+  }
+  const int64_t N = n_pairs ? offsets[n_pairs] : 0;
+  if (N > 0 && (!corr || !inliers)) return fail(B200M_ERR_ARG, "bad arguments");
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  CK(cudaSetDevice(c->device));
+  c->acr.trace.assign((size_t)n_pairs * acrk::kTraceCap, 0); c->acr.trace_nfa.assign((size_t)n_pairs * acrk::kTraceCap, 0);
+  c->acr.n_trace.assign((size_t)n_pairs, 0);
+  for (int t = 0; t < 4; ++t) c->acr.stats[t] = 0;
+  c->acr.last_ms = 0;
+  if (n_pairs == 0) return B200M_OK;
+  // float log10 table of makelogcombi: log10 on the double k, rounded to float (pinned against the compiled reference's tables)
+  std::vector<float> l10((size_t)max_n + 2);
+  for (size_t k = 0; k < l10.size(); ++k) l10[k] = (float)log10((double)k);
+  // one grow-only device buffer
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_pairs = take(sizeof(acrk::Pair) * n_pairs), o_corr = take(sizeof(double) * 4 * N), o_l10 = take(sizeof(float) * l10.size()),
+               o_mt = take(sizeof(uint32_t) * 625), o_pts = take(sizeof(double) * 4 * N), o_idx = take(sizeof(uint32_t) * N),
+               o_logc = take(sizeof(float) * 2 * (N + n_pairs)), o_gk = take(sizeof(unsigned long long) * sort_total),
+               o_gv = take(sizeof(uint32_t) * sort_total), o_inl = take(sizeof(uint32_t) * N),
+               o_tr = take(sizeof(int32_t) * acrk::kTraceCap * n_pairs),
+               o_trn = take(sizeof(double) * acrk::kTraceCap * n_pairs), o_out = take(sizeof(acrk::Out) * n_pairs);
+  if (at > c->acr.bytes) {
+    if (c->acr.d) CK(cudaFree(c->acr.d));
+    c->acr.d = nullptr; c->acr.bytes = 0;
+    CK(cudaMalloc(&c->acr.d, at));
+    c->acr.bytes = at;
+  }
+  if (!c->acr.ev0) { CK(cudaEventCreate(&c->acr.ev0)); CK(cudaEventCreate(&c->acr.ev1)); }
+  char* d = (char*)c->acr.d;
+  cudaStream_t st = c->stream;
+  CK(cudaMemcpyAsync(d + o_pairs, pairs.data(), sizeof(acrk::Pair) * n_pairs, cudaMemcpyHostToDevice, st));
+  if (N) CK(cudaMemcpyAsync(d + o_corr, corr, sizeof(double) * 4 * N, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d + o_l10, l10.data(), sizeof(float) * l10.size(), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d + o_mt, mt_state, sizeof(uint32_t) * 625, cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(c->acr.ev0, st));
+  acrk::acransac_kernel<<<n_pairs, acrk::kThreads, 0, st>>>(
+      (const acrk::Pair*)(d + o_pairs), (const double*)(d + o_corr), (const float*)(d + o_l10), (const uint32_t*)(d + o_mt),
+      (long long)max_iteration, precision, c->acr.skip ? 1 : 0, (double*)(d + o_pts), (uint32_t*)(d + o_idx), (float*)(d + o_logc),
+      (unsigned long long*)(d + o_gk), (uint32_t*)(d + o_gv), (uint32_t*)(d + o_inl), (int*)(d + o_tr), (double*)(d + o_trn), (acrk::Out*)(d + o_out));
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(c->acr.ev1, st));
+  std::vector<acrk::Out> outs((size_t)n_pairs);
+  CK(cudaMemcpyAsync(outs.data(), d + o_out, sizeof(acrk::Out) * n_pairs, cudaMemcpyDeviceToHost, st));
+  if (N) CK(cudaMemcpyAsync(inliers, d + o_inl, sizeof(uint32_t) * N, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(c->acr.trace.data(), d + o_tr, sizeof(int32_t) * acrk::kTraceCap * n_pairs, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(c->acr.trace_nfa.data(), d + o_trn, sizeof(double) * acrk::kTraceCap * n_pairs, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0;
+  CK(cudaEventElapsedTime(&ms, c->acr.ev0, c->acr.ev1));
+  c->acr.last_ms = ms;
+  c->acr.stats[3] = 1;
+  for (int k = 0; k < n_pairs; ++k) {
+    const acrk::Out& o = outs[k];
+    valid[k] = (uint8_t)o.valid; n_inliers[k] = o.n_inl;
+    for (int t = 0; t < 9; ++t) F[9 * k + t] = o.F[t];
+    error_max[k] = o.error_max; min_nfa[k] = o.min_nfa; iterations[k] = o.iterations;
+    c->acr.n_trace[k] = o.n_trace;
+    c->acr.stats[0] += o.evaluated; c->acr.stats[1] += o.skipped; c->acr.stats[2] += o.exact;
+  }
+  return B200M_OK;
+}
+
+double b200m_acransac_last_stats(const b200m_ctx* c, int64_t stats[4]) {
+  if (!c) return 0;
+  std::lock_guard<std::recursive_mutex> api_lock(const_cast<b200m_ctx*>(c)->api_mu);   // a concurrent call rewrites them
+  if (stats) for (int t = 0; t < 4; ++t) stats[t] = c->acr.stats[t];
+  return c->acr.last_ms;
+}
+
+int b200m_acransac_last_trace(const b200m_ctx* c, int pair, int32_t* iters, double* nfa, int cap) {
+  if (!c) return 0;
+  std::lock_guard<std::recursive_mutex> api_lock(const_cast<b200m_ctx*>(c)->api_mu);
+  if (pair < 0 || pair >= (int)c->acr.n_trace.size()) return 0;
+  const int n = c->acr.n_trace[pair];
+  for (int i = 0; i < std::min({n, cap, acrk::kTraceCap}); ++i) {
+    if (iters) iters[i] = c->acr.trace[(size_t)pair * acrk::kTraceCap + i];
+    if (nfa) nfa[i] = c->acr.trace_nfa[(size_t)pair * acrk::kTraceCap + i];
+  }
+  return n;
+}
+
+int b200m_ctx_set_acransac_skip(b200m_ctx* c, int on) {
+  if (!c) return fail(B200M_ERR_ARG, "bad arguments");
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  c->acr.skip = on != 0;
+  return B200M_OK;
+}
+
+void b200m_mt19937_seed(uint32_t seed, uint32_t state[625]) {
+  acr::Mt19937 g;
+  acr::mt_seed(g, seed);
+  std::memcpy(state, g.x, sizeof g.x);
+  state[624] = (uint32_t)g.p;
+}
+
+int b200m_debug_rand_sample(const uint32_t state[625], int range, int draws, uint32_t* out, uint32_t* states) {
+  if (!state || range < 8 || draws < 0 || (draws > 0 && !out) || state[624] > (uint32_t)acr::kMtN) return fail(B200M_ERR_ARG, "bad arguments");
+  acr::Mt19937 g;
+  std::memcpy(g.x, state, sizeof g.x);
+  g.p = (int)state[624];
+  for (int d = 0; d < draws; ++d) {
+    acr::rand_sample7(g, (uint32_t)range, out + 7 * (size_t)d);
+    if (states) { std::memcpy(states + 625 * (size_t)d, g.x, sizeof g.x); states[625 * (size_t)d + 624] = (uint32_t)g.p; }
+  }
   return B200M_OK;
 }
 

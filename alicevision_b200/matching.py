@@ -37,6 +37,8 @@ ABI_SYMBOLS = [
     "b200m_last_search_kernel_ms", "b200m_last_launches", "b200m_last_tc_pairs", "b200m_exactness_errors", "b200m_last_records", "b200m_last_real_tc_pairs", "b200m_last_fallback_rows",
     "b200m_shard_pairs", "b200m_shard_pairs_2d", "b200m_multi_create", "b200m_multi_destroy", "b200m_multi_num_devices", "b200m_multi_ctx", "b200m_multi_match",
     "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model", "b200m_set_view_geometry", "b200m_guided_match_fast_pairs",
+    "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
+    "b200m_mt19937_seed", "b200m_debug_rand_sample",
 ]
 
 
@@ -74,7 +76,8 @@ def load_library() -> C.CDLL:
     lib.b200m_exactness_errors.restype = C.c_uint
     lib.b200m_multi_last_gpu_ms.restype = C.c_double
     lib.b200m_multi_ctx.restype = C.c_void_p
-    for name in ("b200m_ctx_destroy", "b200m_db_destroy", "b200m_result_free", "b200m_multi_destroy"):
+    lib.b200m_acransac_last_stats.restype = C.c_double
+    for name in ("b200m_ctx_destroy", "b200m_db_destroy", "b200m_result_free", "b200m_multi_destroy", "b200m_mt19937_seed"):
         getattr(lib, name).restype = None
     _lib = lib
     return lib
@@ -182,6 +185,72 @@ class Context:
         offsets = _alias(off.value, (n + 1) * 8, np.int64, owner) if n else np.zeros(1, np.int64)
         matches = _alias(mat.value, int(offsets[-1]) * MATCH_DTYPE.itemsize, MATCH_DTYPE, owner)
         return {(int(a), int(b)): matches[offsets[k]:offsets[k + 1]].copy() for k, (a, b) in enumerate(p.tolist())}
+
+    def set_acransac_skip(self, on: bool) -> None:
+        """Debug: the certified skip of models that cannot beat the running minNFA (on by default); results do not depend on it."""
+        _check(self.lib.b200m_ctx_set_acransac_skip(self._h, C.c_int(int(on))), "b200m_ctx_set_acransac_skip")
+
+    def acransac_fundamental_pairs(self, corr_list, wh, mt_state, maxIteration: int = 50000, precision: float = np.inf) -> list[dict]:
+        """b200m_acransac_fundamental_pairs: GeometricFilterMatrix_F_AC::geometricEstimation_Mat_ACRANSAC<Fundamental7PSolver> for
+        every pair.  corr_list: per pair an n x 4 array (xI, yI, xJ, yJ); wh: per pair (widthI, heightI, widthJ, heightJ);
+        mt_state: 625 words (mt19937_state), the same for every pair.  Returns per pair, in input order, {"valid", "inliers" (the
+        reference's order), "F" (3 x 3, x_J^T F x_I = 0), "error_max", "min_nfa", "iterations", "trace" / "trace_nfa" (iterations at
+        which a better model was found and its minNFA, the first 256), "n_trace"}."""
+        cs = [np.ascontiguousarray(c, np.float64).reshape(-1, 4) for c in corr_list]
+        n = len(cs)
+        offsets = np.zeros(n + 1, np.int64)
+        offsets[1:] = np.cumsum([c.shape[0] for c in cs]) if n else []
+        corr = np.ascontiguousarray(np.concatenate(cs) if n and offsets[-1] else np.zeros((1, 4)), np.float64)
+        whm = np.ascontiguousarray(wh, np.int32).reshape(n, 4)
+        st = np.ascontiguousarray(mt_state, np.uint32).reshape(625)
+        valid = np.zeros(max(n, 1), np.uint8); ninl = np.zeros(max(n, 1), np.int32); it = np.zeros(max(n, 1), np.int32)
+        inl = np.zeros(max(int(offsets[-1]), 1), np.uint32); F = np.zeros((max(n, 1), 9)); em = np.zeros(max(n, 1)); nfa = np.zeros(max(n, 1))
+        ptr = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        _check(self.lib.b200m_acransac_fundamental_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st), C.c_int64(maxIteration),
+                                                         C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(F), ptr(em), ptr(nfa), ptr(it)),
+               "b200m_acransac_fundamental_pairs")
+        out = []
+        tr = np.zeros(256, np.int32); trn = np.zeros(256, np.float64)
+        for k in range(n):
+            nt = self.lib.b200m_acransac_last_trace(self._h, C.c_int(k), ptr(tr), ptr(trn), C.c_int(tr.size))
+            out.append({"valid": bool(valid[k]), "inliers": inl[offsets[k]:offsets[k] + ninl[k]].copy(), "F": F[k].reshape(3, 3).copy(),
+                        "error_max": float(em[k]), "min_nfa": float(nfa[k]), "iterations": int(it[k]), "n_trace": int(nt),
+                        "trace": tr[:min(nt, tr.size)].copy(), "trace_nfa": trn[:min(nt, trn.size)].copy()})
+        return out
+
+    def acransac_last_stats(self) -> dict:
+        """Instrumentation of the last acransac_fundamental_pairs call."""
+        st = np.zeros(4, np.int64)
+        ms = self.lib.b200m_acransac_last_stats(self._h, st.ctypes.data_as(C.c_void_p))
+        return {"gpu_ms": ms, "models_evaluated": int(st[0]), "models_skipped": int(st[1]), "models_exact": int(st[2]), "launches": int(st[3])}
+
+
+def mt19937_state(seed: int) -> np.ndarray:
+    """std::mt19937(seed) as the 625 words of its operator<< (b200m_mt19937_seed; host only)."""
+    st = np.zeros(625, np.uint32)
+    load_library().b200m_mt19937_seed(C.c_uint32(seed), st.ctypes.data_as(C.c_void_p))
+    return st
+
+
+def debug_rand_sample(state, rng: int, draws: int):
+    """The engine's sampler on the CPU (b200m_debug_rand_sample): `draws` consecutive randSample(g, 0, rng, 7) from `state`.
+    Returns (draws x 7 samples in their order, draws x 625 generator states after each draw)."""
+    st = np.ascontiguousarray(state, np.uint32).reshape(625)
+    out = np.zeros((draws, 7), np.uint32); sts = np.zeros((draws, 625), np.uint32)
+    _check(load_library().b200m_debug_rand_sample(st.ctypes.data_as(C.c_void_p), C.c_int(rng), C.c_int(draws), out.ctypes.data_as(C.c_void_p),
+                                                  sts.ctypes.data_as(C.c_void_p)), "b200m_debug_rand_sample")
+    return out, sts
+
+
+def geometricEstimation_F_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: int = 50000, precision: float = np.inf,
+                             ctx: Context | None = None) -> dict:
+    """GeometricFilterMatrix_F_AC::geometricEstimation_Mat_ACRANSAC<Fundamental7PSolver, Mat3Model> of one pair on the GPU.
+    xI, xJ: n x 2 positions (the 2 x n matrices of fillMatricesWithUndistortFeaturesMatches, transposed); sizeI / sizeJ: (width,
+    height); seed_or_state: a std::mt19937 seed or its 625-word state.  Returns the dict of Context.acransac_fundamental_pairs."""
+    ctx = ctx or default_context()
+    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else seed_or_state
+    corr = np.concatenate([np.asarray(xI, np.float64).reshape(-1, 2), np.asarray(xJ, np.float64).reshape(-1, 2)], axis=1)
+    return ctx.acransac_fundamental_pairs([corr], [tuple(sizeI) + tuple(sizeJ)], st, maxIteration, precision)[0]
 
 
 _default_ctx: dict[int, Context] = {}

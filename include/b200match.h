@@ -191,6 +191,36 @@ int b200m_multi_match(b200m_multi* m, int n_views, const uint32_t* view_ids, con
 /* max over devices of the GPU time of the last b200m_multi_match, ms */
 double b200m_multi_last_gpu_ms(const b200m_multi* m);
 
+/* ---- geometric filtering: a-contrario RANSAC fundamental matrix (K10) -------------------------------------------- */
+/* GeometricFilterMatrix_F_AC::geometricEstimation_Mat_ACRANSAC<Fundamental7PSolver, Mat3Model> for every pair of a list, results
+ * in input order.  Every pair starts from the same generator state, as the reference passes the std::mt19937 by value.
+ *   offsets    n_pairs + 1 ascending correspondence offsets
+ *   corr       offsets[n_pairs] x 4 doubles (xI, yI, xJ, yJ): the pair's xI / xJ matrices (fillMatricesWithUndistortFeaturesMatches)
+ *   wh         n_pairs x 4 = (widthI, heightI, widthJ, heightJ), each >= 1
+ *   mt_state   625 words: the caller's std::mt19937 as its operator<< writes it (624 words, then the position)
+ *   max_iteration  ACRANSAC's nIter; precision: its upper bound (+inf = pure a-contrario mode)
+ * Out: valid[n_pairs] (minNFA < 0), n_inliers[n_pairs], inliers (at offsets, the reference's order), F[9 * n_pairs] (row-major,
+ * x_J^T F x_I = 0; unnormalised when valid), error_max[n_pairs] (ACRANSAC's first result), min_nfa[n_pairs],
+ * iterations[n_pairs] (loop iterations executed).  A pair with at most 7 correspondences returns (0, 0) and no iteration. */
+int b200m_acransac_fundamental_pairs(b200m_ctx* ctx, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh,
+                                     const uint32_t* mt_state, int64_t max_iteration, double precision, uint8_t* valid,
+                                     int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max, double* min_nfa,
+                                     int32_t* iterations);
+/* instrumentation of the last b200m_acransac_fundamental_pairs: stats = {models evaluated in the a-contrario mode, of them skipped
+ * by the histogram bound, scored exactly, kernel launches}; returns its GPU time in ms */
+double b200m_acransac_last_stats(const b200m_ctx* ctx, int64_t stats[4]);
+/* the `better` events of the last call's pair `pair`: the iterations at which a better model was found and the new minNFA of each
+ * (the first `cap`, at most 256; either pointer may be NULL); returns their number.  The getters of the last call take the context's
+ * lock, so a concurrent call on the same context cannot rewrite what they read. */
+int b200m_acransac_last_trace(const b200m_ctx* ctx, int pair, int32_t* iters, double* nfa, int cap);
+/* debug: 1 (default) = certified skip of models that cannot beat the running minNFA; 0 = score every model exactly */
+int b200m_ctx_set_acransac_skip(b200m_ctx* ctx, int on);
+/* host only: std::mt19937(seed) as 625 words (see mt_state) */
+void b200m_mt19937_seed(uint32_t seed, uint32_t state[625]);
+/* host only (debug): the engine's sampler on the CPU.  `draws` consecutive randSample(g, 0, range, 7) from `state`: the samples in
+ * their order (draws x 7), and the state after each draw (draws x 625) when states != NULL.  range >= 8. */
+int b200m_debug_rand_sample(const uint32_t state[625], int range, int draws, uint32_t* out, uint32_t* states);
+
 /* ---- instrumentation ------------------------------------------------------------------------------------------ */
 /* GPU time of the last b200m_match_pairs between its first and last enqueue (CUDA events on the context's stream), ms */
 double b200m_last_gpu_ms(const b200m_ctx* ctx);
