@@ -1,10 +1,12 @@
-// K10: a-contrario RANSAC fundamental-matrix estimation for a list of pairs (b200m_acransac_fundamental_pairs), sm_90a.
+// K10: a-contrario RANSAC estimation for a list of pairs, sm_90a: the fundamental matrix (b200m_acransac_fundamental_pairs,
+// FPolicy) and the homography (b200m_acransac_homography_pairs, HPolicy).  The kernel is one template over the model policy.
 //
 // One CTA runs one pair's robustEstimation::ACRANSAC loop (robustEstimation/ACRansac.hpp:186-272) iteration by iteration, with the
 // reference's control flow (10 % reserve, strict `<` on minNFA, the switch to sampling among the inliers, the "no model at all"
 // extension, the precision mode and its early exit).  Per iteration thread 0 draws the sample from the pair's own copy of the
-// caller's std::mt19937 (shared memory) and fits the 7-point models (acransac_math.h); then the whole CTA scores each model:
-//   * n residuals (point-to-line error on normalised points);
+// caller's std::mt19937 (shared memory) and fits the models (7-point F or 4-point H, acransac_math.h); then the whole CTA scores
+// each model:
+//   * n residuals (F: point-to-line error, H: point-to-point transfer error, on normalised points);
 //   * certified skip: a shared-memory histogram of the residuals over quarter-binade bins gives, for every k, a lower bound of the
 //     k-th smallest residual (the low edge of its bin), hence of NFA(k), which increases with that residual.  When the least bound
 //     over k is not below the current minNFA (less a 1e-9 relative margin that covers the device log10), the model cannot be
@@ -12,7 +14,8 @@
 //   * exact score: (residual bits, index) keys sorted by a bitonic network, in shared memory up to kSmemSort keys and in a
 //     per-pair global scratch beyond; every k's NFA; the (NFA, k)-lexicographic argmin (bestNFA keeps the first k reaching the
 //     minimum).  NaN residuals sort after +inf, where std::sort is unspecified.
-// The winner's sorted indices are its inlier list in the reference's order.
+// The winner's sorted indices are its inlier list in the reference's order.  When asked, the generator's state after the pair's
+// last draw is written back (HPolicy: the reference passes its std::mt19937 by reference from pair to pair).
 #pragma once
 #include "acransac_math.h"
 
@@ -29,7 +32,7 @@ constexpr int kTraceCap = 256;      // `better` events (iteration, new minNFA) k
 
 struct Pair { long long off, sort_off; int n, w1, h1, w2, h2; };
 struct Out {
-  double F[9]; double error_max, min_nfa;
+  double model[9]; double error_max, min_nfa;
   long long evaluated, skipped, exact;
   int valid, n_inl, iterations, n_trace;
 };
@@ -47,10 +50,31 @@ __device__ __forceinline__ double bin_low(int b) {
   return __longlong_as_double((long long)(((unsigned long long)(kBinLo + q / 4) << 52) | ((unsigned long long)(q & 3) << 50)));
 }
 
-// NFA(k) of bestNFA for the squared residual e of rank k (errorVectorDimension 1)
+// Model policies: sample size, maximum number of models, fit, residual, logalpha0, errorVectorDimension, unnormaliser
+struct FPolicy {   // RelativePoseKernel<Fundamental7PSolver, FundamentalEpipolarDistanceError, UnnormalizerT>
+  static constexpr int kSample = acr::kSample, kMaxModels = acr::kMaxModels, kErrDim = 1;
+  __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) { return acr::fit7(a, b, c, d, m); }
+  __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::epipolar_error(m, x1, y1, x2, y2); }
+  __device__ static double logalpha0(int w2, int h2, const acr::Norm& n2) {
+    return log10(2.0 * sqrt(acr::add(acr::mul((double)w2, (double)w2), acr::mul((double)h2, (double)h2))) / acr::mul((double)w2, (double)h2) / n2.s);
+  }
+  __device__ static void unnormalize(const acr::Norm& n1, const acr::Norm& n2, double* m) { acr::unnormalize(n1, n2, m); }
+};
+struct HPolicy {   // RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError, UnnormalizerI>, point to point
+  static constexpr int kSample = acr::kSampleH, kMaxModels = acr::kMaxModelsH, kErrDim = 2;
+  __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) { return acr::fit4(a, b, c, d, m); }
+  __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::homography_error(m, x1, y1, x2, y2); }
+  __device__ static double logalpha0(int w2, int h2, const acr::Norm& n2) { return acr::logalpha0_h(w2, h2, n2); }
+  __device__ static void unnormalize(const acr::Norm& n1, const acr::Norm& n2, double* m) { acr::unnormalize_h(n1, n2, m); }
+};
+
+// NFA(k) of bestNFA for the squared residual e of rank k: loge0 + (la0 + d log10(sqrt(e) + FLT_EPSILON)) (k - kSample) + logc_n[k]
+// + logc_k[k], d = errorVectorDimension (1: F, 2: H; the product by 2 is exact)
+template <class P>
 __device__ __forceinline__ double nfa_of(double e, int k, double la0, double loge0, const float* lcn, const float* lck) {
-  const double la = acr::add(la0, log10(acr::add(sqrt(e), (double)FLT_EPSILON)));
-  return acr::add(acr::add(acr::add(loge0, acr::mul(la, (double)(k - acr::kSample))), (double)lcn[k]), (double)lck[k]);
+  const double l = log10(acr::add(sqrt(e), (double)FLT_EPSILON));
+  const double la = acr::add(la0, P::kErrDim == 1 ? l : acr::mul((double)P::kErrDim, l));
+  return acr::add(acr::add(acr::add(loge0, acr::mul(la, (double)(k - P::kSample))), (double)lcn[k]), (double)lck[k]);
 }
 
 __device__ __forceinline__ bool lex_less(double v, int k, double v2, int k2) { return v2 < v || (v2 == v && k2 < k); }
@@ -95,22 +119,26 @@ __device__ void bitonic(unsigned long long* K, uint32_t* V, int N2) {
     }
 }
 
-__device__ __forceinline__ double residual(const double* F, const double* pts, int i) {
+template <class P>
+__device__ __forceinline__ double residual(const double* M, const double* pts, int i) {
   const double2 a = reinterpret_cast<const double2*>(pts)[2 * i], b = reinterpret_cast<const double2*>(pts)[2 * i + 1];
-  return acr::epipolar_error(F, a.x, a.y, b.x, b.y);
+  return P::error(M, a.x, a.y, b.x, b.y);
 }
 
 // corr: per correspondence (xI, yI, xJ, yJ) at the pair's offset; l10[k] = (float)log10((double)k) for k <= the largest n.
 // Scratch at the pair's offset: pts (4 doubles), idx (the sampling list), logc (n + 1 floats each of logc_n and logc_k, at
 // 2 * (off + pair)), gkeys / gvals (pow2(n) at sort_off, pairs above kSmemSort only).  inliers: the result list at the offset.
+// mt_state: 625 words at p * mt_stride (mt_stride 0: one state for every pair); mt_out: NULL, or 625 words per pair receiving the
+// generator state after the pair's last draw.
+template <class P>
 __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __restrict__ pairs, const double* __restrict__ corr,
                                                              const float* __restrict__ l10, const uint32_t* __restrict__ mt_state,
-                                                             long long max_iter, double precision, int skip_on, double* pts_all,
+                                                             int mt_stride, long long max_iter, double precision, int skip_on, double* pts_all,
                                                              uint32_t* idx_all, float* logc_all, unsigned long long* gkeys,
                                                              uint32_t* gvals, uint32_t* inliers_all, int* trace_all, double* trace_nfa_all,
-                                                             Out* out_all) {
+                                                             Out* out_all, uint32_t* mt_out) {
   __shared__ acr::Mt19937 g;
-  __shared__ double models[27], bestF[9];
+  __shared__ double models[9 * P::kMaxModels], bestF[9];
   __shared__ int hist[kBins];
   __shared__ unsigned long long skeys[kSmemSort];
   __shared__ uint32_t svals[kSmemSort];
@@ -121,25 +149,28 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
   __shared__ double minNFA, errorMax;
 
   const int p = blockIdx.x, tid = threadIdx.x;
-  const Pair P = pairs[p];
-  const int n = P.n;
+  const Pair Q = pairs[p];
+  const int n = Q.n;
   Out* out = out_all + p;
   const double inf = __longlong_as_double(0x7ff0000000000000ll);
-  if (n <= acr::kSample) {   // ACRANSAC returns (0, 0) at once
+  const uint32_t* st_in = mt_state + (long long)p * mt_stride;
+  if (n <= P::kSample) {   // ACRANSAC returns (0, 0) at once, without a draw
     if (tid == 0) {
-      for (int t = 0; t < 9; ++t) out->F[t] = 0;
+      for (int t = 0; t < 9; ++t) out->model[t] = 0;
       out->error_max = 0; out->min_nfa = 0; out->evaluated = out->skipped = out->exact = 0;
       out->valid = 0; out->n_inl = 0; out->iterations = 0; out->n_trace = 0;
     }
+    if (mt_out)
+      for (int i = tid; i <= acr::kMtN; i += kThreads) mt_out[(long long)p * (acr::kMtN + 1) + i] = st_in[i];
     return;
   }
-  const acr::Norm n1 = acr::precondition(P.w1, P.h1), n2 = acr::precondition(P.w2, P.h2);
-  double* pts = pts_all + 4 * P.off;
-  uint32_t* idx = idx_all + P.off;
-  uint32_t* inl = inliers_all + P.off;
-  float* lcn = logc_all + 2 * (P.off + p);
+  const acr::Norm n1 = acr::precondition(Q.w1, Q.h1), n2 = acr::precondition(Q.w2, Q.h2);
+  double* pts = pts_all + 4 * Q.off;
+  uint32_t* idx = idx_all + Q.off;
+  uint32_t* inl = inliers_all + Q.off;
+  float* lcn = logc_all + 2 * (Q.off + p);
   float* lck = lcn + n + 1;
-  const double* c = corr + 4 * P.off;
+  const double* c = corr + 4 * Q.off;
   for (int i = tid; i < n; i += kThreads) {
     pts[4 * i] = acr::norm_x(n1, c[4 * i]); pts[4 * i + 1] = acr::norm_y(n1, c[4 * i + 1]);
     pts[4 * i + 2] = acr::norm_x(n2, c[4 * i + 2]); pts[4 * i + 3] = acr::norm_y(n2, c[4 * i + 3]);
@@ -157,22 +188,21 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
   }
   __syncthreads();
   for (int k = n / 2 + 1 + tid; k <= n; k += kThreads) lcn[k] = k >= n ? 0.0f : lcn[n - k];
-  for (int k = tid; k <= n; k += kThreads) {   // logcombi(7, k): at most 7 terms
+  for (int k = tid; k <= n; k += kThreads) {   // logcombi(kSample, k): at most kSample terms
     float s = 0.0f;
-    if (!(acr::kSample >= k)) {
-      int kk = acr::kSample;
+    if (!(P::kSample >= k)) {
+      int kk = P::kSample;
       if (k - kk < kk) kk = k - kk;
       for (int i = 1; i <= kk; ++i) s = __fadd_rn(s, __fsub_rn(l10[k - i + 1], l10[i]));
     }
     lck[k] = s;
   }
-  for (int i = tid; i < acr::kMtN; i += kThreads) g.x[i] = mt_state[i];
-  const double la0 = log10(2.0 * sqrt(acr::add(acr::mul((double)P.w2, (double)P.w2), acr::mul((double)P.h2, (double)P.h2)))
-                           / acr::mul((double)P.w2, (double)P.h2) / n2.s);
-  const double loge0 = log10(acr::mul((double)acr::kMaxModels, (double)(n - acr::kSample)));
+  for (int i = tid; i < acr::kMtN; i += kThreads) g.x[i] = st_in[i];
+  const double la0 = P::logalpha0(Q.w2, Q.h2, n2);
+  const double loge0 = log10(acr::mul((double)P::kMaxModels, (double)(n - P::kSample)));
   const double maxThr = precision == inf ? inf : acr::mul(acr::mul(acr::mul(precision, precision), n2.s), n2.s);
   if (tid == 0) {
-    g.p = (int)mt_state[acr::kMtN];
+    g.p = (int)st_in[acr::kMtN];
     nReserve = max_iter / 10; nIter = max_iter - nReserve; iter = 0;
     evaluated = skipped = exact = 0;
     mode = precision == inf; minNFA = inf; errorMax = inf; n_inl = 0; n_idx = n; stop = 0; n_trace = 0;
@@ -185,14 +215,14 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
       if (iter >= nIter) {
         stop = 1;
       } else {
-        uint32_t s[acr::kSample];
-        acr::rand_sample7(g, (uint32_t)(mode ? n_idx : n), s);
-        double a[7], b[7], cc[7], d[7];
-        for (int i = 0; i < acr::kSample; ++i) {
+        uint32_t s[P::kSample];
+        acr::rand_sample<P::kSample>(g, (uint32_t)(mode ? n_idx : n), s);
+        double a[P::kSample], b[P::kSample], cc[P::kSample], d[P::kSample];
+        for (int i = 0; i < P::kSample; ++i) {
           const uint32_t j = mode ? idx[s[i]] : s[i];
           a[i] = pts[4 * j]; b[i] = pts[4 * j + 1]; cc[i] = pts[4 * j + 2]; d[i] = pts[4 * j + 3];
         }
-        nb = acr::fit7(a, b, cc, d, models);
+        nb = P::fit(a, b, cc, d, models);
         better = 0; copy_idx = 0;
       }
     }
@@ -200,11 +230,11 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
     if (stop) break;
     for (int m = 0; m < nb; ++m) {
       const double* F = models + 9 * m;
-      if (!mode) {   // precision mode: a model with more than 2.5 * 7 inliers switches to the a-contrario mode
+      if (!mode) {   // precision mode: a model with more than 2.5 * kSample inliers switches to the a-contrario mode
         int cnt = 0;
-        for (int i = tid; i < n; i += kThreads) cnt += residual(F, pts, i) <= maxThr;
+        for (int i = tid; i < n; i += kThreads) cnt += residual<P>(F, pts, i) <= maxThr;
         cnt = block_sum(cnt, red_k);
-        if (tid == 0 && cnt > 2.5 * acr::kSample) mode = 1;
+        if (tid == 0 && cnt > 2.5 * P::kSample) mode = 1;
         __syncthreads();
         if (!mode) continue;
       }
@@ -212,7 +242,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
       if (skip_on && minNFA < inf) {
         for (int b = tid; b < kBins; b += kThreads) hist[b] = 0;
         __syncthreads();
-        for (int i = tid; i < n; i += kThreads) atomicAdd(&hist[bin_of(residual(F, pts, i))], 1);
+        for (int i = tid; i < n; i += kThreads) atomicAdd(&hist[bin_of(residual<P>(F, pts, i))], 1);
         __syncthreads();
         if (tid < 32) {   // inclusive prefix counts, 17 bins per lane
           constexpr int per = (kBins + 31) / 32;
@@ -225,10 +255,10 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
         }
         __syncthreads();
         double lb = inf; int lk = 0;
-        for (int k = acr::kSample + 1 + tid; k <= n; k += kThreads) {
+        for (int k = P::kSample + 1 + tid; k <= n; k += kThreads) {
           int lo = 0, hi = kBins - 1;   // first bin whose prefix count reaches k
           while (lo < hi) { const int mid = (lo + hi) >> 1; if (hist[mid] >= k) hi = mid; else lo = mid + 1; }
-          const double v = nfa_of(bin_low(lo), k, la0, loge0, lcn, lck);
+          const double v = nfa_of<P>(bin_low(lo), k, la0, loge0, lcn, lck);
           if (v < lb) { lb = v; lk = k; }
         }
         block_min(lb, lk, red_v, red_k);
@@ -240,19 +270,19 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
       if (tid == 0) ++exact;
       int N2 = 1;
       while (N2 < n) N2 <<= 1;
-      unsigned long long* K = N2 <= kSmemSort ? skeys : gkeys + P.sort_off;
-      uint32_t* V = N2 <= kSmemSort ? svals : gvals + P.sort_off;
+      unsigned long long* K = N2 <= kSmemSort ? skeys : gkeys + Q.sort_off;
+      uint32_t* V = N2 <= kSmemSort ? svals : gvals + Q.sort_off;
       for (int i = tid; i < N2; i += kThreads) {
-        K[i] = i < n ? (unsigned long long)__double_as_longlong(residual(F, pts, i)) : ~0ull;
+        K[i] = i < n ? (unsigned long long)__double_as_longlong(residual<P>(F, pts, i)) : ~0ull;
         V[i] = i < n ? (uint32_t)i : ~0u;
       }
       __syncthreads();
       bitonic(K, V, N2);
-      double bv = inf; int bk = acr::kSample;
-      for (int k = acr::kSample + 1 + tid; k <= n; k += kThreads) {
+      double bv = inf; int bk = P::kSample;
+      for (int k = P::kSample + 1 + tid; k <= n; k += kThreads) {
         const double e = __longlong_as_double((long long)K[k - 1]);
         if (!(e <= maxThr)) continue;   // sorted: the ranks with e <= maxThreshold are a prefix
-        const double v = nfa_of(e, k, la0, loge0, lcn, lck);
+        const double v = nfa_of<P>(e, k, la0, loge0, lcn, lck);
         if (lex_less(bv, bk, v, k)) { bv = v; bk = k; }
       }
       block_min(bv, bk, red_v, red_k);
@@ -295,11 +325,16 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
     double Fo[9];
     for (int t = 0; t < 9; ++t) Fo[t] = bestF[t];
     double em = errorMax;
-    if (valid) { acr::unnormalize(n1, n2, Fo); em = sqrt(em) / n2.s; }
-    for (int t = 0; t < 9; ++t) out->F[t] = Fo[t];
+    if (valid) { P::unnormalize(n1, n2, Fo); em = sqrt(em) / n2.s; }
+    for (int t = 0; t < 9; ++t) out->model[t] = Fo[t];
     out->error_max = em; out->min_nfa = minNFA;
     out->evaluated = evaluated; out->skipped = skipped; out->exact = exact;
     out->valid = valid; out->n_inl = valid ? n_inl : 0; out->iterations = (int)iter; out->n_trace = n_trace;
+  }
+  if (mt_out) {   // thread 0's last draw is ordered before the loop's final __syncthreads
+    uint32_t* so = mt_out + (long long)p * (acr::kMtN + 1);
+    for (int i = tid; i < acr::kMtN; i += kThreads) so[i] = g.x[i];
+    if (tid == 0) so[acr::kMtN] = (uint32_t)g.p;
   }
 }
 

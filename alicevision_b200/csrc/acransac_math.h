@@ -1,17 +1,20 @@
-// Host + device building blocks of the a-contrario fundamental-matrix estimation (acransac.cuh):
+// Host + device building blocks of the a-contrario fundamental-matrix and homography estimations (acransac.cuh):
 //   * std::mt19937 (libstdc++), std::uniform_int_distribution<int>(0, d) on it (GCC 13: Lemire's nearly-divisionless reduction
-//     of one 32-bit draw), and the sample of robustEstimation::randSample as ACRANSAC draws it: Floyd's algorithm with the
-//     iteration order of the std::unordered_set<std::size_t> it fills (range >= 11), or std::shuffle with its two-swaps-per-draw
-//     path (range 8..10);
+//     of one 32-bit draw), and the sample of robustEstimation::randSample(g, 0, range, K) as ACRANSAC draws it: Floyd's algorithm
+//     with the iteration order of the std::unordered_set<std::size_t> it fills, or std::shuffle with its two-swaps-per-draw path
+//     when K * 1.5 > range (range 8..10 for K = 7, range 5 for K = 4);
 //   * the F kernel of RelativePoseKernel<Fundamental7PSolver, FundamentalEpipolarDistanceError, UnnormalizerT>: image-size
 //     preconditioning, the 7-point solver (the 2-D null space of the epipolar rows, the cubic det(F1 + a F2) = 0 as written,
-//     SolveCubicPolynomial branch for branch), the point-to-line error and the unnormalisation N2^T F N1.
-// The same code runs in the engine (device) and in the oracle's restated kernel (host, -ffp-contract=off), so the two differ
+//     SolveCubicPolynomial branch for branch), the point-to-line error and the unnormalisation N2^T F N1;
+//   * the H kernel of RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError, UnnormalizerI> (point-to-point): the same
+//     preconditioning, the 4-point DLT and its 1-D null space, the asymmetric transfer error and the unnormalisation N2^-1 H N1.
+// The same code runs in the engine (device) and in the oracle's restated kernels (host, -ffp-contract=off), so the two differ
 // only through acos / cos / pow / log10.  Device double arithmetic goes through __dmul_rn / __dadd_rn / __dsub_rn so that no
 // product is contracted into an FMA.
-// The null space is the one piece that cannot match the reference bit for bit (it comes from Eigen's JacobiSVD there): here it
-// is the last two columns of the Householder QR of A^T.  Any basis of the same 2-D null space gives the same rank-2 matrices up to
-// scale and the error is scale-invariant, so models agree up to rounding.
+// The null spaces are the one piece that cannot match the reference bit for bit (they come from Eigen's JacobiSVD there): here
+// they are the last columns of the Householder QR of A^T.  Any basis of the same null space gives the same models up to scale
+// (F: the same rank-2 matrices; H: the same matrix up to scale and sign) and the errors are scale-invariant, so models agree up to
+// rounding.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -101,11 +104,13 @@ ACR_HD uint32_t uniform_below(Mt19937& g, uint32_t range) {
   return (uint32_t)(prod >> 32);
 }
 
-// The 7 positions in [0, range) that randSample(g, 0, range, 7) returns, in its order; range >= 8.
-ACR_HD void rand_sample7(Mt19937& g, uint32_t range, uint32_t out[kSample]) {
-  if (kSample * 1.5 > range) {
-    // std::shuffle of iota(range): a leading single swap when range is even, then two swap positions per draw
-    uint32_t a[10];
+// The K positions in [0, range) that randSample(g, 0, range, K) returns, in its order; range > K.
+template <int K>
+ACR_HD void rand_sample(Mt19937& g, uint32_t range, uint32_t out[K]) {
+  if (K * 1.5 > range) {
+    // std::shuffle of iota(range) (range 8..10 for K = 7, 5 for K = 4): a leading single swap when range is even, then two swap
+    // positions per draw
+    uint32_t a[K * 3 / 2];
     for (uint32_t i = 0; i < range; ++i) a[i] = i;
     uint32_t i = 1;
     if (range % 2 == 0) {
@@ -118,15 +123,15 @@ ACR_HD void rand_sample7(Mt19937& g, uint32_t range, uint32_t out[kSample]) {
       uint32_t j = x / (sr + 1), t = a[i]; a[i] = a[j]; a[j] = t; ++i;
       j = x % (sr + 1); t = a[i]; a[i] = a[j]; a[j] = t; ++i;
     }
-    for (int k = 0; k < kSample; ++k) out[k] = a[k];
+    for (int k = 0; k < K; ++k) out[k] = a[k];
     return;
   }
   // Floyd's algorithm into a std::unordered_set<std::size_t>: identity hash, 13 buckets from the first insertion on (libstdc++'s
   // prime rehash policy; no rehash below 14 elements).  Its iteration order is the node list: a key goes in front of the first
   // node of its bucket, or at the front of the list when its bucket is empty.
-  uint32_t list[kSample];
+  uint32_t list[K];
   int cnt = 0;
-  for (uint32_t d = range - kSample; d < range; ++d) {
+  for (uint32_t d = range - K; d < range; ++d) {
     const uint32_t t = uniform_below(g, d + 1);
     bool seen = false;
     for (int q = 0; q < cnt; ++q) seen |= (list[q] == t);
@@ -138,8 +143,11 @@ ACR_HD void rand_sample7(Mt19937& g, uint32_t range, uint32_t out[kSample]) {
     list[pos] = key;
     ++cnt;
   }
-  for (int k = 0; k < kSample; ++k) out[k] = list[k];
+  for (int k = 0; k < K; ++k) out[k] = list[k];
 }
+
+// randSample(g, 0, range, 7), the Fundamental7PSolver sample; range >= 8
+ACR_HD void rand_sample7(Mt19937& g, uint32_t range, uint32_t out[kSample]) { rand_sample<kSample>(g, range, out); }
 
 // ---------------------------------------------------------------------------------------------------------------- F kernel
 // preconditionerFromImageSize: N = [s 0 -w/2 s; 0 s -h/2 s; 0 0 1], s = 1 / sqrt(w h) (w h an int product; -.5f * w in float)
@@ -208,15 +216,17 @@ ACR_HD int solve_cubic(const double P[4], double x[3]) {
   return 1;
 }
 
-// Two vectors spanning the null space of the 7 x 9 epipolar system: the last two columns of Q in A^T = Q R (Householder, no
-// pivoting; a column that is already zero below the diagonal gets no reflection).  f1 = Q e8, f2 = Q e7, unit norm.
-ACR_HD void nullspace2(const double A[kSample][9], double f1[9], double f2[9]) {
-  double M[9][kSample];   // A^T
+// The null space of an R x 9 system (R = 7: the epipolar rows, R = 8: the homography DLT rows): the last 9 - R columns of Q in
+// A^T = Q R (Householder, no pivoting; a column that is already zero below the diagonal gets no reflection).  N[0] = Q e8,
+// N[1] = Q e7, unit norm.  A rank-deficient system has a larger null space; the columns returned then lie in it as rounding sets.
+template <int R>
+ACR_HD void nullspace(const double A[R][9], double N[9 - R][9]) {
+  double M[9][R];   // A^T
   for (int r = 0; r < 9; ++r)
-    for (int c = 0; c < kSample; ++c) M[r][c] = A[c][r];
-  double V[kSample][9];   // Householder vectors (zero above their diagonal)
-  double vn[kSample];     // their squared norms (0: no reflection)
-  for (int j = 0; j < kSample; ++j) {
+    for (int c = 0; c < R; ++c) M[r][c] = A[c][r];
+  double V[R][9];   // Householder vectors (zero above their diagonal)
+  double vn[R];     // their squared norms (0: no reflection)
+  for (int j = 0; j < R; ++j) {
     double s = 0;
     for (int r = j; r < 9; ++r) s = add(s, mul(M[r][j], M[r][j]));
     const double nrm = sqrt(s);
@@ -227,20 +237,23 @@ ACR_HD void nullspace2(const double A[kSample][9], double f1[9], double f2[9]) {
     for (int r = j; r < 9; ++r) v2 = add(v2, mul(V[j][r], V[j][r]));
     vn[j] = v2;
     if (v2 == 0) continue;
-    for (int c = j; c < kSample; ++c) {
+    for (int c = j; c < R; ++c) {
       double d = 0;
       for (int r = j; r < 9; ++r) d = add(d, mul(V[j][r], M[r][c]));
       const double f = mul(2.0, d) / v2;
       for (int r = j; r < 9; ++r) M[r][c] = sub(M[r][c], mul(f, V[j][r]));
     }
   }
-  for (int r = 0; r < 9; ++r) { f1[r] = r == 8 ? 1.0 : 0.0; f2[r] = r == 7 ? 1.0 : 0.0; }
-  for (int j = kSample - 1; j >= 0; --j) {
+  for (int q = 0; q < 9 - R; ++q)
+    for (int r = 0; r < 9; ++r) N[q][r] = r == 8 - q ? 1.0 : 0.0;
+  for (int j = R - 1; j >= 0; --j) {
     if (vn[j] == 0) continue;
-    double d1 = 0, d2 = 0;
-    for (int r = j; r < 9; ++r) { d1 = add(d1, mul(V[j][r], f1[r])); d2 = add(d2, mul(V[j][r], f2[r])); }
-    const double g1 = mul(2.0, d1) / vn[j], g2 = mul(2.0, d2) / vn[j];
-    for (int r = j; r < 9; ++r) { f1[r] = sub(f1[r], mul(g1, V[j][r])); f2[r] = sub(f2[r], mul(g2, V[j][r])); }
+    for (int q = 0; q < 9 - R; ++q) {
+      double d = 0;
+      for (int r = j; r < 9; ++r) d = add(d, mul(V[j][r], N[q][r]));
+      const double g = mul(2.0, d) / vn[j];
+      for (int r = j; r < 9; ++r) N[q][r] = sub(N[q][r], mul(g, V[j][r]));
+    }
   }
 }
 
@@ -253,8 +266,10 @@ ACR_HD int fit7(const double* x1, const double* y1, const double* x2, const doub
     A[i][3] = mul(y2[i], x1[i]); A[i][4] = mul(y2[i], y1[i]); A[i][5] = y2[i];
     A[i][6] = x1[i]; A[i][7] = y1[i]; A[i][8] = 1.0;
   }
-  double f1[9], f2[9];
-  nullspace2(A, f1, f2);
+  double f12[2][9];
+  nullspace<kSample>(A, f12);
+  const double* f1 = f12[0];
+  const double* f2 = f12[1];
   const double a = f1[0], j = f2[0], b = f1[1], k = f2[1], c = f1[2], l = f2[2], d = f1[3], m = f2[3], e = f1[4], n = f2[4],
                f = f1[5], o = f2[5], g = f1[6], p = f2[6], h = f1[7], q = f2[7], i = f1[8], r = f2[8];
 #define ACR_T(u, v, w) mul(mul(u, v), w)
@@ -302,5 +317,68 @@ ACR_HD void unnormalize(const Norm& n1, const Norm& n2, double F[9]) {
     for (int c = 0; c < 3; ++c) O[r * 3 + c] = add(add(mul(N2t[r * 3], T[c]), mul(N2t[r * 3 + 1], T[3 + c])), mul(N2t[r * 3 + 2], T[6 + c]));
   for (int t = 0; t < 9; ++t) F[t] = O[t];
 }
+
+// ---------------------------------------------------------------------------------------------------------------- H kernel
+// RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError, UnnormalizerI> (point-to-point): the same preconditioning, the
+// 4-point DLT, the asymmetric transfer error and the unnormalisation N2^-1 H N1.
+constexpr int kSampleH = 4;      // Homography4PSolver::getMinimumNbRequiredSamples
+constexpr int kMaxModelsH = 1;   // Homography4PSolver::getMaximumNbModels
+
+// Homography4PSolver::solve on 4 normalised correspondences: the 8 DLT rows of buildActionMatrix (the non-zero rows of the
+// reference's Mat16_9), their null space, mapped row-major to H[9] (x2 ~ H x1).  Always one model: a degenerate sample
+// (duplicated or collinear points) has a null space of dimension 2 or more, and the vector taken from it is set by rounding.
+ACR_HD int fit4(const double* x1, const double* y1, const double* x2, const double* y2, double* H) {
+  double L[2 * kSampleH][9];
+  for (int i = 0; i < kSampleH; ++i) {
+    double* a = L[2 * i];
+    double* b = L[2 * i + 1];
+    a[0] = x1[i]; a[1] = y1[i]; a[2] = 1.0; a[3] = 0.0; a[4] = 0.0; a[5] = 0.0;
+    a[6] = mul(-x2[i], x1[i]); a[7] = mul(-x2[i], y1[i]); a[8] = -x2[i];
+    b[0] = 0.0; b[1] = 0.0; b[2] = 0.0; b[3] = x1[i]; b[4] = y1[i]; b[5] = 1.0;
+    b[6] = mul(-y2[i], x1[i]); b[7] = mul(-y2[i], y1[i]); b[8] = -y2[i];
+  }
+  double h[1][9];
+  nullspace<2 * kSampleH>(L, h);
+  for (int t = 0; t < 9; ++t) H[t] = h[0][t];
+  return 1;
+}
+
+// HomographyAsymmetricError on normalised points: |x2 - dehomogenised(H (x1, 1))|^2.  A zero third component gives inf or NaN.
+ACR_HD double homography_error(const double* H, double x1, double y1, double x2, double y2) {
+  const double u = add(add(mul(H[0], x1), mul(H[1], y1)), H[2]);
+  const double v = add(add(mul(H[3], x1), mul(H[4], y1)), H[5]);
+  const double w = add(add(mul(H[6], x1), mul(H[7], y1)), H[8]);
+  const double dx = sub(x2, u / w), dy = sub(y2, v / w);
+  return add(mul(dx, dx), mul(dy, dy));
+}
+
+// M^-1 of a 3 x 3 row-major matrix by cofactors: R(i, j) = C(j, i) / det, det expanded along the first column
+ACR_HD void inverse3(const double M[9], double R[9]) {
+  double C[9];   // cofactors C(i, j) = M(i1, j1) M(i2, j2) - M(i1, j2) M(i2, j1), i1 = i + 1, i2 = i + 2 (mod 3)
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      const int i1 = (i + 1) % 3, i2 = (i + 2) % 3, j1 = (j + 1) % 3, j2 = (j + 2) % 3;
+      C[i * 3 + j] = sub(mul(M[i1 * 3 + j1], M[i2 * 3 + j2]), mul(M[i1 * 3 + j2], M[i2 * 3 + j1]));
+    }
+  const double det = add(add(mul(C[0], M[0]), mul(C[3], M[3])), mul(C[6], M[6]));
+  const double inv = 1.0 / det;
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) R[i * 3 + j] = mul(C[j * 3 + i], inv);
+}
+
+// UnnormalizerI: H <- N2^-1 H N1
+ACR_HD void unnormalize_h(const Norm& n1, const Norm& n2, double H[9]) {
+  const double N1[9] = {n1.s, 0, n1.tx, 0, n1.s, n1.ty, 0, 0, 1};
+  const double N2[9] = {n2.s, 0, n2.tx, 0, n2.s, n2.ty, 0, 0, 1};
+  double N2i[9], T[9];
+  inverse3(N2, N2i);
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) T[r * 3 + c] = add(add(mul(N2i[r * 3], H[c]), mul(N2i[r * 3 + 1], H[3 + c])), mul(N2i[r * 3 + 2], H[6 + c]));
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) H[r * 3 + c] = add(add(mul(T[r * 3], N1[c]), mul(T[r * 3 + 1], N1[3 + c])), mul(T[r * 3 + 2], N1[6 + c]));
+}
+
+// logalpha0 of the point-to-point error: log10(pi / (w2 h2) / s2^2), the unit circle over the image area in normalised units
+ACR_HD double logalpha0_h(int w2, int h2, const Norm& n2) { return log10(M_PI / mul((double)w2, (double)h2) / mul(n2.s, n2.s)); }
 
 }  // namespace acr

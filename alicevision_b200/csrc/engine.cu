@@ -243,7 +243,8 @@ struct GuidedFastScratch {
   cudaEvent_t ev_c0 = nullptr, ev_c1 = nullptr;           // candidate-kernel timing
 };
 
-// grow-only scratch of b200m_acransac_fundamental_pairs (acransac.cuh)
+// grow-only scratch of b200m_acransac_fundamental_pairs and b200m_acransac_homography_pairs (acransac.cuh); the last call's
+// instrumentation and trace, whichever model it estimated
 struct AcransacScratch {
   void* d = nullptr; size_t bytes = 0;
   bool skip = true;                                   // certified skip (b200m_ctx_set_acransac_skip)
@@ -1773,13 +1774,17 @@ int b200m_guided_match_fast_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pai
   return B200M_OK;
 }
 
-// ---- K10: a-contrario RANSAC fundamental matrix for a pair list (acransac.cuh) ------------------------------------------
-int b200m_acransac_fundamental_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh,
-                                     const uint32_t* mt_state, int64_t max_iteration, double precision, uint8_t* valid,
-                                     int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max, double* min_nfa,
-                                     int32_t* iterations) {
-  if (!c || n_pairs < 0 || max_iteration < 0 || max_iteration > INT32_MAX || !(precision > 0) ||
-      (n_pairs > 0 && (!offsets || !wh || !mt_state || !valid || !n_inliers || !F || !error_max || !min_nfa || !iterations)))
+}  // extern "C"
+
+// ---- K10: a-contrario RANSAC for a pair list, fundamental matrix or homography (acransac.cuh) ----------------------------
+// One launch of acransac_kernel<Policy> over the list; the two entry points differ in the model and in the generator contract.
+// mt_per_pair: 0 = mt_state is one 625-word state for every pair, 1 = n_pairs x 625.  mt_out: NULL or n_pairs x 625.
+template <class Policy>
+static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh, const uint32_t* mt_state,
+                          int mt_per_pair, int64_t max_iteration, double precision, uint8_t* valid, int32_t* n_inliers, uint32_t* inliers,
+                          double* model, double* error_max, double* min_nfa, int32_t* iterations, uint32_t* mt_out) {
+  if (!c || n_pairs < 0 || max_iteration < 0 || max_iteration > INT32_MAX || !(precision > 0) || (mt_per_pair != 0 && mt_per_pair != 1) ||
+      (n_pairs > 0 && (!offsets || !wh || !mt_state || !valid || !n_inliers || !model || !error_max || !min_nfa || !iterations)))
     return fail(B200M_ERR_ARG, "bad arguments");
   if (n_pairs > 0 && offsets[0] != 0) return fail(B200M_ERR_ARG, "offsets[0] must be 0");
   std::vector<acrk::Pair> pairs((size_t)n_pairs);
@@ -1809,15 +1814,17 @@ int b200m_acransac_fundamental_pairs(b200m_ctx* c, int n_pairs, const int64_t* o
   // float log10 table of makelogcombi: log10 on the double k, rounded to float (pinned against the compiled reference's tables)
   std::vector<float> l10((size_t)max_n + 2);
   for (size_t k = 0; k < l10.size(); ++k) l10[k] = (float)log10((double)k);
-  // one grow-only device buffer
+  const size_t n_states = mt_per_pair ? (size_t)n_pairs : 1;
+  // one grow-only device buffer, shared by both models
   size_t at = 0;
   auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
   const size_t o_pairs = take(sizeof(acrk::Pair) * n_pairs), o_corr = take(sizeof(double) * 4 * N), o_l10 = take(sizeof(float) * l10.size()),
-               o_mt = take(sizeof(uint32_t) * 625), o_pts = take(sizeof(double) * 4 * N), o_idx = take(sizeof(uint32_t) * N),
+               o_mt = take(sizeof(uint32_t) * 625 * n_states), o_pts = take(sizeof(double) * 4 * N), o_idx = take(sizeof(uint32_t) * N),
                o_logc = take(sizeof(float) * 2 * (N + n_pairs)), o_gk = take(sizeof(unsigned long long) * sort_total),
                o_gv = take(sizeof(uint32_t) * sort_total), o_inl = take(sizeof(uint32_t) * N),
                o_tr = take(sizeof(int32_t) * acrk::kTraceCap * n_pairs),
-               o_trn = take(sizeof(double) * acrk::kTraceCap * n_pairs), o_out = take(sizeof(acrk::Out) * n_pairs);
+               o_trn = take(sizeof(double) * acrk::kTraceCap * n_pairs), o_out = take(sizeof(acrk::Out) * n_pairs),
+               o_mto = take(mt_out ? sizeof(uint32_t) * 625 * n_pairs : 0);
   if (at > c->acr.bytes) {
     if (c->acr.d) CK(cudaFree(c->acr.d));
     c->acr.d = nullptr; c->acr.bytes = 0;
@@ -1830,17 +1837,19 @@ int b200m_acransac_fundamental_pairs(b200m_ctx* c, int n_pairs, const int64_t* o
   CK(cudaMemcpyAsync(d + o_pairs, pairs.data(), sizeof(acrk::Pair) * n_pairs, cudaMemcpyHostToDevice, st));
   if (N) CK(cudaMemcpyAsync(d + o_corr, corr, sizeof(double) * 4 * N, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d + o_l10, l10.data(), sizeof(float) * l10.size(), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d + o_mt, mt_state, sizeof(uint32_t) * 625, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d + o_mt, mt_state, sizeof(uint32_t) * 625 * n_states, cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(c->acr.ev0, st));
-  acrk::acransac_kernel<<<n_pairs, acrk::kThreads, 0, st>>>(
+  acrk::acransac_kernel<Policy><<<n_pairs, acrk::kThreads, 0, st>>>(
       (const acrk::Pair*)(d + o_pairs), (const double*)(d + o_corr), (const float*)(d + o_l10), (const uint32_t*)(d + o_mt),
-      (long long)max_iteration, precision, c->acr.skip ? 1 : 0, (double*)(d + o_pts), (uint32_t*)(d + o_idx), (float*)(d + o_logc),
-      (unsigned long long*)(d + o_gk), (uint32_t*)(d + o_gv), (uint32_t*)(d + o_inl), (int*)(d + o_tr), (double*)(d + o_trn), (acrk::Out*)(d + o_out));
+      mt_per_pair ? 625 : 0, (long long)max_iteration, precision, c->acr.skip ? 1 : 0, (double*)(d + o_pts), (uint32_t*)(d + o_idx),
+      (float*)(d + o_logc), (unsigned long long*)(d + o_gk), (uint32_t*)(d + o_gv), (uint32_t*)(d + o_inl), (int*)(d + o_tr),
+      (double*)(d + o_trn), (acrk::Out*)(d + o_out), mt_out ? (uint32_t*)(d + o_mto) : nullptr);
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->acr.ev1, st));
   std::vector<acrk::Out> outs((size_t)n_pairs);
   CK(cudaMemcpyAsync(outs.data(), d + o_out, sizeof(acrk::Out) * n_pairs, cudaMemcpyDeviceToHost, st));
   if (N) CK(cudaMemcpyAsync(inliers, d + o_inl, sizeof(uint32_t) * N, cudaMemcpyDeviceToHost, st));
+  if (mt_out) CK(cudaMemcpyAsync(mt_out, d + o_mto, sizeof(uint32_t) * 625 * n_pairs, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(c->acr.trace.data(), d + o_tr, sizeof(int32_t) * acrk::kTraceCap * n_pairs, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(c->acr.trace_nfa.data(), d + o_trn, sizeof(double) * acrk::kTraceCap * n_pairs, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -1851,12 +1860,30 @@ int b200m_acransac_fundamental_pairs(b200m_ctx* c, int n_pairs, const int64_t* o
   for (int k = 0; k < n_pairs; ++k) {
     const acrk::Out& o = outs[k];
     valid[k] = (uint8_t)o.valid; n_inliers[k] = o.n_inl;
-    for (int t = 0; t < 9; ++t) F[9 * k + t] = o.F[t];
+    for (int t = 0; t < 9; ++t) model[9 * k + t] = o.model[t];
     error_max[k] = o.error_max; min_nfa[k] = o.min_nfa; iterations[k] = o.iterations;
     c->acr.n_trace[k] = o.n_trace;
     c->acr.stats[0] += o.evaluated; c->acr.stats[1] += o.skipped; c->acr.stats[2] += o.exact;
   }
   return B200M_OK;
+}
+
+extern "C" {
+
+int b200m_acransac_fundamental_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh,
+                                     const uint32_t* mt_state, int64_t max_iteration, double precision, uint8_t* valid,
+                                     int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max, double* min_nfa,
+                                     int32_t* iterations) {
+  return acransac_pairs<acrk::FPolicy>(c, n_pairs, offsets, corr, wh, mt_state, 0, max_iteration, precision, valid, n_inliers, inliers, F,
+                                       error_max, min_nfa, iterations, nullptr);
+}
+
+int b200m_acransac_homography_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh,
+                                    const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision, uint8_t* valid,
+                                    int32_t* n_inliers, uint32_t* inliers, double* H, double* error_max, double* min_nfa, int32_t* iterations,
+                                    uint32_t* mt_state_out) {
+  return acransac_pairs<acrk::HPolicy>(c, n_pairs, offsets, corr, wh, mt_state, mt_state_per_pair, max_iteration, precision, valid, n_inliers,
+                                       inliers, H, error_max, min_nfa, iterations, mt_state_out);
 }
 
 double b200m_acransac_last_stats(const b200m_ctx* c, int64_t stats[4]) {
@@ -1892,16 +1919,23 @@ void b200m_mt19937_seed(uint32_t seed, uint32_t state[625]) {
   state[624] = (uint32_t)g.p;
 }
 
-int b200m_debug_rand_sample(const uint32_t state[625], int range, int draws, uint32_t* out, uint32_t* states) {
-  if (!state || range < 8 || draws < 0 || (draws > 0 && !out) || state[624] > (uint32_t)acr::kMtN) return fail(B200M_ERR_ARG, "bad arguments");
+int b200m_debug_rand_sample_k(const uint32_t state[625], int sample_size, int range, int draws, uint32_t* out, uint32_t* states) {
+  if (!state || (sample_size != 4 && sample_size != 7) || range <= sample_size || draws < 0 || (draws > 0 && !out) ||
+      state[624] > (uint32_t)acr::kMtN)
+    return fail(B200M_ERR_ARG, "bad arguments");
   acr::Mt19937 g;
   std::memcpy(g.x, state, sizeof g.x);
   g.p = (int)state[624];
   for (int d = 0; d < draws; ++d) {
-    acr::rand_sample7(g, (uint32_t)range, out + 7 * (size_t)d);
+    if (sample_size == 7) acr::rand_sample<7>(g, (uint32_t)range, out + 7 * (size_t)d);
+    else acr::rand_sample<4>(g, (uint32_t)range, out + 4 * (size_t)d);
     if (states) { std::memcpy(states + 625 * (size_t)d, g.x, sizeof g.x); states[625 * (size_t)d + 624] = (uint32_t)g.p; }
   }
   return B200M_OK;
+}
+
+int b200m_debug_rand_sample(const uint32_t state[625], int range, int draws, uint32_t* out, uint32_t* states) {
+  return b200m_debug_rand_sample_k(state, 7, range, draws, out, states);
 }
 
 // ---- Surface 2 on several GPUs from ONE process ----------------------------------------------------------------------

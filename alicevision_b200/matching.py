@@ -38,7 +38,7 @@ ABI_SYMBOLS = [
     "b200m_shard_pairs", "b200m_shard_pairs_2d", "b200m_multi_create", "b200m_multi_destroy", "b200m_multi_num_devices", "b200m_multi_ctx", "b200m_multi_match",
     "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model", "b200m_set_view_geometry", "b200m_guided_match_fast_pairs",
     "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
-    "b200m_mt19937_seed", "b200m_debug_rand_sample",
+    "b200m_mt19937_seed", "b200m_debug_rand_sample", "b200m_acransac_homography_pairs", "b200m_debug_rand_sample_k",
 ]
 
 
@@ -196,30 +196,55 @@ class Context:
         mt_state: 625 words (mt19937_state), the same for every pair.  Returns per pair, in input order, {"valid", "inliers" (the
         reference's order), "F" (3 x 3, x_J^T F x_I = 0), "error_max", "min_nfa", "iterations", "trace" / "trace_nfa" (iterations at
         which a better model was found and its minNFA, the first 256), "n_trace"}."""
+        return self._acransac_pairs(False, corr_list, wh, np.ascontiguousarray(mt_state, np.uint32).reshape(625), maxIteration, precision)
+
+    def acransac_homography_pairs(self, corr_list, wh, mt_state_or_states, maxIteration: int = 50000, precision: float = np.inf) -> list[dict]:
+        """b200m_acransac_homography_pairs: GeometricFilterMatrix_H_AC::geometricEstimation (ACRANSAC with Homography4PSolver and the
+        point-to-point error) for every pair.  corr_list and wh as in acransac_fundamental_pairs; mt_state_or_states: one 625-word
+        state for every pair, or an n_pairs x 625 array of per-pair start states.  Returns per pair the fields of
+        acransac_fundamental_pairs with "H" (3 x 3, x_J ~ H x_I) in place of "F", and "mt_state_out": the generator state after the
+        pair's estimation (the reference passes its generator on from pair to pair)."""
+        st = np.ascontiguousarray(mt_state_or_states, np.uint32)
+        if st.ndim == 1:
+            st = st.reshape(625)
+        elif st.shape != (len(corr_list), 625):
+            raise ValueError(f"mt_state_or_states: 625 words or n_pairs x 625, got {st.shape}")
+        return self._acransac_pairs(True, corr_list, wh, st, maxIteration, precision)
+
+    def _acransac_pairs(self, homography: bool, corr_list, wh, st, maxIteration, precision) -> list[dict]:
         cs = [np.ascontiguousarray(c, np.float64).reshape(-1, 4) for c in corr_list]
         n = len(cs)
         offsets = np.zeros(n + 1, np.int64)
         offsets[1:] = np.cumsum([c.shape[0] for c in cs]) if n else []
         corr = np.ascontiguousarray(np.concatenate(cs) if n and offsets[-1] else np.zeros((1, 4)), np.float64)
         whm = np.ascontiguousarray(wh, np.int32).reshape(n, 4)
-        st = np.ascontiguousarray(mt_state, np.uint32).reshape(625)
         valid = np.zeros(max(n, 1), np.uint8); ninl = np.zeros(max(n, 1), np.int32); it = np.zeros(max(n, 1), np.int32)
-        inl = np.zeros(max(int(offsets[-1]), 1), np.uint32); F = np.zeros((max(n, 1), 9)); em = np.zeros(max(n, 1)); nfa = np.zeros(max(n, 1))
+        inl = np.zeros(max(int(offsets[-1]), 1), np.uint32); M = np.zeros((max(n, 1), 9)); em = np.zeros(max(n, 1)); nfa = np.zeros(max(n, 1))
         ptr = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-        _check(self.lib.b200m_acransac_fundamental_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st), C.c_int64(maxIteration),
-                                                         C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(F), ptr(em), ptr(nfa), ptr(it)),
-               "b200m_acransac_fundamental_pairs")
+        if homography:
+            sto = np.zeros((max(n, 1), 625), np.uint32)
+            _check(self.lib.b200m_acransac_homography_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st), C.c_int(int(st.ndim == 2)),
+                                                            C.c_int64(maxIteration), C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(M),
+                                                            ptr(em), ptr(nfa), ptr(it), ptr(sto)),
+                   "b200m_acransac_homography_pairs")
+        else:
+            _check(self.lib.b200m_acransac_fundamental_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st), C.c_int64(maxIteration),
+                                                             C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(M), ptr(em), ptr(nfa), ptr(it)),
+                   "b200m_acransac_fundamental_pairs")
         out = []
         tr = np.zeros(256, np.int32); trn = np.zeros(256, np.float64)
         for k in range(n):
             nt = self.lib.b200m_acransac_last_trace(self._h, C.c_int(k), ptr(tr), ptr(trn), C.c_int(tr.size))
-            out.append({"valid": bool(valid[k]), "inliers": inl[offsets[k]:offsets[k] + ninl[k]].copy(), "F": F[k].reshape(3, 3).copy(),
-                        "error_max": float(em[k]), "min_nfa": float(nfa[k]), "iterations": int(it[k]), "n_trace": int(nt),
-                        "trace": tr[:min(nt, tr.size)].copy(), "trace_nfa": trn[:min(nt, trn.size)].copy()})
+            r = {"valid": bool(valid[k]), "inliers": inl[offsets[k]:offsets[k] + ninl[k]].copy(), "H" if homography else "F": M[k].reshape(3, 3).copy(),
+                 "error_max": float(em[k]), "min_nfa": float(nfa[k]), "iterations": int(it[k]), "n_trace": int(nt),
+                 "trace": tr[:min(nt, tr.size)].copy(), "trace_nfa": trn[:min(nt, trn.size)].copy()}
+            if homography:
+                r["mt_state_out"] = sto[k].copy()
+            out.append(r)
         return out
 
     def acransac_last_stats(self) -> dict:
-        """Instrumentation of the last acransac_fundamental_pairs call."""
+        """Instrumentation of the last acransac_fundamental_pairs or acransac_homography_pairs call."""
         st = np.zeros(4, np.int64)
         ms = self.lib.b200m_acransac_last_stats(self._h, st.ctypes.data_as(C.c_void_p))
         return {"gpu_ms": ms, "models_evaluated": int(st[0]), "models_skipped": int(st[1]), "models_exact": int(st[2]), "launches": int(st[3])}
@@ -232,13 +257,14 @@ def mt19937_state(seed: int) -> np.ndarray:
     return st
 
 
-def debug_rand_sample(state, rng: int, draws: int):
-    """The engine's sampler on the CPU (b200m_debug_rand_sample): `draws` consecutive randSample(g, 0, rng, 7) from `state`.
-    Returns (draws x 7 samples in their order, draws x 625 generator states after each draw)."""
+def debug_rand_sample(state, rng: int, draws: int, sample_size: int = 7):
+    """The engine's sampler on the CPU (b200m_debug_rand_sample_k): `draws` consecutive randSample(g, 0, rng, sample_size) from
+    `state`, sample_size 7 (fundamental matrix) or 4 (homography).  Returns (draws x sample_size samples in their order, draws x 625
+    generator states after each draw)."""
     st = np.ascontiguousarray(state, np.uint32).reshape(625)
-    out = np.zeros((draws, 7), np.uint32); sts = np.zeros((draws, 625), np.uint32)
-    _check(load_library().b200m_debug_rand_sample(st.ctypes.data_as(C.c_void_p), C.c_int(rng), C.c_int(draws), out.ctypes.data_as(C.c_void_p),
-                                                  sts.ctypes.data_as(C.c_void_p)), "b200m_debug_rand_sample")
+    out = np.zeros((draws, sample_size), np.uint32); sts = np.zeros((draws, 625), np.uint32)
+    _check(load_library().b200m_debug_rand_sample_k(st.ctypes.data_as(C.c_void_p), C.c_int(sample_size), C.c_int(rng), C.c_int(draws),
+                                                    out.ctypes.data_as(C.c_void_p), sts.ctypes.data_as(C.c_void_p)), "b200m_debug_rand_sample_k")
     return out, sts
 
 
@@ -251,6 +277,17 @@ def geometricEstimation_F_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: 
     st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else seed_or_state
     corr = np.concatenate([np.asarray(xI, np.float64).reshape(-1, 2), np.asarray(xJ, np.float64).reshape(-1, 2)], axis=1)
     return ctx.acransac_fundamental_pairs([corr], [tuple(sizeI) + tuple(sizeJ)], st, maxIteration, precision)[0]
+
+
+def geometricEstimation_H_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: int = 50000, precision: float = np.inf,
+                             ctx: Context | None = None) -> dict:
+    """GeometricFilterMatrix_H_AC::geometricEstimation of one pair on the GPU (arguments as geometricEstimation_F_AC).  Returns the
+    dict of Context.acransac_homography_pairs: "H" and "mt_state_out", the generator advanced past this pair's draws, which the
+    reference's single-threaded filter hands to the next pair."""
+    ctx = ctx or default_context()
+    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else seed_or_state
+    corr = np.concatenate([np.asarray(xI, np.float64).reshape(-1, 2), np.asarray(xJ, np.float64).reshape(-1, 2)], axis=1)
+    return ctx.acransac_homography_pairs([corr], [tuple(sizeI) + tuple(sizeJ)], st, maxIteration, precision)[0]
 
 
 _default_ctx: dict[int, Context] = {}

@@ -206,20 +206,38 @@ int b200m_acransac_fundamental_pairs(b200m_ctx* ctx, int n_pairs, const int64_t*
                                      const uint32_t* mt_state, int64_t max_iteration, double precision, uint8_t* valid,
                                      int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max, double* min_nfa,
                                      int32_t* iterations);
-/* instrumentation of the last b200m_acransac_fundamental_pairs: stats = {models evaluated in the a-contrario mode, of them skipped
- * by the histogram bound, scored exactly, kernel launches}; returns its GPU time in ms */
+/* ---- geometric filtering: a-contrario RANSAC homography (K10, homography_matrix filter) ---------------------------- */
+/* GeometricFilterMatrix_H_AC::geometricEstimation (ACRANSAC over RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError,
+ * UnnormalizerI>, point-to-point error) for every pair of a list, results in input order.  Arguments and outputs as in
+ * b200m_acransac_fundamental_pairs, with H[9 * n_pairs] (row-major, x_J ~ H x_I; unnormalised when valid) in place of F.  A pair
+ * with at most 4 correspondences returns (0, 0) and no iteration.
+ * Generator: the reference passes its std::mt19937 by reference, so a single-threaded filter starts pair k where pair k - 1 left
+ * off.  A batch cannot reproduce that chain (each pair's draw count depends on its data), so:
+ *   mt_state_per_pair  0: mt_state is 625 words, the start state of every pair; 1: n_pairs x 625 words, one per pair
+ *   mt_state_out       NULL, or n_pairs x 625 words: each pair's generator state after its estimation (its input state when the
+ *                      pair is too small to draw).  A caller that needs the sequential chain runs the pairs one call each and
+ *                      passes the previous pair's output state on. */
+int b200m_acransac_homography_pairs(b200m_ctx* ctx, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh,
+                                    const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision, uint8_t* valid,
+                                    int32_t* n_inliers, uint32_t* inliers, double* H, double* error_max, double* min_nfa, int32_t* iterations,
+                                    uint32_t* mt_state_out);
+/* instrumentation of the last a-contrario RANSAC call (b200m_acransac_fundamental_pairs or b200m_acransac_homography_pairs):
+ * stats = {models evaluated in the a-contrario mode, of them skipped by the histogram bound, scored exactly, kernel launches};
+ * returns its GPU time in ms */
 double b200m_acransac_last_stats(const b200m_ctx* ctx, int64_t stats[4]);
-/* the `better` events of the last call's pair `pair`: the iterations at which a better model was found and the new minNFA of each
- * (the first `cap`, at most 256; either pointer may be NULL); returns their number.  The getters of the last call take the context's
- * lock, so a concurrent call on the same context cannot rewrite what they read. */
+/* the `better` events of the last a-contrario RANSAC call's pair `pair` (F or H): the iterations at which a better model was found
+ * and the new minNFA of each (the first `cap`, at most 256; either pointer may be NULL); returns their number.  The getters of the
+ * last call take the context's lock, so a concurrent call on the same context cannot rewrite what they read. */
 int b200m_acransac_last_trace(const b200m_ctx* ctx, int pair, int32_t* iters, double* nfa, int cap);
-/* debug: 1 (default) = certified skip of models that cannot beat the running minNFA; 0 = score every model exactly */
+/* debug, both models: 1 (default) = certified skip of models that cannot beat the running minNFA; 0 = score every model exactly */
 int b200m_ctx_set_acransac_skip(b200m_ctx* ctx, int on);
 /* host only: std::mt19937(seed) as 625 words (see mt_state) */
 void b200m_mt19937_seed(uint32_t seed, uint32_t state[625]);
 /* host only (debug): the engine's sampler on the CPU.  `draws` consecutive randSample(g, 0, range, 7) from `state`: the samples in
  * their order (draws x 7), and the state after each draw (draws x 625) when states != NULL.  range >= 8. */
 int b200m_debug_rand_sample(const uint32_t state[625], int range, int draws, uint32_t* out, uint32_t* states);
+/* the same for sample_size 4 (Homography4PSolver; range >= 5) or 7: out is draws x sample_size */
+int b200m_debug_rand_sample_k(const uint32_t state[625], int sample_size, int range, int draws, uint32_t* out, uint32_t* states);
 
 /* ---- instrumentation ------------------------------------------------------------------------------------------ */
 /* GPU time of the last b200m_match_pairs between its first and last enqueue (CUDA events on the context's stream), ms */
