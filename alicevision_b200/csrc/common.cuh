@@ -25,6 +25,8 @@ struct alignas(128) ViewDev {
   CUtensorMap tmap128;  // fp16 [m x 128], box {64 x 128 rows}, SWIZZLE_128B: one K-block of a query or database tile (only when dim == 128 scalar)
   CUtensorMap tmap_aug; // fp16 [m_pad x 16] half-norm limbs, box {16 x 128 rows}, SWIZZLE_32B (9th K-step of the AUG kernel)
   CUtensorMap tmap_augq; // the same for augq16 (the view as QUERY of the real-valued kernel: its own half-norm limbs as A columns)
+  CUtensorMap tmap_u8;  // uchar-stored views only: `raw` as u8 [m x 128], box {128 B x 128 rows}, SWIZZLE_128B (the u8 kernel's operand tile)
+  const int32_t* nb32;  // uchar-stored views only: ||row||^2 as int32, padded to a multiple of 256 rows with 2^24 (prep.cuh), else nullptr
   const void* raw;      // descriptors as STORED, row-major m x dim: f32 / u8 / 64-byte binary; `dtype` is the storage type (integer-valued
                         // fp32 descriptors are staged and stored as u8: same values, a quarter of the bytes)
   const __half* h16;    // fp16 copy (scalar, dim == 128) or nullptr

@@ -180,6 +180,7 @@ struct ViewHost {
   __half* augq16 = nullptr; float* err = nullptr; uint32_t* stats = nullptr;   // real-valued tensor-core path (prep.cuh): query-side limbs, rounding-error bounds
   void* arena = nullptr; void* raw_own = nullptr;     // the one allocation all device buffers of the view live in; a separately owned `raw`
   bool stored_u8 = false;     // dtype == DT_F32 whose values are integers in 0..255: staged and kept on the device as uchar (hostconv.hpp)
+  int32_t* nb32 = nullptr;    // uchar-stored tensor-core views: int32 squared norms of the u8 kernel (prep.cuh)
   float* d_xy = nullptr; uint32_t* d_yrank = nullptr;   // positions + rank of y on the device (device finishing stage, finish.cuh)
   double2* d_geom = nullptr;  // b200m_set_view_geometry: the (undistorted) positions guided matching uses instead of xy; own allocation
   bool failed = false;       // its upload job failed: the device buffers were never filled
@@ -302,6 +303,7 @@ struct b200m_ctx {
   // last-call instrumentation
   double last_gpu_ms = 0, last_search_ms = 0; int last_launches = 0, last_tc_pairs = 0; int64_t last_records = 0;
   int last_real_pairs = 0; int64_t last_fallback_rows = 0;      // real-valued pairs on the tensor-core filter kernel; queries left to the exact_rows fallback
+  int last_u8_pairs = 0;          // the tensor-core pairs (last_tc_pairs) that ran the u8 kernel
   unsigned err_total = 0;
 };
 
@@ -317,9 +319,10 @@ struct b200m_result {
 // ------------------------------------------------------------------------------------------------ helpers
 // Device buffers of one view (stream-ordered allocations out of the default pool).
 // ONE stream-ordered allocation per view, carved into its buffers (a view of 1024 features paid more for its ten allocations and ten
-// frees than for its copy): raw | h16 | nbh | nrm | aug16 | augq16 | err | stats | yrank | xy, each 256-byte aligned; stats and yrank are
+// frees than for its copy): raw | h16 | nbh | nrm | aug16 | augq16 | err | nb32 | stats | yrank | xy, each 256-byte aligned; stats and yrank are
 // adjacent so that one memset zeroes both.
-static int alloc_view_buffers(b200m_ctx* c, ViewHost& v) {
+// u8_norms: the int32 norms of the u8 search kernel for a uchar-stored view (not for b200m_db_create's databases, which only MODE_KNN reads).
+static int alloc_view_buffers(b200m_ctx* c, ViewHost& v, bool u8_norms = true) {
   const size_t esz = v.store_dtype() == DT_F32 ? 4 : 1;
   auto al = [](size_t x) { return (x + 255) / 256 * 256; };
   const bool tcv = v.tc_capable(), pos = !v.xy.empty();
@@ -329,6 +332,8 @@ static int alloc_view_buffers(b200m_ctx* c, ViewHost& v) {
   const size_t o_raw = take(std::max<size_t>((size_t)v.m * v.dim * esz, 256));
   const size_t o_h16 = tcv ? take((size_t)v.m * 128 * 2) : 0, o_nbh = tcv ? take((size_t)v.m_pad * 4) : 0, o_nrm = tcv ? take((size_t)v.m_pad * 4) : 0;
   const size_t o_aug = tcv ? take((size_t)v.m_pad * 32) : 0, o_augq = tcv ? take((size_t)v.m_pad * 32) : 0, o_err = tcv ? take((size_t)v.m_pad * 4) : 0;
+  const bool nb32 = tcv && u8_norms && v.store_dtype() == DT_U8;
+  const size_t o_nb32 = nb32 ? take((size_t)v.m_pad * 4) : 0;
   const size_t o_stats = tcv ? take(16) : 0;
   const size_t o_yrank = pos ? take((size_t)v.m * 4) : 0, o_xy = pos ? take((size_t)v.m * 8) : 0;
   char* base = nullptr;
@@ -338,6 +343,7 @@ static int alloc_view_buffers(b200m_ctx* c, ViewHost& v) {
   if (tcv) {
     v.h16 = (__half*)(base + o_h16); v.nbh = (float*)(base + o_nbh); v.nrm = (float*)(base + o_nrm); v.aug16 = (__half*)(base + o_aug);
     v.augq16 = (__half*)(base + o_augq); v.err = (float*)(base + o_err); v.stats = (uint32_t*)(base + o_stats);
+    v.nb32 = nb32 ? (int32_t*)(base + o_nb32) : nullptr;
   }
   if (pos) { v.d_yrank = (uint32_t*)(base + o_yrank); v.d_xy = (float*)(base + o_xy); }
   return B200M_OK;
@@ -348,7 +354,7 @@ static void free_view_buffers(b200m_ctx* c, ViewHost& v) {
   if (v.d_geom) cudaFreeAsync(v.d_geom, c->stream);        // re-uploading or removing a view drops its geometry positions
   v.arena = nullptr; v.raw_own = nullptr; v.d_geom = nullptr;
   v.raw = nullptr; v.h16 = nullptr; v.nbh = nullptr; v.nrm = nullptr; v.aug16 = nullptr; v.d_xy = nullptr; v.d_yrank = nullptr;
-  v.augq16 = nullptr; v.err = nullptr; v.stats = nullptr;
+  v.augq16 = nullptr; v.err = nullptr; v.stats = nullptr; v.nb32 = nullptr;
 }
 
 static int make_view_dev(b200m_ctx* c, const ViewHost& v, ViewDev& d) {
@@ -377,6 +383,15 @@ static int make_view_dev(b200m_ctx* c, const ViewHost& v, ViewDev& d) {
                     CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) return fail(B200M_ERR_CUDA, "cuTensorMapEncodeTiled(augq) failed: " + std::to_string((int)r));
     }
+    if (v.nb32 && v.store_dtype() == DT_U8) {
+      // the uchar rows themselves as the u8 kernel's operand: 128-byte rows, the same SWIZZLE_128B layout as one fp16 K-block
+      const cuuint64_t ustr[1] = {128};
+      const cuuint32_t ubox[2] = {128, 128};
+      d.nb32 = v.nb32;
+      CUresult r = c->encode(&d.tmap_u8, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void*)v.raw, gdim, ustr, ubox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) return fail(B200M_ERR_CUDA, "cuTensorMapEncodeTiled(u8) failed: " + std::to_string((int)r));
+    }
   }
   return B200M_OK;
 }
@@ -386,8 +401,8 @@ static int run_prep(b200m_ctx* c, const ViewHost& v, uint32_t* d_flag, cudaStrea
   if (!v.tc_capable()) return B200M_OK;
   const int grid = (v.m_pad + 7) / 8;
   if (zero_stats) CK(cudaMemsetAsync(v.stats, 0, 16, st));
-  if (v.store_dtype() == DT_F32) prep_view_kernel<float><<<grid, 256, 0, st>>>((const float*)v.raw, v.m, v.h16, v.nbh, v.nrm, v.m_pad, d_flag, v.aug16, v.augq16, v.err, v.stats);
-  else prep_view_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)v.raw, v.m, v.h16, v.nbh, v.nrm, v.m_pad, d_flag, v.aug16, v.augq16, v.err, v.stats);
+  if (v.store_dtype() == DT_F32) prep_view_kernel<float><<<grid, 256, 0, st>>>((const float*)v.raw, v.m, v.h16, v.nbh, v.nrm, v.m_pad, d_flag, v.aug16, v.augq16, v.err, v.stats, nullptr);
+  else prep_view_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)v.raw, v.m, v.h16, v.nbh, v.nrm, v.m_pad, d_flag, v.aug16, v.augq16, v.err, v.stats, v.nb32);
   CK(cudaGetLastError());
   return B200M_OK;
 }
@@ -463,6 +478,7 @@ static int ensure_batch_buffers(b200m_ctx* c) {
   CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true, tc::MODE_REAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true, true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true, tc::MODE_KNN>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tc::l2_top2_tc_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<false, false, true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(exact_rows_pairs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XP_SMEM));
   CK(cudaFuncSetAttribute(exact_top2_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, EX_SMEM));
   CK(cudaFuncSetAttribute(exact_top2_kernel<uint8_t, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, EX_SMEM));
@@ -1135,14 +1151,19 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> kernel_events;
   int launches = 0;
   int64_t total_records = 0, fallback_rows = 0;
-  int real_pairs = 0;
+  int real_pairs = 0, u8_pairs = 0;
   const bool real_tc = !c->force_exact && c->real_tc && c->tc_variant == 4;
+  // integer-valued pairs whose views are both stored as uchar run the u8 kernel (8-bit tensor cores, exact int32 distances) under the
+  // default variant; the other tensor-core pairs run the fp16 kernel
+  auto u8_pair = [&](const Directed& d) {
+    return d.mode == PM_TC && c->tc_variant == 4 && c->views[d.slot_i].store_dtype() == DT_U8 && c->views[d.slot_j].store_dtype() == DT_U8;
+  };
 
   auto enqueue = [&](size_t bi) -> int {
     const Batch& B = batches[bi];
     BatchBuf& bb = c->buf[bi & 1];
     const int np = (int)(B.end - B.begin);
-    uint32_t cbase = 0, sbase = 0; int n_items = 0, n_items_real = 0; int max_qblk_exact = 0, max_qblk_ham = 0;
+    uint32_t cbase = 0, sbase = 0; int n_items = 0, n_items_real = 0, n_items_u8 = 0; int max_qblk_exact = 0, max_qblk_ham = 0;
     // In-kernel exactness pass only when a work item lasts long enough (>= 24 database tiles on average) for two warps to
     // re-score the previous item's candidates behind it; shorter images use the stand-alone exactness kernel.
     // the views of this batch must be complete on the device; their exactness flags decide tensor-core vs exact kernel
@@ -1153,18 +1174,20 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       if ((r2 = ensure_view_ready(c, d.slot_i)) || (r2 = ensure_view_ready(c, d.slot_j))) return r2;
       if (d.mode == PM_TC) {
         const ViewHost& vi = c->views[d.slot_i]; const ViewHost& vj = c->views[d.slot_j];
-        if (!c->force_exact && vi.tc_ok() && vj.tc_ok()) ++tc_pairs;
+        if (!c->force_exact && vi.tc_ok() && vj.tc_ok()) { ++tc_pairs; u8_pairs += u8_pair(d); }
         else if (real_tc && vi.real_ok() && vj.real_ok()) { d.mode = PM_TC_REAL; ++real_pairs; }   // real-valued fp32: tensor-core filter + exact re-scoring
         else d.mode = vi.dtype == DT_F32 ? PM_EXACT_F32 : PM_EXACT_U8;
       }
     }
-    long tc_rows = 0, tc_n = 0, real_rows = 0, real_n = 0;
+    long tc_rows = 0, tc_n = 0, real_rows = 0, real_n = 0, u8_rows = 0, u8_n = 0;
     for (int p = 0; p < np; ++p) {
       const Directed& d = dir[seqv[B.begin + p]];
-      if (d.mode == PM_TC) { tc_rows += c->views[d.slot_i].m; ++tc_n; }
+      if (u8_pair(d)) { u8_rows += c->views[d.slot_i].m; ++u8_n; }
+      else if (d.mode == PM_TC) { tc_rows += c->views[d.slot_i].m; ++tc_n; }
       if (d.mode == PM_TC_REAL) { real_rows += c->views[d.slot_i].m; ++real_n; }
     }
     const bool fused = c->tc_variant >= 2 && tc_n > 0 && tc_rows / tc_n >= 6144;
+    const bool fused_u8 = u8_n > 0 && u8_rows / u8_n >= 6144;
     const int tc_ctas_per_item = (c->tc_variant == 2 || c->tc_variant == 4) ? 2 : 1;
     const bool fused_real = real_n > 0 && real_rows / real_n >= c->real_fused_rows;
     bool any_f32 = false, any_u8 = false, any_ham = false, any_gf32 = false, any_gu8 = false; int max_qblk_gen = 0;
@@ -1172,23 +1195,29 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       const Directed& d = dir[seqv[B.begin + p]];
       const ViewHost& vi = c->views[d.slot_i]; const ViewHost& vj = c->views[d.slot_j];
       // the CTA-pair kernel runs the exactness pass itself: its candidates are final records
-      const uint32_t dev_mode = (d.mode == PM_TC && fused) ? (uint32_t)PM_TC_FUSED : d.mode;
+      const bool u8 = u8_pair(d);
+      const uint32_t dev_mode = (d.mode == PM_TC && (u8 ? fused_u8 : fused)) ? (uint32_t)PM_TC_FUSED : d.mode;
       bb.h_pairs[p] = PairDev{(uint32_t)d.slot_i, (uint32_t)d.slot_j, (uint32_t)vi.m, (uint32_t)vj.m, cbase, dev_mode, sbase};
       cbase += (uint32_t)vj.m; sbase += (uint32_t)vi.m;
       const int qrows = tc_ctas_per_item * tc::BM;   // queries per work item
-      if (d.mode == PM_TC) for (int qt = 0; qt < (vj.m + qrows - 1) / qrows; ++qt) bb.h_items[n_items++] = WorkItem{(uint32_t)p, (uint32_t)qt};
+      if (d.mode == PM_TC && !u8) for (int qt = 0; qt < (vj.m + qrows - 1) / qrows; ++qt) bb.h_items[n_items++] = WorkItem{(uint32_t)p, (uint32_t)qt};
       if (d.mode == PM_TC_REAL) for (int qt = 0; qt < (vj.m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items_real[n_items_real++] = WorkItem{(uint32_t)p, (uint32_t)qt};
       if (d.mode == PM_EXACT_F32) { any_f32 = true; max_qblk_exact = std::max(max_qblk_exact, (vj.m + EX_TQ - 1) / EX_TQ); }
       if (d.mode == PM_EXACT_U8) { any_u8 = true; max_qblk_exact = std::max(max_qblk_exact, (vj.m + EX_TQ - 1) / EX_TQ); }
       if (d.mode == PM_HAMMING) { any_ham = true; max_qblk_ham = std::max(max_qblk_ham, (vj.m + HM_TQ - 1) / HM_TQ); }
       if (d.mode == PM_GENERIC_F32 || d.mode == PM_GENERIC_U8) { (d.mode == PM_GENERIC_F32 ? any_gf32 : any_gu8) = true; max_qblk_gen = std::max(max_qblk_gen, (vj.m + 3) / 4); }
     }
+    // the u8 kernel's work items (256 queries each) follow the fp16 kernel's in the same table
+    for (int p = 0; p < np; ++p) {
+      const Directed& d = dir[seqv[B.begin + p]];
+      if (u8_pair(d)) for (int qt = 0; qt < (c->views[d.slot_j].m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items[n_items + n_items_u8++] = WorkItem{(uint32_t)p, (uint32_t)qt};
+    }
     // Three streams so that consecutive batches' search kernels run back to back: the pair / work-item tables of this batch travel on
     // `tab_stream` (issued while the previous batch is still searching), the packing / finishing kernels and the meta read-back of this
     // batch run on `pack_stream` beside the next batch's search kernel.  Buffer set (bi & 1) is free: the host has seen ev_meta of batch bi-2.
     cudaStream_t ts = c->pipe_streams ? c->tab_stream : c->stream, ps = c->pipe_streams ? c->pack_stream : c->stream;
     CK(cudaMemcpyAsync(bb.d_pairs, bb.h_pairs, sizeof(PairDev) * np, cudaMemcpyHostToDevice, ts));
-    if (n_items) CK(cudaMemcpyAsync(bb.d_items, bb.h_items, sizeof(WorkItem) * n_items, cudaMemcpyHostToDevice, ts));
+    if (n_items + n_items_u8) CK(cudaMemcpyAsync(bb.d_items, bb.h_items, sizeof(WorkItem) * (n_items + n_items_u8), cudaMemcpyHostToDevice, ts));
     if (n_items_real) CK(cudaMemcpyAsync(bb.d_items_real, bb.h_items_real, sizeof(WorkItem) * n_items_real, cudaMemcpyHostToDevice, ts));
     CK(cudaMemsetAsync(bb.d_count, 0, sizeof(int) * np, ts));
     CK(cudaMemsetAsync(bb.d_fb_count, 0, 2 * sizeof(int), ts));
@@ -1196,12 +1225,20 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
     if (c->pipe_streams) { CK(cudaEventRecord(bb.ev_tab, ts)); CK(cudaStreamWaitEvent(c->stream, bb.ev_tab, 0)); }
     cudaEvent_t k0 = timing_event(c, tev_used), k1 = timing_event(c, tev_used);
     CK(cudaEventRecord(k0, c->stream));
+    // the debug trace (one kernel's CTA 0) shows the u8 kernel when the batch has u8 pairs, else the fp16 kernel
+    long long* fp16_trace = n_items_u8 ? nullptr : c->d_trace;
     if (n_items) {
       const int grid = tc_ctas_per_item * std::min(n_items, c->num_sms / tc_ctas_per_item);   // one CTA per SM, whole work items per CTA group
       if (c->tc_variant == 4)
-        tc::l2_top2_tc_kernel<true><<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<true>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, tc_ctas_per_item, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->d_err, (int)fused, nullptr, FbSink{});
+        tc::l2_top2_tc_kernel<true><<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<true>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, tc_ctas_per_item, bb.d_cands, bb.d_count, ratio_sq, fp16_trace, c->d_err, (int)fused, nullptr, FbSink{});
       else
-        tc::l2_top2_tc_kernel<false><<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, tc_ctas_per_item, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->d_err, (int)fused, nullptr, FbSink{});
+        tc::l2_top2_tc_kernel<false><<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, tc_ctas_per_item, bb.d_cands, bb.d_count, ratio_sq, fp16_trace, c->d_err, (int)fused, nullptr, FbSink{});
+      ++launches;
+    }
+    if (n_items_u8) {
+      const int grid = 2 * std::min(n_items_u8, c->num_sms / 2);
+      tc::l2_top2_tc_u8_kernel<<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false, false, true>::SMEM_BYTES, c->stream>>>(
+          c->d_views, bb.d_pairs, bb.d_items + n_items, n_items_u8, 2, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->d_err, (int)fused_u8, nullptr, FbSink{});
       ++launches;
     }
     if (n_items_real) {
@@ -1363,7 +1400,7 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
             kernel_events.size(), sk, lead, gaps, gmax, tail);
   }
   c->last_search_ms = sk; c->last_launches = launches; c->last_tc_pairs = tc_pairs; c->last_records = total_records;
-  c->last_real_pairs = real_pairs; c->last_fallback_rows = fallback_rows;
+  c->last_real_pairs = real_pairs; c->last_fallback_rows = fallback_rows; c->last_u8_pairs = u8_pairs;
   unsigned errs = 0;
   CK(cudaMemcpy(&errs, c->d_err, sizeof(unsigned), cudaMemcpyDeviceToHost));
   c->err_total = errs;
@@ -1436,6 +1473,7 @@ int b200m_last_tc_pairs(const b200m_ctx* c) { return c ? c->last_tc_pairs : 0; }
 unsigned b200m_exactness_errors(const b200m_ctx* c) { return c ? c->err_total : 0; }
 int64_t b200m_last_records(const b200m_ctx* c) { return c ? c->last_records : 0; }
 int b200m_last_real_tc_pairs(const b200m_ctx* c) { return c ? c->last_real_pairs : 0; }
+int b200m_last_u8_tc_pairs(const b200m_ctx* c) { return c ? c->last_u8_pairs : 0; }
 int64_t b200m_last_fallback_rows(const b200m_ctx* c) { return c ? c->last_fallback_rows : 0; }
 
 // ---- guided matching (after the path: GeometricFilterMatrix_F_AC.hpp:363-390 -> matching/guidedMatching.hpp:206-268) ----------------
@@ -1516,7 +1554,7 @@ int b200m_guided_match_model(b200m_ctx* c, uint32_t view_left, uint32_t view_rig
     if (n) CK(cudaMemcpy(recs.data(), d_out, sizeof(Rec) * (size_t)n, cudaMemcpyDeviceToHost));
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
-    c->last_gpu_ms = ms; c->last_search_ms = ms; c->last_launches = 3; c->last_records = n; c->last_tc_pairs = 0;
+    c->last_gpu_ms = ms; c->last_search_ms = ms; c->last_launches = 3; c->last_records = n; c->last_tc_pairs = 0; c->last_u8_pairs = 0;
     cudaFreeAsync(d_xy, st); cudaFreeAsync(d_xl, st); cudaFreeAsync(d_xr, st); cudaFreeAsync(d_out, st); cudaFreeAsync(d_cnt, st);
     // IndMatch::getDeduplicated (guidedMatching.hpp:267): one record per left feature, so this is a sort by (i, j)
     std::sort(recs.begin(), recs.end(), [](const Rec& a, const Rec& b) { return a.i < b.i || (a.i == b.i && a.j < b.j); });
@@ -1758,7 +1796,7 @@ int b200m_guided_match_fast_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pai
   for (Open& o : open)
     if (int rc = flush(o)) return rc;
   if (int rc = wait_uploads(c)) return rc;
-  c->last_gpu_ms = gpu_ms; c->last_search_ms = cand_ms; c->last_launches = launches; c->last_records = cands; c->last_tc_pairs = 0;
+  c->last_gpu_ms = gpu_ms; c->last_search_ms = cand_ms; c->last_launches = launches; c->last_records = cands; c->last_tc_pairs = 0; c->last_u8_pairs = 0;
   // one result pair per input pair, in input order (empty lists included)
   std::unique_ptr<b200m_result> res(new b200m_result());
   res->recycler = c->recycler;
@@ -2156,7 +2194,7 @@ int b200m_db_create(b200m_ctx* c, const void* data, int rows, int dim, int dtype
   ViewHost& v = db->v;
   v.m = rows; v.dim = dim; v.dtype = dtype;
   const size_t esz = dtype == DT_F32 ? 4 : 1;
-  if ((rc = alloc_view_buffers(c, v))) return rc;
+  if ((rc = alloc_view_buffers(c, v, false))) return rc;
   CK(cudaMemcpyAsync(v.raw, data, (size_t)rows * dim * esz, cudaMemcpyHostToDevice, c->stream));
   if (v.tc_capable()) {
     uint32_t* d_flag = nullptr;
@@ -2261,10 +2299,10 @@ int b200m_knn(b200m_ctx* c, const b200m_db* db, const void* query, int nq, int n
     CK(cudaMemcpyAsync(&c->err_total, c->d_err, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));               // items / hv / hp are stack objects; results are in the caller's buffers
     done = (qflags & VF_EXACT_MASK) == 0;        // a query batch outside the exact domain (non-integer, huge values): redo on the exact kernels
-    c->last_tc_pairs = done ? 1 : 0;
+    c->last_tc_pairs = done ? 1 : 0; c->last_u8_pairs = 0;
   }
   if (done) return B200M_OK;
-  c->last_tc_pairs = 0;
+  c->last_tc_pairs = 0; c->last_u8_pairs = 0;
 
   const bool tiled_l2 = nn == 2 && v.dim == 128 && v.dtype != DT_BIN && (v.dtype == DT_U8 || db->metric == B200M_L2_VECTORIZED);
   const bool tiled_ham = nn == 2 && v.dim == 64 && v.dtype == DT_BIN;

@@ -65,15 +65,19 @@ constexpr int KB_BYTES = 128 * 64 * 2;    // 16 KB: one K-block (64 fp16) of 128
 constexpr int Q_BYTES = 2 * KB_BYTES;     // 32 KB
 constexpr int DB_BYTES = 2 * KB_BYTES;    // 32 KB
 constexpr int AUG_BYTES = 128 * 16 * 2;   // 4 KB: 16 augmentation columns of 128 rows
-constexpr int NB_BYTES = BN * 4;          // half-norms of one tile
+constexpr int NB_BYTES = BN * 4;          // half-norms (u8: int32 norms) of one tile
+constexpr int U8_BYTES = 128 * 128;       // 16 KB: 128 uchar rows of 128 B = one TMA box of tmap_u8 (the whole K of a u8 query or database tile)
 constexpr int EPI_WARPS = 8;
 enum : int { MODE_MATCH = 0, MODE_KNN = 1, MODE_REAL = 2 };
 
-template <bool AUG, bool REAL = false> struct Lay {
-  static constexpr int NS = AUG ? 3 : 4;                             // database ring slots (AUG: leaves shared memory to L1 for the re-scoring warps)
-  static constexpr int STAGE = DB_BYTES + (AUG ? AUG_BYTES : 1024);  // + augmentation columns, or the half-norms (padded: tiles stay 1024-B aligned)
+template <bool AUG, bool REAL = false, bool U8 = false> struct Lay {
+  // database ring slots (AUG: leaves shared memory to L1 for the re-scoring warps; U8: half-size stages, twice as many in about the same bytes)
+  static constexpr int NS = U8 ? 8 : AUG ? 3 : 4;
+  static constexpr int QT = U8 ? U8_BYTES : Q_BYTES;                 // one query tile buffer
+  // + augmentation columns, or the (half-)norms (padded: tiles stay 1024-B aligned)
+  static constexpr int STAGE = U8 ? U8_BYTES + 1024 : DB_BYTES + (AUG ? AUG_BYTES : 1024);
   static constexpr int OFF_Q = 0;
-  static constexpr int OFF_DB = OFF_Q + 2 * Q_BYTES;
+  static constexpr int OFF_DB = OFF_Q + 2 * QT;
   static constexpr int OFF_A = OFF_DB + NS * STAGE;                  // AUG: the constant A tile of the 9th K-step; REAL: the query's own limb tile, 2 buffers
   static constexpr int OFF_MRG = OFF_A + (AUG ? (REAL ? 2 : 1) * AUG_BYTES : 0);   // per-row merged state, 2 buffers x 128 x 16 B
   static constexpr int OFF_VQ = OFF_MRG + 2 * BM * 16;               // candidate queue: 2 buffers x 128 Cand (32 slots per row quadrant)
@@ -140,22 +144,48 @@ __device__ __forceinline__ void merge_xor(Top4& s, int m) {
   top4_insert(s, o1); top4_insert(s, o2); top4_insert(s, o3); top4_insert(s, o4);
 }
 
+__device__ __forceinline__ float vmin(float a, float b) { return fminf(a, b); }
+__device__ __forceinline__ int32_t vmin(int32_t a, int32_t b) { return min(a, b); }
+// Per row, the thread's minima of the 8 chunks (over its 4 columns of each) -> the full minima of chunks qlane and qlane + 4 (over the quad),
+// v2[row][h] = chunk 4h + qlane: a two-step butterfly, 12 shuffles
+template <typename T>
+__device__ __forceinline__ void quad_chunk_minima(const T (&pm)[2][8], int qlane, T (&v2)[2][2]) {
+  const bool b0 = qlane & 1, b1 = (qlane >> 1) & 1;
+  T v1[2][4];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {        // keep chunks 2i + b0, hand the other to lane ^ 1
+      const T keep = b0 ? pm[r][2 * i + 1] : pm[r][2 * i], send = b0 ? pm[r][2 * i] : pm[r][2 * i + 1];
+      v1[r][i] = vmin(keep, __shfl_xor_sync(0xffffffffu, send, 1));
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {        // keep chunks 4h + 2 b1 + b0 = 4h + qlane
+      const T keep = b1 ? v1[r][2 * h + 1] : v1[r][2 * h], send = b1 ? v1[r][2 * h] : v1[r][2 * h + 1];
+      v2[r][h] = vmin(keep, __shfl_xor_sync(0xffffffffu, send, 2));
+    }
+  }
+}
+
 // The real-valued re-scoring reads 32 fp32 rows per candidate (16 KB, mostly from HBM) and is latency-bound: two warps cannot keep up with
 // the tensor cores, so MODE_REAL adds six re-scoring warps behind the epilogue warps.
 constexpr int REAL_EXTRA_VERIFY_WARPS = 6;
 template <int MODE> constexpr int block_threads() { return 128 + EPI_WARPS * 32 + (MODE == MODE_REAL ? REAL_EXTRA_VERIFY_WARPS * 32 : 0); }
 
-template <bool AUG, int MODE = MODE_MATCH>
-__global__ void __launch_bounds__(block_threads<MODE>(), 1)
-l2_top2_tc_kernel(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs, const WorkItem* __restrict__ items, int n_items,
-                  int ctas_per_item, Cand* __restrict__ cands, int* __restrict__ cand_count, float ratio_sq, long long* __restrict__ trace_buf,
-                  unsigned int* __restrict__ err_count, int fused, uint32_t* __restrict__ candx, FbSink fb) {
+// The kernel body (entry points at the end of the file).  U8: the operands are the views' uchar rows (tmap_u8) on the 8-bit tensor cores,
+// MODE_MATCH only; see the consumer loop.
+template <bool AUG, int MODE, bool U8>
+__device__ __forceinline__ void
+l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs, const WorkItem* __restrict__ items, int n_items,
+           int ctas_per_item, Cand* __restrict__ cands, int* __restrict__ cand_count, float ratio_sq, long long* __restrict__ trace_buf,
+           unsigned int* __restrict__ err_count, int fused, uint32_t* __restrict__ candx, FbSink fb) {
   long long* trace = (blockIdx.x == 0) ? trace_buf : nullptr;
   constexpr bool REAL = MODE == MODE_REAL, KNN = MODE == MODE_KNN;
   constexpr int VERIFY_WARPS_K = REAL ? 2 + REAL_EXTRA_VERIFY_WARPS : 2;   // warps 2, 3 (+ the warps behind the epilogue warps)
   static_assert(!(REAL || KNN) || AUG, "MODE_REAL / MODE_KNN exist for the AUG layout only");
-  using L = Lay<AUG, REAL>;
-  constexpr int NS = L::NS, STAGE = L::STAGE;
+  static_assert(!U8 || (MODE == MODE_MATCH && !AUG), "the u8 kernel is MODE_MATCH with its norms in the database ring");
+  using L = Lay<AUG, REAL, U8>;
+  constexpr int NS = L::NS, STAGE = L::STAGE, QT = L::QT;
   extern __shared__ __align__(1024) uint8_t smem[];   // SWIZZLE_128B operand tiles need 1024-B alignment
   if ((ptx::smem_u32(smem) & 1023u) != 0) { asm volatile("trap;"); }
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
@@ -205,10 +235,14 @@ l2_top2_tc_kernel(const ViewDev* __restrict__ views, const PairDev* __restrict__
         const ViewDev* vj = views + p.view_j;
         const int qrow = ((int)w.qtile * ctas_per_item + rank) * BM;
         ptx::mbar_wait(&q_empty[qb], qph ^ 1);
-        ptx::mbar_arrive_expect_tx(&q_full[qb], Q_BYTES + (REAL ? AUG_BYTES : 0));
-        uint8_t* qs = smem + L::OFF_Q + qb * Q_BYTES;
-        ptx::tma_load_2d(qs, &vj->tmap128, &q_full[qb], 0, qrow);
-        ptx::tma_load_2d(qs + KB_BYTES, &vj->tmap128, &q_full[qb], 64, qrow);
+        ptx::mbar_arrive_expect_tx(&q_full[qb], QT + (REAL ? AUG_BYTES : 0));
+        uint8_t* qs = smem + L::OFF_Q + qb * QT;
+        if (U8) {
+          ptx::tma_load_2d(qs, &vj->tmap_u8, &q_full[qb], 0, qrow);
+        } else {
+          ptx::tma_load_2d(qs, &vj->tmap128, &q_full[qb], 0, qrow);
+          ptx::tma_load_2d(qs + KB_BYTES, &vj->tmap128, &q_full[qb], 64, qrow);
+        }
         if (REAL) ptx::tma_load_2d(smem + L::OFF_A + qb * AUG_BYTES, &vj->tmap_augq, &q_full[qb], 0, qrow);   // the query rows' own half-norm limbs
         qb ^= 1; if (qb == 0) qph ^= 1;
         const int ntiles = ((int)p.m_i + BN - 1) / BN;
@@ -216,11 +250,17 @@ l2_top2_tc_kernel(const ViewDev* __restrict__ views, const PairDev* __restrict__
           ptx::mbar_wait(&db_empty[st], sph ^ 1);
           ptx::trace_stamp(trace, 0, tt, 0);
           uint8_t* ds = smem + L::OFF_DB + st * STAGE;
-          ptx::mbar_arrive_expect_tx(&db_full[st], DB_BYTES + (AUG ? AUG_BYTES : NB_BYTES));
-          ptx::tma_load_2d(ds, &vi->tmap128, &db_full[st], 0, t * BN);
-          ptx::tma_load_2d(ds + KB_BYTES, &vi->tmap128, &db_full[st], 64, t * BN);
-          if (AUG) ptx::tma_load_2d(ds + DB_BYTES, &vi->tmap_aug, &db_full[st], 0, t * BN);
-          else ptx::bulk_load_1d(ds + DB_BYTES, vi->nbh + (size_t)t * BN, NB_BYTES, &db_full[st]);
+          if (U8) {
+            ptx::mbar_arrive_expect_tx(&db_full[st], U8_BYTES + NB_BYTES);
+            ptx::tma_load_2d(ds, &vi->tmap_u8, &db_full[st], 0, t * BN);
+            ptx::bulk_load_1d(ds + U8_BYTES, vi->nb32 + (size_t)t * BN, NB_BYTES, &db_full[st]);
+          } else {
+            ptx::mbar_arrive_expect_tx(&db_full[st], DB_BYTES + (AUG ? AUG_BYTES : NB_BYTES));
+            ptx::tma_load_2d(ds, &vi->tmap128, &db_full[st], 0, t * BN);
+            ptx::tma_load_2d(ds + KB_BYTES, &vi->tmap128, &db_full[st], 64, t * BN);
+            if (AUG) ptx::tma_load_2d(ds + DB_BYTES, &vi->tmap_aug, &db_full[st], 0, t * BN);
+            else ptx::bulk_load_1d(ds + DB_BYTES, vi->nbh + (size_t)t * BN, NB_BYTES, &db_full[st]);
+          }
           ptx::trace_stamp(trace, 0, tt, 1); ++tt;
           if (++st == NS) { st = 0; sph ^= 1; }
         }
@@ -286,54 +326,78 @@ l2_top2_tc_kernel(const ViewDev* __restrict__ views, const PairDev* __restrict__
         ptx::mbar_wait(&db_full[st], sph);
         ptx::trace_stamp(etrace, 1 + wg, tt, 1);
         const uint32_t b_base = db_addr + st * STAGE;
-        float acc[64];
-        ptx::wgmma_fence();
+        auto release_slot = [&] {
+          __syncwarp();
+          if (lane == 0) ptx::mbar_arrive(&db_empty[st]);             // this warp is done with the slot (operands and (half-)norms)
+          if (++st == NS) { st = 0; sph ^= 1; }
+        };
+        float v2[2][2];                        // chunk minima h of chunks 4h + qlane of rows r0, r0 + 8 (quad_chunk_minima)
+        if constexpr (U8) {
+          // acc = a.b, exact in s32.  Per element s = ||b||^2 - 2 a.b = ||a - b||^2 - ||a||^2 (one IMAD), chunk minima in integers, and only
+          // the four surviving minima per thread become h = s / 2: exactly the fp16 kernel's accumulator value (|s| < 2^24), so everything
+          // from the folds on is shared.  Pad rows: a.b = 0 (TMA zero fill), ||b||^2 = 2^24 (prep.cuh) -> h = 2^23, as in the fp16 kernel.
+          int32_t acc[64];
+          ptx::wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t da = ptx::wgmma_desc_k_sw128(q_addr + qb * Q_BYTES + (k >> 2) * KB_BYTES + (k & 3) * 32);
-          const uint64_t db = ptx::wgmma_desc_k_sw128(b_base + (k >> 2) * KB_BYTES + (k & 3) * 32);
-          ptx::wgmma_m64n128k16_f16_negb(acc, da, db, k > 0 ? 1u : 0u);
-        }
-        if (AUG) {  // 9th K-step: constants (or the query's limbs) x the database rows' half-norm limbs
-          const uint64_t da = ptx::wgmma_desc_k_sw32(a_aug + (REAL ? qb * AUG_BYTES : 0));
-          const uint64_t db = ptx::wgmma_desc_k_sw32(b_base + DB_BYTES);
-          ptx::wgmma_m64n128k16_f16_negb(acc, da, db, 1u);
-        }
-        ptx::wgmma_commit();
-        ptx::wgmma_wait_all();
-        ptx::trace_stamp(etrace, 1 + wg, tt, 2);
-        if (!AUG) {
-          const float2* nb2 = reinterpret_cast<const float2*>(smem + L::OFF_DB + st * STAGE + DB_BYTES) + qlane;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float2 nb = nb2[4 * j];
-            acc[4 * j + 0] += nb.x; acc[4 * j + 1] += nb.y; acc[4 * j + 2] += nb.x; acc[4 * j + 3] += nb.y;
+          for (int k = 0; k < 4; ++k) {
+            const uint64_t da = ptx::wgmma_desc_k_sw128(q_addr + qb * QT + k * 32);
+            const uint64_t db = ptx::wgmma_desc_k_sw128(b_base + k * 32);
+            ptx::wgmma_m64n128k32_u8(acc, da, db, k > 0 ? 1u : 0u);
           }
-        }
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&db_empty[st]);             // this warp is done with the slot (operands and half-norms)
-        if (++st == NS) { st = 0; sph ^= 1; }
-        // chunk c of row r0: acc[8c + {0, 1, 4, 5}]; of row r0 + 8: acc[8c + {2, 3, 6, 7}]
-        float pm[2][8];
+          ptx::wgmma_commit();
+          ptx::wgmma_wait_all();
+          ptx::trace_stamp(etrace, 1 + wg, tt, 2);
+          // columns 16c + 2 qlane + {0, 1} and 16c + 8 + 2 qlane + {0, 1} of chunk c: acc[8c + {0, 1}], acc[8c + {4, 5}] (row r0),
+          // acc[8c + {2, 3}], acc[8c + {6, 7}] (row r0 + 8)
+          const int2* nb2 = reinterpret_cast<const int2*>(smem + L::OFF_DB + st * STAGE + U8_BYTES) + qlane;
+          int32_t pm[2][8];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          pm[0][c] = fminf(fminf(acc[8 * c + 0], acc[8 * c + 1]), fminf(acc[8 * c + 4], acc[8 * c + 5]));
-          pm[1][c] = fminf(fminf(acc[8 * c + 2], acc[8 * c + 3]), fminf(acc[8 * c + 6], acc[8 * c + 7]));
-        }
-        const bool b0 = qlane & 1, b1 = (qlane >> 1) & 1;
-        float v1[2][4], v2[2][2];
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {        // keep chunks 2i + b0, hand the other to lane ^ 1
-            const float keep = b0 ? pm[r][2 * i + 1] : pm[r][2 * i], send = b0 ? pm[r][2 * i] : pm[r][2 * i + 1];
-            v1[r][i] = fminf(keep, __shfl_xor_sync(0xffffffffu, send, 1));
+          for (int c = 0; c < 8; ++c) {
+            const int2 n0 = nb2[8 * c], n1 = nb2[8 * c + 4];
+            pm[0][c] = __vimin3_s32(n0.x - 2 * acc[8 * c + 0], n0.y - 2 * acc[8 * c + 1], min(n1.x - 2 * acc[8 * c + 4], n1.y - 2 * acc[8 * c + 5]));
+            pm[1][c] = __vimin3_s32(n0.x - 2 * acc[8 * c + 2], n0.y - 2 * acc[8 * c + 3], min(n1.x - 2 * acc[8 * c + 6], n1.y - 2 * acc[8 * c + 7]));
           }
+          release_slot();
+          int32_t v2i[2][2];
+          quad_chunk_minima(pm, qlane, v2i);
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {        // keep chunks 4h + 2 b1 + b0 = 4h + qlane
-            const float keep = b1 ? v1[r][2 * h + 1] : v1[r][2 * h], send = b1 ? v1[r][2 * h] : v1[r][2 * h + 1];
-            v2[r][h] = fminf(keep, __shfl_xor_sync(0xffffffffu, send, 2));
+          for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) v2[r][h] = 0.5f * (float)v2i[r][h];
+        } else {
+          float acc[64];
+          ptx::wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            const uint64_t da = ptx::wgmma_desc_k_sw128(q_addr + qb * Q_BYTES + (k >> 2) * KB_BYTES + (k & 3) * 32);
+            const uint64_t db = ptx::wgmma_desc_k_sw128(b_base + (k >> 2) * KB_BYTES + (k & 3) * 32);
+            ptx::wgmma_m64n128k16_f16_negb(acc, da, db, k > 0 ? 1u : 0u);
           }
+          if (AUG) {  // 9th K-step: constants (or the query's limbs) x the database rows' half-norm limbs
+            const uint64_t da = ptx::wgmma_desc_k_sw32(a_aug + (REAL ? qb * AUG_BYTES : 0));
+            const uint64_t db = ptx::wgmma_desc_k_sw32(b_base + DB_BYTES);
+            ptx::wgmma_m64n128k16_f16_negb(acc, da, db, 1u);
+          }
+          ptx::wgmma_commit();
+          ptx::wgmma_wait_all();
+          ptx::trace_stamp(etrace, 1 + wg, tt, 2);
+          if (!AUG) {
+            const float2* nb2 = reinterpret_cast<const float2*>(smem + L::OFF_DB + st * STAGE + DB_BYTES) + qlane;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              const float2 nb = nb2[4 * j];
+              acc[4 * j + 0] += nb.x; acc[4 * j + 1] += nb.y; acc[4 * j + 2] += nb.x; acc[4 * j + 3] += nb.y;
+            }
+          }
+          release_slot();
+          // chunk c of row r0: acc[8c + {0, 1, 4, 5}]; of row r0 + 8: acc[8c + {2, 3, 6, 7}]
+          float pm[2][8];
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            pm[0][c] = fminf(fminf(acc[8 * c + 0], acc[8 * c + 1]), fminf(acc[8 * c + 4], acc[8 * c + 5]));
+            pm[1][c] = fminf(fminf(acc[8 * c + 2], acc[8 * c + 3]), fminf(acc[8 * c + 6], acc[8 * c + 7]));
+          }
+          quad_chunk_minima(pm, qlane, v2);
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -435,6 +499,24 @@ l2_top2_tc_kernel(const ViewDev* __restrict__ views, const PairDev* __restrict__
     }
   }
 }
+
+#define B200M_TC_PARAMS const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs, const WorkItem* __restrict__ items, int n_items, \
+    int ctas_per_item, Cand* __restrict__ cands, int* __restrict__ cand_count, float ratio_sq, long long* __restrict__ trace_buf, \
+    unsigned int* __restrict__ err_count, int fused, uint32_t* __restrict__ candx, FbSink fb
+#define B200M_TC_ARGS views, pairs, items, n_items, ctas_per_item, cands, cand_count, ratio_sq, trace_buf, err_count, fused, candx, fb
+
+template <bool AUG, int MODE = MODE_MATCH>
+__global__ void __launch_bounds__(block_threads<MODE>(), 1) l2_top2_tc_kernel(B200M_TC_PARAMS) { l2_top2_tc<AUG, MODE, false>(B200M_TC_ARGS); }
+
+// The u8 kernel is held to 128 registers per thread: the 512-thread, 32-register device finishing kernel (finish.cuh) of the previous batch
+// then still fits beside the persistent CTA of each SM, as it does beside the fp16 kernel.  At 130 registers it waited for the search
+// kernel to end, and consecutive batches' search kernels no longer ran back to back.
+__global__ void __maxnreg__(128) l2_top2_tc_u8_kernel(B200M_TC_PARAMS) {
+  l2_top2_tc<false, MODE_MATCH, true>(B200M_TC_ARGS);
+}
+
+#undef B200M_TC_PARAMS
+#undef B200M_TC_ARGS
 
 }  // namespace tc
 }  // namespace b200m

@@ -69,7 +69,8 @@ int b200m_ctx_set_tc_variant(b200m_ctx* ctx, int variant);
 int b200m_debug_convert_f32_u8(const float* src, uint8_t* dst, size_t n, int which);
 
 /* debug: per-tile SM-clock trace of CTA 0 of the tensor-core kernel (4 roles x 512 tiles x 4 stamps: TMA producer, the two
- * consumer warpgroups, unused); enable!=0 allocates,
+ * consumer warpgroups, unused; of the u8 kernel when the last batch had uchar-stored pairs, else of the fp16 kernel);
+ * enable!=0 allocates,
  * out (may be NULL) receives up to n values after synchronising */
 int b200m_debug_trace(b200m_ctx* ctx, int enable, long long* out, int n);
 
@@ -257,6 +258,9 @@ int64_t b200m_last_records(const b200m_ctx* ctx);
  * exactly over the whole database image (exact_rows fallback) */
 int b200m_last_real_tc_pairs(const b200m_ctx* ctx);
 int64_t b200m_last_fallback_rows(const b200m_ctx* ctx);
+/* the tensor-core pairs of the last call (counted in b200m_last_tc_pairs too) whose two views are stored as uchar and ran on the 8-bit
+ * tensor cores (exact int32 distances) */
+int b200m_last_u8_tc_pairs(const b200m_ctx* ctx);
 
 #ifdef __cplusplus
 }
