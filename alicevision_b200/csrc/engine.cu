@@ -17,6 +17,7 @@
 #include "prep.cuh"
 #include "verify.cuh"
 #include "hostconv.hpp"
+#include "cuda_owner.cuh"
 
 #include <cub/cub.cuh>
 #include <pthread.h>
@@ -48,12 +49,7 @@ using namespace b200m;
 // ------------------------------------------------------------------------------------------------ errors
 static thread_local std::string g_err;
 static int fail(int code, const std::string& msg) { g_err = msg; return code; }
-namespace b200m { int set_error(int code, const std::string& msg) { return fail(code, msg); } }   // for the other translation units of the library
-#define CK(call)                                                                                          \
-  do {                                                                                                    \
-    cudaError_t e_ = (call);                                                                              \
-    if (e_ != cudaSuccess) return fail(B200M_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
-  } while (0)
+namespace b200m { int set_error(int code, const std::string& msg) { return fail(code, msg); } }   // for CK and the other translation units
 
 // ------------------------------------------------------------------------------------------------ small thread pool
 // CPUs of the NUMA node a GPU hangs off (sysfs), intersected with the CPUs this process may use; empty set = unknown / do not pin.
@@ -206,14 +202,14 @@ struct UploadJob {
 };
 
 struct BatchBuf {
-  PairDev* d_pairs = nullptr; WorkItem* d_items = nullptr; Cand* d_cands = nullptr; int* d_count = nullptr; int* d_off = nullptr;
-  Rec* d_out = nullptr;
-  FinMatch* d_fin = nullptr; int* d_fin_count = nullptr; uint32_t* d_scratch = nullptr;   // device finishing stage (finish.cuh)
-  WorkItem* d_items_real = nullptr; WorkItem* h_items_real = nullptr;                     // work items of the real-valued pairs (own launch)
-  uint32_t* d_candx = nullptr; uint4* d_fb = nullptr; int* d_fb_count = nullptr;          // fallback lists: d_fb_count = [overflow count, total]
-  uint4* d_fb_pair = nullptr; int* d_fb_pair_cnt = nullptr;          // real-valued path: 5th candidate word, fallback list (pair, query)
-  PairDev* h_pairs = nullptr; WorkItem* h_items = nullptr; int* h_meta = nullptr; Rec* h_out = nullptr;   // pinned
-  cudaEvent_t ev_meta = nullptr, ev_copy = nullptr, ev_tab = nullptr;
+  DeviceBuffer<PairDev> d_pairs; DeviceBuffer<WorkItem> d_items; DeviceBuffer<Cand> d_cands; DeviceBuffer<int> d_count, d_off;
+  DeviceBuffer<Rec> d_out;
+  DeviceBuffer<FinMatch> d_fin; DeviceBuffer<int> d_fin_count; DeviceBuffer<uint32_t> d_scratch;   // device finishing stage (finish.cuh)
+  DeviceBuffer<WorkItem> d_items_real; PinnedBuffer<WorkItem> h_items_real;                     // work items of the real-valued pairs (own launch)
+  DeviceBuffer<uint32_t> d_candx; DeviceBuffer<uint4> d_fb; DeviceBuffer<int> d_fb_count;      // fallback lists: d_fb_count = [overflow count, total]
+  DeviceBuffer<uint4> d_fb_pair; DeviceBuffer<int> d_fb_pair_cnt;    // real-valued path: 5th candidate word, fallback list (pair, query)
+  PinnedBuffer<PairDev> h_pairs; PinnedBuffer<WorkItem> h_items; PinnedBuffer<int> h_meta; PinnedBuffer<Rec> h_out;
+  Event ev_meta, ev_copy, ev_tab;
 };
 
 constexpr int PAIR_CAP = 4096;            // directed pairs per batch
@@ -228,54 +224,62 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 
 // grow-only device scratch of b200m_knn (Surface 1)
 struct KnnScratch {
-  int cap = 0; size_t raw_bytes = 0;
-  void* raw = nullptr; __half* h16 = nullptr; float* nbh = nullptr; float* nrm = nullptr; __half* aug16 = nullptr; __half* augq16 = nullptr; float* err = nullptr;
-  Cand* cands = nullptr; int32_t* idx = nullptr; uint32_t* dist = nullptr; WorkItem* items = nullptr; uint8_t* small = nullptr;
+  DeviceBuffer<> raw; DeviceBuffer<__half> h16; DeviceBuffer<float> nbh, nrm; DeviceBuffer<__half> aug16, augq16; DeviceBuffer<float> err;
+  DeviceBuffer<Cand> cands; DeviceBuffer<int32_t> idx; DeviceBuffer<uint32_t> dist; DeviceBuffer<WorkItem> items; DeviceBuffer<uint8_t> small;
 };
 
 // grow-only scratch of b200m_guided_match_fast_pairs (guided_fast.cuh): one batch of pairs at a time
 struct GuidedFastScratch {
-  struct Buf { void* p = nullptr; size_t bytes = 0; };
   enum { PAIRS, LBUCKET, BEST, SECOND, BCOUNT, BOFF, CSR, RSTART, RCOUNT, RCOFF, RPAIR, KEEP, KPOS, OUT, PSTART, EXPAND, TEMP, NBUF };
-  Buf d[NBUF];
-  void* h_pairs = nullptr; size_t h_pairs_bytes = 0;      // pinned: FastPair table
-  void* h_meta = nullptr; size_t h_meta_bytes = 0;        // pinned: read-back of the candidate total and the per-pair starts
-  void* h_out = nullptr; size_t h_out_bytes = 0;          // pinned: read-back of the matches
-  cudaEvent_t ev_c0 = nullptr, ev_c1 = nullptr;           // candidate-kernel timing
+  DeviceBuffer<> d[NBUF];
+  PinnedBuffer<FastPair> h_pairs;
+  PinnedBuffer<> h_meta;                      // read-back of the candidate total and the per-pair starts
+  PinnedBuffer<uint2> h_out;                  // read-back of the matches
+  Event ev_c0, ev_c1;                         // candidate-kernel timing
 };
 
 // grow-only scratch of b200m_acransac_fundamental_pairs and b200m_acransac_homography_pairs (acransac.cuh); the last call's
 // instrumentation and trace, whichever model it estimated
 struct AcransacScratch {
-  void* d = nullptr; size_t bytes = 0;
+  DeviceBuffer<char> d;
   bool skip = true;                                   // certified skip (b200m_ctx_set_acransac_skip)
   double last_ms = 0; int64_t stats[4] = {0, 0, 0, 0};
   std::vector<int32_t> trace; std::vector<double> trace_nfa; std::vector<int32_t> n_trace;   // last call: kTraceCap entries per pair
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  Event ev0, ev1;
 };
 
+// What the last b200m_match_pairs, b200m_guided_match_model, b200m_guided_match_fast_pairs or b200m_knn measured (b200m_last_*);
+// a field the call does not measure is 0
+struct LastCall {
+  double gpu_ms, search_ms;
+  int launches, tc_pairs, real_pairs, u8_pairs;
+  int64_t records, fallback_rows;
+};
+
+// Members are released in reverse order of declaration, after ~b200m_ctx has stopped the uploader and the pool and freed the views:
+// the streams go last.
 struct b200m_ctx {
+  ~b200m_ctx();
   int device = 0, num_sms = 148;
+  Stream stream, copy_stream, up_stream, tab_stream, pack_stream;
   AcransacScratch acr;
   KnnScratch knn;
   GuidedFastScratch gf;
   long gf_left_cap = 1l << 21;    // left features per internal batch of b200m_guided_match_fast_pairs (B200M_GUIDED_FAST_LEFT_CAP)
-  cudaStream_t stream = nullptr, copy_stream = nullptr, up_stream = nullptr, tab_stream = nullptr, pack_stream = nullptr;
   bool pipe_streams = true;       // tables / packing+finishing on their own streams (B200M_PIPE_STREAMS=0: everything on the search stream)
-  bool own_stream = false;
   EncodeTiledFn encode = nullptr;
   std::deque<ViewHost> views;     // deque: references stay valid while pool tasks (position checks) run
   std::unordered_map<uint32_t, int> slot_of;
   std::vector<int> free_slots;    // slots of removed views (b200m_remove_view), reused by later uploads
-  ViewDev* d_views = nullptr; uint32_t* d_flags = nullptr; int view_cap = 0;
+  DeviceBuffer<ViewDev> d_views; DeviceBuffer<uint32_t> d_flags; int view_cap = 0;
   BatchBuf buf[2]; bool bufs_ready = false;
   // upload staging: pageable caller memory -> pinned ring (parallel memcpy on the pool) -> async H2D
   static constexpr int NSTG = 24;
-  void* stg[NSTG] = {}; size_t stg_bytes[NSTG] = {}; cudaEvent_t stg_ev[NSTG] = {};
-  ViewDev* h_views = nullptr;     // pinned mirror of the device view table (source of the async table updates)
-  uint32_t* h_flags = nullptr;    // pinned: per-slot exactness flags, copied back behind each view's preparation kernel
-  std::vector<cudaEvent_t> view_ev;   // per slot: recorded on up_stream when the view is complete on the device
-  cudaEvent_t ev_alloc = nullptr;     // search stream -> upload stream: the view buffers of the current job are allocated
+  PinnedBuffer<char> stg[NSTG]; Event stg_ev[NSTG];
+  PinnedBuffer<ViewDev> h_views;  // pinned mirror of the device view table (source of the async table updates)
+  PinnedBuffer<uint32_t> h_flags; // pinned: per-slot exactness flags, copied back behind each view's preparation kernel
+  std::vector<Event> view_ev;     // per slot: recorded on up_stream when the view is complete on the device
+  Event ev_alloc;                 // search stream -> upload stream: the view buffers of the current job are allocated
   // uploader thread (one job at a time, FIFO)
   std::thread up_thread; std::mutex up_mu; std::condition_variable up_cv;
   std::deque<UploadJob> up_jobs; bool up_quit = false; int up_active = 0;
@@ -283,11 +287,11 @@ struct b200m_ctx {
   int up_rc = 0; std::string up_err;
   // the entry points that touch views, batch buffers or the stream serialise on this lock: one context may be shared by
   // several host threads (e.g. IRegionsMatcher adaptors created from an OpenMP region); calls simply queue up
-  std::recursive_mutex api_mu;
-  unsigned int* d_err = nullptr;
-  long long* d_trace = nullptr;   // optional pipeline trace of CTA 0 (debug)
-  std::vector<cudaEvent_t> tev;   // search-kernel timing events, reused across calls
-  cudaEvent_t ev_start = nullptr, ev_end = nullptr;
+  mutable std::recursive_mutex api_mu;
+  DeviceBuffer<unsigned> d_err;
+  DeviceBuffer<long long> d_trace;  // optional pipeline trace of CTA 0 (debug)
+  std::vector<Event> tev;         // search-kernel timing events, reused across calls
+  Event ev_start, ev_end;
   std::unique_ptr<Pool> pool;
   CpuSet cpus;                    // CPUs of the GPU's NUMA node (pool, uploader thread); empty = not pinned
   bool u8_staging = true;         // stage integer-valued fp32 descriptors as uchar (B200M_U8_STAGING=0 disables)
@@ -300,10 +304,7 @@ struct b200m_ctx {
   int tc_variant = 4;             // tensor-core kernel (l2_tc.cuh): 4 (default) = half-norms folded into the GEMM (AUG), 256-query work items;
                                   // half-norms added in the epilogue: 2 = 256-query items, 3 = 128-query items, 1 = 128-query items and
                                   // the stand-alone exactness pass (2-4 re-score in the kernel when the database images are long)
-  // last-call instrumentation
-  double last_gpu_ms = 0, last_search_ms = 0; int last_launches = 0, last_tc_pairs = 0; int64_t last_records = 0;
-  int last_real_pairs = 0; int64_t last_fallback_rows = 0;      // real-valued pairs on the tensor-core filter kernel; queries left to the exact_rows fallback
-  int last_u8_pairs = 0;          // the tensor-core pairs (last_tc_pairs) that ran the u8 kernel
+  LastCall last{};
   unsigned err_total = 0;
 };
 
@@ -355,6 +356,23 @@ static void free_view_buffers(b200m_ctx* c, ViewHost& v) {
   v.arena = nullptr; v.raw_own = nullptr; v.d_geom = nullptr;
   v.raw = nullptr; v.h16 = nullptr; v.nbh = nullptr; v.nrm = nullptr; v.aug16 = nullptr; v.d_xy = nullptr; v.d_yrank = nullptr;
   v.augq16 = nullptr; v.err = nullptr; v.stats = nullptr; v.nb32 = nullptr;
+}
+
+// The shutdown that has to stay in this order; the owners among the members release the rest.  Also runs on the partly built
+// context of a failed b200m_ctx_create (no uploader thread, no pool, streams missing).
+b200m_ctx::~b200m_ctx() {
+  {
+    std::unique_lock<std::mutex> l(up_mu);
+    up_cv.wait(l, [this] { return up_active == 0; });
+    up_quit = true;
+  }
+  up_cv.notify_all();
+  if (up_thread.joinable()) up_thread.join();
+  if (pool) pool->wait();
+  if (up_stream) cudaStreamSynchronize(up_stream);
+  if (stream) cudaStreamSynchronize(stream);
+  for (auto& v : views) free_view_buffers(this, v);      // stream-ordered
+  if (stream) cudaStreamSynchronize(stream);
 }
 
 static int make_view_dev(b200m_ctx* c, const ViewHost& v, ViewDev& d) {
@@ -423,56 +441,44 @@ static int ensure_view_capacity(b200m_ctx* c, int need) {
   if (need <= c->view_cap) return B200M_OK;
   int cap = std::max(256, c->view_cap * 2);
   while (cap < need) cap *= 2;
-  ViewDev* nv = nullptr; uint32_t* nf = nullptr; ViewDev* nh = nullptr; uint32_t* nhf = nullptr;
+  DeviceBuffer<ViewDev> nv; DeviceBuffer<uint32_t> nf; PinnedBuffer<ViewDev> nh; PinnedBuffer<uint32_t> nhf;
+  int rc;
   CK(cudaStreamSynchronize(c->stream));
   CK(cudaStreamSynchronize(c->up_stream));
-  CK(cudaMallocHost((void**)&nh, sizeof(ViewDev) * cap));
-  if (c->h_views) { std::memcpy(nh, c->h_views, sizeof(ViewDev) * c->view_cap); cudaFreeHost(c->h_views); }
-  c->h_views = nh;
-  CK(cudaMallocHost((void**)&nhf, sizeof(uint32_t) * cap));
+  if ((rc = nh.reserve(sizeof(ViewDev) * cap)) || (rc = nhf.reserve(sizeof(uint32_t) * cap)) || (rc = nv.reserve(sizeof(ViewDev) * cap)) ||
+      (rc = nf.reserve(sizeof(uint32_t) * cap)))
+    return rc;
   std::memset(nhf, 0, sizeof(uint32_t) * cap);
-  if (c->h_flags) { std::memcpy(nhf, c->h_flags, sizeof(uint32_t) * c->view_cap); cudaFreeHost(c->h_flags); }
-  c->h_flags = nhf;
-  c->view_ev.resize(cap, nullptr);
-  CK(cudaMalloc((void**)&nv, sizeof(ViewDev) * cap));
-  CK(cudaMalloc((void**)&nf, sizeof(uint32_t) * cap));
   CK(cudaMemset(nf, 0, sizeof(uint32_t) * cap));
-  if (c->d_views) {
+  if (c->view_cap) {
+    std::memcpy(nh, c->h_views, sizeof(ViewDev) * c->view_cap);
+    std::memcpy(nhf, c->h_flags, sizeof(uint32_t) * c->view_cap);
     CK(cudaMemcpy(nv, c->d_views, sizeof(ViewDev) * c->view_cap, cudaMemcpyDeviceToDevice));
     CK(cudaMemcpy(nf, c->d_flags, sizeof(uint32_t) * c->view_cap, cudaMemcpyDeviceToDevice));
-    cudaFree(c->d_views); cudaFree(c->d_flags);
   }
-  c->d_views = nv; c->d_flags = nf; c->view_cap = cap;
+  c->h_views = std::move(nh); c->h_flags = std::move(nhf); c->d_views = std::move(nv); c->d_flags = std::move(nf);   // the old tables go with the locals
+  c->view_ev.resize(cap);
+  c->view_cap = cap;
   return B200M_OK;
 }
 
 static int ensure_batch_buffers(b200m_ctx* c) {
   if (c->bufs_ready) return B200M_OK;
-  for (int s = 0; s < 2; ++s) {
-    BatchBuf& b = c->buf[s];
-    CK(cudaMalloc((void**)&b.d_pairs, sizeof(PairDev) * PAIR_CAP));
-    CK(cudaMalloc((void**)&b.d_items, sizeof(WorkItem) * ITEM_CAP));
-    CK(cudaMalloc((void**)&b.d_cands, sizeof(Cand) * CAND_CAP));
-    CK(cudaMalloc((void**)&b.d_count, sizeof(int) * PAIR_CAP));
-    CK(cudaMalloc((void**)&b.d_off, sizeof(int) * (PAIR_CAP + 1)));
-    CK(cudaMalloc((void**)&b.d_out, sizeof(Rec) * CAND_CAP));
-    CK(cudaMalloc((void**)&b.d_fin, sizeof(FinMatch) * CAND_CAP));
-    CK(cudaMalloc((void**)&b.d_fin_count, sizeof(int) * PAIR_CAP));
-    CK(cudaMalloc((void**)&b.d_scratch, sizeof(uint32_t) * 2 * SLOT_CAP));
-    CK(cudaMalloc((void**)&b.d_items_real, sizeof(WorkItem) * ITEM_CAP));
-    CK(cudaMalloc((void**)&b.d_candx, sizeof(uint32_t) * CAND_CAP));
-    CK(cudaMalloc((void**)&b.d_fb, sizeof(uint4) * CAND_CAP));
-    CK(cudaMalloc((void**)&b.d_fb_count, 2 * sizeof(int)));
-    CK(cudaMalloc((void**)&b.d_fb_pair, sizeof(uint4) * (size_t)PAIR_CAP * FB_PER_PAIR));
-    CK(cudaMalloc((void**)&b.d_fb_pair_cnt, sizeof(int) * PAIR_CAP));
-    CK(cudaMallocHost((void**)&b.h_items_real, sizeof(WorkItem) * ITEM_CAP));
-    CK(cudaMallocHost((void**)&b.h_pairs, sizeof(PairDev) * PAIR_CAP));
-    CK(cudaMallocHost((void**)&b.h_items, sizeof(WorkItem) * ITEM_CAP));
-    CK(cudaMallocHost((void**)&b.h_meta, sizeof(int) * META_INTS));
-    CK(cudaMallocHost((void**)&b.h_out, sizeof(Rec) * CAND_CAP));
-    CK(cudaEventCreateWithFlags(&b.ev_meta, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&b.ev_copy, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&b.ev_tab, cudaEventDisableTiming));
+  for (BatchBuf& b : c->buf) {
+    int rc;
+    if ((rc = b.d_pairs.reserve(sizeof(PairDev) * PAIR_CAP)) || (rc = b.d_items.reserve(sizeof(WorkItem) * ITEM_CAP)) ||
+        (rc = b.d_cands.reserve(sizeof(Cand) * CAND_CAP)) || (rc = b.d_count.reserve(sizeof(int) * PAIR_CAP)) ||
+        (rc = b.d_off.reserve(sizeof(int) * (PAIR_CAP + 1))) || (rc = b.d_out.reserve(sizeof(Rec) * CAND_CAP)) ||
+        (rc = b.d_fin.reserve(sizeof(FinMatch) * CAND_CAP)) || (rc = b.d_fin_count.reserve(sizeof(int) * PAIR_CAP)) ||
+        (rc = b.d_scratch.reserve(sizeof(uint32_t) * 2 * SLOT_CAP)) || (rc = b.d_items_real.reserve(sizeof(WorkItem) * ITEM_CAP)) ||
+        (rc = b.d_candx.reserve(sizeof(uint32_t) * CAND_CAP)) || (rc = b.d_fb.reserve(sizeof(uint4) * CAND_CAP)) ||
+        (rc = b.d_fb_count.reserve(2 * sizeof(int))) || (rc = b.d_fb_pair.reserve(sizeof(uint4) * (size_t)PAIR_CAP * FB_PER_PAIR)) ||
+        (rc = b.d_fb_pair_cnt.reserve(sizeof(int) * PAIR_CAP)) || (rc = b.h_items_real.reserve(sizeof(WorkItem) * ITEM_CAP)) ||
+        (rc = b.h_pairs.reserve(sizeof(PairDev) * PAIR_CAP)) || (rc = b.h_items.reserve(sizeof(WorkItem) * ITEM_CAP)) ||
+        (rc = b.h_meta.reserve(sizeof(int) * META_INTS)) || (rc = b.h_out.reserve(sizeof(Rec) * CAND_CAP)) ||
+        (rc = b.ev_meta.create(cudaEventDisableTiming)) || (rc = b.ev_copy.create(cudaEventDisableTiming)) ||
+        (rc = b.ev_tab.create(cudaEventDisableTiming)))
+      return rc;
   }
   CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<false>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true>::SMEM_BYTES));
@@ -489,7 +495,7 @@ static int ensure_batch_buffers(b200m_ctx* c) {
 }
 
 static cudaEvent_t timing_event(b200m_ctx* c, size_t& used) {
-  if (used == c->tev.size()) { cudaEvent_t e; cudaEventCreate(&e); c->tev.push_back(e); }
+  if (used == c->tev.size()) { c->tev.emplace_back(); c->tev.back().create(); }   // a failed creation shows in the cudaEventRecord that follows
   return c->tev[used++];
 }
 
@@ -573,14 +579,13 @@ int b200m_ctx_create(int device, void* stream, b200m_ctx** out) {
   if (prop.major != 9 || prop.minor != 0) return fail(B200M_ERR_UNSUPPORTED, "this build contains sm_90a code only (found sm_" + std::to_string(prop.major * 10 + prop.minor) + ")");
   std::unique_ptr<b200m_ctx> c(new b200m_ctx());
   c->device = device; c->num_sms = prop.multiProcessorCount;
-  if (stream) { c->stream = (cudaStream_t)stream; }
-  else { CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking)); c->own_stream = true; }
-  CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&c->up_stream, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&c->tab_stream, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&c->pack_stream, cudaStreamNonBlocking));
+  int rc;
+  if (stream) c->stream.borrow((cudaStream_t)stream);
+  else if ((rc = c->stream.create())) return rc;
+  if ((rc = c->copy_stream.create()) || (rc = c->up_stream.create()) || (rc = c->tab_stream.create()) || (rc = c->pack_stream.create()) ||
+      (rc = c->ev_alloc.create(cudaEventDisableTiming)))
+    return rc;
   if (const char* e = getenv("B200M_PIPE_STREAMS")) c->pipe_streams = atoi(e) != 0;
-  CK(cudaEventCreateWithFlags(&c->ev_alloc, cudaEventDisableTiming));
   cudaDriverEntryPointQueryResult qres;
   void* fn = nullptr;
   CK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
@@ -590,10 +595,9 @@ int b200m_ctx_create(int device, void* stream, b200m_ctx** out) {
   CK(cudaDeviceGetDefaultMemPool(&mp, device));
   uint64_t thr = ~0ull;
   CK(cudaMemPoolSetAttribute(mp, cudaMemPoolAttrReleaseThreshold, &thr));
-  CK(cudaMalloc((void**)&c->d_err, sizeof(unsigned int)));
+  if ((rc = c->d_err.reserve(sizeof(unsigned int)))) return rc;
   CK(cudaMemset(c->d_err, 0, sizeof(unsigned int)));
-  CK(cudaEventCreate(&c->ev_start));
-  CK(cudaEventCreate(&c->ev_end));
+  if ((rc = c->ev_start.create()) || (rc = c->ev_end.create())) return rc;
   c->cpus = numa_cpus_of_device(device);
   int ht = c->cpus.count > 0 ? c->cpus.count : (int)std::thread::hardware_concurrency();
   if (const char* e = getenv("B200M_HOST_THREADS")) ht = std::max(1, atoi(e));     // several engine processes sharing one host (one per GPU)
@@ -611,57 +615,6 @@ int b200m_ctx_create(int device, void* stream, b200m_ctx** out) {
 void b200m_ctx_destroy(b200m_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
-  {
-    std::unique_lock<std::mutex> l(c->up_mu);
-    c->up_cv.wait(l, [c] { return c->up_active == 0; });
-    c->up_quit = true;
-  }
-  c->up_cv.notify_all();
-  if (c->up_thread.joinable()) c->up_thread.join();
-  c->pool->wait();
-  cudaStreamSynchronize(c->up_stream);
-  cudaStreamSynchronize(c->stream);
-  for (auto& v : c->views) free_view_buffers(c, v);
-  cudaStreamSynchronize(c->stream);
-  for (int s = 0; s < 2; ++s) {
-    BatchBuf& b = c->buf[s];
-    cudaFree(b.d_pairs); cudaFree(b.d_items); cudaFree(b.d_cands); cudaFree(b.d_count); cudaFree(b.d_off); cudaFree(b.d_out);
-    cudaFree(b.d_fin); cudaFree(b.d_fin_count); cudaFree(b.d_scratch);
-    cudaFree(b.d_items_real); cudaFree(b.d_candx); cudaFree(b.d_fb); cudaFree(b.d_fb_count); cudaFreeHost(b.h_items_real);
-    cudaFree(b.d_fb_pair); cudaFree(b.d_fb_pair_cnt);
-    cudaFreeHost(b.h_pairs); cudaFreeHost(b.h_items); cudaFreeHost(b.h_meta); cudaFreeHost(b.h_out);
-    if (b.ev_meta) cudaEventDestroy(b.ev_meta);
-    if (b.ev_copy) cudaEventDestroy(b.ev_copy);
-    if (b.ev_tab) cudaEventDestroy(b.ev_tab);
-  }
-  for (auto& e : c->tev) cudaEventDestroy(e);
-  for (int k = 0; k < b200m_ctx::NSTG; ++k) { if (c->stg[k]) cudaFreeHost(c->stg[k]); if (c->stg_ev[k]) cudaEventDestroy(c->stg_ev[k]); }
-  if (c->h_views) cudaFreeHost(c->h_views);
-  if (c->h_flags) cudaFreeHost(c->h_flags);
-  for (auto& e : c->view_ev) if (e) cudaEventDestroy(e);
-  cudaEventDestroy(c->ev_alloc);
-  cudaStreamDestroy(c->up_stream);
-  cudaStreamDestroy(c->tab_stream); cudaStreamDestroy(c->pack_stream);
-  if (c->d_trace) cudaFree(c->d_trace);
-  if (c->acr.d) cudaFree(c->acr.d);
-  if (c->acr.ev0) { cudaEventDestroy(c->acr.ev0); cudaEventDestroy(c->acr.ev1); }
-  cudaFree(c->d_views); cudaFree(c->d_flags); cudaFree(c->d_err);
-  {
-    KnnScratch& k = c->knn;
-    for (void* q : {(void*)k.raw, (void*)k.h16, (void*)k.nbh, (void*)k.nrm, (void*)k.aug16, (void*)k.augq16, (void*)k.err, (void*)k.cands, (void*)k.idx, (void*)k.dist, (void*)k.items, (void*)k.small}) if (q) cudaFree(q);
-  }
-  {
-    GuidedFastScratch& g = c->gf;
-    for (auto& b : g.d) if (b.p) cudaFree(b.p);
-    if (g.h_pairs) cudaFreeHost(g.h_pairs);
-    if (g.h_out) cudaFreeHost(g.h_out);
-    if (g.h_meta) cudaFreeHost(g.h_meta);
-    if (g.ev_c0) cudaEventDestroy(g.ev_c0);
-    if (g.ev_c1) cudaEventDestroy(g.ev_c1);
-  }
-  cudaEventDestroy(c->ev_start); cudaEventDestroy(c->ev_end);
-  cudaStreamDestroy(c->copy_stream);
-  if (c->own_stream) cudaStreamDestroy(c->stream);
   delete c;
 }
 
@@ -682,9 +635,9 @@ int b200m_debug_trace(b200m_ctx* c, int enable, long long* out, int n) {
   if (!c) return fail(B200M_ERR_ARG, "ctx is null");
   CK(cudaSetDevice(c->device));
   const size_t total = 4ull * ptx::TRACE_TILES * 4;
-  if (enable && !c->d_trace) { CK(cudaMalloc((void**)&c->d_trace, total * 8)); CK(cudaMemset(c->d_trace, 0, total * 8)); }
+  if (enable && !c->d_trace) { if (int rc = c->d_trace.reserve(total * 8)) return rc; CK(cudaMemset(c->d_trace, 0, total * 8)); }
   if (out && c->d_trace) { CK(cudaStreamSynchronize(c->stream)); CK(cudaMemcpy(out, c->d_trace, std::min<size_t>(total, (size_t)n) * 8, cudaMemcpyDeviceToHost)); }
-  if (!enable && c->d_trace) { cudaFree(c->d_trace); c->d_trace = nullptr; }
+  if (!enable) c->d_trace = DeviceBuffer<long long>();
   return B200M_OK;
 }
 // Debug / test hook (host only, no GPU needed): the checked fp32 -> uchar conversion of the staging path (hostconv.hpp).
@@ -741,11 +694,10 @@ static int run_upload(b200m_ctx* c, const UploadJob& job) {
     }
   }
   for (int k = 0; k < b200m_ctx::NSTG; ++k) {
-    if (c->stg_bytes[k] < CH) {
-      if (c->stg[k]) { CK(cudaEventSynchronize(c->stg_ev[k])); CK(cudaFreeHost(c->stg[k])); c->stg[k] = nullptr; }
-      CK(cudaMallocHost(&c->stg[k], CH)); c->stg_bytes[k] = CH;
-    }
-    if (!c->stg_ev[k]) CK(cudaEventCreateWithFlags(&c->stg_ev[k], cudaEventDisableTiming));
+    int rc;
+    if ((rc = c->stg_ev[k].create(cudaEventDisableTiming))) return rc;
+    if (c->stg[k].capacity() < CH) CK(cudaEventSynchronize(c->stg_ev[k]));   // the last H2D out of the buffer that is replaced is done
+    if ((rc = c->stg[k].reserve(CH))) return rc;
   }
   std::vector<int>& bad = *job.bad;
   double t_ring = 0, t_task = 0, t_fin = 0;                // B200M_TIMING: where the issuing thread waits
@@ -950,7 +902,7 @@ int b200m_upload_views_async(b200m_ctx* c, int n_views, const uint32_t* view_ids
       v.stored_u8 = f32_to_u8_checked((const float*)descs[i], tmp, (size_t)std::min(n, 4) * 128);
     }
     if (n > 0 && (rc = alloc_view_buffers(c, v))) return rc;
-    if (!c->view_ev[slot]) CK(cudaEventCreateWithFlags(&c->view_ev[slot], cudaEventDisableTiming));
+    if ((rc = c->view_ev[slot].create(cudaEventDisableTiming))) return rc;
   }
   // device view table (tensor maps are encoded on the host from the device addresses; valid whatever the upload state)
   for (int i = 0; i < n_views; ++i) {
@@ -1226,7 +1178,7 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
     cudaEvent_t k0 = timing_event(c, tev_used), k1 = timing_event(c, tev_used);
     CK(cudaEventRecord(k0, c->stream));
     // the debug trace (one kernel's CTA 0) shows the u8 kernel when the batch has u8 pairs, else the fp16 kernel
-    long long* fp16_trace = n_items_u8 ? nullptr : c->d_trace;
+    long long* fp16_trace = n_items_u8 ? nullptr : (long long*)c->d_trace;
     if (n_items) {
       const int grid = tc_ctas_per_item * std::min(n_items, c->num_sms / tc_ctas_per_item);   // one CTA per SM, whole work items per CTA group
       if (c->tc_variant == 4)
@@ -1386,7 +1338,6 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
   float ms = 0.f;
   CK(cudaEventSynchronize(c->ev_end));
   CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
-  c->last_gpu_ms = ms;
   double sk = 0;
   for (auto& e : kernel_events) { float t = 0.f; CK(cudaEventElapsedTime(&t, e.first, e.second)); sk += t; }
   if (timing && !kernel_events.empty()) {
@@ -1399,8 +1350,6 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
     fprintf(stderr, "[b200m] device timeline: %zu batches, search kernels %.2f ms, lead-in %.2f, gaps between batches %.2f (max %.2f), tail after the last search kernel %.2f ms\n",
             kernel_events.size(), sk, lead, gaps, gmax, tail);
   }
-  c->last_search_ms = sk; c->last_launches = launches; c->last_tc_pairs = tc_pairs; c->last_records = total_records;
-  c->last_real_pairs = real_pairs; c->last_fallback_rows = fallback_rows; c->last_u8_pairs = u8_pairs;
   unsigned errs = 0;
   CK(cudaMemcpy(&errs, c->d_err, sizeof(unsigned), cudaMemcpyDeviceToHost));
   c->err_total = errs;
@@ -1451,7 +1400,8 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
     g.wait();
   }
   if (timing) fprintf(stderr, "[b200m] match_pairs n=%d stage=%d: setup %.2f ms, batches %.2f ms (gpu %.2f), tail (cross+assemble) %.2f ms, total %.2f ms\n",
-                      n_pairs, stage, t_setup - t_begin, t_gpu_done - t_setup, c->last_gpu_ms, now() - t_gpu_done, now() - t_begin);
+                      n_pairs, stage, t_setup - t_begin, t_gpu_done - t_setup, ms, now() - t_gpu_done, now() - t_begin);
+  c->last = LastCall{ms, sk, launches, tc_pairs, real_pairs, u8_pairs, total_records, fallback_rows};
   *out = res.release();
   return B200M_OK;
 }
@@ -1466,15 +1416,20 @@ int b200m_result_get(const b200m_result* r, const uint32_t** pair_ids, const int
 }
 void b200m_result_free(b200m_result* r) { delete r; }
 
-double b200m_last_gpu_ms(const b200m_ctx* c) { return c ? c->last_gpu_ms : 0; }
-double b200m_last_search_kernel_ms(const b200m_ctx* c) { return c ? c->last_search_ms : 0; }
-int b200m_last_launches(const b200m_ctx* c) { return c ? c->last_launches : 0; }
-int b200m_last_tc_pairs(const b200m_ctx* c) { return c ? c->last_tc_pairs : 0; }
+static LastCall last_call(const b200m_ctx* c) {       // a concurrent call rewrites the record
+  if (!c) return LastCall{};
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  return c->last;
+}
+double b200m_last_gpu_ms(const b200m_ctx* c) { return last_call(c).gpu_ms; }
+double b200m_last_search_kernel_ms(const b200m_ctx* c) { return last_call(c).search_ms; }
+int b200m_last_launches(const b200m_ctx* c) { return last_call(c).launches; }
+int b200m_last_tc_pairs(const b200m_ctx* c) { return last_call(c).tc_pairs; }
 unsigned b200m_exactness_errors(const b200m_ctx* c) { return c ? c->err_total : 0; }
-int64_t b200m_last_records(const b200m_ctx* c) { return c ? c->last_records : 0; }
-int b200m_last_real_tc_pairs(const b200m_ctx* c) { return c ? c->last_real_pairs : 0; }
-int b200m_last_u8_tc_pairs(const b200m_ctx* c) { return c ? c->last_u8_pairs : 0; }
-int64_t b200m_last_fallback_rows(const b200m_ctx* c) { return c ? c->last_fallback_rows : 0; }
+int64_t b200m_last_records(const b200m_ctx* c) { return last_call(c).records; }
+int b200m_last_real_tc_pairs(const b200m_ctx* c) { return last_call(c).real_pairs; }
+int b200m_last_u8_tc_pairs(const b200m_ctx* c) { return last_call(c).u8_pairs; }
+int64_t b200m_last_fallback_rows(const b200m_ctx* c) { return last_call(c).fallback_rows; }
 
 // ---- guided matching (after the path: GeometricFilterMatrix_F_AC.hpp:363-390 -> matching/guidedMatching.hpp:206-268) ----------------
 int b200m_guided_match(b200m_ctx* c, uint32_t view_left, uint32_t view_right, const double* F, double errorTh, double distRatio, b200m_result** out) {
@@ -1554,7 +1509,7 @@ int b200m_guided_match_model(b200m_ctx* c, uint32_t view_left, uint32_t view_rig
     if (n) CK(cudaMemcpy(recs.data(), d_out, sizeof(Rec) * (size_t)n, cudaMemcpyDeviceToHost));
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
-    c->last_gpu_ms = ms; c->last_search_ms = ms; c->last_launches = 3; c->last_records = n; c->last_tc_pairs = 0; c->last_u8_pairs = 0;
+    c->last = LastCall{ms, ms, 3, 0, 0, 0, n, 0};
     cudaFreeAsync(d_xy, st); cudaFreeAsync(d_xl, st); cudaFreeAsync(d_xr, st); cudaFreeAsync(d_out, st); cudaFreeAsync(d_cnt, st);
     // IndMatch::getDeduplicated (guidedMatching.hpp:267): one record per left feature, so this is a sort by (i, j)
     std::sort(recs.begin(), recs.end(), [](const Rec& a, const Rec& b) { return a.i < b.i || (a.i == b.i && a.j < b.j); });
@@ -1563,6 +1518,7 @@ int b200m_guided_match_model(b200m_ctx* c, uint32_t view_left, uint32_t view_rig
     res->offsets[1] = n;
   } else {
     res->matches = c->recycler->take(1);
+    c->last = LastCall{};
   }
   *out = res.release();
   return B200M_OK;
@@ -1587,34 +1543,11 @@ int b200m_set_view_geometry(b200m_ctx* c, uint32_t view_id, const double* xy, in
 }  // extern "C"
 
 // ---- guided matching from known poses: guidedMatchingFundamentalFast for a list of pairs (guided_fast.cuh) -------------------
-template <class T> static int gf_reserve(GuidedFastScratch& g, int which, size_t count, T** p) {
-  GuidedFastScratch::Buf& b = g.d[which];
-  const size_t bytes = std::max<size_t>(count * sizeof(T), 256);
-  if (b.bytes < bytes) {
-    if (b.p) CK(cudaFree(b.p));      // cudaFree synchronises: nothing enqueued still uses the old buffer
-    b.p = nullptr; b.bytes = 0;
-    const size_t nb = bytes + bytes / 4;
-    CK(cudaMalloc(&b.p, nb));
-    b.bytes = nb;
-  }
-  *p = static_cast<T*>(b.p);
-  return B200M_OK;
-}
-static int gf_reserve_host(void*& p, size_t& have, size_t bytes) {
-  if (have >= bytes) return B200M_OK;
-  if (p) CK(cudaFreeHost(p));
-  p = nullptr; have = 0;
-  const size_t nb = std::max<size_t>(bytes + bytes / 4, 4096);
-  CK(cudaMallocHost(&p, nb));
-  have = nb;
-  return B200M_OK;
-}
-
 template <class T> static int gf_exclusive_scan(b200m_ctx* c, const T* in, T* out, size_t n, cudaStream_t st, int& launches) {
   size_t tb = 0;
   CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, (int64_t)n, st));
-  void* tmp = nullptr;
-  if (int rc = gf_reserve(c->gf, GuidedFastScratch::TEMP, tb, (char**)&tmp)) return rc;
+  DeviceBuffer<>& tmp = c->gf.d[GuidedFastScratch::TEMP];
+  if (int rc = tmp.reserve(tb)) return rc;
   CK(cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, (int64_t)n, st));
   launches += 2;
   return B200M_OK;
@@ -1638,11 +1571,11 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
       const int s = c->views[p.slot_l].stored_u8 ? p.slot_l : p.slot_r;
       if (!exp_off.count(s)) { exp_off[s] = exp_elems; exp_elems += (size_t)c->views[s].m * 128; }
     }
+  using G = GuidedFastScratch;
   int rc;
-  if ((rc = gf_reserve_host(g.h_pairs, g.h_pairs_bytes, sizeof(FastPair) * (size_t)np))) return rc;
-  FastPair* hp = static_cast<FastPair*>(g.h_pairs);
-  float* d_exp = nullptr;
-  if (exp_elems && (rc = gf_reserve(g, GuidedFastScratch::EXPAND, exp_elems, &d_exp))) return rc;
+  if ((rc = g.h_pairs.reserve(sizeof(FastPair) * (size_t)np)) || (rc = g.d[G::EXPAND].reserve(sizeof(float) * exp_elems))) return rc;
+  FastPair* hp = g.h_pairs;
+  float* d_exp = g.d[G::EXPAND].as<float>();
   long sum_l = 0, sum_r = 0, sum_b = 0; int max_l = 0, max_r = 0;
   for (int k = 0; k < np; ++k) {
     const GfPairHost& q = batch[k];
@@ -1665,22 +1598,25 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
     sum_l += vl.m; sum_r += vr.m; sum_b += P.nb + 1;
     max_l = std::max(max_l, vl.m); max_r = std::max(max_r, vr.m);
   }
-  FastPair* d_pairs; int *d_lbucket, *d_bcount, *d_boff, *d_csr, *d_rstart, *d_rpair, *d_keep, *d_kpos, *d_pstart;
-  unsigned long long *d_best, *d_second, *d_rcount, *d_rcoff; uint2* d_out;
-  if ((rc = gf_reserve(g, GuidedFastScratch::PAIRS, np, &d_pairs)) || (rc = gf_reserve(g, GuidedFastScratch::LBUCKET, sum_l, &d_lbucket)) ||
-      (rc = gf_reserve(g, GuidedFastScratch::BEST, sum_l, &d_best)) || (rc = gf_reserve(g, GuidedFastScratch::SECOND, sum_l, &d_second)) ||
-      (rc = gf_reserve(g, GuidedFastScratch::BCOUNT, sum_b, &d_bcount)) || (rc = gf_reserve(g, GuidedFastScratch::BOFF, sum_b, &d_boff)) ||
-      (rc = gf_reserve(g, GuidedFastScratch::CSR, sum_l, &d_csr)) || (rc = gf_reserve(g, GuidedFastScratch::RSTART, sum_r, &d_rstart)) ||
-      (rc = gf_reserve(g, GuidedFastScratch::RCOUNT, sum_r + 1, &d_rcount)) || (rc = gf_reserve(g, GuidedFastScratch::RCOFF, sum_r + 1, &d_rcoff)) ||
-      (rc = gf_reserve(g, GuidedFastScratch::RPAIR, sum_r, &d_rpair)) || (rc = gf_reserve(g, GuidedFastScratch::KEEP, sum_l + 1, &d_keep)) ||
-      (rc = gf_reserve(g, GuidedFastScratch::KPOS, sum_l + 1, &d_kpos)) || (rc = gf_reserve(g, GuidedFastScratch::OUT, sum_l, &d_out)) ||
-      (rc = gf_reserve(g, GuidedFastScratch::PSTART, np + 1, &d_pstart)))
+  const size_t i4 = sizeof(int), u8 = sizeof(unsigned long long);
+  if ((rc = g.d[G::PAIRS].reserve(sizeof(FastPair) * np)) || (rc = g.d[G::LBUCKET].reserve(i4 * sum_l)) || (rc = g.d[G::BEST].reserve(u8 * sum_l)) ||
+      (rc = g.d[G::SECOND].reserve(u8 * sum_l)) || (rc = g.d[G::BCOUNT].reserve(i4 * sum_b)) || (rc = g.d[G::BOFF].reserve(i4 * sum_b)) ||
+      (rc = g.d[G::CSR].reserve(i4 * sum_l)) || (rc = g.d[G::RSTART].reserve(i4 * sum_r)) || (rc = g.d[G::RCOUNT].reserve(u8 * (sum_r + 1))) ||
+      (rc = g.d[G::RCOFF].reserve(u8 * (sum_r + 1))) || (rc = g.d[G::RPAIR].reserve(i4 * sum_r)) || (rc = g.d[G::KEEP].reserve(i4 * (sum_l + 1))) ||
+      (rc = g.d[G::KPOS].reserve(i4 * (sum_l + 1))) || (rc = g.d[G::OUT].reserve(sizeof(uint2) * sum_l)) || (rc = g.d[G::PSTART].reserve(i4 * (np + 1))))
     return rc;
+  FastPair* d_pairs = g.d[G::PAIRS].as<FastPair>();
+  int *d_lbucket = g.d[G::LBUCKET].as<int>(), *d_bcount = g.d[G::BCOUNT].as<int>(), *d_boff = g.d[G::BOFF].as<int>(), *d_csr = g.d[G::CSR].as<int>(),
+      *d_rstart = g.d[G::RSTART].as<int>(), *d_rpair = g.d[G::RPAIR].as<int>(), *d_keep = g.d[G::KEEP].as<int>(), *d_kpos = g.d[G::KPOS].as<int>(),
+      *d_pstart = g.d[G::PSTART].as<int>();
+  unsigned long long *d_best = g.d[G::BEST].as<unsigned long long>(), *d_second = g.d[G::SECOND].as<unsigned long long>(),
+                     *d_rcount = g.d[G::RCOUNT].as<unsigned long long>(), *d_rcoff = g.d[G::RCOFF].as<unsigned long long>();
+  uint2* d_out = g.d[G::OUT].as<uint2>();
   // the temporary storage of the three scans is taken inside gf_exclusive_scan; reserve it for the largest one first so that
   // no reallocation (a synchronising cudaFree) happens between launches
   { size_t tb = 0; CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_rcount, d_rcoff, (int64_t)std::max(sum_r + 1, std::max(sum_b, sum_l + 1)), st));
-    char* t; if ((rc = gf_reserve(g, GuidedFastScratch::TEMP, tb, &t))) return rc; }
-  if (!g.ev_c0) { CK(cudaEventCreate(&g.ev_c0)); CK(cudaEventCreate(&g.ev_c1)); }
+    if ((rc = g.d[G::TEMP].reserve(tb))) return rc; }
+  if ((rc = g.ev_c0.create()) || (rc = g.ev_c1.create())) return rc;
   CK(cudaEventRecord(c->ev_start, st));
   CK(cudaMemcpyAsync(d_pairs, hp, sizeof(FastPair) * (size_t)np, cudaMemcpyHostToDevice, st));
   for (const auto& x : exp_off) {
@@ -1712,8 +1648,8 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
   launches += 5;
   CK(cudaEventRecord(c->ev_end, st));
   // read-back: the candidate total + per-pair starts, then the matches
-  if ((rc = gf_reserve_host(g.h_meta, g.h_meta_bytes, sizeof(unsigned long long) + sizeof(int) * (size_t)(np + 1)))) return rc;
-  unsigned long long* h_total = static_cast<unsigned long long*>(g.h_meta);
+  if ((rc = g.h_meta.reserve(sizeof(unsigned long long) + sizeof(int) * (size_t)(np + 1)))) return rc;
+  unsigned long long* h_total = g.h_meta.as<unsigned long long>();
   int* h_pstart = reinterpret_cast<int*>(h_total + 1);
   CK(cudaMemcpyAsync(h_pstart, d_pstart, sizeof(int) * (size_t)(np + 1), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(h_total, d_rcoff + sum_r, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
@@ -1726,10 +1662,10 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
   CK(cudaEventElapsedTime(&cms, g.ev_c0, g.ev_c1));
   gpu_ms += ms; cand_ms += cms;
   if (n_out > 0) {
-    if ((rc = gf_reserve_host(g.h_out, g.h_out_bytes, sizeof(uint2) * (size_t)n_out))) return rc;
+    if ((rc = g.h_out.reserve(sizeof(uint2) * (size_t)n_out))) return rc;
     CK(cudaMemcpyAsync(g.h_out, d_out, sizeof(uint2) * (size_t)n_out, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    const uint2* h = static_cast<const uint2*>(g.h_out);
+    const uint2* h = g.h_out;
     for (int k = 0; k < np; ++k) per_pair[batch[k].index].assign(h + starts[k], h + starts[k + 1]);
   }
   return B200M_OK;
@@ -1796,7 +1732,7 @@ int b200m_guided_match_fast_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pai
   for (Open& o : open)
     if (int rc = flush(o)) return rc;
   if (int rc = wait_uploads(c)) return rc;
-  c->last_gpu_ms = gpu_ms; c->last_search_ms = cand_ms; c->last_launches = launches; c->last_records = cands; c->last_tc_pairs = 0; c->last_u8_pairs = 0;
+  c->last = LastCall{gpu_ms, cand_ms, launches, 0, 0, 0, cands, 0};
   // one result pair per input pair, in input order (empty lists included)
   std::unique_ptr<b200m_result> res(new b200m_result());
   res->recycler = c->recycler;
@@ -1863,14 +1799,9 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
                o_tr = take(sizeof(int32_t) * acrk::kTraceCap * n_pairs),
                o_trn = take(sizeof(double) * acrk::kTraceCap * n_pairs), o_out = take(sizeof(acrk::Out) * n_pairs),
                o_mto = take(mt_out ? sizeof(uint32_t) * 625 * n_pairs : 0);
-  if (at > c->acr.bytes) {
-    if (c->acr.d) CK(cudaFree(c->acr.d));
-    c->acr.d = nullptr; c->acr.bytes = 0;
-    CK(cudaMalloc(&c->acr.d, at));
-    c->acr.bytes = at;
-  }
-  if (!c->acr.ev0) { CK(cudaEventCreate(&c->acr.ev0)); CK(cudaEventCreate(&c->acr.ev1)); }
-  char* d = (char*)c->acr.d;
+  int rc;
+  if ((rc = c->acr.d.reserve(at)) || (rc = c->acr.ev0.create()) || (rc = c->acr.ev1.create())) return rc;
+  char* d = c->acr.d;
   cudaStream_t st = c->stream;
   CK(cudaMemcpyAsync(d + o_pairs, pairs.data(), sizeof(acrk::Pair) * n_pairs, cudaMemcpyHostToDevice, st));
   if (N) CK(cudaMemcpyAsync(d + o_corr, corr, sizeof(double) * 4 * N, cudaMemcpyHostToDevice, st));
@@ -1926,14 +1857,14 @@ int b200m_acransac_homography_pairs(b200m_ctx* c, int n_pairs, const int64_t* of
 
 double b200m_acransac_last_stats(const b200m_ctx* c, int64_t stats[4]) {
   if (!c) return 0;
-  std::lock_guard<std::recursive_mutex> api_lock(const_cast<b200m_ctx*>(c)->api_mu);   // a concurrent call rewrites them
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);   // a concurrent call rewrites them
   if (stats) for (int t = 0; t < 4; ++t) stats[t] = c->acr.stats[t];
   return c->acr.last_ms;
 }
 
 int b200m_acransac_last_trace(const b200m_ctx* c, int pair, int32_t* iters, double* nfa, int cap) {
   if (!c) return 0;
-  std::lock_guard<std::recursive_mutex> api_lock(const_cast<b200m_ctx*>(c)->api_mu);
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
   if (pair < 0 || pair >= (int)c->acr.n_trace.size()) return 0;
   const int n = c->acr.n_trace[pair];
   for (int i = 0; i < std::min({n, cap, acrk::kTraceCap}); ++i) {
@@ -2062,8 +1993,9 @@ int b200m_shard_pairs_2d(const uint32_t* pairs, int n_pairs, int n_shards, int32
 }
 
 struct b200m_multi {
-  std::vector<b200m_ctx*> ctx;
+  std::vector<b200m_ctx*> ctx;      // owned
   double last_gpu_ms_max = 0;
+  ~b200m_multi() { for (auto* c : ctx) b200m_ctx_destroy(c); }
 };
 
 int b200m_multi_create(const int* devices, int n_devices, b200m_multi** out) {
@@ -2073,7 +2005,7 @@ int b200m_multi_create(const int* devices, int n_devices, b200m_multi** out) {
   for (int d = 0; d < n_devices; ++d) {
     b200m_ctx* c = nullptr;
     const int rc = b200m_ctx_create(devices[d], nullptr, &c);
-    if (rc) { for (auto* x : m->ctx) b200m_ctx_destroy(x); return rc; }
+    if (rc) return rc;
     m->ctx.push_back(c);
   }
   // the finishing pools share the host: split the threads
@@ -2083,11 +2015,7 @@ int b200m_multi_create(const int* devices, int n_devices, b200m_multi** out) {
   return B200M_OK;
 }
 
-void b200m_multi_destroy(b200m_multi* m) {
-  if (!m) return;
-  for (auto* c : m->ctx) b200m_ctx_destroy(c);
-  delete m;
-}
+void b200m_multi_destroy(b200m_multi* m) { delete m; }
 
 int b200m_multi_num_devices(const b200m_multi* m) { return m ? (int)m->ctx.size() : 0; }
 b200m_ctx* b200m_multi_ctx(b200m_multi* m, int k) { return (m && k >= 0 && k < (int)m->ctx.size()) ? m->ctx[k] : nullptr; }
@@ -2129,7 +2057,7 @@ int b200m_multi_match(b200m_multi* m, int n_views, const uint32_t* view_ids, con
   for (auto& t : th) t.join();
   m->last_gpu_ms_max = 0;
   for (int d = 0; d < nd; ++d) {
-    m->last_gpu_ms_max = std::max(m->last_gpu_ms_max, m->ctx[d]->last_gpu_ms);
+    m->last_gpu_ms_max = std::max(m->last_gpu_ms_max, b200m_last_gpu_ms(m->ctx[d]));
     if (sh[d].rc) {
       const int code = sh[d].rc; const std::string msg = sh[d].err;
       for (auto& s : sh) if (s.res) b200m_result_free(s.res);
@@ -2224,28 +2152,18 @@ void b200m_db_destroy(b200m_db* db) {
 }
 
 // grow-only scratch of b200m_knn: the query batch as a prepared view + the small tables and outputs of one call
+// (each call ends with a synchronisation: nothing enqueued still uses a buffer that grows)
 static int ensure_knn_scratch(b200m_ctx* c, int nq, int dim, size_t esz) {
   KnnScratch& k = c->knn;
-  const size_t raw_bytes = std::max<size_t>((size_t)nq * dim * esz, 256);
-  if (nq <= k.cap && raw_bytes <= k.raw_bytes) return B200M_OK;
-  CK(cudaStreamSynchronize(c->stream));
-  const int cap = std::max(nq, k.cap * 2);
-  const int cap_pad = (cap + tc::ROW_PAD - 1) / tc::ROW_PAD * tc::ROW_PAD;
-  const size_t rb = std::max(raw_bytes, (size_t)cap * dim * esz);
-  for (void* q : {(void*)k.raw, (void*)k.h16, (void*)k.nbh, (void*)k.nrm, (void*)k.aug16, (void*)k.augq16, (void*)k.err, (void*)k.cands, (void*)k.idx, (void*)k.dist, (void*)k.items}) if (q) cudaFree(q);
-  CK(cudaMalloc(&k.raw, rb));
-  CK(cudaMalloc((void**)&k.h16, (size_t)cap_pad * 256));
-  CK(cudaMalloc((void**)&k.nbh, (size_t)cap_pad * 4));
-  CK(cudaMalloc((void**)&k.nrm, (size_t)cap_pad * 4));
-  CK(cudaMalloc((void**)&k.aug16, (size_t)cap_pad * 32));
-  CK(cudaMalloc((void**)&k.augq16, (size_t)cap_pad * 32));
-  CK(cudaMalloc((void**)&k.err, (size_t)cap_pad * 4));
-  CK(cudaMalloc((void**)&k.cands, sizeof(Cand) * (size_t)cap_pad));
-  CK(cudaMalloc((void**)&k.idx, sizeof(int32_t) * 16 * (size_t)cap));       // NN <= 16 on the generic path
-  CK(cudaMalloc((void**)&k.dist, sizeof(uint32_t) * 16 * (size_t)cap));
-  CK(cudaMalloc((void**)&k.items, sizeof(WorkItem) * (size_t)(cap_pad / 256 + 1)));
-  if (!k.small) CK(cudaMalloc((void**)&k.small, 4096));                        // stats (16 B) | flag (4 B) | PairDev | 2 x ViewDev (aligned 128)
-  k.cap = cap; k.raw_bytes = rb;
+  const size_t pad = (size_t)(nq + tc::ROW_PAD - 1) / tc::ROW_PAD * tc::ROW_PAD;
+  int rc;
+  if ((rc = k.raw.reserve(std::max<size_t>((size_t)nq * dim * esz, 256))) || (rc = k.h16.reserve(pad * 256)) || (rc = k.nbh.reserve(pad * 4)) ||
+      (rc = k.nrm.reserve(pad * 4)) || (rc = k.aug16.reserve(pad * 32)) || (rc = k.augq16.reserve(pad * 32)) || (rc = k.err.reserve(pad * 4)) ||
+      (rc = k.cands.reserve(sizeof(Cand) * pad)) ||
+      (rc = k.idx.reserve(sizeof(int32_t) * 16 * (size_t)nq)) || (rc = k.dist.reserve(sizeof(uint32_t) * 16 * (size_t)nq)) ||   // NN <= 16 on the generic path
+      (rc = k.items.reserve(sizeof(WorkItem) * (pad / 256 + 1))) ||
+      (rc = k.small.reserve(4096)))                  // stats (16 B) | flag (4 B) | PairDev | 2 x ViewDev (aligned 128)
+    return rc;
   return B200M_OK;
 }
 
@@ -2264,7 +2182,7 @@ int b200m_knn(b200m_ctx* c, const b200m_db* db, const void* query, int nq, int n
   KnnScratch& k = c->knn;
   cudaStream_t st = c->stream;
   CK(cudaMemcpyAsync(k.raw, query, (size_t)nq * v.dim * esz, cudaMemcpyHostToDevice, st));
-  uint32_t* d_stats = reinterpret_cast<uint32_t*>(k.small);
+  uint32_t* d_stats = k.small.as<uint32_t>();
   uint32_t* d_flag = d_stats + 4;
   PairDev* d_pair = reinterpret_cast<PairDev*>(k.small + 64);
   ViewDev* d_views = reinterpret_cast<ViewDev*>(k.small + 128);
@@ -2290,7 +2208,7 @@ int b200m_knn(b200m_ctx* c, const b200m_db* db, const void* query, int nq, int n
     const int grid = 2 * std::min(n_items, c->num_sms / 2);
     tc::l2_top2_tc_kernel<true, tc::MODE_KNN><<<grid, tc::block_threads<tc::MODE_KNN>(), tc::Lay<true>::SMEM_BYTES, st>>>(
         d_views, d_pair, k.items, n_items, 2, k.cands, nullptr, 0.f, nullptr, c->d_err, 0, nullptr, FbSink{});
-    knn_finalize_kernel<<<(nq + 7) / 8, 256, 0, st>>>(d_views, d_pair, k.cands, k.idx, (float*)k.dist, c->d_err);
+    knn_finalize_kernel<<<(nq + 7) / 8, 256, 0, st>>>(d_views, d_pair, k.cands, k.idx, k.dist.as<float>(), c->d_err);
     CK(cudaGetLastError());
     uint32_t qflags = 0;
     CK(cudaMemcpyAsync(idx, k.idx, sizeof(int32_t) * (size_t)nq * 2, cudaMemcpyDeviceToHost, st));
@@ -2299,10 +2217,8 @@ int b200m_knn(b200m_ctx* c, const b200m_db* db, const void* query, int nq, int n
     CK(cudaMemcpyAsync(&c->err_total, c->d_err, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));               // items / hv / hp are stack objects; results are in the caller's buffers
     done = (qflags & VF_EXACT_MASK) == 0;        // a query batch outside the exact domain (non-integer, huge values): redo on the exact kernels
-    c->last_tc_pairs = done ? 1 : 0; c->last_u8_pairs = 0;
   }
-  if (done) return B200M_OK;
-  c->last_tc_pairs = 0; c->last_u8_pairs = 0;
+  if (done) { c->last = LastCall{0, 0, 0, 1, 0, 0, 0, 0}; return B200M_OK; }
 
   const bool tiled_l2 = nn == 2 && v.dim == 128 && v.dtype != DT_BIN && (v.dtype == DT_U8 || db->metric == B200M_L2_VECTORIZED);
   const bool tiled_ham = nn == 2 && v.dim == 64 && v.dtype == DT_BIN;
@@ -2315,18 +2231,19 @@ int b200m_knn(b200m_ctx* c, const b200m_db* db, const void* query, int nq, int n
     CK(cudaMemcpyAsync(d_views, hv, sizeof(hv), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_pair, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
     if (tiled_ham) hamming_top2_kernel<true><<<dim3((nq + HM_TQ - 1) / HM_TQ, 1), HM_TQ, 0, st>>>(d_views, d_pair, nullptr, nullptr, 0.f, k.idx, k.dist);
-    else if (v.dtype == DT_F32) exact_top2_kernel<float, true><<<dim3((nq + EX_TQ - 1) / EX_TQ, 1), 256, EX_SMEM, st>>>(d_views, d_pair, mode, nullptr, nullptr, 0.f, k.idx, (float*)k.dist);
-    else exact_top2_kernel<uint8_t, true><<<dim3((nq + EX_TQ - 1) / EX_TQ, 1), 256, EX_SMEM, st>>>(d_views, d_pair, mode, nullptr, nullptr, 0.f, k.idx, (float*)k.dist);
+    else if (v.dtype == DT_F32) exact_top2_kernel<float, true><<<dim3((nq + EX_TQ - 1) / EX_TQ, 1), 256, EX_SMEM, st>>>(d_views, d_pair, mode, nullptr, nullptr, 0.f, k.idx, k.dist.as<float>());
+    else exact_top2_kernel<uint8_t, true><<<dim3((nq + EX_TQ - 1) / EX_TQ, 1), 256, EX_SMEM, st>>>(d_views, d_pair, mode, nullptr, nullptr, 0.f, k.idx, k.dist.as<float>());
     CK(cudaGetLastError());
   } else {
     const int grid = (nq + 3) / 4;
-    if (v.dtype == DT_F32) generic_knn_kernel<float><<<grid, 128, 0, st>>>((const float*)v.raw, v.m, (const float*)k.raw, nq, v.dim, nn, db->metric, k.idx, k.dist);
-    else generic_knn_kernel<uint8_t><<<grid, 128, 0, st>>>((const uint8_t*)v.raw, v.m, (const uint8_t*)k.raw, nq, v.dim, nn, db->metric, k.idx, k.dist);
+    if (v.dtype == DT_F32) generic_knn_kernel<float><<<grid, 128, 0, st>>>((const float*)v.raw, v.m, k.raw.as<const float>(), nq, v.dim, nn, db->metric, k.idx, k.dist);
+    else generic_knn_kernel<uint8_t><<<grid, 128, 0, st>>>((const uint8_t*)v.raw, v.m, k.raw.as<const uint8_t>(), nq, v.dim, nn, db->metric, k.idx, k.dist);
     CK(cudaGetLastError());
   }
   CK(cudaMemcpyAsync(idx, k.idx, sizeof(int32_t) * (size_t)nq * nn, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(dist, k.dist, sizeof(uint32_t) * (size_t)nq * nn, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  c->last = LastCall{};
   return B200M_OK;
 }
 

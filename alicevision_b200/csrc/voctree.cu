@@ -9,6 +9,7 @@
 //   voctree/Database.cpp:44-63,118-137,145-157   insert / find (partial_sort on score only) / computeTfIdfWeights
 //   imageMatching/ImageMatching.cpp:107-143,191-238   convertAllMatchesToPairList, generateFromVoctree (a/a)
 #include "../../include/b200voc.h"
+#include "cuda_owner.cuh"
 
 #include <cub/cub.cuh>
 #include <cuda_runtime.h>
@@ -25,26 +26,20 @@
 #include <string>
 #include <vector>
 
-namespace b200m { int set_error(int code, const std::string& msg); }   // engine.cu: thread-local message behind b200m_last_error()
-using b200m::set_error;
-
-#define VCK(call)                                                                                                  \
-  do {                                                                                                             \
-    cudaError_t e_ = (call);                                                                                       \
-    if (e_ != cudaSuccess) return set_error(B200M_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_));    \
-  } while (0)
+using namespace b200m;
 
 // ------------------------------------------------------------------------------------------------ data model
 struct b200v_tree {
   uint32_t k = 0, levels = 0, num_words = 0, word_start = 0; int dim = 0;
   std::vector<float> centers; std::vector<uint8_t> valid;
   // device copies per GPU ordinal (created on first use)
-  mutable std::map<int, std::pair<float*, uint8_t*>> dev;
+  struct Dev { DeviceBuffer<float> centers; DeviceBuffer<uint8_t> valid; };
+  mutable std::map<int, Dev> dev;
 };
 
 struct b200v_db {
   const b200v_tree* tree = nullptr; int device = 0;
-  cudaStream_t stream = nullptr; cudaEvent_t e0 = nullptr, e1 = nullptr;
+  Stream stream; Event e0, e1;
   std::map<uint32_t, std::vector<int32_t>> docs;     // doc id -> words in feature order (std::map: ascending id, like database_)
   std::vector<float> word_weights;
   std::vector<int32_t> last_scores; int64_t last_n = 0; double last_gpu_ms = 0;
@@ -63,15 +58,15 @@ bool node_count_ok(uint32_t k, uint32_t levels, uint32_t n_nodes, uint32_t& num_
 int tree_to_device(const b200v_tree* t, int device, const float** centers, const uint8_t** valid) {
   auto it = t->dev.find(device);
   if (it == t->dev.end()) {
-    float* dc = nullptr; uint8_t* dv = nullptr;
-    VCK(cudaSetDevice(device));
-    VCK(cudaMalloc((void**)&dc, t->centers.size() * sizeof(float)));
-    VCK(cudaMalloc((void**)&dv, t->valid.size()));
-    VCK(cudaMemcpy(dc, t->centers.data(), t->centers.size() * sizeof(float), cudaMemcpyHostToDevice));
-    VCK(cudaMemcpy(dv, t->valid.data(), t->valid.size(), cudaMemcpyHostToDevice));
-    it = t->dev.emplace(device, std::make_pair(dc, dv)).first;
+    b200v_tree::Dev d;
+    int rc;
+    CK(cudaSetDevice(device));
+    if ((rc = d.centers.reserve(t->centers.size() * sizeof(float))) || (rc = d.valid.reserve(t->valid.size()))) return rc;
+    CK(cudaMemcpy(d.centers, t->centers.data(), t->centers.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d.valid, t->valid.data(), t->valid.size(), cudaMemcpyHostToDevice));
+    it = t->dev.emplace(device, std::move(d)).first;
   }
-  *centers = it->second.first; *valid = it->second.second;
+  *centers = it->second.centers; *valid = it->second.valid;
   return B200M_OK;
 }
 
@@ -191,32 +186,25 @@ weighted_pairs_kernel(const unsigned long long* __restrict__ dkeys, const int* _
   S[(size_t)b * n_docs + a] = score;
 }
 
-struct DevBuf {
-  void* p = nullptr;
-  ~DevBuf() { if (p) cudaFree(p); }
-  int alloc(size_t bytes) { VCK(cudaMalloc(&p, std::max<size_t>(bytes, 16))); return B200M_OK; }
-  template <class T> T* as() const { return static_cast<T*>(p); }
-};
-
 int quantize_on(int device, cudaStream_t stream, const b200v_tree* tree, const void* descs, int64_t n, int dtype, int32_t* words) {
   if (n == 0) return B200M_OK;
   const float* dc; const uint8_t* dv;
   int rc = tree_to_device(tree, device, &dc, &dv);
   if (rc) return rc;
-  VCK(cudaSetDevice(device));
+  CK(cudaSetDevice(device));
   const size_t esz = dtype == B200M_F32 ? 4 : 1;
-  DevBuf dd, dw;
-  if ((rc = dd.alloc((size_t)n * tree->dim * esz)) || (rc = dw.alloc((size_t)n * 4))) return rc;
-  VCK(cudaMemcpyAsync(dd.p, descs, (size_t)n * tree->dim * esz, cudaMemcpyHostToDevice, stream));
+  DeviceBuffer<> dd, dw;
+  if ((rc = dd.reserve((size_t)n * tree->dim * esz)) || (rc = dw.reserve((size_t)n * 4))) return rc;
+  CK(cudaMemcpyAsync(dd, descs, (size_t)n * tree->dim * esz, cudaMemcpyHostToDevice, stream));
   const int grid = (int)((n + QZ_WARPS - 1) / QZ_WARPS);
   const size_t smem = (size_t)QZ_WARPS * tree->dim * sizeof(double);
   if (dtype == B200M_F32)
     quantize_kernel<float><<<grid, QZ_WARPS * 32, smem, stream>>>(dd.as<float>(), n, tree->dim, dc, dv, tree->k, tree->levels, tree->word_start, dw.as<int>());
   else
     quantize_kernel<uint8_t><<<grid, QZ_WARPS * 32, smem, stream>>>(dd.as<uint8_t>(), n, tree->dim, dc, dv, tree->k, tree->levels, tree->word_start, dw.as<int>());
-  VCK(cudaGetLastError());
-  VCK(cudaMemcpyAsync(words, dw.p, (size_t)n * 4, cudaMemcpyDeviceToHost, stream));
-  VCK(cudaStreamSynchronize(stream));
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(words, dw, (size_t)n * 4, cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));
   return B200M_OK;
 }
 
@@ -264,7 +252,7 @@ int b200v_tree_save(const b200v_tree* t, const char* path) {
 
 void b200v_tree_destroy(b200v_tree* t) {
   if (!t) return;
-  for (auto& kv : t->dev) { cudaSetDevice(kv.first); cudaFree(kv.second.first); cudaFree(kv.second.second); }
+  for (auto& kv : t->dev) { cudaSetDevice(kv.first); kv.second = b200v_tree::Dev(); }   // each copy is freed on its own device
   delete t;
 }
 uint32_t b200v_tree_levels(const b200v_tree* t) { return t ? t->levels : 0; }
@@ -288,9 +276,9 @@ int b200v_db_create(const b200v_tree* tree, int device, b200v_db** out) {
   if (device < 0 || device >= nd) return set_error(B200M_ERR_ARG, "bad device ordinal");
   std::unique_ptr<b200v_db> db(new b200v_db());
   db->tree = tree; db->device = device;
-  VCK(cudaSetDevice(device));
-  VCK(cudaStreamCreateWithFlags(&db->stream, cudaStreamNonBlocking));
-  VCK(cudaEventCreate(&db->e0)); VCK(cudaEventCreate(&db->e1));
+  CK(cudaSetDevice(device));
+  int rc;
+  if ((rc = db->stream.create()) || (rc = db->e0.create()) || (rc = db->e1.create())) return rc;
   db->word_weights.assign(tree->num_words, 1.0f);                 // Database::Database (Database.cpp:39-42)
   *out = db.release();
   return B200M_OK;
@@ -299,9 +287,6 @@ int b200v_db_create(const b200v_tree* tree, int device, b200v_db** out) {
 void b200v_db_destroy(b200v_db* db) {
   if (!db) return;
   cudaSetDevice(db->device);
-  if (db->e0) cudaEventDestroy(db->e0);
-  if (db->e1) cudaEventDestroy(db->e1);
-  if (db->stream) cudaStreamDestroy(db->stream);
   delete db;
 }
 
@@ -370,7 +355,7 @@ int b200v_db_query_all(b200v_db* db, size_t numImageQuery, const char* distanceM
   if (n_keep_out) *n_keep_out = n_keep;
   if (n_docs == 0) return B200M_OK;
   if (!query_ids || !match_ids || !scores) return set_error(B200M_ERR_ARG, "null output");
-  VCK(cudaSetDevice(db->device));
+  CK(cudaSetDevice(db->device));
 
   // flatten: words of all documents + their position in ascending-id order
   std::vector<uint32_t> ids; ids.reserve(n_docs);
@@ -389,17 +374,17 @@ int b200v_db_query_all(b200v_db* db, size_t numImageQuery, const char* distanceM
   if (total > 0) {
     if (total > 0x7fffffffull) return set_error(B200M_ERR_UNSUPPORTED, "more than 2^31 features in the database");
     const int n = (int)total;
-    DevBuf d_words, d_pos, d_keys, d_keys2, d_ukeys, d_cnt, d_nu, d_w, d_uw, d_len, d_nw, d_start, d_S, d_tmp;
+    DeviceBuffer<> d_words, d_pos, d_keys, d_keys2, d_ukeys, d_cnt, d_nu, d_w, d_uw, d_len, d_nw, d_start, d_S, d_tmp;
     int rc;
-    if ((rc = d_words.alloc(total * 4)) || (rc = d_pos.alloc(total * 4)) || (rc = d_keys.alloc(total * 8)) || (rc = d_keys2.alloc(total * 8)) ||
-        (rc = d_ukeys.alloc(total * 8)) || (rc = d_cnt.alloc(total * 4)) || (rc = d_nu.alloc(4)) || (rc = d_w.alloc(total * 4)) || (rc = d_uw.alloc(total * 4)) ||
-        (rc = d_len.alloc(total * 4)) || (rc = d_nw.alloc(4)) || (rc = d_start.alloc(total * 4)) || (rc = d_S.alloc(n_docs * n_docs * 4)))
+    if ((rc = d_words.reserve(total * 4)) || (rc = d_pos.reserve(total * 4)) || (rc = d_keys.reserve(total * 8)) || (rc = d_keys2.reserve(total * 8)) ||
+        (rc = d_ukeys.reserve(total * 8)) || (rc = d_cnt.reserve(total * 4)) || (rc = d_nu.reserve(4)) || (rc = d_w.reserve(total * 4)) || (rc = d_uw.reserve(total * 4)) ||
+        (rc = d_len.reserve(total * 4)) || (rc = d_nw.reserve(4)) || (rc = d_start.reserve(total * 4)) || (rc = d_S.reserve(n_docs * n_docs * 4)))
       return rc;
     cudaStream_t st = db->stream;
-    VCK(cudaMemcpyAsync(d_words.p, flat.data(), total * 4, cudaMemcpyHostToDevice, st));
-    VCK(cudaMemcpyAsync(d_pos.p, pos.data(), total * 4, cudaMemcpyHostToDevice, st));
-    VCK(cudaMemsetAsync(d_S.p, 0, n_docs * n_docs * 4, st));
-    VCK(cudaEventRecord(db->e0, st));
+    CK(cudaMemcpyAsync(d_words, flat.data(), total * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_pos, pos.data(), total * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(d_S, 0, n_docs * n_docs * 4, st));
+    CK(cudaEventRecord(db->e0, st));
     make_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_words.as<int>(), d_pos.as<unsigned>(), n, d_keys.as<unsigned long long>());
     size_t tb = 0, tb2 = 0;
     cub::DeviceRadixSort::SortKeys(nullptr, tb, d_keys.as<unsigned long long>(), d_keys2.as<unsigned long long>(), n, 0, 64, st);
@@ -409,46 +394,46 @@ int b200v_db_query_all(b200v_db* db, size_t numImageQuery, const char* distanceM
     tb = std::max(tb, tb2);
     cub::DeviceScan::ExclusiveSum(nullptr, tb2, d_len.as<int>(), d_start.as<int>(), n, st);
     tb = std::max(tb, tb2);
-    if ((rc = d_tmp.alloc(tb))) return rc;
-    VCK(cub::DeviceRadixSort::SortKeys(d_tmp.p, tb, d_keys.as<unsigned long long>(), d_keys2.as<unsigned long long>(), n, 0, 64, st));
-    VCK(cub::DeviceRunLengthEncode::Encode(d_tmp.p, tb, d_keys2.as<unsigned long long>(), d_ukeys.as<unsigned long long>(), d_cnt.as<int>(), d_nu.as<int>(), n, st));
+    if ((rc = d_tmp.reserve(tb))) return rc;
+    CK(cub::DeviceRadixSort::SortKeys(d_tmp, tb, d_keys.as<unsigned long long>(), d_keys2.as<unsigned long long>(), n, 0, 64, st));
+    CK(cub::DeviceRunLengthEncode::Encode(d_tmp, tb, d_keys2.as<unsigned long long>(), d_ukeys.as<unsigned long long>(), d_cnt.as<int>(), d_nu.as<int>(), n, st));
     int nu = 0;
-    VCK(cudaMemcpyAsync(&nu, d_nu.p, 4, cudaMemcpyDeviceToHost, st));
-    VCK(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(&nu, d_nu, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     key_words_kernel<<<(nu + 255) / 256, 256, 0, st>>>(d_ukeys.as<unsigned long long>(), nu, d_w.as<unsigned>());
-    VCK(cub::DeviceRunLengthEncode::Encode(d_tmp.p, tb, d_w.as<unsigned>(), d_uw.as<unsigned>(), d_len.as<int>(), d_nw.as<int>(), nu, st));
+    CK(cub::DeviceRunLengthEncode::Encode(d_tmp, tb, d_w.as<unsigned>(), d_uw.as<unsigned>(), d_len.as<int>(), d_nw.as<int>(), nu, st));
     int nw = 0;
-    VCK(cudaMemcpyAsync(&nw, d_nw.p, 4, cudaMemcpyDeviceToHost, st));
-    VCK(cudaStreamSynchronize(st));
-    VCK(cub::DeviceScan::ExclusiveSum(d_tmp.p, tb, d_len.as<int>(), d_start.as<int>(), nw, st));
+    CK(cudaMemcpyAsync(&nw, d_nw, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_len.as<int>(), d_start.as<int>(), nw, st));
     if (mode == 2) {
       // per-document sorted (word, count) lists: re-key the unique pairs by (document, word), sort them with their counts
-      DevBuf d_dk, d_dk2, d_dc2, d_ds, d_wt, d_tmp2;
-      if ((rc = d_dk.alloc((size_t)nu * 8)) || (rc = d_dk2.alloc((size_t)nu * 8)) || (rc = d_dc2.alloc((size_t)nu * 4)) || (rc = d_ds.alloc((n_docs + 2) * 4)) ||
-          (rc = d_wt.alloc(db->word_weights.size() * 4)))
+      DeviceBuffer<> d_dk, d_dk2, d_dc2, d_ds, d_wt, d_tmp2;
+      if ((rc = d_dk.reserve((size_t)nu * 8)) || (rc = d_dk2.reserve((size_t)nu * 8)) || (rc = d_dc2.reserve((size_t)nu * 4)) || (rc = d_ds.reserve((n_docs + 2) * 4)) ||
+          (rc = d_wt.reserve(db->word_weights.size() * 4)))
         return rc;
-      VCK(cudaMemcpyAsync(d_wt.p, db->word_weights.data(), db->word_weights.size() * 4, cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(d_wt, db->word_weights.data(), db->word_weights.size() * 4, cudaMemcpyHostToDevice, st));
       doc_keys_kernel<<<(nu + 255) / 256, 256, 0, st>>>(d_ukeys.as<unsigned long long>(), nu, d_dk.as<unsigned long long>());
       size_t tb3 = 0;
       cub::DeviceRadixSort::SortPairs(nullptr, tb3, d_dk.as<unsigned long long>(), d_dk2.as<unsigned long long>(), d_cnt.as<int>(), d_dc2.as<int>(), nu, 0, 64, st);
-      if ((rc = d_tmp2.alloc(tb3))) return rc;
-      VCK(cub::DeviceRadixSort::SortPairs(d_tmp2.p, tb3, d_dk.as<unsigned long long>(), d_dk2.as<unsigned long long>(), d_cnt.as<int>(), d_dc2.as<int>(), nu, 0, 64, st));
+      if ((rc = d_tmp2.reserve(tb3))) return rc;
+      CK(cub::DeviceRadixSort::SortPairs(d_tmp2, tb3, d_dk.as<unsigned long long>(), d_dk2.as<unsigned long long>(), d_cnt.as<int>(), d_dc2.as<int>(), nu, 0, 64, st));
       doc_starts_kernel<<<(nu + 1 + 255) / 256, 256, 0, st>>>(d_dk2.as<unsigned long long>(), nu, (int)n_docs, d_ds.as<int>());
       weighted_pairs_kernel<<<dim3((unsigned)((n_docs + 127) / 128), (unsigned)n_docs), 128, 0, st>>>(d_dk2.as<unsigned long long>(), d_dc2.as<int>(), d_ds.as<int>(), d_wt.as<float>(),
-                                                                                                  (int)n_docs, reinterpret_cast<float*>(d_S.p));
-      VCK(cudaGetLastError());
-      VCK(cudaEventRecord(db->e1, st));
-      VCK(cudaMemcpyAsync(wscores.data(), d_S.p, n_docs * n_docs * 4, cudaMemcpyDeviceToHost, st));
-      VCK(cudaStreamSynchronize(st));
+                                                                                                  (int)n_docs, d_S.as<float>());
+      CK(cudaGetLastError());
+      CK(cudaEventRecord(db->e1, st));
+      CK(cudaMemcpyAsync(wscores.data(), d_S, n_docs * n_docs * 4, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
     } else {
     score_postings_kernel<<<(int)(((size_t)nw * 32 + 255) / 256), 256, 0, st>>>(d_ukeys.as<unsigned long long>(), d_cnt.as<int>(), d_start.as<int>(), d_len.as<int>(), nw, mode, (int)n_docs, d_S.as<int>());
-    VCK(cudaGetLastError());
-    VCK(cudaEventRecord(db->e1, st));
-    VCK(cudaMemcpyAsync(db->last_scores.data(), d_S.p, n_docs * n_docs * 4, cudaMemcpyDeviceToHost, st));
-    VCK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(db->e1, st));
+    CK(cudaMemcpyAsync(db->last_scores.data(), d_S, n_docs * n_docs * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     }
     float ms = 0.f;
-    VCK(cudaEventElapsedTime(&ms, db->e0, db->e1));
+    CK(cudaEventElapsedTime(&ms, db->e0, db->e1));
     db->last_gpu_ms = ms;
   }
 

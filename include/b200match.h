@@ -241,17 +241,23 @@ int b200m_debug_rand_sample(const uint32_t state[625], int range, int draws, uin
 int b200m_debug_rand_sample_k(const uint32_t state[625], int sample_size, int range, int draws, uint32_t* out, uint32_t* states);
 
 /* ---- instrumentation ------------------------------------------------------------------------------------------ */
-/* GPU time of the last b200m_match_pairs between its first and last enqueue (CUDA events on the context's stream), ms */
+/* The b200m_last_* getters report the last successful b200m_match_pairs, b200m_guided_match(_model), b200m_guided_match_fast_pairs
+ * or b200m_knn on the context, whichever came last; a value that call does not measure reads 0 (b200m_knn sets only
+ * b200m_last_tc_pairs: 1 when it ran on the tensor-core kernel).  They take the context's lock.  The a-contrario RANSAC calls have
+ * their own (b200m_acransac_last_stats) and leave these alone. */
+/* GPU time of the last call between its first and last enqueue (CUDA events on the context's stream), ms */
 double b200m_last_gpu_ms(const b200m_ctx* ctx);
-/* summed device time of the search kernel launches (tensor-core / exact / Hamming) in the last call, ms */
+/* summed device time of the search kernel launches (tensor-core / exact / Hamming) in the last call, ms; the guided calls: their
+ * search kernel (b200m_guided_match_fast_pairs: its candidate kernel) */
 double b200m_last_search_kernel_ms(const b200m_ctx* ctx);
 /* kernel launches issued by the last call */
 int b200m_last_launches(const b200m_ctx* ctx);
 /* pairs of the last call that ran on the tensor-core kernel */
 int b200m_last_tc_pairs(const b200m_ctx* ctx);
-/* candidates whose re-scored best distance differed from the tensor-core value (must stay 0) */
+/* candidates whose re-scored best distance differed from the tensor-core value (must stay 0); cumulative over the context's life */
 unsigned b200m_exactness_errors(const b200m_ctx* ctx);
-/* total raw records (matches before host finishing) produced by the last call */
+/* total raw records (matches before host finishing) produced by the last call; b200m_guided_match(_model): its matches,
+ * b200m_guided_match_fast_pairs: the candidate distances it evaluated */
 int64_t b200m_last_records(const b200m_ctx* ctx);
 /* pairs of the last call that ran on the tensor-core FILTER kernel for real-valued fp32 descriptors (fp16-rounded GEMM + rigorous error
  * bound + exact re-scoring in the reference's arithmetic), and the queries among them the bound could not decide, which were searched
