@@ -1,0 +1,277 @@
+// Reference-side adaptor for the `fundamental_matrix` geometric filter: matchingImageCollection::robustModelEstimation with
+// GeometricFilterMatrix_F_AC (ACRANSAC, Fundamental7PSolver; GeometricFilter.hpp:40-88, GeometricFilterMatrix_F_AC.hpp:90-174,
+// :266-299, :357-392) for a whole putative list on the b200match engine (H100): one b200m_acransac_fundamental_pairs call, the
+// reference's inlier copy and support rules, then one b200m_guided_match_pairs call for every kept pair and common descriptor type.
+// Header-only; compiled inside an AliceVision build and linked against libb200match.so.  The caller gathers xI / xJ with the
+// reference's fillMatricesWithUndistortFeaturesMatches and the guided positions with camera::IntrinsicBase::getUndistortedPixel.
+// Inside the AliceVision build (ALICEVISION_B200_REFERENCE_FILTER_UTILS defined) the library's own copyInlierMatches and
+// hasStrongSupport run; elsewhere their restatement below.
+#pragma once
+
+#include <aliceVision/matching/IndMatch.hpp>
+#include <aliceVision/feature/Regions.hpp>
+#include <aliceVision/feature/imageDescriberCommon.hpp>
+#ifdef ALICEVISION_B200_REFERENCE_FILTER_UTILS
+#include <aliceVision/matchingImageCollection/geometricFilterUtils.hpp>
+#include <aliceVision/matching/supportEstimation.hpp>
+#endif
+
+#include <b200match.h>
+
+// matching::b200detail: sharedContext / nextViewId / regionsDtype / uploadRegions (matching/ in an AliceVision tree, alongside here otherwise)
+#if __has_include(<aliceVision/matching/RegionsMatcher_b200.hpp>)
+#include <aliceVision/matching/RegionsMatcher_b200.hpp>
+#else
+#include "RegionsMatcher_b200.hpp"
+#endif
+
+#include <algorithm>
+#include <cmath>
+#include <cstdint>
+#include <limits>
+#include <map>
+#include <random>
+#include <sstream>
+#include <utility>
+#include <vector>
+
+namespace aliceVision {
+namespace matchingImageCollection {
+
+namespace b200detail {
+/// copyInlierMatches (geometricFilterUtils.cpp:13-37)
+inline void copyInlierMatches(const std::vector<std::size_t>& inliers,
+                              const matching::MatchesPerDescType& putatives,
+                              const std::vector<feature::EImageDescriberType>& descTypes,
+                              matching::MatchesPerDescType& out)
+{
+#ifdef ALICEVISION_B200_REFERENCE_FILTER_UTILS
+    matchingImageCollection::copyInlierMatches(inliers, putatives, descTypes, out);
+#else
+    std::vector<std::size_t> ordered = inliers;
+    std::sort(ordered.begin(), ordered.end());
+    std::size_t type = 0, start = 0, end = putatives.getNbMatches(descTypes[0]);
+    for (const std::size_t g : ordered)
+    {
+        while (g >= end)
+        {
+            ++type;
+            start = end;
+            end += putatives.getNbMatches(descTypes[type]);
+        }
+        out[descTypes[type]].push_back(putatives.at(descTypes[type])[g - start]);
+    }
+#endif
+}
+
+/// matching::hasStrongSupport(MatchesPerDescType, minimumSamples) (supportEstimation.cpp:48-59)
+inline bool hasStrongSupport(const matching::MatchesPerDescType& matches, std::size_t minimumSamples)
+{
+#ifdef ALICEVISION_B200_REFERENCE_FILTER_UTILS
+    return matching::hasStrongSupport(matches, minimumSamples);
+#else
+    float score = 0;
+    for (const auto& m : matches)
+        score += feature::getStrongSupportCoeff(m.first) * m.second.size();
+    return score > minimumSamples;
+#endif
+}
+
+/// The generator as its operator<< writes it: 624 words, then the position.
+inline void mtState(const std::mt19937& g, uint32_t state[625])
+{
+    std::stringstream ss;
+    ss << g;
+    for (int k = 0; k < 625; ++k)
+        ss >> state[k];
+}
+}  // namespace b200detail
+
+/// A putative list over views that are uploaded ONCE per descriptor type: addView every (view, type) with its guided positions,
+/// addPair every pair, then run().  The views are removed from the engine when the batch is destroyed.
+class GeometricFilterMatrix_F_AC_Batch_b200
+{
+public:
+    /// What the estimation of one pair gave (in addPair order): ACRANSAC's validity, F (row-major, x_J^T F x_I = 0), errorMax
+    /// (m_dPrecision_robust; infinite when not valid) and the support decision.
+    struct Estimate
+    {
+        bool valid = false, strongSupport = false;
+        double F[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        double errorMax = std::numeric_limits<double>::infinity();
+    };
+
+    explicit GeometricFilterMatrix_F_AC_Batch_b200(b200m_ctx* ctx = matching::b200detail::sharedContext())
+      : _ctx(ctx)
+    {}
+    ~GeometricFilterMatrix_F_AC_Batch_b200()
+    {
+        if (_ctx)
+            for (const auto& v : _views)
+                b200m_remove_view(_ctx, v.second);
+    }
+    GeometricFilterMatrix_F_AC_Batch_b200(const GeometricFilterMatrix_F_AC_Batch_b200&) = delete;
+    GeometricFilterMatrix_F_AC_Batch_b200& operator=(const GeometricFilterMatrix_F_AC_Batch_b200&) = delete;
+
+    bool available() const { return _ctx != nullptr && _ok; }
+
+    /// Uploads one (view, type) once; guidedPos: n x 2 positions guided matching uses (getUndistortedPixel when the camera isValid()),
+    /// or nullptr for the regions' own positions.
+    bool addView(IndexT viewId, feature::EImageDescriberType type, const feature::Regions& regions, const double* guidedPos = nullptr)
+    {
+        if (!available())
+            return false;
+        const auto key = std::make_pair(viewId, type);
+        if (_views.count(key))
+            return true;
+        const int dtype = matching::b200detail::regionsDtype(regions);
+        if (dtype < 0)
+            return _ok = false;
+        const uint32_t id = matching::b200detail::nextViewId();
+        if (!matching::b200detail::uploadRegions(_ctx, id, regions, dtype))
+            return _ok = false;
+        _views[key] = id;
+        if (guidedPos != nullptr && b200m_set_view_geometry(_ctx, id, guidedPos, (int)regions.RegionCount()) != B200M_OK)
+            return _ok = false;
+        return true;
+    }
+
+    /// descTypes: getCommonDescTypes of the pair (an empty list: the pair is not estimated, as the reference returns
+    /// EstimationStatus(false, false)); xI / xJ: 2 x n (fillMatricesWithUndistortFeaturesMatches); sizes: (width, height).
+    template<class MatT>
+    void addPair(const Pair& pair,
+                 const matching::MatchesPerDescType& putatives,
+                 const std::vector<feature::EImageDescriberType>& descTypes,
+                 const MatT& xI,
+                 const MatT& xJ,
+                 const std::pair<std::size_t, std::size_t>& sizeI,
+                 const std::pair<std::size_t, std::size_t>& sizeJ)
+    {
+        PairIn p{pair, putatives, descTypes, _corr.size() / 4};
+        if (!descTypes.empty())
+            for (int c = 0; c < (int)xI.cols(); ++c)
+            {
+                _corr.push_back(xI(0, c));
+                _corr.push_back(xI(1, c));
+                _corr.push_back(xJ(0, c));
+                _corr.push_back(xJ(1, c));
+            }
+        _wh.insert(_wh.end(), {(int32_t)sizeI.first, (int32_t)sizeI.second, (int32_t)sizeJ.first, (int32_t)sizeJ.second});
+        _pairs.push_back(std::move(p));
+    }
+
+    /// robustModelEstimation over every pair added so far: each pair starts from `rng` (geometricEstimation_Mat_ACRANSAC takes it
+    /// by value).  Pairs with strong support enter out; with guidedMatching their lists are the guided ones (errorTh = errorMax^2,
+    /// distRatio = distanceRatio^2, every common type, empty lists included; nothing when errorMax is infinite).  Returns false
+    /// (out untouched) when the engine is unavailable or fails.
+    bool run(const std::mt19937& rng, std::size_t maxIteration, double precision, bool guidedMatching, double distanceRatio,
+             matching::PairwiseMatches& out)
+    {
+        if (!available())
+            return false;
+        const int n = (int)_pairs.size();
+        uint32_t state[625];
+        b200detail::mtState(rng, state);
+        std::vector<int64_t> offsets(n + 1, 0);
+        for (int k = 0; k < n; ++k)
+            offsets[k + 1] = (k + 1 < n ? (int64_t)_pairs[k + 1].offset : (int64_t)(_corr.size() / 4));
+        const std::size_t total = std::max<std::size_t>(_corr.size() / 4, 1);
+        std::vector<uint8_t> valid(std::max(n, 1));
+        std::vector<int32_t> nInl(std::max(n, 1)), iters(std::max(n, 1));
+        std::vector<uint32_t> inl(total);
+        std::vector<double> F(9 * std::max(n, 1)), errMax(std::max(n, 1)), nfa(std::max(n, 1));
+        const double dummy[4] = {0, 0, 0, 0};
+        if (n > 0 && b200m_acransac_fundamental_pairs(_ctx, n, offsets.data(), _corr.empty() ? dummy : _corr.data(), _wh.data(), state,
+                                                      (int64_t)maxIteration, precision, valid.data(), nInl.data(), inl.data(), F.data(),
+                                                      errMax.data(), nfa.data(), iters.data()) != B200M_OK)
+            return false;
+        _estimates.assign(n, Estimate());
+        std::map<Pair, matching::MatchesPerDescType> result;
+        std::vector<int> kept;
+        for (int k = 0; k < n; ++k)
+        {
+            Estimate& e = _estimates[k];
+            e.valid = valid[k] != 0;
+            std::copy(F.begin() + 9 * k, F.begin() + 9 * k + 9, e.F);
+            if (!e.valid)
+                continue;
+            e.errorMax = errMax[k];
+            const std::vector<std::size_t> inliers(inl.begin() + offsets[k], inl.begin() + offsets[k] + nInl[k]);
+            matching::MatchesPerDescType perType;
+            b200detail::copyInlierMatches(inliers, _pairs[k].putatives, _pairs[k].descTypes, perType);
+            e.strongSupport = b200detail::hasStrongSupport(perType, 7);   // Fundamental7PSolver::getMinimumNbRequiredSamples
+            if (!e.strongSupport)
+                continue;
+            kept.push_back(k);
+            result[_pairs[k].pair] = std::move(perType);
+        }
+        if (guidedMatching)
+        {
+            std::vector<uint32_t> ids;
+            std::vector<double> M, th;
+            std::vector<std::pair<Pair, feature::EImageDescriberType>> items;
+            for (const int k : kept)
+            {
+                result[_pairs[k].pair] = matching::MatchesPerDescType();       // the guided result replaces the inliers, even when empty
+                if (_estimates[k].errorMax == std::numeric_limits<double>::infinity())
+                    continue;                                                  // GeometricFilterMatrix_F_AC.hpp:363
+                for (const feature::EImageDescriberType t : _pairs[k].descTypes)
+                {
+                    const auto l = _views.find(std::make_pair(_pairs[k].pair.first, t)), r = _views.find(std::make_pair(_pairs[k].pair.second, t));
+                    if (l == _views.end() || r == _views.end())
+                        return false;
+                    ids.push_back(l->second);
+                    ids.push_back(r->second);
+                    M.insert(M.end(), _estimates[k].F, _estimates[k].F + 9);
+                    th.push_back(_estimates[k].errorMax * _estimates[k].errorMax);
+                    items.emplace_back(_pairs[k].pair, t);
+                }
+            }
+            if (!items.empty())
+            {
+                b200m_result* res = nullptr;
+                if (b200m_guided_match_pairs(_ctx, ids.data(), (int)items.size(), B200M_MODEL_FUNDAMENTAL, M.data(), th.data(),
+                                             distanceRatio * distanceRatio, &res) != B200M_OK)
+                {
+                    b200m_result_free(res);
+                    return false;
+                }
+                const int64_t* off = nullptr;
+                const b200m_match* m = nullptr;
+                b200m_result_get(res, nullptr, &off, &m);
+                for (std::size_t q = 0; q < items.size(); ++q)
+                {
+                    matching::IndMatches& dst = result[items[q].first][items[q].second];
+                    for (int64_t e = off[q]; e < off[q + 1]; ++e)
+                        dst.emplace_back(m[e].i, m[e].j);
+                }
+                b200m_result_free(res);
+            }
+        }
+        for (auto& r : result)
+            out[r.first] = std::move(r.second);
+        return true;
+    }
+
+    /// The estimation of the k-th pair added, after run().
+    const Estimate& estimate(std::size_t k) const { return _estimates.at(k); }
+
+private:
+    struct PairIn
+    {
+        Pair pair;
+        matching::MatchesPerDescType putatives;
+        std::vector<feature::EImageDescriberType> descTypes;
+        std::size_t offset;
+    };
+    b200m_ctx* _ctx;
+    bool _ok = true;
+    std::map<std::pair<IndexT, feature::EImageDescriberType>, uint32_t> _views;
+    std::vector<PairIn> _pairs;
+    std::vector<double> _corr;
+    std::vector<int32_t> _wh;
+    std::vector<Estimate> _estimates;
+};
+
+}  // namespace matchingImageCollection
+}  // namespace aliceVision

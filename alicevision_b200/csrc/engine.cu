@@ -238,6 +238,15 @@ struct GuidedFastScratch {
   Event ev_c0, ev_c1;                         // candidate-kernel timing
 };
 
+// grow-only scratch of b200m_guided_match_pairs (guided.cuh): one batch of pairs at a time
+struct GuidedScratch {
+  enum { PAIRS, BESTJ, KEEP, KPOS, OUT, EXPAND, TEMP, NBUF };
+  DeviceBuffer<> d[NBUF];
+  PinnedBuffer<GuidedPair> h_pairs;
+  PinnedBuffer<> h_out;                       // read-back of the per-pair starts and the matches, one copy
+  Event ev_k0, ev_k1;                         // search-kernel timing
+};
+
 // grow-only scratch of b200m_acransac_fundamental_pairs and b200m_acransac_homography_pairs (acransac.cuh); the last call's
 // instrumentation and trace, whichever model it estimated
 struct AcransacScratch {
@@ -248,7 +257,7 @@ struct AcransacScratch {
   Event ev0, ev1;
 };
 
-// What the last b200m_match_pairs, b200m_guided_match_model, b200m_guided_match_fast_pairs or b200m_knn measured (b200m_last_*);
+// What the last b200m_match_pairs, b200m_guided_match_pairs (and its one-pair forms), b200m_guided_match_fast_pairs or b200m_knn measured (b200m_last_*);
 // a field the call does not measure is 0
 struct LastCall {
   double gpu_ms, search_ms;
@@ -266,6 +275,8 @@ struct b200m_ctx {
   KnnScratch knn;
   GuidedFastScratch gf;
   long gf_left_cap = 1l << 21;    // left features per internal batch of b200m_guided_match_fast_pairs (B200M_GUIDED_FAST_LEFT_CAP)
+  GuidedScratch gm;
+  long gm_left_cap = 1l << 21;    // left features per internal batch of b200m_guided_match_pairs (B200M_GUIDED_LEFT_CAP)
   bool pipe_streams = true;       // tables / packing+finishing on their own streams (B200M_PIPE_STREAMS=0: everything on the search stream)
   EncodeTiledFn encode = nullptr;
   std::deque<ViewHost> views;     // deque: references stay valid while pool tasks (position checks) run
@@ -608,6 +619,7 @@ int b200m_ctx_create(int device, void* stream, b200m_ctx** out) {
   if (const char* e = getenv("B200M_REAL_TC")) c->real_tc = atoi(e) != 0;
   if (const char* e = getenv("B200M_REAL_FUSED_ROWS")) c->real_fused_rows = std::max(0l, atol(e));
   if (const char* e = getenv("B200M_GUIDED_FAST_LEFT_CAP")) c->gf_left_cap = std::max(1l, atol(e));
+  if (const char* e = getenv("B200M_GUIDED_LEFT_CAP")) c->gm_left_cap = std::max(1l, atol(e));
   *out = c.release();
   return B200M_OK;
 }
@@ -1438,90 +1450,8 @@ int b200m_guided_match(b200m_ctx* c, uint32_t view_left, uint32_t view_right, co
 
 int b200m_guided_match_model(b200m_ctx* c, uint32_t view_left, uint32_t view_right, int model, const double* F, double errorTh, double distRatio,
                              b200m_result** out) {
-  if (!c || !out || !F || (model != B200M_MODEL_FUNDAMENTAL && model != B200M_MODEL_HOMOGRAPHY)) return fail(B200M_ERR_ARG, "bad arguments");
-  *out = nullptr;
-  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
-  CK(cudaSetDevice(c->device));
-  auto sl = c->slot_of.find(view_left), sr = c->slot_of.find(view_right);
-  if (sl == c->slot_of.end() || sr == c->slot_of.end()) return fail(B200M_ERR_ARG, "guided matching references a view that was never uploaded");
-  int rc;
-  if ((rc = ensure_view_ready(c, sl->second)) || (rc = ensure_view_ready(c, sr->second))) return rc;
-  if ((rc = wait_uploads(c))) return rc;
-  const ViewHost& vl = c->views[sl->second]; const ViewHost& vr = c->views[sr->second];
-  std::unique_ptr<b200m_result> res(new b200m_result());
-  res->pair_ids = {view_left, view_right};
-  res->offsets = {0, 0};
-  res->recycler = c->recycler;
-  const bool usable = vl.m > 0 && vr.m > 0 && vl.dtype == vr.dtype && vl.dim == vr.dim;      // common descriptor type, :300-306
-  if (usable) {
-    if (!((vl.dtype == DT_BIN && vl.dim == 64) || (vl.dtype != DT_BIN && vl.dim == 128)))
-      return fail(B200M_ERR_UNSUPPORTED, "guided matching takes 128-component scalar or 64-byte binary descriptors");
-    if ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom))
-      return fail(B200M_ERR_ARG, "guided matching needs feature positions (or geometry positions) for both views");
-    float* d_xy = nullptr; double2* d_xl = nullptr; double2* d_xr = nullptr; Rec* d_out = nullptr; int* d_cnt = nullptr;
-    cudaStream_t st = c->stream;
-    CK(cudaMallocAsync((void**)&d_xy, sizeof(float) * 2 * (size_t)std::max(vl.m, vr.m), st));
-    CK(cudaMallocAsync((void**)&d_xl, sizeof(double2) * (size_t)vl.m, st));
-    CK(cudaMallocAsync((void**)&d_xr, sizeof(double2) * (size_t)vr.m, st));
-    CK(cudaMallocAsync((void**)&d_out, sizeof(Rec) * (size_t)vl.m, st));
-    CK(cudaMallocAsync((void**)&d_cnt, sizeof(int), st));
-    CK(cudaMemsetAsync(d_cnt, 0, sizeof(int), st));
-    // a view's geometry positions (b200m_set_view_geometry) replace its widened float upload positions
-    if (!vl.d_geom) {
-      CK(cudaMemcpyAsync(d_xy, vl.xy.data(), sizeof(float) * 2 * (size_t)vl.m, cudaMemcpyHostToDevice, st));
-      positions_to_double_kernel<<<(vl.m + 255) / 256, 256, 0, st>>>(d_xy, vl.m, d_xl);
-      CK(cudaStreamSynchronize(st));                   // d_xy is reused for the right view
-    }
-    if (!vr.d_geom) {
-      CK(cudaMemcpyAsync(d_xy, vr.xy.data(), sizeof(float) * 2 * (size_t)vr.m, cudaMemcpyHostToDevice, st));
-      positions_to_double_kernel<<<(vr.m + 255) / 256, 256, 0, st>>>(d_xy, vr.m, d_xr);
-    }
-    const double2* xl = vl.d_geom ? vl.d_geom : d_xl;
-    const double2* xr = vr.d_geom ? vr.d_geom : d_xr;
-    GuidedParams P;
-    P.model = model == B200M_MODEL_HOMOGRAPHY ? GM_HOMOGRAPHY : GM_FUNDAMENTAL;
-    for (int k = 0; k < 9; ++k) P.F[k] = F[k];
-    P.errorTh = errorTh; P.distRatio = distRatio;
-    const int grid = (vl.m + GM_WARPS - 1) / GM_WARPS;
-    CK(cudaEventRecord(c->ev_start, st));
-    // integer-valued fp32 views are stored as uchar (same distances: exact integers); a pair of one such view and one real-valued
-    // fp32 view gets a temporary fp32 expansion of the former
-    const void* rawl = vl.raw; const void* rawr = vr.raw; float* tmp32 = nullptr;
-    int kdt = vl.store_dtype();
-    if (vl.store_dtype() != vr.store_dtype()) {
-      const ViewHost& vu = vl.stored_u8 ? vl : vr;
-      const size_t ne = (size_t)vu.m * 128;
-      CK(cudaMallocAsync((void**)&tmp32, ne * 4, st));
-      u8_to_f32_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>((const uint8_t*)vu.raw, tmp32, ne);
-      (vl.stored_u8 ? rawl : rawr) = tmp32;
-      kdt = DT_F32;
-    }
-    if (kdt == DT_F32) guided_top2_kernel<DT_F32><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, xl, xr, vl.m, vr.m, P, d_out, d_cnt);
-    else if (kdt == DT_U8) guided_top2_kernel<DT_U8><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, xl, xr, vl.m, vr.m, P, d_out, d_cnt);
-    else guided_top2_kernel<DT_BIN><<<grid, GM_WARPS * 32, 0, st>>>(rawl, rawr, xl, xr, vl.m, vr.m, P, d_out, d_cnt);
-    if (tmp32) cudaFreeAsync(tmp32, st);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(c->ev_end, st));
-    int n = 0;
-    CK(cudaMemcpyAsync(&n, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    std::vector<Rec> recs((size_t)n);
-    if (n) CK(cudaMemcpy(recs.data(), d_out, sizeof(Rec) * (size_t)n, cudaMemcpyDeviceToHost));
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
-    c->last = LastCall{ms, ms, 3, 0, 0, 0, n, 0};
-    cudaFreeAsync(d_xy, st); cudaFreeAsync(d_xl, st); cudaFreeAsync(d_xr, st); cudaFreeAsync(d_out, st); cudaFreeAsync(d_cnt, st);
-    // IndMatch::getDeduplicated (guidedMatching.hpp:267): one record per left feature, so this is a sort by (i, j)
-    std::sort(recs.begin(), recs.end(), [](const Rec& a, const Rec& b) { return a.i < b.i || (a.i == b.i && a.j < b.j); });
-    res->matches = c->recycler->take((size_t)std::max(n, 1));
-    for (int k = 0; k < n; ++k) res->matches.p[k] = b200m_match{recs[k].i, recs[k].j, 0.f, 0.f};    // IndMatch(i, j): ratio and distance default to 0
-    res->offsets[1] = n;
-  } else {
-    res->matches = c->recycler->take(1);
-    c->last = LastCall{};
-  }
-  *out = res.release();
-  return B200M_OK;
+  const uint32_t pair[2] = {view_left, view_right};
+  return b200m_guided_match_pairs(c, pair, 1, model, F, &errorTh, distRatio, out);
 }
 
 int b200m_set_view_geometry(b200m_ctx* c, uint32_t view_id, const double* xy, int n) {
@@ -1543,10 +1473,9 @@ int b200m_set_view_geometry(b200m_ctx* c, uint32_t view_id, const double* xy, in
 }  // extern "C"
 
 // ---- guided matching from known poses: guidedMatchingFundamentalFast for a list of pairs (guided_fast.cuh) -------------------
-template <class T> static int gf_exclusive_scan(b200m_ctx* c, const T* in, T* out, size_t n, cudaStream_t st, int& launches) {
+template <class T> static int exclusive_scan(DeviceBuffer<>& tmp, const T* in, T* out, size_t n, cudaStream_t st, int& launches) {
   size_t tb = 0;
   CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, (int64_t)n, st));
-  DeviceBuffer<>& tmp = c->gf.d[GuidedFastScratch::TEMP];
   if (int rc = tmp.reserve(tb)) return rc;
   CK(cub::DeviceScan::ExclusiveSum(tmp, tb, in, out, (int64_t)n, st));
   launches += 2;
@@ -1612,7 +1541,7 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
   unsigned long long *d_best = g.d[G::BEST].as<unsigned long long>(), *d_second = g.d[G::SECOND].as<unsigned long long>(),
                      *d_rcount = g.d[G::RCOUNT].as<unsigned long long>(), *d_rcoff = g.d[G::RCOFF].as<unsigned long long>();
   uint2* d_out = g.d[G::OUT].as<uint2>();
-  // the temporary storage of the three scans is taken inside gf_exclusive_scan; reserve it for the largest one first so that
+  // the temporary storage of the three scans is taken inside exclusive_scan; reserve it for the largest one first so that
   // no reallocation (a synchronising cudaFree) happens between launches
   { size_t tb = 0; CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_rcount, d_rcoff, (int64_t)std::max(sum_r + 1, std::max(sum_b, sum_l + 1)), st));
     if ((rc = g.d[G::TEMP].reserve(tb))) return rc; }
@@ -1630,11 +1559,11 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
   CK(cudaMemsetAsync(d_keep + sum_l, 0, sizeof(int), st));
   const dim3 gl((max_l + GF_THREADS - 1) / GF_THREADS, np), gr((max_r + GF_THREADS - 1) / GF_THREADS, np);
   guided_fast_left_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, d_lbucket, d_bcount, d_best, d_second);
-  if ((rc = gf_exclusive_scan(c, d_bcount, d_boff, (size_t)sum_b, st, launches))) return rc;
+  if ((rc = exclusive_scan(g.d[G::TEMP], d_bcount, d_boff, (size_t)sum_b, st, launches))) return rc;
   CK(cudaMemcpyAsync(d_bcount, d_boff, sizeof(int) * (size_t)sum_b, cudaMemcpyDeviceToDevice, st));   // scatter cursors
   guided_fast_scatter_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, d_lbucket, d_bcount, d_csr);
   guided_fast_right_kernel<<<gr, GF_THREADS, 0, st>>>(d_pairs, std::sqrt(errorTh), d_boff, d_rstart, d_rcount, d_rpair);
-  if ((rc = gf_exclusive_scan(c, d_rcount, d_rcoff, (size_t)sum_r + 1, st, launches))) return rc;
+  if ((rc = exclusive_scan(g.d[G::TEMP], d_rcount, d_rcoff, (size_t)sum_r + 1, st, launches))) return rc;
   CK(cudaEventRecord(g.ev_c0, st));
   const int cgrid = c->num_sms * 8;
   if (kclass == DT_U8) guided_fast_cand_kernel<DT_U8><<<cgrid, GF_THREADS, 0, st>>>(d_pairs, (int)sum_r, d_rcoff, d_rstart, d_rpair, d_csr, d_best, d_second);
@@ -1642,7 +1571,7 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
   else guided_fast_cand_kernel<DT_F32><<<cgrid, GF_THREADS, 0, st>>>(d_pairs, (int)sum_r, d_rcoff, d_rstart, d_rpair, d_csr, d_best, d_second);
   CK(cudaEventRecord(g.ev_c1, st));
   guided_fast_keep_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, distRatio, d_best, d_second, d_keep);
-  if ((rc = gf_exclusive_scan(c, d_keep, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+  if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
   guided_fast_emit_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, np, (int)sum_l, d_keep, d_kpos, d_best, d_out, d_pstart);
   CK(cudaGetLastError());
   launches += 5;
@@ -1739,6 +1668,166 @@ int b200m_guided_match_fast_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pai
   res->pair_ids.assign(pairs, pairs + 2 * (size_t)n_pairs);
   res->offsets.assign((size_t)n_pairs + 1, 0);
   for (int k = 0; k < n_pairs; ++k) res->offsets[k + 1] = res->offsets[k] + (int64_t)per_pair[k].size();
+  res->matches = c->recycler->take((size_t)std::max<int64_t>(res->offsets[n_pairs], 1));
+  for (int k = 0; k < n_pairs; ++k) {
+    b200m_match* m = res->matches.p + res->offsets[k];
+    for (const uint2& x : per_pair[k]) *m++ = b200m_match{x.x, x.y, 0.f, 0.f};     // IndMatch(i, j): ratio and distance 0
+  }
+  *out = res.release();
+  return B200M_OK;
+}
+
+}  // extern "C"
+
+// ---- guided matching for a list of pairs, one model each (guided.cuh); b200m_guided_match(_model) are lists of one -------------
+// One batch of pairs of one kernel class.  per_pair[index] receives the pair's matches.
+static int gm_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int model, const double* M, const double* errorTh, double distRatio,
+                        std::vector<std::vector<uint2>>& per_pair, double& gpu_ms, double& search_ms, int& launches) {
+  GuidedScratch& g = c->gm;
+  using G = GuidedScratch;
+  cudaStream_t st = c->stream;
+  const int np = (int)batch.size();
+  const int kclass = batch[0].kclass;
+  // uchar-stored views of mixed pairs: one fp32 expansion each
+  std::map<int, size_t> exp_off; size_t exp_elems = 0;
+  if (kclass == 3)
+    for (const auto& p : batch) {
+      const int s = c->views[p.slot_l].stored_u8 ? p.slot_l : p.slot_r;
+      if (!exp_off.count(s)) { exp_off[s] = exp_elems; exp_elems += (size_t)c->views[s].m * 128; }
+    }
+  int rc;
+  if ((rc = g.h_pairs.reserve(sizeof(GuidedPair) * (size_t)np)) || (rc = g.d[G::EXPAND].reserve(sizeof(float) * exp_elems))) return rc;
+  GuidedPair* hp = g.h_pairs;
+  float* d_exp = g.d[G::EXPAND].as<float>();
+  long sum_l = 0, blocks = 0;
+  for (int k = 0; k < np; ++k) {
+    const GfPairHost& q = batch[k];
+    const ViewHost& vl = c->views[q.slot_l]; const ViewHost& vr = c->views[q.slot_r];
+    GuidedPair& P = hp[k];
+    std::memset(&P, 0, sizeof(P));
+    P.rawl = vl.raw; P.rawr = vr.raw;
+    if (kclass == 3) {
+      if (vl.stored_u8) P.rawl = d_exp + exp_off[q.slot_l]; else P.rawr = d_exp + exp_off[q.slot_r];
+    }
+    P.gl = vl.d_geom; P.gr = vr.d_geom; P.fl = (const float2*)vl.d_xy; P.fr = (const float2*)vr.d_xy;
+    for (int t = 0; t < 9; ++t) P.M[t] = M[9 * (size_t)q.index + t];
+    P.errorTh = errorTh[q.index];
+    P.model = model == B200M_MODEL_HOMOGRAPHY ? GM_HOMOGRAPHY : GM_FUNDAMENTAL;
+    P.ml = vl.m; P.mr = vr.m;
+    P.block_base = (int)blocks; P.left_base = (int)sum_l;
+    blocks += (vl.m + GM_WARPS - 1) / GM_WARPS; sum_l += vl.m;
+  }
+  const size_t i4 = sizeof(int), hdr = (size_t)(np + 2) / 2;      // hdr: uint2 words in front of the matches holding the np + 1 starts
+  if ((rc = g.d[G::PAIRS].reserve(sizeof(GuidedPair) * np)) || (rc = g.d[G::BESTJ].reserve(i4 * sum_l)) || (rc = g.d[G::KEEP].reserve(i4 * (sum_l + 1))) ||
+      (rc = g.d[G::KPOS].reserve(i4 * (sum_l + 1))) || (rc = g.d[G::OUT].reserve(sizeof(uint2) * (hdr + sum_l))) ||
+      (rc = g.h_out.reserve(sizeof(uint2) * (hdr + sum_l))))
+    return rc;
+  GuidedPair* d_pairs = g.d[G::PAIRS].as<GuidedPair>();
+  int *d_bestj = g.d[G::BESTJ].as<int>(), *d_keep = g.d[G::KEEP].as<int>(), *d_kpos = g.d[G::KPOS].as<int>();
+  uint2* d_out = g.d[G::OUT].as<uint2>();
+  // reserve the scan's temporary storage before the first launch: no reallocation (a synchronising cudaFree) between launches
+  { size_t tb = 0; CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_keep, d_kpos, (int64_t)(sum_l + 1), st));
+    if ((rc = g.d[G::TEMP].reserve(tb))) return rc; }
+  if ((rc = g.ev_k0.create()) || (rc = g.ev_k1.create())) return rc;
+  CK(cudaEventRecord(c->ev_start, st));
+  CK(cudaMemcpyAsync(d_pairs, hp, sizeof(GuidedPair) * (size_t)np, cudaMemcpyHostToDevice, st));
+  for (const auto& x : exp_off) {
+    const ViewHost& vu = c->views[x.first];
+    const size_t ne = (size_t)vu.m * 128;
+    u8_to_f32_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>((const uint8_t*)vu.raw, d_exp + x.second, ne);
+    ++launches;
+  }
+  CK(cudaMemsetAsync(d_keep + sum_l, 0, sizeof(int), st));
+  CK(cudaEventRecord(g.ev_k0, st));
+  if (kclass == DT_U8) guided_pairs_kernel<DT_U8><<<(unsigned)blocks, GM_WARPS * 32, 0, st>>>(d_pairs, np, distRatio, d_bestj, d_keep);
+  else if (kclass == DT_BIN) guided_pairs_kernel<DT_BIN><<<(unsigned)blocks, GM_WARPS * 32, 0, st>>>(d_pairs, np, distRatio, d_bestj, d_keep);
+  else guided_pairs_kernel<DT_F32><<<(unsigned)blocks, GM_WARPS * 32, 0, st>>>(d_pairs, np, distRatio, d_bestj, d_keep);
+  CK(cudaEventRecord(g.ev_k1, st));
+  if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+  const long emit_threads = std::max(sum_l, (long)np + 1);
+  guided_pairs_emit_kernel<<<(unsigned)((emit_threads + 255) / 256), 256, 0, st>>>(d_pairs, np, (int)sum_l, d_bestj, d_keep, d_kpos, d_out + hdr,
+                                                                                  reinterpret_cast<int*>(d_out));
+  CK(cudaGetLastError());
+  launches += 2;
+  CK(cudaEventRecord(c->ev_end, st));
+  // one read-back: the per-pair starts and every slot the matches may occupy
+  CK(cudaMemcpyAsync(g.h_out, d_out, sizeof(uint2) * (hdr + sum_l), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0.f, kms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
+  CK(cudaEventElapsedTime(&kms, g.ev_k0, g.ev_k1));
+  gpu_ms += ms; search_ms += kms;
+  const int* h_pstart = g.h_out.as<int>();
+  const uint2* h = g.h_out.as<uint2>() + hdr;
+  for (int k = 0; k < np; ++k) per_pair[batch[k].index].assign(h + h_pstart[k], h + h_pstart[k + 1]);
+  return B200M_OK;
+}
+
+extern "C" {
+
+int b200m_guided_match_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, int model, const double* M, const double* errorTh, double distRatio,
+                             b200m_result** out) {
+  if (!c || !out || n_pairs < 0 || (model != B200M_MODEL_FUNDAMENTAL && model != B200M_MODEL_HOMOGRAPHY) ||
+      (n_pairs > 0 && (!pairs || !M || !errorTh)))
+    return fail(B200M_ERR_ARG, "bad arguments");
+  *out = nullptr;
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  CK(cudaSetDevice(c->device));
+  // checks first: nothing runs for a list with a bad entry
+  std::vector<GfPairHost> work;
+  for (int k = 0; k < n_pairs; ++k) {
+    auto sl = c->slot_of.find(pairs[2 * k]), sr = c->slot_of.find(pairs[2 * k + 1]);
+    if (sl == c->slot_of.end() || sr == c->slot_of.end()) return fail(B200M_ERR_ARG, "guided matching references a view that was never uploaded");
+    const ViewHost& vl = c->views[sl->second]; const ViewHost& vr = c->views[sr->second];
+    if (!(vl.m > 0 && vr.m > 0 && vl.dtype == vr.dtype && vl.dim == vr.dim)) continue;     // common descriptor type, :300-306; else empty
+    if (!((vl.dtype == DT_BIN && vl.dim == 64) || (vl.dtype != DT_BIN && vl.dim == 128)))
+      return fail(B200M_ERR_UNSUPPORTED, "guided matching takes 128-component scalar or 64-byte binary descriptors");
+    if ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom))
+      return fail(B200M_ERR_ARG, "guided matching needs feature positions (or geometry positions) for both views");
+    work.push_back({k, sl->second, sr->second, 0});
+  }
+  std::vector<std::vector<uint2>> per_pair((size_t)n_pairs);
+  double gpu_ms = 0, search_ms = 0; int launches = 0;
+  // Batches as in b200m_guided_match_fast_pairs: the list is walked once in input order and every pair joins the open batch of its
+  // kernel class (uchar, fp32, mixed, binary); a batch runs when its pairs (the pinned and device pair tables), left features (a pair
+  // larger than the bound runs alone) or fp32 expansions would pass their bound, and the rest at the end.  Each view is waited for when
+  // its first pair is reached.
+  const long pair_cap = 8192, exp_cap = 64l << 20;
+  struct Open { std::vector<GfPairHost> pairs; long l = 0, e = 0; std::set<int> exp_views; };
+  Open open[4];
+  auto flush = [&](Open& o) -> int {
+    if (o.pairs.empty()) return B200M_OK;
+    const int rc = gm_run_batch(c, o.pairs, model, M, errorTh, distRatio, per_pair, gpu_ms, search_ms, launches);
+    o = Open();
+    return rc;
+  };
+  for (GfPairHost p : work) {
+    int rc;
+    if ((rc = ensure_view_ready(c, p.slot_l)) || (rc = ensure_view_ready(c, p.slot_r))) return rc;
+    // the stored type is final once the view is ready (a uchar-staged view that met a non-integer value was re-uploaded as fp32)
+    const ViewHost& vl = c->views[p.slot_l]; const ViewHost& vr = c->views[p.slot_r];
+    p.kclass = vl.store_dtype() == vr.store_dtype() ? vl.store_dtype() : 3;
+    Open& o = open[p.kclass];
+    const int su = p.kclass == 3 ? (vl.stored_u8 ? p.slot_l : p.slot_r) : -1;
+    long ne = su >= 0 && !o.exp_views.count(su) ? (long)c->views[su].m * 128 : 0;
+    if (!o.pairs.empty() && ((long)o.pairs.size() + 1 > pair_cap || o.l + vl.m > c->gm_left_cap || o.e + ne > exp_cap)) {
+      if ((rc = flush(o))) return rc;
+      ne = su >= 0 ? (long)c->views[su].m * 128 : 0;
+    }
+    o.pairs.push_back(p);
+    o.l += vl.m; o.e += ne;
+    if (su >= 0) o.exp_views.insert(su);
+  }
+  for (Open& o : open)
+    if (int rc = flush(o)) return rc;
+  if (int rc = wait_uploads(c)) return rc;
+  // one result pair per input pair, in input order (empty lists included)
+  std::unique_ptr<b200m_result> res(new b200m_result());
+  res->recycler = c->recycler;
+  res->pair_ids.assign(pairs, pairs + 2 * (size_t)n_pairs);
+  res->offsets.assign((size_t)n_pairs + 1, 0);
+  for (int k = 0; k < n_pairs; ++k) res->offsets[k + 1] = res->offsets[k] + (int64_t)per_pair[k].size();
+  c->last = LastCall{gpu_ms, search_ms, launches, 0, 0, 0, res->offsets[n_pairs], 0};
   res->matches = c->recycler->take((size_t)std::max<int64_t>(res->offsets[n_pairs], 1));
   for (int k = 0; k < n_pairs; ++k) {
     b200m_match* m = res->matches.p + res->offsets[k];

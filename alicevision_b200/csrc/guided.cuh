@@ -12,6 +12,11 @@
 //
 // One warp per left feature; the right positions stream through shared memory; survivors are queued per warp and their
 // distances evaluated eight at a time (4 lanes per candidate = the 4 SSE lanes).
+//
+// A whole list of pairs runs per launch (b200m_guided_match_pairs; the one-pair calls are lists of one): the work items are
+// (pair, block of GM_WARPS left features), the items of one pair adjacent; per-pair parameters sit in a device table.  Each
+// (pair, left i) writes its best j or -1 to a flat slot array, and an exclusive scan of the keep flags places each pair's list in
+// ascending i.  There is one record per left feature, so IndMatch::getDeduplicated (guidedMatching.hpp:267) changes nothing.
 #pragma once
 #include "common.cuh"
 
@@ -25,12 +30,23 @@ constexpr int GM_QUEUE = 40;         // >= 8 + 32: survivors of one 32-wide step
 
 enum : int { GM_FUNDAMENTAL = 0, GM_HOMOGRAPHY = 1 };
 
-struct GuidedParams {
-  int model;            // GM_FUNDAMENTAL: FundamentalEpipolarDistanceError; GM_HOMOGRAPHY: HomographyAsymmetricError (HomographyError.hpp:23-31)
-  double F[9];          // row-major model matrix: fundamental (x_right^T F x_left = 0) or homography (x_right ~ H x_left)
+struct GuidedPair {
+  const void* rawl; const void* rawr;           // descriptors (kernel dtype: a uchar-stored view of a mixed pair points at its fp32 expansion)
+  const double2* gl; const double2* gr;         // geometry positions, or nullptr: the float upload positions below, widened
+  const float2* fl; const float2* fr;
+  double M[9];          // row-major model matrix: fundamental (x_right^T F x_left = 0) or homography (x_right ~ H x_left)
   double errorTh;       // Square(precision), guidedMatching.hpp:211 / GeometricFilterMatrix_F_AC.hpp:387
-  double distRatio;     // Square(distance ratio), :388
+  int model;            // GM_FUNDAMENTAL: FundamentalEpipolarDistanceError; GM_HOMOGRAPHY: HomographyAsymmetricError (HomographyError.hpp:23-31)
+  int ml, mr;
+  int block_base;       // first block of this pair in the launch (blocks of one pair are adjacent: the right view is reused out of L2)
+  int left_base;        // first slot of this pair in the flat per-batch arrays
 };
+
+__device__ __forceinline__ double2 guided_pos(const double2* g, const float2* f, int k) {
+  if (g) return g[k];
+  const float2 v = f[k];
+  return make_double2((double)v.x, (double)v.y);
+}
 
 // distance of candidate descriptors a (left) and b (right) evaluated by the 4 lanes of a group; returns the value on every lane of the group
 template <int DTYPE>
@@ -67,24 +83,24 @@ __device__ __forceinline__ double guided_distance(const void* __restrict__ left,
   return (double)__fadd_rn(__fadd_rn(s0123, s2), s3);                 // ((s0+s1)+s2)+s3, metric.hpp:112-116
 }
 
+// The K7 body for left feature i of pair P, one warp per left feature; every thread of the block calls it for the same pair (the
+// right positions stream through the block's shared tile).  The geometric gate, the survivor queue, the descriptor distances and
+// the distanceRatio fold; returns the kept right feature, or -1, on every lane.
 template <int DTYPE>
-__global__ void __launch_bounds__(GM_WARPS * 32)
-guided_top2_kernel(const void* __restrict__ left, const void* __restrict__ right, const double2* __restrict__ xl, const double2* __restrict__ xr,
-                   int m_l, int m_r, GuidedParams P, Rec* __restrict__ out, int* __restrict__ out_count) {
-  __shared__ double2 tile[GM_TILE];
-  __shared__ int queue[GM_WARPS][GM_QUEUE];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int i = blockIdx.x * GM_WARPS + warp;
-  const bool live = i < m_l;
+__device__ __forceinline__ int guided_row(const GuidedPair& P, int i, double distRatio, double2* tile, int* queue) {
+  const int lane = threadIdx.x & 31;
+  const bool live = i < P.ml;
+  const int model = P.model, m_r = P.mr;
+  const double errorTh = P.errorTh;
   // epipolar line of the left point in the right image: F_x = F * (x, y, 1), row r = (F(r,0)*x + F(r,1)*y) + F(r,2)*1
   double fx0 = 0, fx1 = 0, fx2 = 0, nrm = 1;
   if (live) {
-    const double2 x = xl[i];
-    fx0 = __dadd_rn(__dadd_rn(__dmul_rn(P.F[0], x.x), __dmul_rn(P.F[1], x.y)), P.F[2]);
-    fx1 = __dadd_rn(__dadd_rn(__dmul_rn(P.F[3], x.x), __dmul_rn(P.F[4], x.y)), P.F[5]);
-    fx2 = __dadd_rn(__dadd_rn(__dmul_rn(P.F[6], x.x), __dmul_rn(P.F[7], x.y)), P.F[8]);
+    const double2 x = guided_pos(P.gl, P.fl, i);
+    fx0 = __dadd_rn(__dadd_rn(__dmul_rn(P.M[0], x.x), __dmul_rn(P.M[1], x.y)), P.M[2]);
+    fx1 = __dadd_rn(__dadd_rn(__dmul_rn(P.M[3], x.x), __dmul_rn(P.M[4], x.y)), P.M[5]);
+    fx2 = __dadd_rn(__dadd_rn(__dmul_rn(P.M[6], x.x), __dmul_rn(P.M[7], x.y)), P.M[8]);
     nrm = __dadd_rn(__dmul_rn(fx0, fx0), __dmul_rn(fx1, fx1));      // F_x.head<2>().squaredNorm()
-    if (P.model == GM_HOMOGRAPHY) { fx0 = __ddiv_rn(fx0, fx2); fx1 = __ddiv_rn(fx1, fx2); }   // x2_est = x2h_est.head<2>() / x2h_est[2]
+    if (model == GM_HOMOGRAPHY) { fx0 = __ddiv_rn(fx0, fx2); fx1 = __ddiv_rn(fx1, fx2); }   // x2_est = x2h_est.head<2>() / x2h_est[2]
   }
   double bd = DBL_MAX, sbd = DBL_MAX; int idx = 0;                   // distanceRatio<double>, guidedMatching.hpp:77-90
   int nq = 0;
@@ -92,9 +108,9 @@ guided_top2_kernel(const void* __restrict__ left, const void* __restrict__ right
   const unsigned gmask = 0xFu << (grp * 4);
 
   auto drain = [&](int count) {                                       // evaluate `count` (<= 8) queued candidates, oldest first
-    const int j = grp < count ? queue[warp][grp] : -1;
+    const int j = grp < count ? queue[grp] : -1;
     double d = 0;
-    if (j >= 0) d = guided_distance<DTYPE>(left, right, i, j, sub, gmask);
+    if (j >= 0) d = guided_distance<DTYPE>(P.rawl, P.rawr, i, j, sub, gmask);
     for (int g = 0; g < count; ++g) {                                 // distanceRatio::update in ascending j (:95-110)
       const double dist = __shfl_sync(0xffffffffu, d, g * 4);
       const int jj = __shfl_sync(0xffffffffu, j, g * 4);
@@ -105,7 +121,7 @@ guided_top2_kernel(const void* __restrict__ left, const void* __restrict__ right
 
   for (int t0 = 0; t0 < m_r; t0 += GM_TILE) {
     __syncthreads();
-    for (int e = threadIdx.x; e < GM_TILE && t0 + e < m_r; e += GM_WARPS * 32) tile[e] = xr[t0 + e];
+    for (int e = threadIdx.x; e < GM_TILE && t0 + e < m_r; e += GM_WARPS * 32) tile[e] = guided_pos(P.gr, P.fr, t0 + e);
     __syncthreads();
     if (!live) continue;
     const int n = min(GM_TILE, m_r - t0);
@@ -115,45 +131,63 @@ guided_top2_kernel(const void* __restrict__ left, const void* __restrict__ right
       if (e < n) {
         const double2 y = tile[e];
         double err;
-        if (P.model == GM_HOMOGRAPHY) {
+        if (model == GM_HOMOGRAPHY) {
           const double d0 = __dsub_rn(y.x, fx0), d1 = __dsub_rn(y.y, fx1);                            // (x2 - x2_est).squaredNorm()
           err = __dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1));
         } else {
           const double dot = __dadd_rn(__dadd_rn(__dmul_rn(fx0, y.x), __dmul_rn(fx1, y.y)), fx2);    // F_x.dot((y, 1))
           err = __ddiv_rn(__dmul_rn(dot, dot), nrm);                                                  // Square(dot) / squaredNorm
         }
-        pass = err < P.errorTh;                                                                       // guidedMatching.hpp:252
+        pass = err < errorTh;                                                                         // guidedMatching.hpp:252
       }
       const unsigned m = __ballot_sync(0xffffffffu, pass);
       if (m) {
-        if (pass) queue[warp][nq + __popc(m & ((1u << lane) - 1))] = t0 + e;
+        if (pass) queue[nq + __popc(m & ((1u << lane) - 1))] = t0 + e;
         nq += __popc(m);
         __syncwarp();
         while (nq >= 8) {
           drain(8);
           __syncwarp();
           const int rest = nq - 8;                                    // shift the remaining entries to the front
-          const int v = lane < rest ? queue[warp][8 + lane] : 0;
+          const int v = lane < rest ? queue[8 + lane] : 0;
           __syncwarp();
-          if (lane < rest) queue[warp][lane] = v;
+          if (lane < rest) queue[lane] = v;
           nq = rest;
           __syncwarp();
         }
       }
     }
   }
-  if (!live) return;
+  if (!live) return -1;
   if (nq > 0) drain(nq);
   // distanceRatio::isValid (:115-118) and the emitted pair (:259-263)
-  if (lane == 0 && sbd != DBL_MAX && bd < __dmul_rn(P.distRatio, sbd)) {
-    const int slot = atomicAdd(out_count, 1);
-    out[slot] = Rec{(uint32_t)i, (uint32_t)idx, (float)bd, (float)sbd};
-  }
+  return sbd != DBL_MAX && bd < __dmul_rn(distRatio, sbd) ? idx : -1;
 }
 
-__global__ void positions_to_double_kernel(const float* __restrict__ xy, int n, double2* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = make_double2((double)xy[2 * i], (double)xy[2 * i + 1]);
+// One launch per kernel class and batch: block b runs GM_WARPS left features of the pair whose blocks contain b.  Every (pair, left i)
+// writes its kept right feature or -1 to best_j and the keep flag of the ordered compaction to keep.
+template <int DTYPE>
+__global__ void __launch_bounds__(GM_WARPS * 32)
+guided_pairs_kernel(const GuidedPair* __restrict__ pairs, int n_pairs, double distRatio, int* __restrict__ best_j, int* __restrict__ keep) {
+  __shared__ double2 tile[GM_TILE];
+  __shared__ int queue[GM_WARPS][GM_QUEUE];
+  int lo = 0, hi = n_pairs;                                           // last pair with block_base <= blockIdx.x
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pairs[mid].block_base <= (int)blockIdx.x) lo = mid; else hi = mid; }
+  const GuidedPair& P = pairs[lo];
+  const int warp = threadIdx.x >> 5;
+  const int i = ((int)blockIdx.x - P.block_base) * GM_WARPS + warp;
+  const int j = guided_row<DTYPE>(P, i, distRatio, tile, queue[warp]);
+  if (i < P.ml && (threadIdx.x & 31) == 0) { best_j[P.left_base + i] = j; keep[P.left_base + i] = j >= 0; }
 }
 
+// ordered compaction: kept (i, j) at kpos[g] (ascending i per pair, pairs in batch order); pstart[p] = first output of pair p
+__global__ void guided_pairs_emit_kernel(const GuidedPair* __restrict__ pairs, int n_pairs, int n_left, const int* __restrict__ best_j,
+                                         const int* __restrict__ keep, const int* __restrict__ kpos, uint2* __restrict__ out, int* __restrict__ pstart) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g <= n_pairs) pstart[g] = kpos[g < n_pairs ? pairs[g].left_base : n_left];
+  if (g >= n_left || !keep[g]) return;
+  int lo = 0, hi = n_pairs;                                           // last pair with left_base <= g
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pairs[mid].left_base <= g) lo = mid; else hi = mid; }
+  out[kpos[g]] = make_uint2((unsigned)(g - pairs[lo].left_base), (unsigned)best_j[g]);
+}
 }  // namespace b200m

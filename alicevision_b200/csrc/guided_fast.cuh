@@ -83,12 +83,6 @@ __device__ __forceinline__ void gf_cross(const FastPair& P, double x, double y, 
   l2 = __dsub_rn(__dmul_rn(P.e0, y), __dmul_rn(P.e1, x));
 }
 
-__device__ __forceinline__ double2 gf_pos(const double2* g, const float2* f, int k) {
-  if (g) return g[k];
-  const float2 v = f[k];
-  return make_double2((double)v.x, (double)v.y);
-}
-
 // grid (features / GF_THREADS, pairs): bucket of every left feature, counts per (pair, bucket); keys reset to the sentinel
 __global__ void __launch_bounds__(GF_THREADS)
 guided_fast_left_kernel(const FastPair* __restrict__ pairs, int* __restrict__ lbucket, int* __restrict__ bcount,
@@ -96,7 +90,7 @@ guided_fast_left_kernel(const FastPair* __restrict__ pairs, int* __restrict__ lb
   const FastPair& P = pairs[blockIdx.y];
   const int i = blockIdx.x * GF_THREADS + threadIdx.x;
   if (i >= P.ml) return;
-  const double2 x = gf_pos(P.gl, P.fl, i);
+  const double2 x = guided_pos(P.gl, P.fl, i);
   // line = F * (x, y, 1), row r = (F(r,0) x + F(r,1) y) + F(r,2)
   const double a = __dadd_rn(__dadd_rn(__dmul_rn(P.F[0], x.x), __dmul_rn(P.F[1], x.y)), P.F[2]);
   const double b = __dadd_rn(__dadd_rn(__dmul_rn(P.F[3], x.x), __dmul_rn(P.F[4], x.y)), P.F[5]);
@@ -126,7 +120,7 @@ guided_fast_right_kernel(const FastPair* __restrict__ pairs, double sqrt_th, con
   const int j = blockIdx.x * GF_THREADS + threadIdx.x;
   if (j >= P.mr) return;
   const int r = P.right_base + j;
-  const double2 x = gf_pos(P.gr, P.fr, j);
+  const double2 x = guided_pos(P.gr, P.fr, j);
   double l0, l1, l2;
   gf_cross(P, x.x, x.y, l0, l1, l2);
   const double s = __ddiv_rn(sqrt_th, __dsqrt_rn(__dadd_rn(__dmul_rn(l0, l0), __dmul_rn(l1, l1))));   // sqrt(errorTh) / l2.head<2>().norm()

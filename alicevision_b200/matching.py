@@ -26,6 +26,7 @@ LIB_PATH = os.path.join(_HERE, "libb200match.so")
 F32, U8, BIN = 0, 1, 2
 L2_SIMPLE, L2_VECTORIZED, HAMMING = 0, 1, 2
 STAGE_DEVICE, STAGE_RAW, STAGE_FULL = 0, 1, 2
+MODEL_FUNDAMENTAL, MODEL_HOMOGRAPHY = 0, 1
 
 MATCH_DTYPE = np.dtype([("i", np.uint32), ("j", np.uint32), ("ratio", np.float32), ("dist", np.float32)])
 
@@ -38,7 +39,7 @@ ABI_SYMBOLS = [
     "b200m_shard_pairs", "b200m_shard_pairs_2d", "b200m_multi_create", "b200m_multi_destroy", "b200m_multi_num_devices", "b200m_multi_ctx", "b200m_multi_match",
     "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model", "b200m_set_view_geometry", "b200m_guided_match_fast_pairs",
     "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
-    "b200m_mt19937_seed", "b200m_debug_rand_sample", "b200m_acransac_homography_pairs", "b200m_debug_rand_sample_k",
+    "b200m_mt19937_seed", "b200m_debug_rand_sample", "b200m_acransac_homography_pairs", "b200m_debug_rand_sample_k", "b200m_guided_match_pairs",
 ]
 
 
@@ -187,6 +188,25 @@ class Context:
         matches = _alias(mat.value, int(offsets[-1]) * MATCH_DTYPE.itemsize, MATCH_DTYPE, owner)
         return {(int(a), int(b)): matches[offsets[k]:offsets[k + 1]].copy() for k, (a, b) in enumerate(p.tolist())}
 
+    def guided_match_pairs(self, pairs, M, errorTh, distRatio: float, model: int = MODEL_FUNDAMENTAL) -> list:
+        """b200m_guided_match_pairs on resident views: guidedMatching (matching/guidedMatching.hpp:206-268) for every (L, R) of `pairs`
+        with its own model M [n, 3, 3] (MODEL_FUNDAMENTAL: x_R^T F x_L = 0; MODEL_HOMOGRAPHY: x_R ~ H x_L) and errorTh [n], already
+        squared; distRatio already squared, one for the call.  Returns one matches[MATCH_DTYPE] per input pair, in input order (a pair
+        may appear more than once): ascending i, ratio and distance 0."""
+        p = np.ascontiguousarray(pairs, np.uint32).reshape(-1, 2)
+        n = p.shape[0]
+        Mm = np.ascontiguousarray(M, np.float64).reshape(n, 9)
+        th = np.ascontiguousarray(errorTh, np.float64).reshape(n)
+        res = C.c_void_p()
+        _check(self.lib.b200m_guided_match_pairs(self._h, p.ctypes.data_as(C.c_void_p), C.c_int(n), C.c_int(model), Mm.ctypes.data_as(C.c_void_p),
+                                                 th.ctypes.data_as(C.c_void_p), C.c_double(distRatio), C.byref(res)), "b200m_guided_match_pairs")
+        owner = _ResultOwner(self.lib, res)
+        off, mat = C.c_void_p(), C.c_void_p()
+        _check(self.lib.b200m_result_get(res, None, C.byref(off), C.byref(mat)), "b200m_result_get")
+        offsets = _alias(off.value, (n + 1) * 8, np.int64, owner) if n else np.zeros(1, np.int64)
+        matches = _alias(mat.value, int(offsets[-1]) * MATCH_DTYPE.itemsize, MATCH_DTYPE, owner)
+        return [matches[offsets[k]:offsets[k + 1]].copy() for k in range(n)]
+
     def set_acransac_skip(self, on: bool) -> None:
         """Debug: the certified skip of models that cannot beat the running minNFA (on by default); results do not depend on it."""
         _check(self.lib.b200m_ctx_set_acransac_skip(self._h, C.c_int(int(on))), "b200m_ctx_set_acransac_skip")
@@ -289,6 +309,116 @@ def geometricEstimation_H_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: 
     st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else seed_or_state
     corr = np.concatenate([np.asarray(xI, np.float64).reshape(-1, 2), np.asarray(xJ, np.float64).reshape(-1, 2)], axis=1)
     return ctx.acransac_homography_pairs([corr], [tuple(sizeI) + tuple(sizeJ)], st, maxIteration, precision)[0]
+
+
+# EImageDescriberType in enum order (feature/imageDescriberCommon.hpp:19-55): getCommonDescTypes returns the common types in this order
+DESCRIBER_TYPES = ["sift", "sift_float", "sift_upright", "dspsift", "akaze", "akaze_liop", "akaze_mldb", "cctag3", "cctag4", "sift_ocv", "akaze_ocv",
+                   "tag16h5"]
+# feature::getStrongSupportCoeff (imageDescriberCommon.hpp:103-140)
+STRONG_SUPPORT_COEFF = {t: 1.0 if t in ("cctag3", "cctag4", "tag16h5") else 0.14 for t in DESCRIBER_TYPES}
+
+
+def copyInlierMatches(inliers, putatives_per_type: dict, desc_types) -> dict:
+    """matchingImageCollection::copyInlierMatches (geometricFilterUtils.cpp:13-37): the inlier indices, sorted ascending, index the
+    putative matches concatenated in `desc_types` order; each is copied (ratio and distance kept) into the list of its type.  Types
+    without an inlier get no entry."""
+    order = np.sort(np.asarray(inliers, np.int64))
+    out, start = {}, 0
+    for t in desc_types:
+        m = putatives_per_type.get(t, np.zeros(0, MATCH_DTYPE))
+        sel = order[(order >= start) & (order < start + len(m))] - start
+        if sel.size:
+            out[t] = m[sel].copy()
+        start += len(m)
+    return out
+
+
+def hasStrongSupport(matches_per_type: dict, minimumSamples: int = 7) -> bool:
+    """matching::hasStrongSupport(MatchesPerDescType, minimumSamples) (supportEstimation.cpp:48-59): the float sum over the types, in
+    enum order, of getStrongSupportCoeff(type) * count must exceed minimumSamples (7 for Fundamental7PSolver)."""
+    score = np.float32(0)
+    for t in sorted(matches_per_type, key=DESCRIBER_TYPES.index):
+        score = np.float32(score + np.float32(STRONG_SUPPORT_COEFF[t]) * np.float32(len(matches_per_type[t])))
+    return bool(score > minimumSamples)
+
+
+def robustModelEstimation_F_AC(putatives: dict, regions_per_view: dict, image_sizes: dict, seed_or_state, maxIteration: int = 50000,
+                               precision: float = np.inf, guidedMatching: bool = False, distanceRatio: float = 0.6, geometry: dict | None = None,
+                               guided_geometry: dict | None = None, desc_types=None, ctx: Context | None = None):
+    """matchingImageCollection::robustModelEstimation with GeometricFilterMatrix_F_AC (ACRANSAC, Fundamental7PSolver; GeometricFilter.hpp:40-88),
+    the default `fundamental_matrix` filter of featureMatching, for a whole putative list: one a-contrario RANSAC call for every pair
+    (b200m_acransac_fundamental_pairs), then, with guidedMatching, one guided-matching call for every kept pair and common descriptor
+    type (b200m_guided_match_pairs).
+
+    putatives        {(I, J): {describer type: matches[MATCH_DTYPE]}}
+    regions_per_view {view: {describer type: Regions}}
+    image_sizes      {view: (width, height)}
+    seed_or_state    the caller's std::mt19937 (seed or 625-word state): every pair starts from it, as geometricEstimation_Mat_ACRANSAC
+                     takes the generator by value (GeometricFilterMatrix_F_AC.hpp:271)
+    geometry         optional {view: {type: n x 2 double}}: the undistorted positions of a view whose camera isValid() && hasDistortion()
+                     (fillMatricesWithUndistortFeaturesMatches, geometricFilterUtils.hpp:36-66); otherwise the regions' positions
+    guided_geometry  optional {view: {type: n x 2 double}}: getUndistortedPixel of every feature of a view whose camera isValid()
+                     (guidedMatching.hpp:229-248), the positions guided matching uses
+    desc_types       the describer types in EImageDescriberType order (default DESCRIBER_TYPES)
+
+    Returns (geometric matches {(I, J): {type: matches}} of the pairs with strong support, per-pair estimation
+    {(I, J): {"valid", "strong_support", "F", "error_max"}}).  Without guided matching the kept lists are the inlier putatives (ratio
+    and distance kept); with it, the guided lists of every common type (empty ones included) replace them, or nothing when error_max
+    is infinite (GeometricFilterMatrix_F_AC.hpp:363)."""
+    ctx = ctx or default_context()
+    order = list(desc_types) if desc_types is not None else DESCRIBER_TYPES
+    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
+    geometry = geometry or {}
+    pairs = list(putatives)
+    common = {p: [t for t in order if t in regions_per_view[p[0]] and t in regions_per_view[p[1]]] for p in pairs}
+
+    def positions(v, t):
+        g = geometry.get(v, {}).get(t)
+        return np.asarray(g, np.float64).reshape(-1, 2) if g is not None else regions_per_view[v][t].positions.astype(np.float64)
+
+    est = [p for p in pairs if common[p]]                     # no common type: EstimationStatus(false, false)
+    corrs, whs = [], []
+    for I, J in est:
+        parts = [np.zeros((0, 4))]
+        for t in common[(I, J)]:
+            m = putatives[(I, J)].get(t)
+            if m is not None and len(m):
+                parts.append(np.concatenate([positions(I, t)[m["i"]], positions(J, t)[m["j"]]], axis=1))
+        corrs.append(np.concatenate(parts))
+        whs.append(tuple(image_sizes[I]) + tuple(image_sizes[J]))
+    res = ctx.acransac_fundamental_pairs(corrs, whs, st, maxIteration, precision) if est else []
+    info = {p: {"valid": False, "strong_support": False, "F": np.zeros((3, 3)), "error_max": np.inf} for p in pairs}
+    out = {}
+    for p, r in zip(est, res):
+        info[p].update(valid=r["valid"], F=r["F"], error_max=r["error_max"])
+        if not r["valid"]:
+            continue
+        inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
+        info[p]["strong_support"] = hasStrongSupport(inl)
+        if info[p]["strong_support"]:
+            out[p] = inl
+    if guidedMatching and out:
+        guided = [p for p in out if np.isfinite(info[p]["error_max"])]
+        for p in out:
+            out[p] = {}
+        ids, up = {}, []
+        try:
+            for I, J in guided:
+                for t in common[(I, J)]:
+                    for v in (I, J):
+                        if (v, t) not in ids:
+                            ids[(v, t)] = _new_view_id()
+                            xy = (guided_geometry or {}).get(v, {}).get(t)
+                            _upload_pair(ctx, [ids[(v, t)]], [regions_per_view[v][t]], [xy], up)
+            items = [(p, t) for p in guided for t in common[p]]
+            lists = ctx.guided_match_pairs([(ids[(p[0], t)], ids[(p[1], t)]) for p, t in items], [info[p]["F"] for p, _ in items],
+                                           [info[p]["error_max"] * info[p]["error_max"] for p, _ in items], distanceRatio * distanceRatio) if items else []
+            for (p, t), m in zip(items, lists):
+                out[p][t] = m
+        finally:
+            for vid in up:
+                ctx.lib.b200m_remove_view(ctx._h, C.c_uint32(vid))
+    return out, info
 
 
 _default_ctx: dict[int, Context] = {}
@@ -581,9 +711,6 @@ for _n in ("__getitem__", "__contains__", "__iter__", "__len__", "__eq__", "__ne
         setattr(PairwiseMatches, _n, _lazy(_n))
 PairwiseMatches.__bool__ = lambda self: len(self) > 0
 PairwiseMatches.__hash__ = None
-
-
-MODEL_FUNDAMENTAL, MODEL_HOMOGRAPHY = 0, 1
 
 
 def _upload_pair(ctx: Context, ids, regions, geometry, up: list) -> None:

@@ -136,11 +136,23 @@ int b200m_guided_match(b200m_ctx* ctx, uint32_t view_left, uint32_t view_right, 
 enum { B200M_MODEL_FUNDAMENTAL = 0, B200M_MODEL_HOMOGRAPHY = 1 };
 int b200m_guided_match_model(b200m_ctx* ctx, uint32_t view_left, uint32_t view_right, int model, const double* M, double errorTh, double distRatio,
                              b200m_result** out);
+/* matching::guidedMatching<Mat3Model, FundamentalEpipolarDistanceError | HomographyAsymmetricError> + IndMatch::getDeduplicated
+ * (guidedMatching.hpp:206-268) for every pair (L = pairs[2k], R = pairs[2k+1]) of resident views, one model per pair:
+ *   M        n_pairs x 9 row-major (F: x_R^T F x_L = 0; H: x_R ~ H x_L), model = B200M_MODEL_FUNDAMENTAL | B200M_MODEL_HOMOGRAPHY
+ *   errorTh  n_pairs values, already squared (Square(m_dPrecision_robust) differs per pair)
+ *   distRatio already squared, one for the call
+ * The result holds one pair per input pair, in input order (empty lists included); each list is what b200m_guided_match_model
+ * returns for that pair: IndMatch(i = left, j = right) in ascending i, ratio and distance 0.  A pair whose views differ in
+ * descriptor type, or with an empty view, gets an empty list.  Waits only for the views the list references; long lists run in
+ * internal batches of at most 8192 pairs and a bounded left-feature total (B200M_GUIDED_LEFT_CAP overrides that bound).  b200m_guided_match and
+ * b200m_guided_match_model are this call on a list of one pair. */
+int b200m_guided_match_pairs(b200m_ctx* ctx, const uint32_t* pairs, int n_pairs, int model, const double* M, const double* errorTh, double distRatio,
+                             b200m_result** out);
 
 /* Positions guided matching uses for one uploaded view instead of its (float) upload positions: n x 2 doubles, typically
  * camera::IntrinsicBase::getUndistortedPixel of every feature (matching/guidedMatching.hpp:229-248, :395, :416): the reference
- * matches on undistorted positions whenever the intrinsic is valid.  b200m_guided_match, b200m_guided_match_model and
- * b200m_guided_match_fast_pairs use them when they are set; a view with geometry positions needs no upload positions.
+ * matches on undistorted positions whenever the intrinsic is valid.  b200m_guided_match, b200m_guided_match_model,
+ * b200m_guided_match_pairs and b200m_guided_match_fast_pairs use them when they are set; a view with geometry positions needs no upload positions.
  * n must equal the view's feature count (else B200M_ERR_ARG); xy == NULL drops them; unknown view -> B200M_ERR_ARG.
  * Re-uploading or removing the view drops them.  The array is copied before the call returns. */
 int b200m_set_view_geometry(b200m_ctx* ctx, uint32_t view_id, const double* xy, int n);
@@ -241,7 +253,7 @@ int b200m_debug_rand_sample(const uint32_t state[625], int range, int draws, uin
 int b200m_debug_rand_sample_k(const uint32_t state[625], int sample_size, int range, int draws, uint32_t* out, uint32_t* states);
 
 /* ---- instrumentation ------------------------------------------------------------------------------------------ */
-/* The b200m_last_* getters report the last successful b200m_match_pairs, b200m_guided_match(_model), b200m_guided_match_fast_pairs
+/* The b200m_last_* getters report the last successful b200m_match_pairs, b200m_guided_match(_model, _pairs), b200m_guided_match_fast_pairs
  * or b200m_knn on the context, whichever came last; a value that call does not measure reads 0 (b200m_knn sets only
  * b200m_last_tc_pairs: 1 when it ran on the tensor-core kernel).  They take the context's lock.  The a-contrario RANSAC calls have
  * their own (b200m_acransac_last_stats) and leave these alone. */
@@ -256,7 +268,7 @@ int b200m_last_launches(const b200m_ctx* ctx);
 int b200m_last_tc_pairs(const b200m_ctx* ctx);
 /* candidates whose re-scored best distance differed from the tensor-core value (must stay 0); cumulative over the context's life */
 unsigned b200m_exactness_errors(const b200m_ctx* ctx);
-/* total raw records (matches before host finishing) produced by the last call; b200m_guided_match(_model): its matches,
+/* total raw records (matches before host finishing) produced by the last call; b200m_guided_match(_model, _pairs): its matches,
  * b200m_guided_match_fast_pairs: the candidate distances it evaluated */
 int64_t b200m_last_records(const b200m_ctx* ctx);
 /* pairs of the last call that ran on the tensor-core FILTER kernel for real-valued fp32 descriptors (fp16-rounded GEMM + rigorous error
