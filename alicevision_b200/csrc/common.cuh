@@ -26,7 +26,7 @@ struct alignas(128) ViewDev {
   CUtensorMap tmap_aug; // fp16 [m_pad x 16] half-norm limbs, box {16 x 128 rows}, SWIZZLE_32B (9th K-step of the AUG kernel)
   CUtensorMap tmap_augq; // the same for augq16 (the view as QUERY of the real-valued kernel: its own half-norm limbs as A columns)
   CUtensorMap tmap_u8;  // uchar-stored views only: `raw` as u8 [m x 128], box {128 B x 128 rows}, SWIZZLE_128B (the u8 kernel's operand tile)
-  const int32_t* nb32;  // uchar-stored views only: ||row||^2 as int32, padded to a multiple of 256 rows with 2^24 (prep.cuh), else nullptr
+  const int32_t* nb32;  // uchar-stored views only: ||row||^2 + U8_NORM_BIAS as int32, padded to a multiple of 256 rows with 2^24 + U8_NORM_BIAS (prep.cuh), else nullptr
   const void* raw;      // descriptors as STORED, row-major m x dim: f32 / u8 / 64-byte binary; `dtype` is the storage type (integer-valued
                         // fp32 descriptors are staged and stored as u8: same values, a quarter of the bytes)
   const __half* h16;    // fp16 copy (scalar, dim == 128) or nullptr
@@ -51,6 +51,7 @@ struct PairDev {
   uint32_t cand_base;        // first candidate slot of this pair (prefix sum of m_j over the batch)
   uint32_t mode;             // PM_*
   uint32_t slot_base;        // prefix sum of m_i over the batch: this pair's scratch range of the device finishing stage (finish.cuh)
+  uint32_t thread_chunks;    // PM_TC: 1 when the pair's candidates come from the u8 kernel (chunk ids in its per-thread layout, chunk_row)
 };
 enum : uint32_t { PM_TC = 0, PM_EXACT_F32 = 1, PM_EXACT_U8 = 2, PM_HAMMING = 3, PM_SKIP = 4,
                   PM_TC_FUSED = 5 /* tensor-core pair whose kernel also ran the exactness pass: candidates are final */,
@@ -62,11 +63,22 @@ enum : uint32_t { PM_TC = 0, PM_EXACT_F32 = 1, PM_EXACT_U8 = 2, PM_HAMMING = 3, 
 struct WorkItem { uint32_t pair, qtile; };
 
 // Candidate produced by a search kernel, one per query that passed the (pre-)ratio test.
-//   PM_TC:   a = query row, b = 16-row chunk id of the best database row, d1 exact, d2 = upper bound (exactness pass needed)
+//   PM_TC:   a = query row, b = 16-row chunk id of the best database row (chunk_row), d1 exact, d2 = upper bound (exactness pass needed)
 //   others:  a = query row, b = database row of the nearest neighbour, d1/d2 exact (float bits, or uint32 bits for Hamming)
 //   PM_TC_REAL (before re-scoring): q = query row, b / d1 / d2 = bit patterns p1 / p2 / p3 of the three smallest packed chunk minima
 //            (value with the chunk id in the low REAL_IDBITS bits), p4 in the parallel `candx` word
 struct Cand { uint32_t q, b; float d1, d2; };
+
+// ViewDev::nb32 holds ||row||^2 + U8_NORM_BIAS: with it the u8 kernel's per-element value ||b||^2 - 2 a.b > -||a||^2 > -2^22 is positive, and
+// positive values order the same as integers and as float bit patterns (l2_tc.cuh u8_elem)
+constexpr int32_t U8_NORM_BIAS = 1 << 22;
+
+// Database row r (0..15, ascending) of 16-row chunk g of a tensor-core candidate.  The fp16 kernels' chunks are contiguous rows.  The u8
+// kernel's chunk g = 8t + 4h + q is what ONE thread (lane % 4 = q) holds of a query row in the 64-column half h of tile t:
+// rows 128t + 64h + 8j + 2q + e (j = 0..7, e = 0, 1), so that a chunk minimum needs no exchange between threads.
+__device__ __forceinline__ uint32_t chunk_row(uint32_t g, int r, bool thread_chunks) {
+  return thread_chunks ? (g >> 2) * 64 + (uint32_t)(r >> 1) * 8 + (g & 3) * 2 + (uint32_t)(r & 1) : g * 16 + (uint32_t)r;
+}
 
 // Real-valued filter: chunk ids ride in the low mantissa bits of the (non-negative) chunk minima
 constexpr int REAL_IDBITS = 13;                       // 8191 chunks of 16 rows = 131056 database rows at most

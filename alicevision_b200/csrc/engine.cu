@@ -1161,7 +1161,7 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       // the CTA-pair kernel runs the exactness pass itself: its candidates are final records
       const bool u8 = u8_pair(d);
       const uint32_t dev_mode = (d.mode == PM_TC && (u8 ? fused_u8 : fused)) ? (uint32_t)PM_TC_FUSED : d.mode;
-      bb.h_pairs[p] = PairDev{(uint32_t)d.slot_i, (uint32_t)d.slot_j, (uint32_t)vi.m, (uint32_t)vj.m, cbase, dev_mode, sbase};
+      bb.h_pairs[p] = PairDev{(uint32_t)d.slot_i, (uint32_t)d.slot_j, (uint32_t)vi.m, (uint32_t)vj.m, cbase, dev_mode, sbase, u8 ? 1u : 0u};
       cbase += (uint32_t)vj.m; sbase += (uint32_t)vi.m;
       const int qrows = tc_ctas_per_item * tc::BM;   // queries per work item
       if (d.mode == PM_TC && !u8) for (int qt = 0; qt < (vj.m + qrows - 1) / qrows; ++qt) bb.h_items[n_items++] = WorkItem{(uint32_t)p, (uint32_t)qt};

@@ -45,7 +45,8 @@
 //               whatever the rounding did.
 //
 // Accumulator layout (ptx::wgmma_m64n128k16_f16_negb): a thread holds two query rows and, per row, 4 of the 16 columns of each
-// chunk; the four threads of a quad (lanes 4k..4k+3) hold the same rows.  A chunk minimum is a min over the thread's 4 values
+// chunk; the four threads of a quad (lanes 4k..4k+3) hold the same rows.  (The u8 kernel defines its chunks per thread instead and
+// skips what follows: see its branch of the consumer loop.)  A chunk minimum is a min over the thread's 4 values
 // and then over the quad: a two-step butterfly (xor 1, xor 2) that leaves each lane the full minima of chunks {q, q + 4}
 // (q = lane % 4) of both rows - 12 shuffles per tile instead of 32 - and each lane keeps its own running state over its chunks.
 // The four disjoint states are merged once per work item.
@@ -145,7 +146,6 @@ __device__ __forceinline__ void merge_xor(Top4& s, int m) {
 }
 
 __device__ __forceinline__ float vmin(float a, float b) { return fminf(a, b); }
-__device__ __forceinline__ int32_t vmin(int32_t a, int32_t b) { return min(a, b); }
 // Per row, the thread's minima of the 8 chunks (over its 4 columns of each) -> the full minima of chunks qlane and qlane + 4 (over the quad),
 // v2[row][h] = chunk 4h + qlane: a two-step butterfly, 12 shuffles
 template <typename T>
@@ -165,6 +165,19 @@ __device__ __forceinline__ void quad_chunk_minima(const T (&pm)[2][8], int qlane
       v2[r][h] = vmin(keep, __shfl_xor_sync(0xffffffffu, send, 2));
     }
   }
+}
+
+// u8 kernel, per element: s + U8_NORM_BIAS = (||b||^2 + U8_NORM_BIAS) - 2 a.b on the fp32 pipe.  Both operands are integers in [0, 2^24]; read as
+// floats their bit patterns are the (sub)normal numbers x * 2^-149, the product and the sum are exact, and the result (positive: the bias
+// exceeds ||a||^2) read back as an integer is the integer result: one full-rate FFMA where an IMAD issues at half rate.  This needs
+// denormals kept: the library is built without -ftz / fast-math.  A pad row (a.b = 0) gives back its norm word unchanged.
+__device__ __forceinline__ int32_t u8_elem(int32_t nb, int32_t ab) { return __float_as_int(fmaf(-2.f, __int_as_float(ab), __int_as_float(nb))); }
+// ... and of a chunk minimum, h = s / 2: what the fp16 kernel's accumulator holds (exact, |s| <= 2^24)
+__device__ __forceinline__ float u8_half_dist(int32_t biased) { return fmaf(0.5f, (float)biased, -0.5f * (float)U8_NORM_BIAS); }
+__device__ __forceinline__ int32_t min16(const int32_t (&x)[16]) {
+  const int32_t a = __vimin3_s32(x[0], x[1], x[2]), b = __vimin3_s32(x[3], x[4], x[5]), c = __vimin3_s32(x[6], x[7], x[8]);
+  const int32_t d = __vimin3_s32(x[9], x[10], x[11]), e = __vimin3_s32(x[12], x[13], x[14]);
+  return min(__vimin3_s32(a, b, c), __vimin3_s32(d, e, x[15]));
 }
 
 // The real-valued re-scoring reads 32 fp32 rows per candidate (16 KB, mostly from HBM) and is latency-bound: two warps cannot keep up with
@@ -290,7 +303,7 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
           Rec rec;
           int verdict;                                                          // 0 drop, 1 keep, 2 undecided -> exact_rows fallback
           if (REAL) verdict = rescore_real(views[p.view_i], views[p.view_j], p.m_i, k, queuex[quad * 32 + e], ratio_sq, lane, err_count, rec);
-          else verdict = rescore_candidate(db16, q16, p.m_i, k, ratio_sq, lane, err_count, rec) ? 1 : 0;
+          else verdict = rescore_candidate(db16, q16, p.m_i, k, U8, ratio_sq, lane, err_count, rec) ? 1 : 0;
           if (verdict == 1 && lane == 0) {
             const int slot = atomicAdd(&cand_count[hdr[4]], 1);
             cands[p.cand_base + slot] = Cand{rec.j, rec.i, rec.d1, rec.d2};     // final record, (query, database row) order like the exact kernels
@@ -331,11 +344,13 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
           if (lane == 0) ptx::mbar_arrive(&db_empty[st]);             // this warp is done with the slot (operands and (half-)norms)
           if (++st == NS) { st = 0; sph ^= 1; }
         };
-        float v2[2][2];                        // chunk minima h of chunks 4h + qlane of rows r0, r0 + 8 (quad_chunk_minima)
+        float v2[2][2];                        // chunk minima h of chunks 4h + qlane of rows r0, r0 + 8
         if constexpr (U8) {
-          // acc = a.b, exact in s32.  Per element s = ||b||^2 - 2 a.b = ||a - b||^2 - ||a||^2 (one IMAD), chunk minima in integers, and only
-          // the four surviving minima per thread become h = s / 2: exactly the fp16 kernel's accumulator value (|s| < 2^24), so everything
+          // acc = a.b, exact in s32.  Per element s = ||b||^2 - 2 a.b = ||a - b||^2 - ||a||^2 (u8_elem), chunk minima in integers, and only
+          // the four minima per thread become h = s / 2: exactly the fp16 kernel's accumulator value (|s| < 2^24), so everything
           // from the folds on is shared.  Pad rows: a.b = 0 (TMA zero fill), ||b||^2 = 2^24 (prep.cuh) -> h = 2^23, as in the fp16 kernel.
+          // A chunk is the 16 columns THIS thread holds of a query row in one 64-column half of the tile (common.cuh chunk_row), so its
+          // minimum needs no shuffle; pad rows of a partial last tile share chunks with real rows and lose to them.
           int32_t acc[64];
           ptx::wgmma_fence();
 #pragma unroll
@@ -345,25 +360,31 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
             ptx::wgmma_m64n128k32_u8(acc, da, db, k > 0 ? 1u : 0u);
           }
           ptx::wgmma_commit();
+          // column 8j + 2 qlane + e of the tile (j = 0..15, e = 0, 1): acc[4j + e] (row r0), acc[4j + 2 + e] (row r0 + 8); norms nb2[4j]
+          const int2* nb2 = reinterpret_cast<const int2*>(smem + L::OFF_DB + st * STAGE + U8_BYTES) + qlane;
+          // half of the norms are loaded under the MMAs (they depend on db_full only); all 16 there would not fit in 128 registers
+          constexpr int U8_NB_EARLY = 8;
+          int2 nb[16];
+#pragma unroll
+          for (int j = 0; j < U8_NB_EARLY; ++j) nb[j] = nb2[4 * j];
           ptx::wgmma_wait_all();
           ptx::trace_stamp(etrace, 1 + wg, tt, 2);
-          // columns 16c + 2 qlane + {0, 1} and 16c + 8 + 2 qlane + {0, 1} of chunk c: acc[8c + {0, 1}], acc[8c + {4, 5}] (row r0),
-          // acc[8c + {2, 3}], acc[8c + {6, 7}] (row r0 + 8)
-          const int2* nb2 = reinterpret_cast<const int2*>(smem + L::OFF_DB + st * STAGE + U8_BYTES) + qlane;
-          int32_t pm[2][8];
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const int2 n0 = nb2[8 * c], n1 = nb2[8 * c + 4];
-            pm[0][c] = __vimin3_s32(n0.x - 2 * acc[8 * c + 0], n0.y - 2 * acc[8 * c + 1], min(n1.x - 2 * acc[8 * c + 4], n1.y - 2 * acc[8 * c + 5]));
-            pm[1][c] = __vimin3_s32(n0.x - 2 * acc[8 * c + 2], n0.y - 2 * acc[8 * c + 3], min(n1.x - 2 * acc[8 * c + 6], n1.y - 2 * acc[8 * c + 7]));
+          for (int j = U8_NB_EARLY; j < 16; ++j) nb[j] = nb2[4 * j];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            int32_t x[2][16];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int2 n = nb[8 * h + j];
+              const int a = 32 * h + 4 * j;
+              x[0][2 * j] = u8_elem(n.x, acc[a + 0]); x[0][2 * j + 1] = u8_elem(n.y, acc[a + 1]);
+              x[1][2 * j] = u8_elem(n.x, acc[a + 2]); x[1][2 * j + 1] = u8_elem(n.y, acc[a + 3]);
+            }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) v2[r][h] = u8_half_dist(min16(x[r]));
           }
           release_slot();
-          int32_t v2i[2][2];
-          quad_chunk_minima(pm, qlane, v2i);
-#pragma unroll
-          for (int r = 0; r < 2; ++r)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) v2[r][h] = 0.5f * (float)v2i[r][h];
         } else {
           float acc[64];
           ptx::wgmma_fence();

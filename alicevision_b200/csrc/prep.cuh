@@ -37,7 +37,7 @@ __device__ __forceinline__ void halfnorm_limbs(float s, bool integer_valued, flo
 //         cols 3-5, so the extra database columns cost it nothing.
 //   err   ||row - fp16(row)||_2 inflated by 2^-9 (upper bound of the rounding error norm), 0 for integer-valued rows
 //   stats [0] = max err over the view, [1] = max nrm  (float bits, atomicMax on the non-negative patterns)
-//   nb32  (uchar-stored views, else nullptr) m_pad x int32 ||row||^2 for the u8 kernel; pad rows 2^24 (see below)
+//   nb32  (uchar-stored views, else nullptr) m_pad x int32 ||row||^2 + U8_NORM_BIAS for the u8 kernel; pad rows 2^24 + U8_NORM_BIAS (see below)
 template <typename T>
 __global__ void __launch_bounds__(256)
 prep_view_kernel(const T* __restrict__ raw, int m, __half* __restrict__ h16, float* __restrict__ nbh, float* __restrict__ nrm,
@@ -53,7 +53,7 @@ prep_view_kernel(const T* __restrict__ raw, int m, __half* __restrict__ h16, flo
     // So a chunk of padding never wins and never ties with another; it is the second chunk minimum only when m <= 16, and then the
     // exactness pass re-scores the one real chunk.  (A pad half-norm below 2^21 + 2^22 lost to anti-correlated queries.)
     // The u8 kernel's pad rows (zero-filled by TMA, a.b = 0) get s = ||b||^2 - 2 a.b = 2^24 and h = s/2 = 2^23: the same value as here.
-    if (lane == 0) { nbh[row] = 1e30f; err[row] = 0.f; if (nb32) nb32[row] = 1 << 24; }
+    if (lane == 0) { nbh[row] = 1e30f; err[row] = 0.f; if (nb32) nb32[row] = (1 << 24) + U8_NORM_BIAS; }
     if (lane < 16) {
       aug16[(size_t)row * 16 + lane] = __float2half_rn(lane == 2 ? 4096.f : (lane >= 3 && lane < 6) ? (lane == 3 ? -0.5f : lane == 4 ? -1.f : -2048.f) : 0.f);
       augq16[(size_t)row * 16 + lane] = __float2half_rn(cst);
@@ -83,7 +83,7 @@ prep_view_kernel(const T* __restrict__ raw, int m, __half* __restrict__ h16, flo
     nrm[row] = s;
     nbh[row] = 0.5f * s;
     err[row] = er;
-    if (nb32) nb32[row] = (int32_t)s;       // exact: at most 128 * 255^2 < 2^24
+    if (nb32) nb32[row] = (int32_t)s + U8_NORM_BIAS;       // exact: at most 128 * 255^2 < 2^24
     if (f) atomicOr(flags, f);
     atomicMax(&stats[0], __float_as_uint(er));
     atomicMax(&stats[1], __float_as_uint(s));

@@ -62,12 +62,13 @@ __global__ void scan_counts_kernel(const int* __restrict__ cand_count, int n, in
 }
 
 // Warp-level exact re-scoring of one tensor-core candidate (see the header comment). All 32 lanes call it with the same
-// candidate; lane l handles database row 16*k.b + (l & 15), components 64*(l >> 4)..+63. Returns (on every lane)
+// candidate; lane l handles row (l & 15) of chunk k.b (chunk_row: ascending in l, so ties go to the smallest database row in either
+// layout), components 64*(l >> 4)..+63. Returns (on every lane)
 // whether the match survives the ratio test; `rec` is the final record (i = database row, j = query row, d1, d2).
 __device__ __forceinline__ bool rescore_candidate(const __half* __restrict__ db16, const __half* __restrict__ q16, uint32_t m_i, const Cand& k,
-                                                  float ratio_sq, int lane, unsigned int* __restrict__ err_count, Rec& rec) {
+                                                  bool thread_chunks, float ratio_sq, int lane, unsigned int* __restrict__ err_count, Rec& rec) {
   const int r = lane & 15, hv = lane >> 4;
-  const uint32_t row = k.b * 16 + r;
+  const uint32_t row = chunk_row(k.b, r, thread_chunks);
   float acc = INFINITY;
   if (row < m_i) {
     const uint4* a = reinterpret_cast<const uint4*>(q16 + (size_t)k.q * 128 + hv * 64);
@@ -100,7 +101,7 @@ __device__ __forceinline__ bool rescore_candidate(const __half* __restrict__ db1
   for (int o = 8; o >= 1; o >>= 1) second = fminf(second, __shfl_xor_sync(0xffffffffu, second, o));
   if (lane == 0 && best != k.d1) atomicAdd(err_count, 1u);             // tensor-core accumulation was not exact
   const float d2 = fminf(k.d2, second);
-  rec = Rec{k.b * 16 + (uint32_t)arg, k.q, best, d2};
+  rec = Rec{chunk_row(k.b, arg, thread_chunks), k.q, best, d2};
   return best < __fmul_rn(ratio_sq, d2);                                // matching/filters.hpp:60
 }
 
@@ -478,7 +479,7 @@ verify_pack_kernel(const ViewDev* __restrict__ views, const PairDev* __restrict_
   for (int c = wid; c < n; c += nwarps) {
     const Cand k = src[c];
     Rec rec;
-    const bool keep = rescore_candidate(vi.h16, vj.h16, p.m_i, k, ratio_sq, lane, err_count, rec);
+    const bool keep = rescore_candidate(vi.h16, vj.h16, p.m_i, k, p.thread_chunks != 0, ratio_sq, lane, err_count, rec);
     if (lane == 0) dst[c] = keep ? rec : Rec{0xFFFFFFFFu, k.q, rec.d1, rec.d2};
   }
 }
