@@ -1,7 +1,10 @@
-// Reference-side adaptor for the `fundamental_matrix` geometric filter: matchingImageCollection::robustModelEstimation with
-// GeometricFilterMatrix_F_AC (ACRANSAC, Fundamental7PSolver; GeometricFilter.hpp:40-88, GeometricFilterMatrix_F_AC.hpp:90-174,
-// :266-299, :357-392) for a whole putative list on the b200match engine (H100): one b200m_acransac_fundamental_pairs call, the
-// reference's inlier copy and support rules, then one b200m_guided_match_pairs call for every kept pair and common descriptor type.
+// Reference-side adaptors for the `fundamental_matrix` and `homography_matrix` geometric filters: matchingImageCollection::
+// robustModelEstimation with GeometricFilterMatrix_F_AC (ACRANSAC, Fundamental7PSolver; GeometricFilter.hpp:40-88,
+// GeometricFilterMatrix_F_AC.hpp:90-174, :266-299, :357-392) or GeometricFilterMatrix_H_AC (Homography4PSolver;
+// GeometricFilterMatrix_H_AC.hpp:43-103, :160-212) for a whole putative list on the b200match engine (H100): one a-contrario RANSAC
+// call (b200m_acransac_fundamental_pairs / b200m_acransac_homography_pairs), the reference's inlier copy and support rules, then one
+// guided-matching call for every kept pair and common descriptor type (b200m_guided_match_pairs, or for H with distanceRatio < 0
+// b200m_guided_match_positions_pairs).
 // Header-only; compiled inside an AliceVision build and linked against libb200match.so.  The caller gathers xI / xJ with the
 // reference's fillMatricesWithUndistortFeaturesMatches and the guided positions with camera::IntrinsicBase::getUndistortedPixel.
 // Inside the AliceVision build (ALICEVISION_B200_REFERENCE_FILTER_UTILS defined) the library's own copyInlierMatches and
@@ -87,36 +90,28 @@ inline void mtState(const std::mt19937& g, uint32_t state[625])
 }
 }  // namespace b200detail
 
-/// A putative list over views that are uploaded ONCE per descriptor type: addView every (view, type) with its guided positions,
-/// addPair every pair, then run().  The views are removed from the engine when the batch is destroyed.
-class GeometricFilterMatrix_F_AC_Batch_b200
+/// The bookkeeping both batch adaptors share: a putative list over views that are uploaded ONCE per descriptor type.  addView every
+/// (view, type) with its guided positions, addPair every pair, then the derived class's run().  The views are removed from the engine
+/// when the batch is destroyed.
+class GeometricFilterBatchBase_b200
 {
 public:
-    /// What the estimation of one pair gave (in addPair order): ACRANSAC's validity, F (row-major, x_J^T F x_I = 0), errorMax
-    /// (m_dPrecision_robust; infinite when not valid) and the support decision.
-    struct Estimate
-    {
-        bool valid = false, strongSupport = false;
-        double F[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-        double errorMax = std::numeric_limits<double>::infinity();
-    };
-
-    explicit GeometricFilterMatrix_F_AC_Batch_b200(b200m_ctx* ctx = matching::b200detail::sharedContext())
+    explicit GeometricFilterBatchBase_b200(b200m_ctx* ctx)
       : _ctx(ctx)
     {}
-    ~GeometricFilterMatrix_F_AC_Batch_b200()
+    ~GeometricFilterBatchBase_b200()
     {
         if (_ctx)
             for (const auto& v : _views)
                 b200m_remove_view(_ctx, v.second);
     }
-    GeometricFilterMatrix_F_AC_Batch_b200(const GeometricFilterMatrix_F_AC_Batch_b200&) = delete;
-    GeometricFilterMatrix_F_AC_Batch_b200& operator=(const GeometricFilterMatrix_F_AC_Batch_b200&) = delete;
+    GeometricFilterBatchBase_b200(const GeometricFilterBatchBase_b200&) = delete;
+    GeometricFilterBatchBase_b200& operator=(const GeometricFilterBatchBase_b200&) = delete;
 
     bool available() const { return _ctx != nullptr && _ok; }
 
-    /// Uploads one (view, type) once; guidedPos: n x 2 positions guided matching uses (getUndistortedPixel when the camera isValid()),
-    /// or nullptr for the regions' own positions.
+    /// Uploads one (view, type) once, with the regions' own positions; guidedPos: n x 2 positions guided matching uses
+    /// (getUndistortedPixel when the camera isValid()), or nullptr for the regions' own positions.
     bool addView(IndexT viewId, feature::EImageDescriberType type, const feature::Regions& regions, const double* guidedPos = nullptr)
     {
         if (!available())
@@ -160,6 +155,131 @@ public:
         _pairs.push_back(std::move(p));
     }
 
+protected:
+    struct PairIn
+    {
+        Pair pair;
+        matching::MatchesPerDescType putatives;
+        std::vector<feature::EImageDescriberType> descTypes;
+        std::size_t offset;
+    };
+
+    /// What one K10 call over the list returned, per pair in addPair order.
+    struct K10Out
+    {
+        std::vector<int64_t> offsets;
+        std::vector<uint8_t> valid;
+        std::vector<int32_t> nInl, iters;
+        std::vector<uint32_t> inl;
+        std::vector<double> M, errMax, nfa;
+        explicit K10Out(const std::vector<PairIn>& pairs, std::size_t nCorr)
+          : offsets(pairs.size() + 1, 0)
+        {
+            const int n = (int)pairs.size();
+            for (int k = 0; k < n; ++k)
+                offsets[k + 1] = (k + 1 < n ? (int64_t)pairs[k + 1].offset : (int64_t)nCorr);
+            valid.resize(std::max(n, 1));
+            nInl.resize(std::max(n, 1));
+            iters.resize(std::max(n, 1));
+            inl.resize(std::max<std::size_t>(nCorr, 1));
+            M.resize(9 * std::max(n, 1));
+            errMax.resize(std::max(n, 1));
+            nfa.resize(std::max(n, 1));
+        }
+    };
+
+    const double* corrData() const
+    {
+        static const double dummy[4] = {0, 0, 0, 0};
+        return _corr.empty() ? dummy : _corr.data();
+    }
+
+    /// copyInlierMatches and hasStrongSupport(minimumSamples) of pair k; returns whether it has strong support (then result[pair]
+    /// holds its inliers).
+    bool keepInliers(int k, const K10Out& r, std::size_t minimumSamples, std::map<Pair, matching::MatchesPerDescType>& result) const
+    {
+        const std::vector<std::size_t> inliers(r.inl.begin() + r.offsets[k], r.inl.begin() + r.offsets[k] + r.nInl[k]);
+        matching::MatchesPerDescType perType;
+        b200detail::copyInlierMatches(inliers, _pairs[k].putatives, _pairs[k].descTypes, perType);
+        if (!b200detail::hasStrongSupport(perType, minimumSamples))
+            return false;
+        result[_pairs[k].pair] = std::move(perType);
+        return true;
+    }
+
+    /// The guided step of the kept pairs: their lists are replaced by one entry per common type (empty ones included) when errorMax
+    /// is finite, else by nothing.  M(k) is pair k's 9 model coefficients; call(ids, n, M, errorTh, &res) makes the one batched call.
+    template<class ModelOf, class Call>
+    bool guided(const std::vector<int>& kept, const std::vector<double>& errorMax, ModelOf M_of, Call call,
+                std::map<Pair, matching::MatchesPerDescType>& result) const
+    {
+        std::vector<uint32_t> ids;
+        std::vector<double> M, th;
+        std::vector<std::pair<Pair, feature::EImageDescriberType>> items;
+        for (const int k : kept)
+        {
+            result[_pairs[k].pair] = matching::MatchesPerDescType();       // the guided result replaces the inliers, even when empty
+            if (errorMax[k] == std::numeric_limits<double>::infinity())
+                continue;                                                  // Geometry_guided_matching: m_dPrecision_robust infinite
+            for (const feature::EImageDescriberType t : _pairs[k].descTypes)
+            {
+                const auto l = _views.find(std::make_pair(_pairs[k].pair.first, t)), r = _views.find(std::make_pair(_pairs[k].pair.second, t));
+                if (l == _views.end() || r == _views.end())
+                    return false;
+                ids.push_back(l->second);
+                ids.push_back(r->second);
+                const double* m = M_of(k);
+                M.insert(M.end(), m, m + 9);
+                th.push_back(errorMax[k] * errorMax[k]);
+                items.emplace_back(_pairs[k].pair, t);
+            }
+        }
+        if (items.empty())
+            return true;
+        b200m_result* res = nullptr;
+        if (call(ids.data(), (int)items.size(), M.data(), th.data(), &res) != B200M_OK)
+        {
+            b200m_result_free(res);
+            return false;
+        }
+        const int64_t* off = nullptr;
+        const b200m_match* m = nullptr;
+        b200m_result_get(res, nullptr, &off, &m);
+        for (std::size_t q = 0; q < items.size(); ++q)
+        {
+            matching::IndMatches& dst = result[items[q].first][items[q].second];
+            for (int64_t e = off[q]; e < off[q + 1]; ++e)
+                dst.emplace_back(m[e].i, m[e].j);
+        }
+        b200m_result_free(res);
+        return true;
+    }
+
+    b200m_ctx* _ctx;
+    bool _ok = true;
+    std::map<std::pair<IndexT, feature::EImageDescriberType>, uint32_t> _views;
+    std::vector<PairIn> _pairs;
+    std::vector<double> _corr;
+    std::vector<int32_t> _wh;
+};
+
+/// robustModelEstimation with GeometricFilterMatrix_F_AC for the pairs added (addView / addPair of the base), then run().
+class GeometricFilterMatrix_F_AC_Batch_b200 : public GeometricFilterBatchBase_b200
+{
+public:
+    /// What the estimation of one pair gave (in addPair order): ACRANSAC's validity, F (row-major, x_J^T F x_I = 0), errorMax
+    /// (m_dPrecision_robust; infinite when not valid) and the support decision.
+    struct Estimate
+    {
+        bool valid = false, strongSupport = false;
+        double F[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        double errorMax = std::numeric_limits<double>::infinity();
+    };
+
+    explicit GeometricFilterMatrix_F_AC_Batch_b200(b200m_ctx* ctx = matching::b200detail::sharedContext())
+      : GeometricFilterBatchBase_b200(ctx)
+    {}
+
     /// robustModelEstimation over every pair added so far: each pair starts from `rng` (geometricEstimation_Mat_ACRANSAC takes it
     /// by value).  Pairs with strong support enter out; with guidedMatching their lists are the guided ones (errorTh = errorMax^2,
     /// distRatio = distanceRatio^2, every common type, empty lists included; nothing when errorMax is infinite).  Returns false
@@ -172,84 +292,36 @@ public:
         const int n = (int)_pairs.size();
         uint32_t state[625];
         b200detail::mtState(rng, state);
-        std::vector<int64_t> offsets(n + 1, 0);
-        for (int k = 0; k < n; ++k)
-            offsets[k + 1] = (k + 1 < n ? (int64_t)_pairs[k + 1].offset : (int64_t)(_corr.size() / 4));
-        const std::size_t total = std::max<std::size_t>(_corr.size() / 4, 1);
-        std::vector<uint8_t> valid(std::max(n, 1));
-        std::vector<int32_t> nInl(std::max(n, 1)), iters(std::max(n, 1));
-        std::vector<uint32_t> inl(total);
-        std::vector<double> F(9 * std::max(n, 1)), errMax(std::max(n, 1)), nfa(std::max(n, 1));
-        const double dummy[4] = {0, 0, 0, 0};
-        if (n > 0 && b200m_acransac_fundamental_pairs(_ctx, n, offsets.data(), _corr.empty() ? dummy : _corr.data(), _wh.data(), state,
-                                                      (int64_t)maxIteration, precision, valid.data(), nInl.data(), inl.data(), F.data(),
-                                                      errMax.data(), nfa.data(), iters.data()) != B200M_OK)
+        K10Out r(_pairs, _corr.size() / 4);
+        if (n > 0 && b200m_acransac_fundamental_pairs(_ctx, n, r.offsets.data(), corrData(), _wh.data(), state, (int64_t)maxIteration, precision,
+                                                      r.valid.data(), r.nInl.data(), r.inl.data(), r.M.data(), r.errMax.data(), r.nfa.data(),
+                                                      r.iters.data()) != B200M_OK)
             return false;
         _estimates.assign(n, Estimate());
         std::map<Pair, matching::MatchesPerDescType> result;
         std::vector<int> kept;
+        std::vector<double> errorMax(n, std::numeric_limits<double>::infinity());
         for (int k = 0; k < n; ++k)
         {
             Estimate& e = _estimates[k];
-            e.valid = valid[k] != 0;
-            std::copy(F.begin() + 9 * k, F.begin() + 9 * k + 9, e.F);
+            e.valid = r.valid[k] != 0;
+            std::copy(r.M.begin() + 9 * k, r.M.begin() + 9 * k + 9, e.F);
             if (!e.valid)
                 continue;
-            e.errorMax = errMax[k];
-            const std::vector<std::size_t> inliers(inl.begin() + offsets[k], inl.begin() + offsets[k] + nInl[k]);
-            matching::MatchesPerDescType perType;
-            b200detail::copyInlierMatches(inliers, _pairs[k].putatives, _pairs[k].descTypes, perType);
-            e.strongSupport = b200detail::hasStrongSupport(perType, 7);   // Fundamental7PSolver::getMinimumNbRequiredSamples
-            if (!e.strongSupport)
-                continue;
-            kept.push_back(k);
-            result[_pairs[k].pair] = std::move(perType);
+            e.errorMax = errorMax[k] = r.errMax[k];
+            e.strongSupport = keepInliers(k, r, 7, result);             // Fundamental7PSolver::getMinimumNbRequiredSamples
+            if (e.strongSupport)
+                kept.push_back(k);
         }
-        if (guidedMatching)
-        {
-            std::vector<uint32_t> ids;
-            std::vector<double> M, th;
-            std::vector<std::pair<Pair, feature::EImageDescriberType>> items;
-            for (const int k : kept)
-            {
-                result[_pairs[k].pair] = matching::MatchesPerDescType();       // the guided result replaces the inliers, even when empty
-                if (_estimates[k].errorMax == std::numeric_limits<double>::infinity())
-                    continue;                                                  // GeometricFilterMatrix_F_AC.hpp:363
-                for (const feature::EImageDescriberType t : _pairs[k].descTypes)
-                {
-                    const auto l = _views.find(std::make_pair(_pairs[k].pair.first, t)), r = _views.find(std::make_pair(_pairs[k].pair.second, t));
-                    if (l == _views.end() || r == _views.end())
-                        return false;
-                    ids.push_back(l->second);
-                    ids.push_back(r->second);
-                    M.insert(M.end(), _estimates[k].F, _estimates[k].F + 9);
-                    th.push_back(_estimates[k].errorMax * _estimates[k].errorMax);
-                    items.emplace_back(_pairs[k].pair, t);
-                }
-            }
-            if (!items.empty())
-            {
-                b200m_result* res = nullptr;
-                if (b200m_guided_match_pairs(_ctx, ids.data(), (int)items.size(), B200M_MODEL_FUNDAMENTAL, M.data(), th.data(),
-                                             distanceRatio * distanceRatio, &res) != B200M_OK)
-                {
-                    b200m_result_free(res);
-                    return false;
-                }
-                const int64_t* off = nullptr;
-                const b200m_match* m = nullptr;
-                b200m_result_get(res, nullptr, &off, &m);
-                for (std::size_t q = 0; q < items.size(); ++q)
-                {
-                    matching::IndMatches& dst = result[items[q].first][items[q].second];
-                    for (int64_t e = off[q]; e < off[q + 1]; ++e)
-                        dst.emplace_back(m[e].i, m[e].j);
-                }
-                b200m_result_free(res);
-            }
-        }
-        for (auto& r : result)
-            out[r.first] = std::move(r.second);
+        if (guidedMatching &&
+            !guided(kept, errorMax, [&](int k) { return _estimates[k].F; },
+                    [&](const uint32_t* ids, int np, const double* M, const double* th, b200m_result** res) {
+                        return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distanceRatio * distanceRatio, res);
+                    },
+                    result))
+            return false;
+        for (auto& x : result)
+            out[x.first] = std::move(x.second);
         return true;
     }
 
@@ -257,19 +329,82 @@ public:
     const Estimate& estimate(std::size_t k) const { return _estimates.at(k); }
 
 private:
-    struct PairIn
+    std::vector<Estimate> _estimates;
+};
+
+/// robustModelEstimation with GeometricFilterMatrix_H_AC (ACRANSAC, Homography4PSolver, point-to-point error;
+/// GeometricFilterMatrix_H_AC.hpp:43-103, :160-212) for the pairs added (addView / addPair of the base), then run().
+class GeometricFilterMatrix_H_AC_Batch_b200 : public GeometricFilterBatchBase_b200
+{
+public:
+    /// What the estimation of one pair gave (in addPair order): ACRANSAC's validity, H (row-major, x_J ~ H x_I), errorMax
+    /// (m_dPrecision_robust; infinite when not valid) and the support decision.
+    struct Estimate
     {
-        Pair pair;
-        matching::MatchesPerDescType putatives;
-        std::vector<feature::EImageDescriberType> descTypes;
-        std::size_t offset;
+        bool valid = false, strongSupport = false;
+        double H[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        double errorMax = std::numeric_limits<double>::infinity();
     };
-    b200m_ctx* _ctx;
-    bool _ok = true;
-    std::map<std::pair<IndexT, feature::EImageDescriberType>, uint32_t> _views;
-    std::vector<PairIn> _pairs;
-    std::vector<double> _corr;
-    std::vector<int32_t> _wh;
+
+    explicit GeometricFilterMatrix_H_AC_Batch_b200(b200m_ctx* ctx = matching::b200detail::sharedContext())
+      : GeometricFilterBatchBase_b200(ctx)
+    {}
+
+    /// robustModelEstimation over every pair added so far.  Every pair starts from `rng`: the reference hands one generator from pair
+    /// to pair by reference, which featureMatching's OpenMP loop shares between threads without order, so no run of it is
+    /// reproducible; starting every pair from the same state is deterministic and independent of the thread count.  Pairs with strong
+    /// support (hasStrongSupport(.., 4)) enter out; with guidedMatching their lists are the guided ones, errorTh = errorMax^2, every
+    /// common type, empty lists included, nothing when errorMax is infinite:
+    ///   distanceRatio < 0   position-only guidedMatching and IndMatchDecorator on the regions' positions (featureMatching's case)
+    ///   distanceRatio >= 0  guidedMatching with descriptors, distRatio = distanceRatio^2
+    /// Returns false (out untouched) when the engine is unavailable or fails.
+    bool run(const std::mt19937& rng, std::size_t maxIteration, double precision, bool guidedMatching, double distanceRatio,
+             matching::PairwiseMatches& out)
+    {
+        if (!available())
+            return false;
+        const int n = (int)_pairs.size();
+        uint32_t state[625];
+        b200detail::mtState(rng, state);
+        K10Out r(_pairs, _corr.size() / 4);
+        if (n > 0 && b200m_acransac_homography_pairs(_ctx, n, r.offsets.data(), corrData(), _wh.data(), state, 0, (int64_t)maxIteration, precision,
+                                                     r.valid.data(), r.nInl.data(), r.inl.data(), r.M.data(), r.errMax.data(), r.nfa.data(),
+                                                     r.iters.data(), nullptr) != B200M_OK)
+            return false;
+        _estimates.assign(n, Estimate());
+        std::map<Pair, matching::MatchesPerDescType> result;
+        std::vector<int> kept;
+        std::vector<double> errorMax(n, std::numeric_limits<double>::infinity());
+        for (int k = 0; k < n; ++k)
+        {
+            Estimate& e = _estimates[k];
+            e.valid = r.valid[k] != 0;
+            std::copy(r.M.begin() + 9 * k, r.M.begin() + 9 * k + 9, e.H);
+            if (!e.valid)
+                continue;
+            e.errorMax = errorMax[k] = r.errMax[k];
+            e.strongSupport = keepInliers(k, r, 4, result);             // Homography4PSolver::getMinimumNbRequiredSamples
+            if (e.strongSupport)
+                kept.push_back(k);
+        }
+        if (guidedMatching &&
+            !guided(kept, errorMax, [&](int k) { return _estimates[k].H; },
+                    [&](const uint32_t* ids, int np, const double* M, const double* th, b200m_result** res) {
+                        if (distanceRatio < 0)
+                            return b200m_guided_match_positions_pairs(_ctx, ids, np, B200M_MODEL_HOMOGRAPHY, M, th, 1, res);
+                        return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_HOMOGRAPHY, M, th, distanceRatio * distanceRatio, res);
+                    },
+                    result))
+            return false;
+        for (auto& x : result)
+            out[x.first] = std::move(x.second);
+        return true;
+    }
+
+    /// The estimation of the k-th pair added, after run().
+    const Estimate& estimate(std::size_t k) const { return _estimates.at(k); }
+
+private:
     std::vector<Estimate> _estimates;
 };
 

@@ -238,11 +238,12 @@ struct GuidedFastScratch {
   Event ev_c0, ev_c1;                         // candidate-kernel timing
 };
 
-// grow-only scratch of b200m_guided_match_pairs (guided.cuh): one batch of pairs at a time
+// grow-only scratch of b200m_guided_match_pairs and b200m_guided_match_positions_pairs (guided.cuh): one batch of pairs at a time
 struct GuidedScratch {
-  enum { PAIRS, BESTJ, KEEP, KPOS, OUT, EXPAND, TEMP, NBUF };
+  enum { PAIRS, BESTJ, KEEP, KPOS, OUT, EXPAND, TEMP, YRANK, REC, KEEP2, NBUF };
   DeviceBuffer<> d[NBUF];
   PinnedBuffer<GuidedPair> h_pairs;
+  PinnedBuffer<const uint32_t*> h_yrank;      // position-only call: per pair, the left view's yrank when it is decorated on the device
   PinnedBuffer<> h_out;                       // read-back of the per-pair starts and the matches, one copy
   Event ev_k0, ev_k1;                         // search-kernel timing
 };
@@ -257,7 +258,8 @@ struct AcransacScratch {
   Event ev0, ev1;
 };
 
-// What the last b200m_match_pairs, b200m_guided_match_pairs (and its one-pair forms), b200m_guided_match_fast_pairs or b200m_knn measured (b200m_last_*);
+// What the last b200m_match_pairs, b200m_guided_match_pairs (and its one-pair forms), b200m_guided_match_positions_pairs, b200m_guided_match_fast_pairs
+// or b200m_knn measured (b200m_last_*);
 // a field the call does not measure is 0
 struct LastCall {
   double gpu_ms, search_ms;
@@ -524,6 +526,17 @@ struct DecoBefore {
   }
 };
 
+// IndMatchDecorator<float>::getDeduplicated (IndMatchDecorator.hpp:57-69,84-98) of out[0..cnt) with the positions xi (left) and xj
+// (right), m x 2 each, literally: the same container and insertion order.  Returns the number kept, written back to out.
+int decorator_dedup(b200m_match* out, int cnt, const float* xi, const float* xj) {
+  std::vector<DecoKey> keys; keys.reserve(cnt);
+  for (int k = 0; k < cnt; ++k) { const b200m_match& m = out[k]; keys.push_back(DecoKey{xi[2 * m.i], xi[2 * m.i + 1], xj[2 * m.j], xj[2 * m.j + 1], m}); }
+  std::set<DecoKey, DecoBefore> st(keys.begin(), keys.end());
+  cnt = 0;
+  for (const auto& k : st) out[cnt++] = k.m;
+  return cnt;
+}
+
 // recs -> final IndMatches of one directed pair, written to out[0..n) (capacity n). Returns the number kept.
 int finish_directed(const Rec* recs, int n, bool hamming, bool full, const ViewHost& vi, const ViewHost& vj, b200m_match* out) {
   int cnt = 0;
@@ -556,11 +569,7 @@ int finish_directed(const Rec* recs, int n, bool hamming, bool full, const ViewH
     cnt = w;
     std::sort(out, out + cnt, [xi](const b200m_match& a, const b200m_match& b) { return xi[2 * a.i + 1] < xi[2 * b.i + 1]; });
   } else {
-    std::vector<DecoKey> keys; keys.reserve(cnt);
-    for (int k = 0; k < cnt; ++k) { const b200m_match& m = out[k]; keys.push_back(DecoKey{xi[2 * m.i], xi[2 * m.i + 1], xj[2 * m.j], xj[2 * m.j + 1], m}); }
-    std::set<DecoKey, DecoBefore> st(keys.begin(), keys.end());
-    cnt = 0;
-    for (const auto& k : st) out[cnt++] = k.m;
+    cnt = decorator_dedup(out, cnt, xi, xj);
   }
   return cnt;
 }
@@ -1833,6 +1842,157 @@ int b200m_guided_match_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, i
     b200m_match* m = res->matches.p + res->offsets[k];
     for (const uint2& x : per_pair[k]) *m++ = b200m_match{x.x, x.y, 0.f, 0.f};     // IndMatch(i, j): ratio and distance 0
   }
+  *out = res.release();
+  return B200M_OK;
+}
+
+}  // extern "C"
+
+// ---- position-only guided matching for a list of pairs (guided.cuh, guided_positions_pairs_kernel) ---------------------------------
+// One batch.  per_pair[index] receives the pair's guidedMatching list (the phantom (0, 0) included), decorated when `decorate`.
+static int gp_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int model, const double* M, const double* errorTh, bool decorate,
+                        std::vector<std::vector<b200m_match>>& per_pair, double& gpu_ms, double& search_ms, int& launches) {
+  GuidedScratch& g = c->gm;
+  using G = GuidedScratch;
+  cudaStream_t st = c->stream;
+  const int np = (int)batch.size();
+  int rc;
+  if ((rc = g.h_pairs.reserve(sizeof(GuidedPair) * (size_t)np)) || (rc = g.h_yrank.reserve(sizeof(uint32_t*) * (size_t)np))) return rc;
+  GuidedPair* hp = g.h_pairs;
+  const uint32_t** hy = g.h_yrank;
+  long sum_l = 0, blocks = 0;
+  bool dev_deco = false;
+  for (int k = 0; k < np; ++k) {
+    const GfPairHost& q = batch[k];
+    const ViewHost& vl = c->views[q.slot_l]; const ViewHost& vr = c->views[q.slot_r];
+    GuidedPair& P = hp[k];
+    std::memset(&P, 0, sizeof(P));
+    P.gl = vl.d_geom; P.gr = vr.d_geom; P.fl = (const float2*)vl.d_xy; P.fr = (const float2*)vr.d_xy;
+    for (int t = 0; t < 9; ++t) P.M[t] = M[9 * (size_t)q.index + t];
+    P.errorTh = errorTh[q.index];
+    P.model = model == B200M_MODEL_HOMOGRAPHY ? GM_HOMOGRAPHY : GM_FUNDAMENTAL;
+    P.ml = vl.m; P.mr = vr.m;
+    P.block_base = (int)blocks; P.left_base = (int)sum_l;
+    blocks += (vl.m + GP_THREADS - 1) / GP_THREADS; sum_l += vl.m;
+    // the decorator on the device: left view in general position (pos_rank_kernel's flag, read back with the view)
+    hy[k] = decorate && c->device_finish && vl.d_yrank && !(vl.flags & VF_POS_NONGENERIC) ? vl.d_yrank : nullptr;
+    dev_deco |= hy[k] != nullptr;
+  }
+  // d_out: np + 1 pair starts and np phantom flags (ints) in hdr uint2 words, then the matches
+  const size_t i4 = sizeof(int), hdr = (size_t)np + 1;
+  if ((rc = g.d[G::PAIRS].reserve(sizeof(GuidedPair) * np)) || (rc = g.d[G::BESTJ].reserve(i4 * sum_l)) || (rc = g.d[G::KEEP].reserve(i4 * (sum_l + 1))) ||
+      (rc = g.d[G::KPOS].reserve(i4 * (sum_l + 1))) || (rc = g.d[G::OUT].reserve(sizeof(uint2) * (hdr + sum_l))) ||
+      (rc = g.h_out.reserve(sizeof(uint2) * (hdr + sum_l))))
+    return rc;
+  if (dev_deco && ((rc = g.d[G::YRANK].reserve(sizeof(uint32_t*) * np)) || (rc = g.d[G::REC].reserve(sizeof(uint2) * sum_l)) ||
+                   (rc = g.d[G::KEEP2].reserve(i4 * (sum_l + 1)))))
+    return rc;
+  GuidedPair* d_pairs = g.d[G::PAIRS].as<GuidedPair>();
+  int *d_bestj = g.d[G::BESTJ].as<int>(), *d_keep = g.d[G::KEEP].as<int>(), *d_kpos = g.d[G::KPOS].as<int>();
+  uint2* d_out = g.d[G::OUT].as<uint2>();
+  int* d_pstart = reinterpret_cast<int*>(d_out);
+  int* d_phantom = d_pstart + np + 1;
+  int* d_scan_in = dev_deco ? g.d[G::KEEP2].as<int>() : d_keep;      // the slots the compaction reads
+  { size_t tb = 0; CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_scan_in, d_kpos, (int64_t)(sum_l + 1), st));
+    if ((rc = g.d[G::TEMP].reserve(tb))) return rc; }
+  if ((rc = g.ev_k0.create()) || (rc = g.ev_k1.create())) return rc;
+  CK(cudaEventRecord(c->ev_start, st));
+  CK(cudaMemcpyAsync(d_pairs, hp, sizeof(GuidedPair) * (size_t)np, cudaMemcpyHostToDevice, st));
+  if (dev_deco) CK(cudaMemcpyAsync(g.d[G::YRANK], hy, sizeof(uint32_t*) * (size_t)np, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(d_phantom, 0, i4 * np, st));
+  CK(cudaMemsetAsync(d_scan_in + sum_l, 0, sizeof(int), st));
+  CK(cudaEventRecord(g.ev_k0, st));
+  guided_positions_pairs_kernel<<<(unsigned)blocks, GP_THREADS, 0, st>>>(d_pairs, np, d_bestj, d_keep, d_phantom);
+  CK(cudaEventRecord(g.ev_k1, st));
+  ++launches;
+  const long emit_threads = std::max(sum_l, (long)np + 1);
+  const unsigned emit_blocks = (unsigned)((emit_threads + 255) / 256);
+  if (dev_deco) {
+    uint2* d_rec = g.d[G::REC].as<uint2>();
+    guided_positions_deco_kernel<<<(unsigned)((sum_l + 255) / 256), 256, 0, st>>>(d_pairs, g.d[G::YRANK].as<const uint32_t*>(), np, (int)sum_l, d_bestj,
+                                                                                 d_phantom, d_rec, d_scan_in);
+    if ((rc = exclusive_scan(g.d[G::TEMP], d_scan_in, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+    guided_positions_emit_kernel<<<emit_blocks, 256, 0, st>>>(d_pairs, np, (int)sum_l, d_rec, d_scan_in, d_kpos, d_out + hdr, d_pstart);
+  } else {
+    if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+    guided_pairs_emit_kernel<<<emit_blocks, 256, 0, st>>>(d_pairs, np, (int)sum_l, d_bestj, d_keep, d_kpos, d_out + hdr, d_pstart);
+  }
+  CK(cudaGetLastError());
+  launches += dev_deco ? 2 : 1;
+  CK(cudaEventRecord(c->ev_end, st));
+  CK(cudaMemcpyAsync(g.h_out, d_out, sizeof(uint2) * (hdr + sum_l), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0.f, kms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
+  CK(cudaEventElapsedTime(&kms, g.ev_k0, g.ev_k1));
+  gpu_ms += ms; search_ms += kms;
+  const int* h_pstart = g.h_out.as<int>();
+  const int* h_phantom = h_pstart + np + 1;
+  const uint2* h = g.h_out.as<uint2>() + hdr;
+  for (int k = 0; k < np; ++k) {
+    std::vector<b200m_match>& L = per_pair[batch[k].index];
+    L.clear();
+    if (h_phantom[k] && !hy[k] && !(h_pstart[k + 1] > h_pstart[k] && h[h_pstart[k]].x == 0 && h[h_pstart[k]].y == 0))
+      L.push_back(b200m_match{0, 0, 0.f, 0.f});                       // IndMatch() sorts first; a real (0, 0) is the same match
+    for (int e = h_pstart[k]; e < h_pstart[k + 1]; ++e) L.push_back(b200m_match{h[e].x, h[e].y, 0.f, 0.f});
+    if (decorate && !hy[k] && !L.empty()) {
+      const ViewHost& vl = c->views[batch[k].slot_l]; const ViewHost& vr = c->views[batch[k].slot_r];
+      L.resize((size_t)decorator_dedup(L.data(), (int)L.size(), vl.xy.data(), vr.xy.data()));
+    }
+  }
+  return B200M_OK;
+}
+
+extern "C" {
+
+int b200m_guided_match_positions_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, int model, const double* M, const double* errorTh,
+                                       int decorate, b200m_result** out) {
+  if (!c || !out || n_pairs < 0 || (model != B200M_MODEL_FUNDAMENTAL && model != B200M_MODEL_HOMOGRAPHY) || (decorate != 0 && decorate != 1) ||
+      (n_pairs > 0 && (!pairs || !M || !errorTh)))
+    return fail(B200M_ERR_ARG, "bad arguments");
+  *out = nullptr;
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  CK(cudaSetDevice(c->device));
+  // checks first: nothing runs for a list with a bad entry
+  std::vector<GfPairHost> work;
+  for (int k = 0; k < n_pairs; ++k) {
+    auto sl = c->slot_of.find(pairs[2 * k]), sr = c->slot_of.find(pairs[2 * k + 1]);
+    if (sl == c->slot_of.end() || sr == c->slot_of.end()) return fail(B200M_ERR_ARG, "guided matching references a view that was never uploaded");
+    const ViewHost& vl = c->views[sl->second]; const ViewHost& vr = c->views[sr->second];
+    if (!(vl.m > 0 && vr.m > 0 && vl.dtype == vr.dtype && vl.dim == vr.dim)) continue;     // common describer type; else empty
+    if (decorate ? (vl.xy.empty() || vr.xy.empty()) : ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom)))
+      return fail(B200M_ERR_ARG, decorate ? "the decorator needs the upload positions of both views"
+                                          : "guided matching needs feature positions (or geometry positions) for both views");
+    work.push_back({k, sl->second, sr->second, 0});
+  }
+  std::vector<std::vector<b200m_match>> per_pair((size_t)n_pairs);
+  double gpu_ms = 0, search_ms = 0; int launches = 0;
+  // Batches as in b200m_guided_match_pairs, one kernel class (no descriptors are read): a batch runs when its pairs or left features
+  // would pass their bound (a pair larger than the bound runs alone).  Each view is waited for when its first pair is reached.
+  const long pair_cap = 8192;
+  std::vector<GfPairHost> open; long open_l = 0;
+  for (const GfPairHost& p : work) {
+    int rc;
+    if ((rc = ensure_view_ready(c, p.slot_l)) || (rc = ensure_view_ready(c, p.slot_r))) return rc;
+    const long ml = c->views[p.slot_l].m;
+    if (!open.empty() && ((long)open.size() + 1 > pair_cap || open_l + ml > c->gm_left_cap)) {
+      if ((rc = gp_run_batch(c, open, model, M, errorTh, decorate != 0, per_pair, gpu_ms, search_ms, launches))) return rc;
+      open.clear(); open_l = 0;
+    }
+    open.push_back(p); open_l += ml;
+  }
+  if (!open.empty())
+    if (int rc = gp_run_batch(c, open, model, M, errorTh, decorate != 0, per_pair, gpu_ms, search_ms, launches)) return rc;
+  if (int rc = wait_uploads(c)) return rc;
+  // one result pair per input pair, in input order (empty lists included)
+  std::unique_ptr<b200m_result> res(new b200m_result());
+  res->recycler = c->recycler;
+  res->pair_ids.assign(pairs, pairs + 2 * (size_t)n_pairs);
+  res->offsets.assign((size_t)n_pairs + 1, 0);
+  for (int k = 0; k < n_pairs; ++k) res->offsets[k + 1] = res->offsets[k] + (int64_t)per_pair[k].size();
+  c->last = LastCall{gpu_ms, search_ms, launches, 0, 0, 0, res->offsets[n_pairs], 0};
+  res->matches = c->recycler->take((size_t)std::max<int64_t>(res->offsets[n_pairs], 1));
+  for (int k = 0; k < n_pairs; ++k) std::copy(per_pair[k].begin(), per_pair[k].end(), res->matches.p + res->offsets[k]);
   *out = res.release();
   return B200M_OK;
 }

@@ -48,6 +48,27 @@ __device__ __forceinline__ double2 guided_pos(const double2* g, const float2* f,
   return make_double2((double)v.x, (double)v.y);
 }
 
+// The model applied to left point x, once per left feature.  F_x = F * (x, y, 1), row r = (F(r,0)*x + F(r,1)*y) + F(r,2)*1, and
+// nrm = F_x.head<2>().squaredNorm(); for a homography (fx0, fx1) = x2_est = x2h_est.head<2>() / x2h_est[2] (HomographyError.hpp:27-28).
+__device__ __forceinline__ void guided_left(const double* M, int model, double2 x, double& fx0, double& fx1, double& fx2, double& nrm) {
+  fx0 = __dadd_rn(__dadd_rn(__dmul_rn(M[0], x.x), __dmul_rn(M[1], x.y)), M[2]);
+  fx1 = __dadd_rn(__dadd_rn(__dmul_rn(M[3], x.x), __dmul_rn(M[4], x.y)), M[5]);
+  fx2 = __dadd_rn(__dadd_rn(__dmul_rn(M[6], x.x), __dmul_rn(M[7], x.y)), M[8]);
+  nrm = __dadd_rn(__dmul_rn(fx0, fx0), __dmul_rn(fx1, fx1));
+  if (model == GM_HOMOGRAPHY) { fx0 = __ddiv_rn(fx0, fx2); fx1 = __ddiv_rn(fx1, fx2); }
+}
+
+// ErrorT::error of right point y against the left point's guided_left values: HomographyAsymmetricError (x2 - x2_est).squaredNorm()
+// or FundamentalEpipolarDistanceError Square(F_x.dot((y, 1))) / squaredNorm, separate multiply / add as the reference evaluates them
+__device__ __forceinline__ double guided_error(int model, double fx0, double fx1, double fx2, double nrm, double2 y) {
+  if (model == GM_HOMOGRAPHY) {
+    const double d0 = __dsub_rn(y.x, fx0), d1 = __dsub_rn(y.y, fx1);
+    return __dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1));
+  }
+  const double dot = __dadd_rn(__dadd_rn(__dmul_rn(fx0, y.x), __dmul_rn(fx1, y.y)), fx2);
+  return __ddiv_rn(__dmul_rn(dot, dot), nrm);
+}
+
 // distance of candidate descriptors a (left) and b (right) evaluated by the 4 lanes of a group; returns the value on every lane of the group
 template <int DTYPE>
 __device__ __forceinline__ double guided_distance(const void* __restrict__ left, const void* __restrict__ right, int i, int j, int sub, unsigned gmask) {
@@ -92,16 +113,9 @@ __device__ __forceinline__ int guided_row(const GuidedPair& P, int i, double dis
   const bool live = i < P.ml;
   const int model = P.model, m_r = P.mr;
   const double errorTh = P.errorTh;
-  // epipolar line of the left point in the right image: F_x = F * (x, y, 1), row r = (F(r,0)*x + F(r,1)*y) + F(r,2)*1
+  // epipolar line of the left point in the right image, or its homography transfer
   double fx0 = 0, fx1 = 0, fx2 = 0, nrm = 1;
-  if (live) {
-    const double2 x = guided_pos(P.gl, P.fl, i);
-    fx0 = __dadd_rn(__dadd_rn(__dmul_rn(P.M[0], x.x), __dmul_rn(P.M[1], x.y)), P.M[2]);
-    fx1 = __dadd_rn(__dadd_rn(__dmul_rn(P.M[3], x.x), __dmul_rn(P.M[4], x.y)), P.M[5]);
-    fx2 = __dadd_rn(__dadd_rn(__dmul_rn(P.M[6], x.x), __dmul_rn(P.M[7], x.y)), P.M[8]);
-    nrm = __dadd_rn(__dmul_rn(fx0, fx0), __dmul_rn(fx1, fx1));      // F_x.head<2>().squaredNorm()
-    if (model == GM_HOMOGRAPHY) { fx0 = __ddiv_rn(fx0, fx2); fx1 = __ddiv_rn(fx1, fx2); }   // x2_est = x2h_est.head<2>() / x2h_est[2]
-  }
+  if (live) guided_left(P.M, model, guided_pos(P.gl, P.fl, i), fx0, fx1, fx2, nrm);
   double bd = DBL_MAX, sbd = DBL_MAX; int idx = 0;                   // distanceRatio<double>, guidedMatching.hpp:77-90
   int nq = 0;
   const int sub = lane & 3, grp = lane >> 2;
@@ -128,18 +142,7 @@ __device__ __forceinline__ int guided_row(const GuidedPair& P, int i, double dis
     for (int b = 0; b < n; b += 32) {
       const int e = b + lane;
       bool pass = false;
-      if (e < n) {
-        const double2 y = tile[e];
-        double err;
-        if (model == GM_HOMOGRAPHY) {
-          const double d0 = __dsub_rn(y.x, fx0), d1 = __dsub_rn(y.y, fx1);                            // (x2 - x2_est).squaredNorm()
-          err = __dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1));
-        } else {
-          const double dot = __dadd_rn(__dadd_rn(__dmul_rn(fx0, y.x), __dmul_rn(fx1, y.y)), fx2);    // F_x.dot((y, 1))
-          err = __ddiv_rn(__dmul_rn(dot, dot), nrm);                                                  // Square(dot) / squaredNorm
-        }
-        pass = err < errorTh;                                                                         // guidedMatching.hpp:252
-      }
+      if (e < n) pass = guided_error(model, fx0, fx1, fx2, nrm, tile[e]) < errorTh;                 // guidedMatching.hpp:252
       const unsigned m = __ballot_sync(0xffffffffu, pass);
       if (m) {
         if (pass) queue[nq + __popc(m & ((1u << lane) - 1))] = t0 + e;
@@ -189,5 +192,89 @@ __global__ void guided_pairs_emit_kernel(const GuidedPair* __restrict__ pairs, i
   int lo = 0, hi = n_pairs;                                           // last pair with left_base <= g
   while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pairs[mid].left_base <= g) lo = mid; else hi = mid; }
   out[kpos[g]] = make_uint2((unsigned)(g - pairs[lo].left_base), (unsigned)best_j[g]);
+}
+
+// ---- position-only guided matching (b200m_guided_match_positions_pairs) -------------------------------------------------------------
+// matching::guidedMatching<Mat3Model, ErrorT>(model, xLeft, xRight, errorTh, matches) (guidedMatching.hpp:37-70): for every left
+// feature, the right feature of smallest error among those with err < errorTh, the first j on ties; no descriptors.  What
+// GeometricFilterMatrix_H_AC::Geometry_guided_matching runs with distanceRatio < 0 (featureMatching's guided H filter).
+//
+// One thread per left feature: the block reads each right position of the shared tile by broadcast, so every thread scans j in
+// ascending order and the reference's strict `err < errorTh && err < min` keeps the first j of a tie with no reduction.  Both tests
+// are one compare against bound = min(errorTh, min) (errorTh NaN: bound NaN, nothing passes).  ~5 FP64 instructions per candidate
+// for a homography.  The pair table and the work-item layout are K7's, with GP_THREADS left features per block.
+//
+// The reference's `match` is a default IndMatch() = (0, 0), pushed whenever min < errorTh: with errorTh = +inf a left feature whose
+// errors are all inf / NaN / >= DBL_MAX contributes (0, 0), not (i, -).  Such a row writes -1 and raises the pair's `phantom`
+// flag; the host (or guided_positions_deco_kernel) puts (0, 0) where IndMatch::getDeduplicated's sort puts it.
+constexpr int GP_THREADS = 256;
+
+template <int MODEL>
+__device__ __forceinline__ void guided_positions_scan(const double2* tile, int n, int t0, double fx0, double fx1, double fx2, double nrm,
+                                                      double& bound, int& bj) {
+#pragma unroll 4
+  for (int e = 0; e < n; ++e) {
+    const double err = guided_error(MODEL, fx0, fx1, fx2, nrm, tile[e]);
+    if (err < bound) { bound = err; bj = t0 + e; }
+  }
+}
+
+__global__ void __launch_bounds__(GP_THREADS)
+guided_positions_pairs_kernel(const GuidedPair* __restrict__ pairs, int n_pairs, int* __restrict__ best_j, int* __restrict__ keep,
+                              int* __restrict__ phantom) {
+  __shared__ double2 tile[GM_TILE];
+  int lo = 0, hi = n_pairs;                                           // last pair with block_base <= blockIdx.x
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pairs[mid].block_base <= (int)blockIdx.x) lo = mid; else hi = mid; }
+  const GuidedPair& P = pairs[lo];
+  const int i = ((int)blockIdx.x - P.block_base) * GP_THREADS + (int)threadIdx.x;
+  const bool live = i < P.ml;
+  const int model = P.model, m_r = P.mr;
+  const double errorTh = P.errorTh;
+  double fx0 = 0, fx1 = 0, fx2 = 0, nrm = 1;
+  if (live) guided_left(P.M, model, guided_pos(P.gl, P.fl, i), fx0, fx1, fx2, nrm);
+  double bound = errorTh > DBL_MAX ? DBL_MAX : errorTh;               // min(errorTh, min = DBL_MAX)
+  int bj = -1;
+  for (int t0 = 0; t0 < m_r; t0 += GM_TILE) {
+    __syncthreads();
+    for (int e = threadIdx.x; e < GM_TILE && t0 + e < m_r; e += GP_THREADS) tile[e] = guided_pos(P.gr, P.fr, t0 + e);
+    __syncthreads();
+    if (!live) continue;
+    const int n = min(GM_TILE, m_r - t0);
+    if (model == GM_HOMOGRAPHY) guided_positions_scan<GM_HOMOGRAPHY>(tile, n, t0, fx0, fx1, fx2, nrm, bound, bj);
+    else guided_positions_scan<GM_FUNDAMENTAL>(tile, n, t0, fx0, fx1, fx2, nrm, bound, bj);
+  }
+  if (!live) return;
+  if (bj < 0 && errorTh > DBL_MAX) phantom[lo] = 1;                  // min = DBL_MAX < errorTh = +inf: IndMatch() is pushed
+  best_j[P.left_base + i] = bj;
+  keep[P.left_base + i] = bj >= 0;
+}
+
+// IndMatchDecorator::getDeduplicated on the device (see finish.cuh): for a pair whose left view is in general position (yrank[p] set)
+// the decorated list is the kept matches by ascending left y, so row i goes to slot left_base + yrank[i].  IndMatch::getDeduplicated
+// puts a phantom (0, 0) first, and the decorator keeps the first match of left feature 0, so the phantom replaces row 0's match.
+// Other pairs are copied in ascending i and finished on the host.  rec / keep2 are then compacted like K7's slots.
+__global__ void guided_positions_deco_kernel(const GuidedPair* __restrict__ pairs, const uint32_t* const* __restrict__ yrank, int n_pairs, int n_left,
+                                             const int* __restrict__ best_j, const int* __restrict__ phantom, uint2* __restrict__ rec,
+                                             int* __restrict__ keep2) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_left) return;
+  int lo = 0, hi = n_pairs;                                           // last pair with left_base <= g
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pairs[mid].left_base <= g) lo = mid; else hi = mid; }
+  const int base = pairs[lo].left_base, i = g - base;
+  const uint32_t* yr = yrank[lo];
+  int j = best_j[g];
+  if (yr && i == 0 && phantom[lo]) j = 0;
+  const int slot = yr ? base + (int)yr[i] : g;
+  rec[slot] = make_uint2((unsigned)i, (unsigned)j);
+  keep2[slot] = j >= 0;
+}
+
+// ordered compaction of guided_positions_deco_kernel's slots, as guided_pairs_emit_kernel does for K7's
+__global__ void guided_positions_emit_kernel(const GuidedPair* __restrict__ pairs, int n_pairs, int n_left, const uint2* __restrict__ rec,
+                                             const int* __restrict__ keep, const int* __restrict__ kpos, uint2* __restrict__ out, int* __restrict__ pstart) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g <= n_pairs) pstart[g] = kpos[g < n_pairs ? pairs[g].left_base : n_left];
+  if (g >= n_left || !keep[g]) return;
+  out[kpos[g]] = rec[g];
 }
 }  // namespace b200m

@@ -40,6 +40,7 @@ ABI_SYMBOLS = [
     "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model", "b200m_set_view_geometry", "b200m_guided_match_fast_pairs",
     "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
     "b200m_mt19937_seed", "b200m_debug_rand_sample", "b200m_acransac_homography_pairs", "b200m_debug_rand_sample_k", "b200m_guided_match_pairs",
+    "b200m_guided_match_positions_pairs",
 ]
 
 
@@ -200,6 +201,25 @@ class Context:
         res = C.c_void_p()
         _check(self.lib.b200m_guided_match_pairs(self._h, p.ctypes.data_as(C.c_void_p), C.c_int(n), C.c_int(model), Mm.ctypes.data_as(C.c_void_p),
                                                  th.ctypes.data_as(C.c_void_p), C.c_double(distRatio), C.byref(res)), "b200m_guided_match_pairs")
+        return self._pair_lists(res, n)
+
+    def guided_match_positions_pairs(self, pairs, M, errorTh, model: int = MODEL_HOMOGRAPHY, decorate: bool = True) -> list:
+        """b200m_guided_match_positions_pairs on resident views: position-only guidedMatching (matching/guidedMatching.hpp:37-70) for
+        every (L, R) of `pairs`, with its own model M [n, 3, 3] and errorTh [n] (already squared): per left feature the right feature of
+        smallest error below errorTh, the first on ties; no descriptors.  decorate=True then applies IndMatchDecorator::getDeduplicated
+        on the upload positions, as GeometricFilterMatrix_H_AC does with distanceRatio < 0.  Returns one matches[MATCH_DTYPE] per input
+        pair, in input order: sorted by (i, j) without decoration, in the decorator's order with it; ratio and distance 0."""
+        p = np.ascontiguousarray(pairs, np.uint32).reshape(-1, 2)
+        n = p.shape[0]
+        Mm = np.ascontiguousarray(M, np.float64).reshape(n, 9)
+        th = np.ascontiguousarray(errorTh, np.float64).reshape(n)
+        res = C.c_void_p()
+        _check(self.lib.b200m_guided_match_positions_pairs(self._h, p.ctypes.data_as(C.c_void_p), C.c_int(n), C.c_int(model),
+                                                           Mm.ctypes.data_as(C.c_void_p), th.ctypes.data_as(C.c_void_p), C.c_int(int(bool(decorate))),
+                                                           C.byref(res)), "b200m_guided_match_positions_pairs")
+        return self._pair_lists(res, n)
+
+    def _pair_lists(self, res, n: int) -> list:
         owner = _ResultOwner(self.lib, res)
         off, mat = C.c_void_p(), C.c_void_p()
         _check(self.lib.b200m_result_get(res, None, C.byref(off), C.byref(mat)), "b200m_result_get")
@@ -366,8 +386,31 @@ def robustModelEstimation_F_AC(putatives: dict, regions_per_view: dict, image_si
     and distance kept); with it, the guided lists of every common type (empty ones included) replace them, or nothing when error_max
     is infinite (GeometricFilterMatrix_F_AC.hpp:363)."""
     ctx = ctx or default_context()
-    order = list(desc_types) if desc_types is not None else DESCRIBER_TYPES
     st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
+    pairs, common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
+    res = ctx.acransac_fundamental_pairs(corrs, whs, st, maxIteration, precision) if est else []
+    info = {p: {"valid": False, "strong_support": False, "F": np.zeros((3, 3)), "error_max": np.inf} for p in pairs}
+    out = {}
+    for p, r in zip(est, res):
+        info[p].update(valid=r["valid"], F=r["F"], error_max=r["error_max"])
+        if not r["valid"]:
+            continue
+        inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
+        info[p]["strong_support"] = hasStrongSupport(inl)
+        if info[p]["strong_support"]:
+            out[p] = inl
+    if guidedMatching and out:
+        _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry,
+                      lambda vp, items: ctx.guided_match_pairs(vp, [info[p]["F"] for p, _ in items],
+                                                               [info[p]["error_max"] * info[p]["error_max"] for p, _ in items],
+                                                               distanceRatio * distanceRatio))
+    return out, info
+
+
+def _estimation_inputs(putatives: dict, regions_per_view: dict, image_sizes: dict, geometry: dict | None, desc_types):
+    """The pair list, each pair's common describer types (EImageDescriberType order), the pairs that have one, and for those the
+    correspondences of fillMatricesWithUndistortFeaturesMatches (n x 4: xI, yI, xJ, yJ, types concatenated in order) and image sizes."""
+    order = list(desc_types) if desc_types is not None else DESCRIBER_TYPES
     geometry = geometry or {}
     pairs = list(putatives)
     common = {p: [t for t in order if t in regions_per_view[p[0]] and t in regions_per_view[p[1]]] for p in pairs}
@@ -386,38 +429,86 @@ def robustModelEstimation_F_AC(putatives: dict, regions_per_view: dict, image_si
                 parts.append(np.concatenate([positions(I, t)[m["i"]], positions(J, t)[m["j"]]], axis=1))
         corrs.append(np.concatenate(parts))
         whs.append(tuple(image_sizes[I]) + tuple(image_sizes[J]))
-    res = ctx.acransac_fundamental_pairs(corrs, whs, st, maxIteration, precision) if est else []
-    info = {p: {"valid": False, "strong_support": False, "F": np.zeros((3, 3)), "error_max": np.inf} for p in pairs}
+    return pairs, common, est, corrs, whs
+
+
+def _guided_stage(ctx: Context, out: dict, info: dict, common: dict, regions_per_view: dict, guided_geometry: dict | None, run) -> None:
+    """The guided-matching step of a geometric filter stage: every kept pair's lists are replaced by one entry per common type (empty
+    ones included) when its error_max is finite, else by nothing.  The views of those pairs are uploaded once per (view, type), with
+    their guided positions, and run(view_pairs, items) makes the one batched call over items = [(pair, type)]."""
+    guided = [p for p in out if np.isfinite(info[p]["error_max"])]
+    for p in out:
+        out[p] = {}
+    ids, up = {}, []
+    try:
+        for I, J in guided:
+            for t in common[(I, J)]:
+                for v in (I, J):
+                    if (v, t) not in ids:
+                        ids[(v, t)] = _new_view_id()
+                        xy = (guided_geometry or {}).get(v, {}).get(t)
+                        _upload_pair(ctx, [ids[(v, t)]], [regions_per_view[v][t]], [xy], up)
+        items = [(p, t) for p in guided for t in common[p]]
+        lists = run([(ids[(p[0], t)], ids[(p[1], t)]) for p, t in items], items) if items else []
+        for (p, t), m in zip(items, lists):
+            out[p][t] = m
+    finally:
+        for vid in up:
+            ctx.lib.b200m_remove_view(ctx._h, C.c_uint32(vid))
+
+
+def robustModelEstimation_H_AC(putatives: dict, regions_per_view: dict, image_sizes: dict, seed_or_state, maxIteration: int = 50000,
+                               precision: float = np.inf, guidedMatching: bool = False, distanceRatio: float = -1.0, geometry: dict | None = None,
+                               guided_geometry: dict | None = None, desc_types=None, chain: bool = False, ctx: Context | None = None):
+    """matchingImageCollection::robustModelEstimation with GeometricFilterMatrix_H_AC (ACRANSAC, Homography4PSolver, point-to-point
+    error; GeometricFilterMatrix_H_AC.hpp:43-103), the `homography_matrix` filter of featureMatching, for a whole putative list: a-contrario
+    RANSAC for every pair (b200m_acransac_homography_pairs), copyInlierMatches and hasStrongSupport(.., 4); then, with guidedMatching,
+    one guided-matching call for every kept pair with a finite error_max and every common type, errorTh = error_max^2:
+      distanceRatio < 0   position-only guidedMatching + IndMatchDecorator (b200m_guided_match_positions_pairs), what featureMatching
+                          runs (it passes distanceRatio = -1 with --guidedMatching)
+      distanceRatio >= 0  guidedMatching with descriptors and distRatio = distanceRatio^2 (b200m_guided_match_pairs, homography model)
+
+    Arguments as robustModelEstimation_F_AC, except the generator contract.  geometricEstimation takes the std::mt19937 by reference, so
+    the reference's filter hands one generator from pair to pair; under featureMatching's OpenMP loop every thread draws from it without
+    synchronisation, and no run is reproducible.
+      chain=False  every pair starts from the caller's state (as the F stage does): deterministic, one K10 call for the whole list.
+      chain=True   the single-threaded reference: K10 runs one pair per call in putative-list order, each starting from the state the
+                   previous pair left (pairs without a common type draw nothing).  Bit for bit the reference's run; meant for tests and
+                   short lists.
+
+    Returns (geometric matches {(I, J): {type: matches}} of the pairs with strong support, per-pair estimation
+    {(I, J): {"valid", "strong_support", "H", "error_max"}, plus "mt_state_out" for the estimated pairs}).  The kept lists are as in
+    robustModelEstimation_F_AC; the position-only guided lists are in the decorator's order (ratio and distance 0)."""
+    ctx = ctx or default_context()
+    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
+    pairs, common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
+    if not est:
+        res = []
+    elif chain:
+        res = []
+        for c, wh in zip(corrs, whs):
+            res.append(ctx.acransac_homography_pairs([c], [wh], st, maxIteration, precision)[0])
+            st = res[-1]["mt_state_out"]
+    else:
+        res = ctx.acransac_homography_pairs(corrs, whs, st, maxIteration, precision)
+    info = {p: {"valid": False, "strong_support": False, "H": np.zeros((3, 3)), "error_max": np.inf} for p in pairs}
     out = {}
     for p, r in zip(est, res):
-        info[p].update(valid=r["valid"], F=r["F"], error_max=r["error_max"])
+        info[p].update(valid=r["valid"], H=r["H"], error_max=r["error_max"], mt_state_out=r["mt_state_out"])
         if not r["valid"]:
             continue
         inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
-        info[p]["strong_support"] = hasStrongSupport(inl)
+        info[p]["strong_support"] = hasStrongSupport(inl, 4)          # Homography4PSolver::getMinimumNbRequiredSamples
         if info[p]["strong_support"]:
             out[p] = inl
     if guidedMatching and out:
-        guided = [p for p in out if np.isfinite(info[p]["error_max"])]
-        for p in out:
-            out[p] = {}
-        ids, up = {}, []
-        try:
-            for I, J in guided:
-                for t in common[(I, J)]:
-                    for v in (I, J):
-                        if (v, t) not in ids:
-                            ids[(v, t)] = _new_view_id()
-                            xy = (guided_geometry or {}).get(v, {}).get(t)
-                            _upload_pair(ctx, [ids[(v, t)]], [regions_per_view[v][t]], [xy], up)
-            items = [(p, t) for p in guided for t in common[p]]
-            lists = ctx.guided_match_pairs([(ids[(p[0], t)], ids[(p[1], t)]) for p, t in items], [info[p]["F"] for p, _ in items],
-                                           [info[p]["error_max"] * info[p]["error_max"] for p, _ in items], distanceRatio * distanceRatio) if items else []
-            for (p, t), m in zip(items, lists):
-                out[p][t] = m
-        finally:
-            for vid in up:
-                ctx.lib.b200m_remove_view(ctx._h, C.c_uint32(vid))
+        def run(vp, items):
+            Hs = [info[p]["H"] for p, _ in items]
+            th = [info[p]["error_max"] * info[p]["error_max"] for p, _ in items]
+            if distanceRatio < 0:
+                return ctx.guided_match_positions_pairs(vp, Hs, th, MODEL_HOMOGRAPHY, decorate=True)
+            return ctx.guided_match_pairs(vp, Hs, th, distanceRatio * distanceRatio, MODEL_HOMOGRAPHY)
+        _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry, run)
     return out, info
 
 

@@ -148,6 +148,20 @@ int b200m_guided_match_model(b200m_ctx* ctx, uint32_t view_left, uint32_t view_r
  * b200m_guided_match_model are this call on a list of one pair. */
 int b200m_guided_match_pairs(b200m_ctx* ctx, const uint32_t* pairs, int n_pairs, int model, const double* M, const double* errorTh, double distRatio,
                              b200m_result** out);
+/* Position-only guided matching, what GeometricFilterMatrix_H_AC::Geometry_guided_matching runs with distanceRatio < 0 (featureMatching's
+ * guided homography filter): matching::guidedMatching<Mat3Model, ErrorT>(model, xLeft, xRight, errorTh, matches) (guidedMatching.hpp:37-70)
+ * for every pair of resident views.  For every left feature, the right feature of smallest error (HomographyAsymmetricError or
+ * FundamentalEpipolarDistanceError) below errorTh, the first j on ties; no descriptor is read.  Then IndMatch::getDeduplicated.
+ * Arguments as in b200m_guided_match_pairs, without distRatio.  The positions are the geometry positions when set
+ * (b200m_set_view_geometry), else the upload positions.
+ *   decorate = 0: that list, IndMatch(i = left, j = right) sorted by (i, j), ratio and distance 0.  As in the reference, with
+ *                 errorTh = +inf a left feature without a finite error below DBL_MAX contributes IndMatch() = (0, 0).
+ *   decorate = 1: then IndMatchDecorator<float>::getDeduplicated on the upload positions of both views (GeometricFilterMatrix_H_AC.hpp:197-199):
+ *                 on the device for a left view in general position (all x distinct, all y distinct), else the reference's std::set.
+ *                 Both views need upload positions (else B200M_ERR_ARG).
+ * A pair with an empty view, or whose views differ in describer type, gets an empty list.  Batches as b200m_guided_match_pairs. */
+int b200m_guided_match_positions_pairs(b200m_ctx* ctx, const uint32_t* pairs, int n_pairs, int model, const double* M, const double* errorTh,
+                                       int decorate, b200m_result** out);
 
 /* Positions guided matching uses for one uploaded view instead of its (float) upload positions: n x 2 doubles, typically
  * camera::IntrinsicBase::getUndistortedPixel of every feature (matching/guidedMatching.hpp:229-248, :395, :416): the reference
@@ -253,8 +267,8 @@ int b200m_debug_rand_sample(const uint32_t state[625], int range, int draws, uin
 int b200m_debug_rand_sample_k(const uint32_t state[625], int sample_size, int range, int draws, uint32_t* out, uint32_t* states);
 
 /* ---- instrumentation ------------------------------------------------------------------------------------------ */
-/* The b200m_last_* getters report the last successful b200m_match_pairs, b200m_guided_match(_model, _pairs), b200m_guided_match_fast_pairs
- * or b200m_knn on the context, whichever came last; a value that call does not measure reads 0 (b200m_knn sets only
+/* The b200m_last_* getters report the last successful b200m_match_pairs, b200m_guided_match(_model, _pairs), b200m_guided_match_positions_pairs,
+ * b200m_guided_match_fast_pairs or b200m_knn on the context, whichever came last; a value that call does not measure reads 0 (b200m_knn sets only
  * b200m_last_tc_pairs: 1 when it ran on the tensor-core kernel).  They take the context's lock.  The a-contrario RANSAC calls have
  * their own (b200m_acransac_last_stats) and leave these alone. */
 /* GPU time of the last call between its first and last enqueue (CUDA events on the context's stream), ms */
@@ -268,8 +282,8 @@ int b200m_last_launches(const b200m_ctx* ctx);
 int b200m_last_tc_pairs(const b200m_ctx* ctx);
 /* candidates whose re-scored best distance differed from the tensor-core value (must stay 0); cumulative over the context's life */
 unsigned b200m_exactness_errors(const b200m_ctx* ctx);
-/* total raw records (matches before host finishing) produced by the last call; b200m_guided_match(_model, _pairs): its matches,
- * b200m_guided_match_fast_pairs: the candidate distances it evaluated */
+/* total raw records (matches before host finishing) produced by the last call; b200m_guided_match(_model, _pairs) and
+ * b200m_guided_match_positions_pairs: its matches, b200m_guided_match_fast_pairs: the candidate distances it evaluated */
 int64_t b200m_last_records(const b200m_ctx* ctx);
 /* pairs of the last call that ran on the tensor-core FILTER kernel for real-valued fp32 descriptors (fp16-rounded GEMM + rigorous error
  * bound + exact re-scoring in the reference's arithmetic), and the queries among them the bound could not decide, which were searched
