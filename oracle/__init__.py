@@ -58,6 +58,25 @@ def available(kind: str) -> bool:
     return os.path.exists(_lib_path(kind))
 
 
+def exports(path: str, names) -> bool:
+    """Whether the shared library at `path` defines every symbol in `names`.  Read with nm rather than loaded: a library dlopen'ed in
+    this process stays the one its path resolves to, even after a rebuild replaces the file."""
+    r = subprocess.run(["nm", "-D", "--defined-only", path], capture_output=True, text=True)
+    return r.returncode == 0 and set(names) <= {ln.split()[-1] for ln in r.stdout.splitlines() if ln.strip()}
+
+
+def make_current(makefile: str, targets: dict, make_args) -> None:
+    """make -f makefile <make_args>, then rebuild (make -B) every target of `targets` ({target: (library path, symbols)}) whose
+    library was not rebuilt but lacks symbols: make goes by modification times, and a library compiled from older sources can be
+    newer than a fresh checkout of the sources."""
+    subprocess.run(["make", "-C", _HERE, "-f", makefile] + list(make_args), check=True, stdout=subprocess.DEVNULL)
+    for target, (path, names) in targets.items():
+        if os.path.exists(path) and not exports(path, names):
+            extra = [a for a in make_args if "=" in a]
+            subprocess.run(["make", "-C", _HERE, "-f", makefile, "-B", target] + extra, check=True, stdout=subprocess.DEVNULL)
+            assert exports(path, names), f"{path} lacks {sorted(names)} after a rebuild"
+
+
 def _lib_path(kind: str) -> str:
     return os.path.join(_HERE, "_ref", "libref_oracle.so") if kind == "ref" else os.path.join(_HERE, "libport_oracle.so")
 

@@ -13,7 +13,6 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
@@ -33,12 +32,25 @@ def available(kind: str) -> bool:
     return os.path.exists(_lib_path(kind))
 
 
+# the primitives the exact-arithmetic tests call (test_acransac_exact.py); the estimation entry points predate them
+PRIMITIVES = ("acr_solve_cubic", "acr_nullspace7", "acr_epipolar_error", "acr_precondition", "acr_unnormalize", "acr_logalpha0",
+                "acr_unnormalize_error")
+
+
+def current(kind: str) -> bool:
+    """The library is built and has every entry point of this source (an older build lacks PRIMITIVES)."""
+    return available(kind) and oracle.exports(_lib_path(kind), PRIMITIVES)
+
+
 def build(ref: bool | None = None) -> None:
-    """Compile the port always, the "ref" build when oracle.reference_src() finds an AliceVision tree."""
+    """Compile the port always, the "ref" build when oracle.reference_src() finds an AliceVision tree; a library older than these
+    sources' entry points is rebuilt even when make finds it up to date."""
     src = oracle.reference_src()
     ref = (src is not None) if ref is None else ref
-    subprocess.run(["make", "-C", _HERE, "-f", "acransac.mk", "all"] + (["ref", f"REF={src}"] if ref else []), check=True,
-                   stdout=subprocess.DEVNULL)
+    targets = {"libport_acransac.so": (_lib_path("port"), PRIMITIVES)}
+    if ref:
+        targets["_ref/libref_acransac.so"] = (_lib_path("ref"), PRIMITIVES)
+    oracle.make_current("acransac.mk", targets, ["all"] + (["ref", f"REF={src}"] if ref else []))
 
 
 def _p(a: np.ndarray):
@@ -78,6 +90,53 @@ class AcransacOracle:
         F = np.zeros((3, 9), np.float64)
         nb = self.lib.acr_fit7(_p(c), _p(F))
         return F[:nb].reshape(-1, 3, 3)
+
+    # -- the F kernel's primitives (the tests of test_acransac_exact.py check them against mpmath)
+    def solve_cubic(self, P) -> np.ndarray:
+        """SolveCubicPolynomial(P, x), P in ascending powers: the roots it returns (0, 1 or 3)."""
+        p = np.ascontiguousarray(P, np.float64).reshape(4)
+        x = np.zeros(3, np.float64)
+        f = self.lib.acr_solve_cubic
+        f.restype = C.c_int
+        nb = f(_p(p), _p(x))
+        return x[:nb].copy()
+
+    def nullspace7(self, A) -> np.ndarray:
+        a = np.ascontiguousarray(A, np.float64).reshape(7, 9)
+        N = np.zeros((2, 9), np.float64)
+        self.lib.acr_nullspace7(_p(a), _p(N))
+        return N
+
+    def errors(self, F, corr) -> np.ndarray:
+        """FundamentalEpipolarDistanceError of F on the correspondences as given (no normalisation)."""
+        c = np.ascontiguousarray(corr, np.float64).reshape(-1, 4)
+        f = np.ascontiguousarray(F, np.float64).reshape(9)
+        e = np.zeros(c.shape[0])
+        self.lib.acr_epipolar_error(_p(f), C.c_int(c.shape[0]), _p(c), _p(e))
+        return e
+
+    def precondition(self, w: int, h: int, x=(), y=()):
+        """((s, tx, ty), x normalised, y normalised) of preconditionerFromImageSize(w, h)."""
+        sxy = np.zeros(3)
+        xs = np.array(x, np.float64).reshape(-1).copy(); ys = np.array(y, np.float64).reshape(-1).copy()
+        assert xs.size == ys.size
+        self.lib.acr_precondition(C.c_int(w), C.c_int(h), _p(sxy), C.c_int(xs.size), _p(xs), _p(ys))
+        return sxy, xs, ys
+
+    def unnormalize(self, wh, F) -> np.ndarray:
+        f = np.ascontiguousarray(F, np.float64).reshape(9).copy()
+        self.lib.acr_unnormalize(*(C.c_int(int(v)) for v in wh), _p(f))
+        return f.reshape(3, 3)
+
+    def logalpha0(self, wh) -> float:
+        f = self.lib.acr_logalpha0
+        f.restype = C.c_double
+        return f(*(C.c_int(int(v)) for v in wh))
+
+    def unnormalize_error(self, wh, v: float) -> float:
+        f = self.lib.acr_unnormalize_error
+        f.restype = C.c_double
+        return f(*(C.c_int(int(x)) for x in wh), C.c_double(v))
 
     def estimate(self, corr, wh, state, max_iteration: int = 50000, precision: float = np.inf) -> dict:
         """One pair: corr n x 4 (xI, yI, xJ, yJ), wh = (wI, hI, wJ, hJ), state = 625 generator words."""

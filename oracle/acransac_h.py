@@ -13,7 +13,6 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
@@ -33,12 +32,24 @@ def available(kind: str) -> bool:
     return os.path.exists(_lib_path(kind))
 
 
+# the primitives the exact-arithmetic tests call (test_acransac_exact.py); the estimation entry points predate them
+PRIMITIVES = ("acr_nullspace8", "acr_inverse3", "acr_unnormalize_h", "acr_logalpha0_h", "acr_unnormalize_error_h")
+
+
+def current(kind: str) -> bool:
+    """The library is built and has every entry point of this source (an older build lacks PRIMITIVES)."""
+    return available(kind) and oracle.exports(_lib_path(kind), PRIMITIVES)
+
+
 def build(ref: bool | None = None) -> None:
-    """Compile the port always, the "ref" build when oracle.reference_src() finds an AliceVision tree."""
+    """Compile the port always, the "ref" build when oracle.reference_src() finds an AliceVision tree; a library older than these
+    sources' entry points is rebuilt even when make finds it up to date."""
     src = oracle.reference_src()
     ref = (src is not None) if ref is None else ref
-    subprocess.run(["make", "-C", _HERE, "-f", "acransac_h.mk", "all"] + (["ref", f"REF={src}"] if ref else []), check=True,
-                   stdout=subprocess.DEVNULL)
+    targets = {"libport_acransac_h.so": (_lib_path("port"), PRIMITIVES)}
+    if ref:
+        targets["_ref/libref_acransac_h.so"] = (_lib_path("ref"), PRIMITIVES)
+    oracle.make_current("acransac_h.mk", targets, ["all"] + (["ref", f"REF={src}"] if ref else []))
 
 
 def _p(a: np.ndarray):
@@ -85,6 +96,34 @@ class AcransacHOracle:
         e = np.zeros(c.shape[0])
         self.lib.acr_homography_error(_p(h), C.c_int(c.shape[0]), _p(c), _p(e))
         return e
+
+    # -- the H kernel's primitives (the tests of test_acransac_exact.py check them against mpmath)
+    def nullspace8(self, A) -> np.ndarray:
+        a = np.ascontiguousarray(A, np.float64).reshape(8, 9)
+        N = np.zeros(9, np.float64)
+        self.lib.acr_nullspace8(_p(a), _p(N))
+        return N
+
+    def inverse3(self, M) -> np.ndarray:
+        m = np.ascontiguousarray(M, np.float64).reshape(9)
+        R = np.zeros(9, np.float64)
+        self.lib.acr_inverse3(_p(m), _p(R))
+        return R.reshape(3, 3)
+
+    def unnormalize(self, wh, H) -> np.ndarray:
+        h = np.ascontiguousarray(H, np.float64).reshape(9).copy()
+        self.lib.acr_unnormalize_h(*(C.c_int(int(v)) for v in wh), _p(h))
+        return h.reshape(3, 3)
+
+    def logalpha0(self, wh) -> float:
+        f = self.lib.acr_logalpha0_h
+        f.restype = C.c_double
+        return f(*(C.c_int(int(v)) for v in wh))
+
+    def unnormalize_error(self, wh, v: float) -> float:
+        f = self.lib.acr_unnormalize_error_h
+        f.restype = C.c_double
+        return f(*(C.c_int(int(x)) for x in wh), C.c_double(v))
 
     def estimate(self, corr, wh, state, max_iteration: int = 50000, precision: float = np.inf) -> dict:
         """One pair: corr n x 4 (xI, yI, xJ, yJ), wh = (wI, hI, wJ, hJ), state = 625 generator words (left unchanged; the state

@@ -278,6 +278,31 @@ void acr_homography_error(const double* H, int n, const double* corr, double* e)
   for (int i = 0; i < n; ++i) e[i] = acr::homography_error(H, corr[4 * i], corr[4 * i + 1], corr[4 * i + 2], corr[4 * i + 3]);
 }
 
+// The H kernel's primitives one by one, for the tests that check them against an independent high-precision reference.
+// the null space of an 8 x 9 row-major system: N[9] = Q e8
+void acr_nullspace8(const double* A, double* N) {
+  double a[8][9], n[1][9];
+  std::memcpy(a, A, sizeof a);
+  acr::nullspace<8>(a, n);
+  std::memcpy(N, n, sizeof n);
+}
+
+// the restated 3 x 3 inverse (cofactors over the first-column determinant), row-major
+void acr_inverse3(const double* M, double* R) { acr::inverse3(M, R); }
+
+// UnnormalizerI in place (H <- N2^-1 H N1), with the kernel's preconditioners of (w1, h1) and (w2, h2)
+void acr_unnormalize_h(int w1, int h1, int w2, int h2, double* H) {
+  const HKernel k(nullptr, 0, w1, h1, w2, h2);
+  Model m;
+  std::memcpy(m.M, H, sizeof m.M);
+  k.unnormalize(m);
+  std::memcpy(H, m.M, sizeof m.M);
+}
+
+// the kernel's logalpha0() and unormalizeError(v) for image J = (w2, h2)
+double acr_logalpha0_h(int w1, int h1, int w2, int h2) { return HKernel(nullptr, 0, w1, h1, w2, h2).logalpha0(); }
+double acr_unnormalize_error_h(int w1, int h1, int w2, int h2, double v) { return HKernel(nullptr, 0, w1, h1, w2, h2).unormalizeError(v); }
+
 // GeometricFilterMatrix_H_AC::geometricEstimation's ACRANSAC of one pair.  corr: n x (xI, yI, xJ, yJ).  inliers: capacity n.
 // state: the generator on entry; state_out: the generator after the estimation (the reference's std::mt19937& afterwards).
 // trace: the iterations at which a better model was found (first trace_cap of *n_trace); trace_nfa: the new minNFA of each (NaN in

@@ -272,6 +272,49 @@ int acr_fit7(const double* corr, double* F) {
   return acr::fit7(a, b, c, d, F);
 }
 
+// The F kernel's primitives one by one, for the tests that check them against an independent high-precision reference.
+// SolveCubicPolynomial(P, x): the compiled reference's own in the "ref" build, the restated one in "port"; returns the root count.
+int acr_solve_cubic(const double* P, double* x) {
+#ifdef ACR_USE_REFERENCE
+  return aliceVision::SolveCubicPolynomial<double>(P, x);
+#else
+  return acr::solve_cubic(P, x);
+#endif
+}
+
+// the null space of a 7 x 9 row-major system: N[2 x 9], rows N[0] = Q e8 and N[1] = Q e7
+void acr_nullspace7(const double* A, double* N) {
+  double a[7][9], n[2][9];
+  std::memcpy(a, A, sizeof a);
+  acr::nullspace<7>(a, n);
+  std::memcpy(N, n, sizeof n);
+}
+
+// FundamentalEpipolarDistanceError of F on n correspondences as given (no normalisation): e[i]
+void acr_epipolar_error(const double* F, int n, const double* corr, double* e) {
+  for (int i = 0; i < n; ++i) e[i] = acr::epipolar_error(F, corr[4 * i], corr[4 * i + 1], corr[4 * i + 2], corr[4 * i + 3]);
+}
+
+// preconditionerFromImageSize(w, h): (s, tx, ty), and the n coordinates x[i], y[i] mapped through it in place
+void acr_precondition(int w, int h, double* sxy, int n, double* x, double* y) {
+  const acr::Norm nm = acr::precondition(w, h);
+  sxy[0] = nm.s; sxy[1] = nm.tx; sxy[2] = nm.ty;
+  for (int i = 0; i < n; ++i) { x[i] = acr::norm_x(nm, x[i]); y[i] = acr::norm_y(nm, y[i]); }
+}
+
+// UnnormalizerT in place (F <- N2^T F N1), with the kernel's preconditioners of (w1, h1) and (w2, h2)
+void acr_unnormalize(int w1, int h1, int w2, int h2, double* F) {
+  const FKernel k(nullptr, 0, w1, h1, w2, h2);
+  Model m;
+  std::memcpy(m.F, F, sizeof m.F);
+  k.unnormalize(m);
+  std::memcpy(F, m.F, sizeof m.F);
+}
+
+// the kernel's logalpha0() and unormalizeError(v) for image J = (w2, h2)
+double acr_logalpha0(int w1, int h1, int w2, int h2) { return FKernel(nullptr, 0, w1, h1, w2, h2).logalpha0(); }
+double acr_unnormalize_error(int w1, int h1, int w2, int h2, double v) { return FKernel(nullptr, 0, w1, h1, w2, h2).unormalizeError(v); }
+
 // geometricEstimation_Mat_ACRANSAC<Fundamental7PSolver, Mat3Model> of one pair.  corr: n x (xI, yI, xJ, yJ).  inliers: capacity n.
 // trace: the iterations at which a better model was found (first trace_cap of *n_trace); trace_nfa: the new minNFA of each
 // (NaN in the "ref" build).  Returns the iterations executed.
