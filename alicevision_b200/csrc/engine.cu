@@ -25,6 +25,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <atomic>
@@ -1481,7 +1482,10 @@ int b200m_set_view_geometry(b200m_ctx* c, uint32_t view_id, const double* xy, in
 
 }  // extern "C"
 
-// ---- guided matching from known poses: guidedMatchingFundamentalFast for a list of pairs (guided_fast.cuh) -------------------
+// ---- guided matching of a pair list: b200m_guided_match_fast_pairs (K9, guided_fast.cuh), b200m_guided_match_pairs (K7, guided.cuh)
+// and b200m_guided_match_positions_pairs (position-only, guided.cuh).  The three calls share one path: guided_work checks the whole
+// list before anything runs, run_batches groups it into batches (the rule is DESIGN.md K7), the call's own *_run_batch runs one batch
+// and appends each pair's matches to its list, and guided_result returns one list per input pair, in input order. ---------------------
 template <class T> static int exclusive_scan(DeviceBuffer<>& tmp, const T* in, T* out, size_t n, cudaStream_t st, int& launches) {
   size_t tb = 0;
   CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, in, out, (int64_t)n, st));
@@ -1493,27 +1497,129 @@ template <class T> static int exclusive_scan(DeviceBuffer<>& tmp, const T* in, T
 
 namespace {
 struct GfPairHost { int index, slot_l, slot_r, kclass; };   // kclass: kernel dtype, or 3 = mixed (uchar-stored view expanded to fp32)
+// One batch: pairs of one kernel class, and the uchar-stored views of its mixed pairs, each expanded to fp32 once
+struct GuidedBatch { std::vector<GfPairHost> pairs; std::set<int> expand; };
+// What a call measured, summed over its batches
+struct GuidedTotals { double gpu_ms = 0, search_ms = 0; int launches = 0; int64_t cands = 0; };
+using PairLists = std::vector<std::vector<b200m_match>>;
 }
 
-// One batch of pairs of one kernel class.  Appends the pair's matches to per_pair[index].
-static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, const double* F, const double* ep2, const int32_t* wh, double errorTh,
-                        double distRatio, std::vector<std::vector<uint2>>& per_pair, double& gpu_ms, double& cand_ms, int& launches, int64_t& cands) {
+// The work list of pairs[0 .. n_pairs), checked whole before anything runs; check(k) runs first for each entry.  A pair with an empty
+// view or no common descriptor type gets an empty list (guidedMatching.hpp:300-306).  `descriptors`: the call reads descriptors (128
+// scalars or 64 bytes); `upload_xy`: it needs the upload positions of both views, geometry positions are not enough.
+template <class Check>
+static int guided_work(b200m_ctx* c, const uint32_t* pairs, int n_pairs, bool descriptors, bool upload_xy, Check check,
+                       std::vector<GfPairHost>& work) {
+  for (int k = 0; k < n_pairs; ++k) {
+    if (int rc = check(k)) return rc;
+    auto sl = c->slot_of.find(pairs[2 * k]), sr = c->slot_of.find(pairs[2 * k + 1]);
+    if (sl == c->slot_of.end() || sr == c->slot_of.end()) return fail(B200M_ERR_ARG, "guided matching references a view that was never uploaded");
+    const ViewHost& vl = c->views[sl->second]; const ViewHost& vr = c->views[sr->second];
+    if (!(vl.m > 0 && vr.m > 0 && vl.dtype == vr.dtype && vl.dim == vr.dim)) continue;
+    if (descriptors && !((vl.dtype == DT_BIN && vl.dim == 64) || (vl.dtype != DT_BIN && vl.dim == 128)))
+      return fail(B200M_ERR_UNSUPPORTED, "guided matching takes 128-component scalar or 64-byte binary descriptors");
+    if (upload_xy ? (vl.xy.empty() || vr.xy.empty()) : ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom)))
+      return fail(B200M_ERR_ARG, upload_xy ? "the decorator needs the upload positions of both views"
+                                           : "guided matching needs feature positions (or geometry positions) for both views");
+    work.push_back({k, sl->second, sr->second, 0});
+  }
+  return B200M_OK;
+}
+
+// Walks the work list once in input order; each pair joins the open batch of its kernel class (uchar, fp32, mixed, binary; one class
+// when `by_class` is false), and run(batch) runs a batch when one more pair would pass one of its bounds: 8192 pairs, left_cap left
+// features (a larger pair runs alone), right_cap right features, bucket_cap buckets (buckets_of(index) per pair) or 64 Mi fp32
+// expansion elements.  The open batches run at the end, class by class.  Each view is waited for when its first pair is reached.
+template <class BucketsOf, class Run>
+static int run_batches(b200m_ctx* c, const std::vector<GfPairHost>& work, bool by_class, long left_cap, long right_cap, long bucket_cap,
+                       BucketsOf buckets_of, Run run) {
+  const long pair_cap = 8192, exp_cap = 64l << 20;
+  struct Open { GuidedBatch b; long l = 0, r = 0, nb = 0, e = 0; };
+  Open open[4];
+  auto flush = [&](Open& o) -> int {
+    if (o.b.pairs.empty()) return B200M_OK;
+    const int rc = run(o.b);
+    o = Open();
+    return rc;
+  };
+  for (GfPairHost p : work) {
+    int rc;
+    if ((rc = ensure_view_ready(c, p.slot_l)) || (rc = ensure_view_ready(c, p.slot_r))) return rc;
+    // the stored type is final once the view is ready (a uchar-staged view that met a non-integer value was re-uploaded as fp32)
+    const ViewHost& vl = c->views[p.slot_l]; const ViewHost& vr = c->views[p.slot_r];
+    p.kclass = !by_class ? 0 : vl.store_dtype() == vr.store_dtype() ? vl.store_dtype() : 3;
+    Open& o = open[p.kclass];
+    const long nb = buckets_of(p.index);
+    const int su = p.kclass == 3 ? (vl.stored_u8 ? p.slot_l : p.slot_r) : -1;
+    auto expansion = [&] { return su >= 0 && !o.b.expand.count(su) ? (long)c->views[su].m * 128 : 0l; };   // elements the pair adds
+    if (!o.b.pairs.empty() && ((long)o.b.pairs.size() + 1 > pair_cap || o.l + vl.m > left_cap || o.r + vr.m > right_cap ||
+                               o.nb + nb > bucket_cap || o.e + expansion() > exp_cap))
+      if ((rc = flush(o))) return rc;
+    o.e += expansion();
+    if (su >= 0) o.b.expand.insert(su);
+    o.b.pairs.push_back(p);
+    o.l += vl.m; o.r += vr.m; o.nb += nb;
+  }
+  for (Open& o : open)
+    if (int rc = flush(o)) return rc;
+  return B200M_OK;
+}
+
+// The fp32 copies of a batch's uchar-stored views in `buf`, one u8_to_f32_kernel each; x[slot] is the copy of view `slot`
+static int expand_views(b200m_ctx* c, DeviceBuffer<>& buf, const std::set<int>& views, std::map<int, const float*>& x, int& launches) {
+  size_t total = 0;
+  for (int s : views) total += (size_t)c->views[s].m * 128;
+  if (int rc = buf.reserve(sizeof(float) * total)) return rc;
+  float* d = buf.as<float>();
+  for (int s : views) {
+    const ViewHost& vu = c->views[s];
+    const size_t ne = (size_t)vu.m * 128;
+    u8_to_f32_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, c->stream>>>((const uint8_t*)vu.raw, d, ne);
+    x[s] = d; d += ne; ++launches;
+  }
+  return B200M_OK;
+}
+
+// Adds the batch's GPU time (ev_start .. ev_end) and its search kernel's (k0 .. k1) to t, once the stream is synchronised
+static int add_times(b200m_ctx* c, cudaEvent_t k0, cudaEvent_t k1, GuidedTotals& t) {
+  float ms = 0.f, kms = 0.f;
+  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
+  CK(cudaEventElapsedTime(&kms, k0, k1));
+  t.gpu_ms += ms; t.search_ms += kms;
+  return B200M_OK;
+}
+
+// Appends the (i, j) of h[b .. e) to L as IndMatch(i, j): ratio and distance 0
+static void append_matches(std::vector<b200m_match>& L, const uint2* h, int b, int e) {
+  const size_t n0 = L.size();
+  L.resize(n0 + (size_t)std::max(e - b, 0));
+  for (b200m_match* m = L.data() + n0; b < e; ++b) *m++ = b200m_match{h[b].x, h[b].y, 0.f, 0.f};
+}
+
+// One result pair per input pair, in input order (empty lists included)
+static b200m_result* guided_result(b200m_ctx* c, const uint32_t* pairs, int n_pairs, const PairLists& per_pair) {
+  std::unique_ptr<b200m_result> res(new b200m_result());
+  res->recycler = c->recycler;
+  res->pair_ids.assign(pairs, pairs + 2 * (size_t)n_pairs);
+  res->offsets.assign((size_t)n_pairs + 1, 0);
+  for (int k = 0; k < n_pairs; ++k) res->offsets[k + 1] = res->offsets[k] + (int64_t)per_pair[k].size();
+  res->matches = c->recycler->take((size_t)std::max<int64_t>(res->offsets[n_pairs], 1));
+  for (int k = 0; k < n_pairs; ++k) std::copy(per_pair[k].begin(), per_pair[k].end(), res->matches.p + res->offsets[k]);
+  return res.release();
+}
+
+// One K9 batch (guidedMatchingFundamentalFast, one kernel class)
+static int gf_run_batch(b200m_ctx* c, const GuidedBatch& b, const double* F, const double* ep2, const int32_t* wh, double errorTh,
+                        double distRatio, PairLists& per_pair, GuidedTotals& t) {
   GuidedFastScratch& g = c->gf;
+  using G = GuidedFastScratch;
   cudaStream_t st = c->stream;
+  const std::vector<GfPairHost>& batch = b.pairs;
   const int np = (int)batch.size();
   const int kclass = batch[0].kclass;
-  // uchar-stored views of mixed pairs: one fp32 expansion each
-  std::map<int, size_t> exp_off; size_t exp_elems = 0;
-  if (kclass == 3)
-    for (const auto& p : batch) {
-      const int s = c->views[p.slot_l].stored_u8 ? p.slot_l : p.slot_r;
-      if (!exp_off.count(s)) { exp_off[s] = exp_elems; exp_elems += (size_t)c->views[s].m * 128; }
-    }
-  using G = GuidedFastScratch;
   int rc;
-  if ((rc = g.h_pairs.reserve(sizeof(FastPair) * (size_t)np)) || (rc = g.d[G::EXPAND].reserve(sizeof(float) * exp_elems))) return rc;
+  if ((rc = g.h_pairs.reserve(sizeof(FastPair) * (size_t)np))) return rc;
   FastPair* hp = g.h_pairs;
-  float* d_exp = g.d[G::EXPAND].as<float>();
   long sum_l = 0, sum_r = 0, sum_b = 0; int max_l = 0, max_r = 0;
   for (int k = 0; k < np; ++k) {
     const GfPairHost& q = batch[k];
@@ -1521,14 +1627,11 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
     FastPair& P = hp[k];
     std::memset(&P, 0, sizeof(P));
     P.rawl = vl.raw; P.rawr = vr.raw;
-    if (kclass == 3) {
-      if (vl.stored_u8) P.rawl = d_exp + exp_off[q.slot_l]; else P.rawr = d_exp + exp_off[q.slot_r];
-    }
     P.gl = vl.d_geom; P.gr = vr.d_geom; P.fl = (const float2*)vl.d_xy; P.fr = (const float2*)vr.d_xy;
     // normalise once (guidedMatching.hpp:378-385): F and ep2 negated when ep2(2) > 0, then ep2 / ep2(2)
     const double* f = F + 9 * (size_t)q.index; const double* e = ep2 + 3 * (size_t)q.index;
     const bool neg = e[2] > 0.0;
-    for (int t = 0; t < 9; ++t) P.F[t] = neg ? -f[t] : f[t];
+    for (int u = 0; u < 9; ++u) P.F[u] = neg ? -f[u] : f[u];
     const double e0 = neg ? -e[0] : e[0], e1 = neg ? -e[1] : e[1], e2 = neg ? -e[2] : e[2];
     P.e0 = e0 / e2; P.e1 = e1 / e2; P.e2 = e2 / e2;
     P.ml = vl.m; P.mr = vr.m; P.W = wh[2 * q.index]; P.H = wh[2 * q.index + 1]; P.nb = 2 * (P.W + P.H - 2);
@@ -1556,23 +1659,21 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
     if ((rc = g.d[G::TEMP].reserve(tb))) return rc; }
   if ((rc = g.ev_c0.create()) || (rc = g.ev_c1.create())) return rc;
   CK(cudaEventRecord(c->ev_start, st));
+  std::map<int, const float*> x;
+  if ((rc = expand_views(c, g.d[G::EXPAND], b.expand, x, t.launches))) return rc;
+  for (int k = 0; k < np && kclass == 3; ++k)      // mixed pairs read the fp32 copy of their uchar-stored view
+    if (c->views[batch[k].slot_l].stored_u8) hp[k].rawl = x[batch[k].slot_l]; else hp[k].rawr = x[batch[k].slot_r];
   CK(cudaMemcpyAsync(d_pairs, hp, sizeof(FastPair) * (size_t)np, cudaMemcpyHostToDevice, st));
-  for (const auto& x : exp_off) {
-    const ViewHost& vu = c->views[x.first];
-    const size_t ne = (size_t)vu.m * 128;
-    u8_to_f32_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>((const uint8_t*)vu.raw, d_exp + x.second, ne);
-    ++launches;
-  }
   CK(cudaMemsetAsync(d_bcount, 0, sizeof(int) * (size_t)sum_b, st));
   CK(cudaMemsetAsync(d_rcount + sum_r, 0, sizeof(unsigned long long), st));
   CK(cudaMemsetAsync(d_keep + sum_l, 0, sizeof(int), st));
   const dim3 gl((max_l + GF_THREADS - 1) / GF_THREADS, np), gr((max_r + GF_THREADS - 1) / GF_THREADS, np);
   guided_fast_left_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, d_lbucket, d_bcount, d_best, d_second);
-  if ((rc = exclusive_scan(g.d[G::TEMP], d_bcount, d_boff, (size_t)sum_b, st, launches))) return rc;
+  if ((rc = exclusive_scan(g.d[G::TEMP], d_bcount, d_boff, (size_t)sum_b, st, t.launches))) return rc;
   CK(cudaMemcpyAsync(d_bcount, d_boff, sizeof(int) * (size_t)sum_b, cudaMemcpyDeviceToDevice, st));   // scatter cursors
   guided_fast_scatter_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, d_lbucket, d_bcount, d_csr);
   guided_fast_right_kernel<<<gr, GF_THREADS, 0, st>>>(d_pairs, std::sqrt(errorTh), d_boff, d_rstart, d_rcount, d_rpair);
-  if ((rc = exclusive_scan(g.d[G::TEMP], d_rcount, d_rcoff, (size_t)sum_r + 1, st, launches))) return rc;
+  if ((rc = exclusive_scan(g.d[G::TEMP], d_rcount, d_rcoff, (size_t)sum_r + 1, st, t.launches))) return rc;
   CK(cudaEventRecord(g.ev_c0, st));
   const int cgrid = c->num_sms * 8;
   if (kclass == DT_U8) guided_fast_cand_kernel<DT_U8><<<cgrid, GF_THREADS, 0, st>>>(d_pairs, (int)sum_r, d_rcoff, d_rstart, d_rpair, d_csr, d_best, d_second);
@@ -1580,10 +1681,10 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
   else guided_fast_cand_kernel<DT_F32><<<cgrid, GF_THREADS, 0, st>>>(d_pairs, (int)sum_r, d_rcoff, d_rstart, d_rpair, d_csr, d_best, d_second);
   CK(cudaEventRecord(g.ev_c1, st));
   guided_fast_keep_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, distRatio, d_best, d_second, d_keep);
-  if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+  if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, t.launches))) return rc;
   guided_fast_emit_kernel<<<gl, GF_THREADS, 0, st>>>(d_pairs, np, (int)sum_l, d_keep, d_kpos, d_best, d_out, d_pstart);
   CK(cudaGetLastError());
-  launches += 5;
+  t.launches += 5;
   CK(cudaEventRecord(c->ev_end, st));
   // read-back: the candidate total + per-pair starts, then the matches
   if ((rc = g.h_meta.reserve(sizeof(unsigned long long) + sizeof(int) * (size_t)(np + 1)))) return rc;
@@ -1594,120 +1695,29 @@ static int gf_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, cons
   CK(cudaStreamSynchronize(st));
   const int n_out = h_pstart[np];
   std::vector<int> starts(h_pstart, h_pstart + np + 1);
-  cands += (int64_t)*h_total;
-  float ms = 0.f, cms = 0.f;
-  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
-  CK(cudaEventElapsedTime(&cms, g.ev_c0, g.ev_c1));
-  gpu_ms += ms; cand_ms += cms;
+  t.cands += (int64_t)*h_total;
+  if ((rc = add_times(c, g.ev_c0, g.ev_c1, t))) return rc;
   if (n_out > 0) {
     if ((rc = g.h_out.reserve(sizeof(uint2) * (size_t)n_out))) return rc;
     CK(cudaMemcpyAsync(g.h_out, d_out, sizeof(uint2) * (size_t)n_out, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    const uint2* h = g.h_out;
-    for (int k = 0; k < np; ++k) per_pair[batch[k].index].assign(h + starts[k], h + starts[k + 1]);
+    for (int k = 0; k < np; ++k) append_matches(per_pair[batch[k].index], g.h_out, starts[k], starts[k + 1]);
   }
   return B200M_OK;
 }
 
-extern "C" {
-
-int b200m_guided_match_fast_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, const double* F, const double* epipole2, const int32_t* wh,
-                                  double errorTh, double distRatio, b200m_result** out) {
-  if (!c || !out || n_pairs < 0 || (n_pairs > 0 && (!pairs || !F || !epipole2 || !wh))) return fail(B200M_ERR_ARG, "bad arguments");
-  *out = nullptr;
-  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
-  CK(cudaSetDevice(c->device));
-  // checks first: nothing runs for a list with a bad entry
-  std::vector<GfPairHost> work;
-  for (int k = 0; k < n_pairs; ++k) {
-    const int W = wh[2 * k], H = wh[2 * k + 1];
-    if (W < 2 || H < 2 || W > (1 << 24) || H > (1 << 24))
-      return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": the right image must be at least 2 x 2 pixels (and at most 2^24 on a side)");
-    auto sl = c->slot_of.find(pairs[2 * k]), sr = c->slot_of.find(pairs[2 * k + 1]);
-    if (sl == c->slot_of.end() || sr == c->slot_of.end()) return fail(B200M_ERR_ARG, "guided matching references a view that was never uploaded");
-    const ViewHost& vl = c->views[sl->second]; const ViewHost& vr = c->views[sr->second];
-    if (!(vl.m > 0 && vr.m > 0 && vl.dtype == vr.dtype && vl.dim == vr.dim)) continue;     // no common descriptor type / empty view: empty list
-    if (!((vl.dtype == DT_BIN && vl.dim == 64) || (vl.dtype != DT_BIN && vl.dim == 128)))
-      return fail(B200M_ERR_UNSUPPORTED, "guided matching takes 128-component scalar or 64-byte binary descriptors");
-    if ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom))
-      return fail(B200M_ERR_ARG, "guided matching needs feature positions (or geometry positions) for both views");
-    work.push_back({k, sl->second, sr->second, 0});
-  }
-  std::vector<std::vector<uint2>> per_pair((size_t)n_pairs);
-  double gpu_ms = 0, cand_ms = 0; int launches = 0; int64_t cands = 0;
-  // Batches: the list is walked once in input order and every pair joins the open batch of its kernel class (uchar, fp32, mixed,
-  // binary); a batch runs when it is full - bounded by left features (a pair larger than the bound runs alone), right features,
-  // buckets and fp32 expansions - and the rest at the end.  Each view is waited for when its first pair is reached.
-  const long pair_cap = 8192, right_cap = std::max(c->gf_left_cap, 1l << 20), bucket_cap = 16l << 20, exp_cap = 64l << 20;
-  struct Open { std::vector<GfPairHost> pairs; long l = 0, r = 0, b = 0, e = 0; std::set<int> exp_views; };
-  Open open[4];
-  auto flush = [&](Open& o) -> int {
-    if (o.pairs.empty()) return B200M_OK;
-    const int rc = gf_run_batch(c, o.pairs, F, epipole2, wh, errorTh, distRatio, per_pair, gpu_ms, cand_ms, launches, cands);
-    o = Open();
-    return rc;
-  };
-  for (GfPairHost p : work) {
-    int rc;
-    if ((rc = ensure_view_ready(c, p.slot_l)) || (rc = ensure_view_ready(c, p.slot_r))) return rc;
-    // the stored type is final once the view is ready (a uchar-staged view that met a non-integer value was re-uploaded as fp32)
-    const ViewHost& vl = c->views[p.slot_l]; const ViewHost& vr = c->views[p.slot_r];
-    p.kclass = vl.store_dtype() == vr.store_dtype() ? vl.store_dtype() : 3;
-    Open& o = open[p.kclass];
-    const int W = wh[2 * p.index], H = wh[2 * p.index + 1];
-    const long nb = 2l * (W + H - 2) + 1;
-    const int su = p.kclass == 3 ? (vl.stored_u8 ? p.slot_l : p.slot_r) : -1;
-    long ne = su >= 0 && !o.exp_views.count(su) ? (long)c->views[su].m * 128 : 0;
-    if (!o.pairs.empty() && ((long)o.pairs.size() + 1 > pair_cap || o.l + vl.m > c->gf_left_cap || o.r + vr.m > right_cap || o.b + nb > bucket_cap ||
-                             o.e + ne > exp_cap)) {
-      if ((rc = flush(o))) return rc;
-      ne = su >= 0 ? (long)c->views[su].m * 128 : 0;
-    }
-    o.pairs.push_back(p);
-    o.l += vl.m; o.r += vr.m; o.b += nb; o.e += ne;
-    if (su >= 0) o.exp_views.insert(su);
-  }
-  for (Open& o : open)
-    if (int rc = flush(o)) return rc;
-  if (int rc = wait_uploads(c)) return rc;
-  c->last = LastCall{gpu_ms, cand_ms, launches, 0, 0, 0, cands, 0};
-  // one result pair per input pair, in input order (empty lists included)
-  std::unique_ptr<b200m_result> res(new b200m_result());
-  res->recycler = c->recycler;
-  res->pair_ids.assign(pairs, pairs + 2 * (size_t)n_pairs);
-  res->offsets.assign((size_t)n_pairs + 1, 0);
-  for (int k = 0; k < n_pairs; ++k) res->offsets[k + 1] = res->offsets[k] + (int64_t)per_pair[k].size();
-  res->matches = c->recycler->take((size_t)std::max<int64_t>(res->offsets[n_pairs], 1));
-  for (int k = 0; k < n_pairs; ++k) {
-    b200m_match* m = res->matches.p + res->offsets[k];
-    for (const uint2& x : per_pair[k]) *m++ = b200m_match{x.x, x.y, 0.f, 0.f};     // IndMatch(i, j): ratio and distance 0
-  }
-  *out = res.release();
-  return B200M_OK;
-}
-
-}  // extern "C"
-
-// ---- guided matching for a list of pairs, one model each (guided.cuh); b200m_guided_match(_model) are lists of one -------------
-// One batch of pairs of one kernel class.  per_pair[index] receives the pair's matches.
-static int gm_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int model, const double* M, const double* errorTh, double distRatio,
-                        std::vector<std::vector<uint2>>& per_pair, double& gpu_ms, double& search_ms, int& launches) {
+// One K7 batch (guidedMatching with descriptors, one kernel class)
+static int gm_run_batch(b200m_ctx* c, const GuidedBatch& b, int model, const double* M, const double* errorTh, double distRatio,
+                        PairLists& per_pair, GuidedTotals& t) {
   GuidedScratch& g = c->gm;
   using G = GuidedScratch;
   cudaStream_t st = c->stream;
+  const std::vector<GfPairHost>& batch = b.pairs;
   const int np = (int)batch.size();
   const int kclass = batch[0].kclass;
-  // uchar-stored views of mixed pairs: one fp32 expansion each
-  std::map<int, size_t> exp_off; size_t exp_elems = 0;
-  if (kclass == 3)
-    for (const auto& p : batch) {
-      const int s = c->views[p.slot_l].stored_u8 ? p.slot_l : p.slot_r;
-      if (!exp_off.count(s)) { exp_off[s] = exp_elems; exp_elems += (size_t)c->views[s].m * 128; }
-    }
   int rc;
-  if ((rc = g.h_pairs.reserve(sizeof(GuidedPair) * (size_t)np)) || (rc = g.d[G::EXPAND].reserve(sizeof(float) * exp_elems))) return rc;
+  if ((rc = g.h_pairs.reserve(sizeof(GuidedPair) * (size_t)np))) return rc;
   GuidedPair* hp = g.h_pairs;
-  float* d_exp = g.d[G::EXPAND].as<float>();
   long sum_l = 0, blocks = 0;
   for (int k = 0; k < np; ++k) {
     const GfPairHost& q = batch[k];
@@ -1715,11 +1725,8 @@ static int gm_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int 
     GuidedPair& P = hp[k];
     std::memset(&P, 0, sizeof(P));
     P.rawl = vl.raw; P.rawr = vr.raw;
-    if (kclass == 3) {
-      if (vl.stored_u8) P.rawl = d_exp + exp_off[q.slot_l]; else P.rawr = d_exp + exp_off[q.slot_r];
-    }
     P.gl = vl.d_geom; P.gr = vr.d_geom; P.fl = (const float2*)vl.d_xy; P.fr = (const float2*)vr.d_xy;
-    for (int t = 0; t < 9; ++t) P.M[t] = M[9 * (size_t)q.index + t];
+    for (int u = 0; u < 9; ++u) P.M[u] = M[9 * (size_t)q.index + u];
     P.errorTh = errorTh[q.index];
     P.model = model == B200M_MODEL_HOMOGRAPHY ? GM_HOMOGRAPHY : GM_FUNDAMENTAL;
     P.ml = vl.m; P.mr = vr.m;
@@ -1739,122 +1746,41 @@ static int gm_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int 
     if ((rc = g.d[G::TEMP].reserve(tb))) return rc; }
   if ((rc = g.ev_k0.create()) || (rc = g.ev_k1.create())) return rc;
   CK(cudaEventRecord(c->ev_start, st));
+  std::map<int, const float*> x;
+  if ((rc = expand_views(c, g.d[G::EXPAND], b.expand, x, t.launches))) return rc;
+  for (int k = 0; k < np && kclass == 3; ++k)      // mixed pairs read the fp32 copy of their uchar-stored view
+    if (c->views[batch[k].slot_l].stored_u8) hp[k].rawl = x[batch[k].slot_l]; else hp[k].rawr = x[batch[k].slot_r];
   CK(cudaMemcpyAsync(d_pairs, hp, sizeof(GuidedPair) * (size_t)np, cudaMemcpyHostToDevice, st));
-  for (const auto& x : exp_off) {
-    const ViewHost& vu = c->views[x.first];
-    const size_t ne = (size_t)vu.m * 128;
-    u8_to_f32_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>((const uint8_t*)vu.raw, d_exp + x.second, ne);
-    ++launches;
-  }
   CK(cudaMemsetAsync(d_keep + sum_l, 0, sizeof(int), st));
   CK(cudaEventRecord(g.ev_k0, st));
   if (kclass == DT_U8) guided_pairs_kernel<DT_U8><<<(unsigned)blocks, GM_WARPS * 32, 0, st>>>(d_pairs, np, distRatio, d_bestj, d_keep);
   else if (kclass == DT_BIN) guided_pairs_kernel<DT_BIN><<<(unsigned)blocks, GM_WARPS * 32, 0, st>>>(d_pairs, np, distRatio, d_bestj, d_keep);
   else guided_pairs_kernel<DT_F32><<<(unsigned)blocks, GM_WARPS * 32, 0, st>>>(d_pairs, np, distRatio, d_bestj, d_keep);
   CK(cudaEventRecord(g.ev_k1, st));
-  if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+  if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, t.launches))) return rc;
   const long emit_threads = std::max(sum_l, (long)np + 1);
   guided_pairs_emit_kernel<<<(unsigned)((emit_threads + 255) / 256), 256, 0, st>>>(d_pairs, np, (int)sum_l, d_bestj, d_keep, d_kpos, d_out + hdr,
                                                                                   reinterpret_cast<int*>(d_out));
   CK(cudaGetLastError());
-  launches += 2;
+  t.launches += 2;
   CK(cudaEventRecord(c->ev_end, st));
   // one read-back: the per-pair starts and every slot the matches may occupy
   CK(cudaMemcpyAsync(g.h_out, d_out, sizeof(uint2) * (hdr + sum_l), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  float ms = 0.f, kms = 0.f;
-  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
-  CK(cudaEventElapsedTime(&kms, g.ev_k0, g.ev_k1));
-  gpu_ms += ms; search_ms += kms;
+  if ((rc = add_times(c, g.ev_k0, g.ev_k1, t))) return rc;
   const int* h_pstart = g.h_out.as<int>();
   const uint2* h = g.h_out.as<uint2>() + hdr;
-  for (int k = 0; k < np; ++k) per_pair[batch[k].index].assign(h + h_pstart[k], h + h_pstart[k + 1]);
+  for (int k = 0; k < np; ++k) append_matches(per_pair[batch[k].index], h, h_pstart[k], h_pstart[k + 1]);
   return B200M_OK;
 }
 
-extern "C" {
-
-int b200m_guided_match_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, int model, const double* M, const double* errorTh, double distRatio,
-                             b200m_result** out) {
-  if (!c || !out || n_pairs < 0 || (model != B200M_MODEL_FUNDAMENTAL && model != B200M_MODEL_HOMOGRAPHY) ||
-      (n_pairs > 0 && (!pairs || !M || !errorTh)))
-    return fail(B200M_ERR_ARG, "bad arguments");
-  *out = nullptr;
-  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
-  CK(cudaSetDevice(c->device));
-  // checks first: nothing runs for a list with a bad entry
-  std::vector<GfPairHost> work;
-  for (int k = 0; k < n_pairs; ++k) {
-    auto sl = c->slot_of.find(pairs[2 * k]), sr = c->slot_of.find(pairs[2 * k + 1]);
-    if (sl == c->slot_of.end() || sr == c->slot_of.end()) return fail(B200M_ERR_ARG, "guided matching references a view that was never uploaded");
-    const ViewHost& vl = c->views[sl->second]; const ViewHost& vr = c->views[sr->second];
-    if (!(vl.m > 0 && vr.m > 0 && vl.dtype == vr.dtype && vl.dim == vr.dim)) continue;     // common descriptor type, :300-306; else empty
-    if (!((vl.dtype == DT_BIN && vl.dim == 64) || (vl.dtype != DT_BIN && vl.dim == 128)))
-      return fail(B200M_ERR_UNSUPPORTED, "guided matching takes 128-component scalar or 64-byte binary descriptors");
-    if ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom))
-      return fail(B200M_ERR_ARG, "guided matching needs feature positions (or geometry positions) for both views");
-    work.push_back({k, sl->second, sr->second, 0});
-  }
-  std::vector<std::vector<uint2>> per_pair((size_t)n_pairs);
-  double gpu_ms = 0, search_ms = 0; int launches = 0;
-  // Batches as in b200m_guided_match_fast_pairs: the list is walked once in input order and every pair joins the open batch of its
-  // kernel class (uchar, fp32, mixed, binary); a batch runs when its pairs (the pinned and device pair tables), left features (a pair
-  // larger than the bound runs alone) or fp32 expansions would pass their bound, and the rest at the end.  Each view is waited for when
-  // its first pair is reached.
-  const long pair_cap = 8192, exp_cap = 64l << 20;
-  struct Open { std::vector<GfPairHost> pairs; long l = 0, e = 0; std::set<int> exp_views; };
-  Open open[4];
-  auto flush = [&](Open& o) -> int {
-    if (o.pairs.empty()) return B200M_OK;
-    const int rc = gm_run_batch(c, o.pairs, model, M, errorTh, distRatio, per_pair, gpu_ms, search_ms, launches);
-    o = Open();
-    return rc;
-  };
-  for (GfPairHost p : work) {
-    int rc;
-    if ((rc = ensure_view_ready(c, p.slot_l)) || (rc = ensure_view_ready(c, p.slot_r))) return rc;
-    // the stored type is final once the view is ready (a uchar-staged view that met a non-integer value was re-uploaded as fp32)
-    const ViewHost& vl = c->views[p.slot_l]; const ViewHost& vr = c->views[p.slot_r];
-    p.kclass = vl.store_dtype() == vr.store_dtype() ? vl.store_dtype() : 3;
-    Open& o = open[p.kclass];
-    const int su = p.kclass == 3 ? (vl.stored_u8 ? p.slot_l : p.slot_r) : -1;
-    long ne = su >= 0 && !o.exp_views.count(su) ? (long)c->views[su].m * 128 : 0;
-    if (!o.pairs.empty() && ((long)o.pairs.size() + 1 > pair_cap || o.l + vl.m > c->gm_left_cap || o.e + ne > exp_cap)) {
-      if ((rc = flush(o))) return rc;
-      ne = su >= 0 ? (long)c->views[su].m * 128 : 0;
-    }
-    o.pairs.push_back(p);
-    o.l += vl.m; o.e += ne;
-    if (su >= 0) o.exp_views.insert(su);
-  }
-  for (Open& o : open)
-    if (int rc = flush(o)) return rc;
-  if (int rc = wait_uploads(c)) return rc;
-  // one result pair per input pair, in input order (empty lists included)
-  std::unique_ptr<b200m_result> res(new b200m_result());
-  res->recycler = c->recycler;
-  res->pair_ids.assign(pairs, pairs + 2 * (size_t)n_pairs);
-  res->offsets.assign((size_t)n_pairs + 1, 0);
-  for (int k = 0; k < n_pairs; ++k) res->offsets[k + 1] = res->offsets[k] + (int64_t)per_pair[k].size();
-  c->last = LastCall{gpu_ms, search_ms, launches, 0, 0, 0, res->offsets[n_pairs], 0};
-  res->matches = c->recycler->take((size_t)std::max<int64_t>(res->offsets[n_pairs], 1));
-  for (int k = 0; k < n_pairs; ++k) {
-    b200m_match* m = res->matches.p + res->offsets[k];
-    for (const uint2& x : per_pair[k]) *m++ = b200m_match{x.x, x.y, 0.f, 0.f};     // IndMatch(i, j): ratio and distance 0
-  }
-  *out = res.release();
-  return B200M_OK;
-}
-
-}  // extern "C"
-
-// ---- position-only guided matching for a list of pairs (guided.cuh, guided_positions_pairs_kernel) ---------------------------------
-// One batch.  per_pair[index] receives the pair's guidedMatching list (the phantom (0, 0) included), decorated when `decorate`.
-static int gp_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int model, const double* M, const double* errorTh, bool decorate,
-                        std::vector<std::vector<b200m_match>>& per_pair, double& gpu_ms, double& search_ms, int& launches) {
+// One position-only batch: each pair's guidedMatching list (the phantom (0, 0) included), decorated when `decorate`
+static int gp_run_batch(b200m_ctx* c, const GuidedBatch& b, int model, const double* M, const double* errorTh, bool decorate,
+                        PairLists& per_pair, GuidedTotals& t) {
   GuidedScratch& g = c->gm;
   using G = GuidedScratch;
   cudaStream_t st = c->stream;
+  const std::vector<GfPairHost>& batch = b.pairs;
   const int np = (int)batch.size();
   int rc;
   if ((rc = g.h_pairs.reserve(sizeof(GuidedPair) * (size_t)np)) || (rc = g.h_yrank.reserve(sizeof(uint32_t*) * (size_t)np))) return rc;
@@ -1868,7 +1794,7 @@ static int gp_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int 
     GuidedPair& P = hp[k];
     std::memset(&P, 0, sizeof(P));
     P.gl = vl.d_geom; P.gr = vr.d_geom; P.fl = (const float2*)vl.d_xy; P.fr = (const float2*)vr.d_xy;
-    for (int t = 0; t < 9; ++t) P.M[t] = M[9 * (size_t)q.index + t];
+    for (int u = 0; u < 9; ++u) P.M[u] = M[9 * (size_t)q.index + u];
     P.errorTh = errorTh[q.index];
     P.model = model == B200M_MODEL_HOMOGRAPHY ? GM_HOMOGRAPHY : GM_FUNDAMENTAL;
     P.ml = vl.m; P.mr = vr.m;
@@ -1904,37 +1830,33 @@ static int gp_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int 
   CK(cudaEventRecord(g.ev_k0, st));
   guided_positions_pairs_kernel<<<(unsigned)blocks, GP_THREADS, 0, st>>>(d_pairs, np, d_bestj, d_keep, d_phantom);
   CK(cudaEventRecord(g.ev_k1, st));
-  ++launches;
+  ++t.launches;
   const long emit_threads = std::max(sum_l, (long)np + 1);
   const unsigned emit_blocks = (unsigned)((emit_threads + 255) / 256);
   if (dev_deco) {
     uint2* d_rec = g.d[G::REC].as<uint2>();
     guided_positions_deco_kernel<<<(unsigned)((sum_l + 255) / 256), 256, 0, st>>>(d_pairs, g.d[G::YRANK].as<const uint32_t*>(), np, (int)sum_l, d_bestj,
                                                                                  d_phantom, d_rec, d_scan_in);
-    if ((rc = exclusive_scan(g.d[G::TEMP], d_scan_in, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+    if ((rc = exclusive_scan(g.d[G::TEMP], d_scan_in, d_kpos, (size_t)sum_l + 1, st, t.launches))) return rc;
     guided_positions_emit_kernel<<<emit_blocks, 256, 0, st>>>(d_pairs, np, (int)sum_l, d_rec, d_scan_in, d_kpos, d_out + hdr, d_pstart);
   } else {
-    if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, launches))) return rc;
+    if ((rc = exclusive_scan(g.d[G::TEMP], d_keep, d_kpos, (size_t)sum_l + 1, st, t.launches))) return rc;
     guided_pairs_emit_kernel<<<emit_blocks, 256, 0, st>>>(d_pairs, np, (int)sum_l, d_bestj, d_keep, d_kpos, d_out + hdr, d_pstart);
   }
   CK(cudaGetLastError());
-  launches += dev_deco ? 2 : 1;
+  t.launches += dev_deco ? 2 : 1;
   CK(cudaEventRecord(c->ev_end, st));
   CK(cudaMemcpyAsync(g.h_out, d_out, sizeof(uint2) * (hdr + sum_l), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  float ms = 0.f, kms = 0.f;
-  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
-  CK(cudaEventElapsedTime(&kms, g.ev_k0, g.ev_k1));
-  gpu_ms += ms; search_ms += kms;
+  if ((rc = add_times(c, g.ev_k0, g.ev_k1, t))) return rc;
   const int* h_pstart = g.h_out.as<int>();
   const int* h_phantom = h_pstart + np + 1;
   const uint2* h = g.h_out.as<uint2>() + hdr;
   for (int k = 0; k < np; ++k) {
     std::vector<b200m_match>& L = per_pair[batch[k].index];
-    L.clear();
     if (h_phantom[k] && !hy[k] && !(h_pstart[k + 1] > h_pstart[k] && h[h_pstart[k]].x == 0 && h[h_pstart[k]].y == 0))
       L.push_back(b200m_match{0, 0, 0.f, 0.f});                       // IndMatch() sorts first; a real (0, 0) is the same match
-    for (int e = h_pstart[k]; e < h_pstart[k + 1]; ++e) L.push_back(b200m_match{h[e].x, h[e].y, 0.f, 0.f});
+    append_matches(L, h, h_pstart[k], h_pstart[k + 1]);
     if (decorate && !hy[k] && !L.empty()) {
       const ViewHost& vl = c->views[batch[k].slot_l]; const ViewHost& vr = c->views[batch[k].slot_r];
       L.resize((size_t)decorator_dedup(L.data(), (int)L.size(), vl.xy.data(), vr.xy.data()));
@@ -1945,6 +1867,51 @@ static int gp_run_batch(b200m_ctx* c, const std::vector<GfPairHost>& batch, int 
 
 extern "C" {
 
+int b200m_guided_match_fast_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, const double* F, const double* epipole2, const int32_t* wh,
+                                  double errorTh, double distRatio, b200m_result** out) {
+  if (!c || !out || n_pairs < 0 || (n_pairs > 0 && (!pairs || !F || !epipole2 || !wh))) return fail(B200M_ERR_ARG, "bad arguments");
+  *out = nullptr;
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  CK(cudaSetDevice(c->device));
+  auto check_wh = [wh](int k) {
+    const int W = wh[2 * k], H = wh[2 * k + 1];
+    if (W < 2 || H < 2 || W > (1 << 24) || H > (1 << 24))
+      return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": the right image must be at least 2 x 2 pixels (and at most 2^24 on a side)");
+    return (int)B200M_OK;
+  };
+  std::vector<GfPairHost> work;
+  if (int rc = guided_work(c, pairs, n_pairs, true, false, check_wh, work)) return rc;
+  PairLists per_pair((size_t)n_pairs);
+  GuidedTotals t;
+  auto buckets = [wh](int k) { return 2l * (wh[2 * k] + wh[2 * k + 1] - 2) + 1; };
+  auto run = [&](const GuidedBatch& b) { return gf_run_batch(c, b, F, epipole2, wh, errorTh, distRatio, per_pair, t); };
+  if (int rc = run_batches(c, work, true, c->gf_left_cap, std::max(c->gf_left_cap, 1l << 20), 16l << 20, buckets, run)) return rc;
+  if (int rc = wait_uploads(c)) return rc;
+  c->last = LastCall{t.gpu_ms, t.search_ms, t.launches, 0, 0, 0, t.cands, 0};
+  *out = guided_result(c, pairs, n_pairs, per_pair);
+  return B200M_OK;
+}
+
+int b200m_guided_match_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, int model, const double* M, const double* errorTh, double distRatio,
+                             b200m_result** out) {
+  if (!c || !out || n_pairs < 0 || (model != B200M_MODEL_FUNDAMENTAL && model != B200M_MODEL_HOMOGRAPHY) ||
+      (n_pairs > 0 && (!pairs || !M || !errorTh)))
+    return fail(B200M_ERR_ARG, "bad arguments");
+  *out = nullptr;
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  CK(cudaSetDevice(c->device));
+  std::vector<GfPairHost> work;
+  if (int rc = guided_work(c, pairs, n_pairs, true, false, [](int) { return 0; }, work)) return rc;
+  PairLists per_pair((size_t)n_pairs);
+  GuidedTotals t;
+  auto run = [&](const GuidedBatch& b) { return gm_run_batch(c, b, model, M, errorTh, distRatio, per_pair, t); };
+  if (int rc = run_batches(c, work, true, c->gm_left_cap, LONG_MAX, LONG_MAX, [](int) { return 0l; }, run)) return rc;
+  if (int rc = wait_uploads(c)) return rc;
+  *out = guided_result(c, pairs, n_pairs, per_pair);
+  c->last = LastCall{t.gpu_ms, t.search_ms, t.launches, 0, 0, 0, (*out)->offsets[n_pairs], 0};
+  return B200M_OK;
+}
+
 int b200m_guided_match_positions_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, int model, const double* M, const double* errorTh,
                                        int decorate, b200m_result** out) {
   if (!c || !out || n_pairs < 0 || (model != B200M_MODEL_FUNDAMENTAL && model != B200M_MODEL_HOMOGRAPHY) || (decorate != 0 && decorate != 1) ||
@@ -1953,47 +1920,15 @@ int b200m_guided_match_positions_pairs(b200m_ctx* c, const uint32_t* pairs, int 
   *out = nullptr;
   std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
   CK(cudaSetDevice(c->device));
-  // checks first: nothing runs for a list with a bad entry
   std::vector<GfPairHost> work;
-  for (int k = 0; k < n_pairs; ++k) {
-    auto sl = c->slot_of.find(pairs[2 * k]), sr = c->slot_of.find(pairs[2 * k + 1]);
-    if (sl == c->slot_of.end() || sr == c->slot_of.end()) return fail(B200M_ERR_ARG, "guided matching references a view that was never uploaded");
-    const ViewHost& vl = c->views[sl->second]; const ViewHost& vr = c->views[sr->second];
-    if (!(vl.m > 0 && vr.m > 0 && vl.dtype == vr.dtype && vl.dim == vr.dim)) continue;     // common describer type; else empty
-    if (decorate ? (vl.xy.empty() || vr.xy.empty()) : ((vl.xy.empty() && !vl.d_geom) || (vr.xy.empty() && !vr.d_geom)))
-      return fail(B200M_ERR_ARG, decorate ? "the decorator needs the upload positions of both views"
-                                          : "guided matching needs feature positions (or geometry positions) for both views");
-    work.push_back({k, sl->second, sr->second, 0});
-  }
-  std::vector<std::vector<b200m_match>> per_pair((size_t)n_pairs);
-  double gpu_ms = 0, search_ms = 0; int launches = 0;
-  // Batches as in b200m_guided_match_pairs, one kernel class (no descriptors are read): a batch runs when its pairs or left features
-  // would pass their bound (a pair larger than the bound runs alone).  Each view is waited for when its first pair is reached.
-  const long pair_cap = 8192;
-  std::vector<GfPairHost> open; long open_l = 0;
-  for (const GfPairHost& p : work) {
-    int rc;
-    if ((rc = ensure_view_ready(c, p.slot_l)) || (rc = ensure_view_ready(c, p.slot_r))) return rc;
-    const long ml = c->views[p.slot_l].m;
-    if (!open.empty() && ((long)open.size() + 1 > pair_cap || open_l + ml > c->gm_left_cap)) {
-      if ((rc = gp_run_batch(c, open, model, M, errorTh, decorate != 0, per_pair, gpu_ms, search_ms, launches))) return rc;
-      open.clear(); open_l = 0;
-    }
-    open.push_back(p); open_l += ml;
-  }
-  if (!open.empty())
-    if (int rc = gp_run_batch(c, open, model, M, errorTh, decorate != 0, per_pair, gpu_ms, search_ms, launches)) return rc;
+  if (int rc = guided_work(c, pairs, n_pairs, false, decorate != 0, [](int) { return 0; }, work)) return rc;
+  PairLists per_pair((size_t)n_pairs);
+  GuidedTotals t;
+  auto run = [&](const GuidedBatch& b) { return gp_run_batch(c, b, model, M, errorTh, decorate != 0, per_pair, t); };
+  if (int rc = run_batches(c, work, false, c->gm_left_cap, LONG_MAX, LONG_MAX, [](int) { return 0l; }, run)) return rc;
   if (int rc = wait_uploads(c)) return rc;
-  // one result pair per input pair, in input order (empty lists included)
-  std::unique_ptr<b200m_result> res(new b200m_result());
-  res->recycler = c->recycler;
-  res->pair_ids.assign(pairs, pairs + 2 * (size_t)n_pairs);
-  res->offsets.assign((size_t)n_pairs + 1, 0);
-  for (int k = 0; k < n_pairs; ++k) res->offsets[k + 1] = res->offsets[k] + (int64_t)per_pair[k].size();
-  c->last = LastCall{gpu_ms, search_ms, launches, 0, 0, 0, res->offsets[n_pairs], 0};
-  res->matches = c->recycler->take((size_t)std::max<int64_t>(res->offsets[n_pairs], 1));
-  for (int k = 0; k < n_pairs; ++k) std::copy(per_pair[k].begin(), per_pair[k].end(), res->matches.p + res->offsets[k]);
-  *out = res.release();
+  *out = guided_result(c, pairs, n_pairs, per_pair);
+  c->last = LastCall{t.gpu_ms, t.search_ms, t.launches, 0, 0, 0, (*out)->offsets[n_pairs], 0};
   return B200M_OK;
 }
 

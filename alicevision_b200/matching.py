@@ -182,12 +182,7 @@ class Context:
         _check(self.lib.b200m_guided_match_fast_pairs(self._h, p.ctypes.data_as(C.c_void_p), C.c_int(n), Fm.ctypes.data_as(C.c_void_p),
                                                       ep.ctypes.data_as(C.c_void_p), whm.ctypes.data_as(C.c_void_p), C.c_double(errorTh),
                                                       C.c_double(distRatio), C.byref(res)), "b200m_guided_match_fast_pairs")
-        owner = _ResultOwner(self.lib, res)
-        off, mat = C.c_void_p(), C.c_void_p()
-        _check(self.lib.b200m_result_get(res, None, C.byref(off), C.byref(mat)), "b200m_result_get")
-        offsets = _alias(off.value, (n + 1) * 8, np.int64, owner) if n else np.zeros(1, np.int64)
-        matches = _alias(mat.value, int(offsets[-1]) * MATCH_DTYPE.itemsize, MATCH_DTYPE, owner)
-        return {(int(a), int(b)): matches[offsets[k]:offsets[k + 1]].copy() for k, (a, b) in enumerate(p.tolist())}
+        return {(int(a), int(b)): m for (a, b), m in zip(p.tolist(), self._pair_lists(res, n))}
 
     def guided_match_pairs(self, pairs, M, errorTh, distRatio: float, model: int = MODEL_FUNDAMENTAL) -> list:
         """b200m_guided_match_pairs on resident views: guidedMatching (matching/guidedMatching.hpp:206-268) for every (L, R) of `pairs`
