@@ -2,7 +2,9 @@
 // robustModelEstimation with GeometricFilterMatrix_F_AC (ACRANSAC, Fundamental7PSolver; GeometricFilter.hpp:40-88,
 // GeometricFilterMatrix_F_AC.hpp:90-174, :266-299, :357-392) or GeometricFilterMatrix_H_AC (Homography4PSolver;
 // GeometricFilterMatrix_H_AC.hpp:43-103, :160-212) for a whole putative list on the b200match engine (H100): one a-contrario RANSAC
-// call (b200m_acransac_fundamental_pairs / b200m_acransac_homography_pairs), the reference's inlier copy and support rules, then one
+// call (b200m_acransac_fundamental_pairs / b200m_acransac_homography_pairs; for F a second one, b200m_acransac_fundamental_spherical_pairs,
+// over the pairs whose two cameras are camera::Equidistant, GeometricFilterMatrix_F_AC.hpp:186-253), the reference's inlier copy and
+// support rules, then one
 // guided-matching call for every kept pair and common descriptor type (b200m_guided_match_pairs, or for H with distanceRatio < 0
 // b200m_guided_match_positions_pairs).
 // Header-only; compiled inside an AliceVision build and linked against libb200match.so.  The caller gathers xI / xJ with the
@@ -173,11 +175,14 @@ protected:
         std::vector<uint32_t> inl;
         std::vector<double> M, errMax, nfa;
         explicit K10Out(const std::vector<PairIn>& pairs, std::size_t nCorr)
-          : offsets(pairs.size() + 1, 0)
+          : K10Out(offsetsOf(pairs, nCorr))
+        {}
+        /// offs: the n + 1 correspondence offsets of the call's pairs
+        explicit K10Out(std::vector<int64_t> offs)
+          : offsets(std::move(offs))
         {
-            const int n = (int)pairs.size();
-            for (int k = 0; k < n; ++k)
-                offsets[k + 1] = (k + 1 < n ? (int64_t)pairs[k + 1].offset : (int64_t)nCorr);
+            const int n = (int)offsets.size() - 1;
+            const std::size_t nCorr = (std::size_t)offsets.back();
             valid.resize(std::max(n, 1));
             nInl.resize(std::max(n, 1));
             iters.resize(std::max(n, 1));
@@ -185,6 +190,13 @@ protected:
             M.resize(9 * std::max(n, 1));
             errMax.resize(std::max(n, 1));
             nfa.resize(std::max(n, 1));
+        }
+        static std::vector<int64_t> offsetsOf(const std::vector<PairIn>& pairs, std::size_t nCorr)
+        {
+            std::vector<int64_t> o(pairs.size() + 1, 0);
+            for (std::size_t k = 0; k < pairs.size(); ++k)
+                o[k + 1] = (k + 1 < pairs.size() ? (int64_t)pairs[k + 1].offset : (int64_t)nCorr);
+            return o;
         }
     };
 
@@ -194,11 +206,11 @@ protected:
         return _corr.empty() ? dummy : _corr.data();
     }
 
-    /// copyInlierMatches and hasStrongSupport(minimumSamples) of pair k; returns whether it has strong support (then result[pair]
-    /// holds its inliers).
-    bool keepInliers(int k, const K10Out& r, std::size_t minimumSamples, std::map<Pair, matching::MatchesPerDescType>& result) const
+    /// copyInlierMatches and hasStrongSupport(minimumSamples) of pair k, entry q of the call r that estimated it; returns whether it
+    /// has strong support (then result[pair] holds its inliers).
+    bool keepInliers(int k, const K10Out& r, int q, std::size_t minimumSamples, std::map<Pair, matching::MatchesPerDescType>& result) const
     {
-        const std::vector<std::size_t> inliers(r.inl.begin() + r.offsets[k], r.inl.begin() + r.offsets[k] + r.nInl[k]);
+        const std::vector<std::size_t> inliers(r.inl.begin() + r.offsets[q], r.inl.begin() + r.offsets[q] + r.nInl[q]);
         matching::MatchesPerDescType perType;
         b200detail::copyInlierMatches(inliers, _pairs[k].putatives, _pairs[k].descTypes, perType);
         if (!b200detail::hasStrongSupport(perType, minimumSamples))
@@ -263,7 +275,8 @@ protected:
     std::vector<int32_t> _wh;
 };
 
-/// robustModelEstimation with GeometricFilterMatrix_F_AC for the pairs added (addView / addPair of the base), then run().
+/// robustModelEstimation with GeometricFilterMatrix_F_AC for the pairs added (addView / addPair of the base, addPairSpherical for
+/// pairs of two equidistant cameras), then run().
 class GeometricFilterMatrix_F_AC_Batch_b200 : public GeometricFilterBatchBase_b200
 {
 public:
@@ -280,39 +293,88 @@ public:
       : GeometricFilterBatchBase_b200(ctx)
     {}
 
-    /// robustModelEstimation over every pair added so far: each pair starts from `rng` (geometricEstimation_Mat_ACRANSAC takes it
-    /// by value).  Pairs with strong support enter out; with guidedMatching their lists are the guided ones (errorTh = errorMax^2,
-    /// distRatio = distanceRatio^2, every common type, empty lists included; nothing when errorMax is infinite).  Returns false
-    /// (out untouched) when the engine is unavailable or fails.
+    /// addPair for a pair whose two cameras are camera::Equidistant (geometricEstimation_Spherical_Mat): bI / bJ are 3 x n, column c
+    /// the unit vector toUnitSphere(removeDistortion(ima2cam(x))) of column c of the xI / xJ addPair would take.  No image size.
+    template<class MatT>
+    void addPairSpherical(const Pair& pair,
+                          const matching::MatchesPerDescType& putatives,
+                          const std::vector<feature::EImageDescriberType>& descTypes,
+                          const MatT& bI,
+                          const MatT& bJ)
+    {
+        _spherical.resize(_pairs.size() + 1, 0);
+        _spherical.back() = 1;
+        PairIn p{pair, putatives, descTypes, _bear.size() / 6};
+        if (!descTypes.empty())
+            for (int c = 0; c < (int)bI.cols(); ++c)
+            {
+                for (int a = 0; a < 3; ++a)
+                    _bear.push_back(bI(a, c));
+                for (int a = 0; a < 3; ++a)
+                    _bear.push_back(bJ(a, c));
+            }
+        _wh.insert(_wh.end(), {0, 0, 0, 0});
+        _pairs.push_back(std::move(p));
+    }
+
+    /// robustModelEstimation over every pair added so far: each pair starts from `rng`.  geometricEstimation_Mat_ACRANSAC takes the
+    /// generator by value; geometricEstimation_Spherical_Mat takes it by reference, so a single-threaded reference run hands it on
+    /// from a spherical pair to the next pair, which no batch reproduces.  The planar pairs go through one K10 call, the spherical
+    /// ones through another.  Pairs with strong support enter out; with guidedMatching their lists are the guided ones (errorTh =
+    /// errorMax^2, distRatio = distanceRatio^2, every common type, empty lists included; nothing when errorMax is infinite; a
+    /// spherical F is applied to the guided positions, as the reference does).  Returns false (out untouched) when the engine is
+    /// unavailable or fails.
     bool run(const std::mt19937& rng, std::size_t maxIteration, double precision, bool guidedMatching, double distanceRatio,
              matching::PairwiseMatches& out)
     {
         if (!available())
             return false;
         const int n = (int)_pairs.size();
+        _spherical.resize(n, 0);
         uint32_t state[625];
         b200detail::mtState(rng, state);
-        K10Out r(_pairs, _corr.size() / 4);
-        if (n > 0 && b200m_acransac_fundamental_pairs(_ctx, n, r.offsets.data(), corrData(), _wh.data(), state, (int64_t)maxIteration, precision,
-                                                      r.valid.data(), r.nInl.data(), r.inl.data(), r.M.data(), r.errMax.data(), r.nfa.data(),
-                                                      r.iters.data()) != B200M_OK)
+        std::vector<int> sub[2];                                        // in addPair order: the planar pairs, the spherical pairs
+        for (int k = 0; k < n; ++k)
+            sub[(int)_spherical[k]].push_back(k);
+        std::vector<int64_t> offs[2];
+        for (int s = 0; s < 2; ++s)
+        {
+            for (const int k : sub[s])
+                offs[s].push_back((int64_t)_pairs[k].offset);
+            offs[s].push_back(s == 0 ? (int64_t)(_corr.size() / 4) : (int64_t)(_bear.size() / 6));
+        }
+        std::vector<int32_t> wh;
+        for (const int k : sub[0])
+            wh.insert(wh.end(), _wh.begin() + 4 * k, _wh.begin() + 4 * k + 4);
+        K10Out r[2] = {K10Out(offs[0]), K10Out(offs[1])};
+        const int n0 = (int)sub[0].size(), n1 = (int)sub[1].size();
+        if (n0 > 0 && b200m_acransac_fundamental_pairs(_ctx, n0, r[0].offsets.data(), corrData(), wh.data(), state, (int64_t)maxIteration,
+                                                       precision, r[0].valid.data(), r[0].nInl.data(), r[0].inl.data(), r[0].M.data(),
+                                                       r[0].errMax.data(), r[0].nfa.data(), r[0].iters.data()) != B200M_OK)
+            return false;
+        if (n1 > 0 && b200m_acransac_fundamental_spherical_pairs(_ctx, n1, r[1].offsets.data(), _bear.data(), state, 0, (int64_t)maxIteration,
+                                                                 precision, r[1].valid.data(), r[1].nInl.data(), r[1].inl.data(), r[1].M.data(),
+                                                                 r[1].errMax.data(), r[1].nfa.data(), r[1].iters.data(), nullptr) != B200M_OK)
             return false;
         _estimates.assign(n, Estimate());
         std::map<Pair, matching::MatchesPerDescType> result;
         std::vector<int> kept;
         std::vector<double> errorMax(n, std::numeric_limits<double>::infinity());
-        for (int k = 0; k < n; ++k)
-        {
-            Estimate& e = _estimates[k];
-            e.valid = r.valid[k] != 0;
-            std::copy(r.M.begin() + 9 * k, r.M.begin() + 9 * k + 9, e.F);
-            if (!e.valid)
-                continue;
-            e.errorMax = errorMax[k] = r.errMax[k];
-            e.strongSupport = keepInliers(k, r, 7, result);             // Fundamental7PSolver::getMinimumNbRequiredSamples
-            if (e.strongSupport)
-                kept.push_back(k);
-        }
+        for (int s = 0; s < 2; ++s)
+            for (int q = 0; q < (int)sub[s].size(); ++q)
+            {
+                const int k = sub[s][q];
+                Estimate& e = _estimates[k];
+                e.valid = r[s].valid[q] != 0;
+                std::copy(r[s].M.begin() + 9 * q, r[s].M.begin() + 9 * q + 9, e.F);
+                if (!e.valid)
+                    continue;
+                e.errorMax = errorMax[k] = r[s].errMax[q];
+                e.strongSupport = keepInliers(k, r[s], q, 7, result);   // getMinimumNbRequiredSamples of both 7-point solvers
+                if (e.strongSupport)
+                    kept.push_back(k);
+            }
+        std::sort(kept.begin(), kept.end());
         if (guidedMatching &&
             !guided(kept, errorMax, [&](int k) { return _estimates[k].F; },
                     [&](const uint32_t* ids, int np, const double* M, const double* th, b200m_result** res) {
@@ -330,6 +392,8 @@ public:
 
 private:
     std::vector<Estimate> _estimates;
+    std::vector<char> _spherical;   // per pair added: 1 = addPairSpherical (its offset indexes _bear)
+    std::vector<double> _bear;      // 6 doubles per correspondence (xI, yI, zI, xJ, yJ, zJ)
 };
 
 /// robustModelEstimation with GeometricFilterMatrix_H_AC (ACRANSAC, Homography4PSolver, point-to-point error;
@@ -383,7 +447,7 @@ public:
             if (!e.valid)
                 continue;
             e.errorMax = errorMax[k] = r.errMax[k];
-            e.strongSupport = keepInliers(k, r, 4, result);             // Homography4PSolver::getMinimumNbRequiredSamples
+            e.strongSupport = keepInliers(k, r, k, 4, result);             // Homography4PSolver::getMinimumNbRequiredSamples
             if (e.strongSupport)
                 kept.push_back(k);
         }

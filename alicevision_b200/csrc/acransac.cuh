@@ -1,12 +1,13 @@
 // K10: a-contrario RANSAC estimation for a list of pairs, sm_90a: the fundamental matrix (b200m_acransac_fundamental_pairs,
-// FPolicy) and the homography (b200m_acransac_homography_pairs, HPolicy).  The kernel is one template over the model policy.
+// FPolicy), the homography (b200m_acransac_homography_pairs, HPolicy) and the fundamental matrix of two equidistant cameras on
+// lifted unit vectors (b200m_acransac_fundamental_spherical_pairs, SPolicy).  The kernel is one template over the model policy.
 //
 // One CTA runs one pair's robustEstimation::ACRANSAC loop (robustEstimation/ACRansac.hpp:186-272) iteration by iteration, with the
 // reference's control flow (10 % reserve, strict `<` on minNFA, the switch to sampling among the inliers, the "no model at all"
 // extension, the precision mode and its early exit).  Per iteration thread 0 draws the sample from the pair's own copy of the
 // caller's std::mt19937 (shared memory) and fits the models (7-point F or 4-point H, acransac_math.h); then the whole CTA scores
 // each model:
-//   * n residuals (F: point-to-line error, H: point-to-point transfer error, on normalised points);
+//   * n residuals (F: point-to-line error, H: point-to-point transfer error, on normalised points; S: (F x_I . x_J)^2 on bearings);
 //   * certified skip: a shared-memory histogram of the residuals over quarter-binade bins gives, for every k, a lower bound of the
 //     k-th smallest residual (the low edge of its bin), hence of NFA(k), which increases with that residual.  When the least bound
 //     over k is not below the current minNFA (less a 1e-9 relative margin that covers the device log10), the model cannot be
@@ -15,7 +16,7 @@
 //     per-pair global scratch beyond; every k's NFA; the (NFA, k)-lexicographic argmin (bestNFA keeps the first k reaching the
 //     minimum).  NaN residuals sort after +inf, where std::sort is unspecified.
 // The winner's sorted indices are its inlier list in the reference's order.  When asked, the generator's state after the pair's
-// last draw is written back (HPolicy: the reference passes its std::mt19937 by reference from pair to pair).
+// last draw is written back (HPolicy, SPolicy: the reference passes its std::mt19937 by reference from pair to pair).
 #pragma once
 #include "acransac_math.h"
 
@@ -50,10 +51,15 @@ __device__ __forceinline__ double bin_low(int b) {
   return __longlong_as_double((long long)(((unsigned long long)(kBinLo + q / 4) << 52) | ((unsigned long long)(q & 3) << 50)));
 }
 
-// Model policies: sample size, maximum number of models, fit, residual, logalpha0, errorVectorDimension, unnormaliser
+// Model policies: sample size, maximum number of models, fit, residual, logalpha0, errorVectorDimension, unnormaliser, and the
+// correspondence layout: kPlanar = pixel pairs (xI, yI, xJ, yJ) preconditioned by the image sizes, else lifted unit vectors
+// (xI, yI, zI, xJ, yJ, zJ) used as given; kWidth doubles per correspondence.
 struct FPolicy {   // RelativePoseKernel<Fundamental7PSolver, FundamentalEpipolarDistanceError, UnnormalizerT>
-  static constexpr int kSample = acr::kSample, kMaxModels = acr::kMaxModels, kErrDim = 1;
-  __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) { return acr::fit7(a, b, c, d, m); }
+  static constexpr int kSample = acr::kSample, kMaxModels = acr::kMaxModels, kErrDim = 1, kWidth = 4;
+  static constexpr bool kPlanar = true;
+  __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) {
+    return acr::fit7_solve<false>(a, b, c, d, m);   // = acr::fit7, one inlining level shallower
+  }
   __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::epipolar_error(m, x1, y1, x2, y2); }
   __device__ static double logalpha0(int w2, int h2, const acr::Norm& n2) {
     return log10(2.0 * sqrt(acr::add(acr::mul((double)w2, (double)w2), acr::mul((double)h2, (double)h2))) / acr::mul((double)w2, (double)h2) / n2.s);
@@ -61,15 +67,24 @@ struct FPolicy {   // RelativePoseKernel<Fundamental7PSolver, FundamentalEpipola
   __device__ static void unnormalize(const acr::Norm& n1, const acr::Norm& n2, double* m) { acr::unnormalize(n1, n2, m); }
 };
 struct HPolicy {   // RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError, UnnormalizerI>, point to point
-  static constexpr int kSample = acr::kSampleH, kMaxModels = acr::kMaxModelsH, kErrDim = 2;
+  static constexpr int kSample = acr::kSampleH, kMaxModels = acr::kMaxModelsH, kErrDim = 2, kWidth = 4;
+  static constexpr bool kPlanar = true;
   __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) { return acr::fit4(a, b, c, d, m); }
   __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::homography_error(m, x1, y1, x2, y2); }
   __device__ static double logalpha0(int w2, int h2, const acr::Norm& n2) { return acr::logalpha0_h(w2, h2, n2); }
   __device__ static void unnormalize(const acr::Norm& n1, const acr::Norm& n2, double* m) { acr::unnormalize_h(n1, n2, m); }
 };
+struct SPolicy {   // RelativePoseSphericalKernel<Fundamental7PSphericalSolver, EpipolarSphericalDistanceError>
+  static constexpr int kSample = acr::kSample, kMaxModels = acr::kMaxModels, kErrDim = 2, kWidth = 6;
+  static constexpr bool kPlanar = false;
+  __device__ static int fit(const double* x1, const double* x2, double* m) { return acr::fit7s(x1, x2, m); }
+  __device__ static double error(const double* m, const double* x1, const double* x2) { return acr::spherical_error(m, x1, x2); }
+  __device__ static double logalpha0(int, int, const acr::Norm&) { return M_PI; }   // the value itself, not its log10
+  __device__ static void unnormalize(const acr::Norm&, const acr::Norm&, double*) {}
+};
 
 // NFA(k) of bestNFA for the squared residual e of rank k: loge0 + (la0 + d log10(sqrt(e) + FLT_EPSILON)) (k - kSample) + logc_n[k]
-// + logc_k[k], d = errorVectorDimension (1: F, 2: H; the product by 2 is exact)
+// + logc_k[k], d = errorVectorDimension (1: F, 2: H and S; the product by 2 is exact)
 template <class P>
 __device__ __forceinline__ double nfa_of(double e, int k, double la0, double loge0, const float* lcn, const float* lck) {
   const double l = log10(acr::add(sqrt(e), (double)FLT_EPSILON));
@@ -121,12 +136,20 @@ __device__ void bitonic(unsigned long long* K, uint32_t* V, int N2) {
 
 template <class P>
 __device__ __forceinline__ double residual(const double* M, const double* pts, int i) {
-  const double2 a = reinterpret_cast<const double2*>(pts)[2 * i], b = reinterpret_cast<const double2*>(pts)[2 * i + 1];
-  return P::error(M, a.x, a.y, b.x, b.y);
+  if constexpr (P::kPlanar) {
+    const double2 a = reinterpret_cast<const double2*>(pts)[2 * i], b = reinterpret_cast<const double2*>(pts)[2 * i + 1];
+    return P::error(M, a.x, a.y, b.x, b.y);
+  } else {   // 48 bytes a correspondence: three aligned 16-byte loads
+    const double2* q = reinterpret_cast<const double2*>(pts) + 3 * i;
+    const double2 a = q[0], b = q[1], c = q[2];
+    const double x1[3] = {a.x, a.y, b.x}, x2[3] = {b.y, c.x, c.y};
+    return P::error(M, x1, x2);
+  }
 }
 
-// corr: per correspondence (xI, yI, xJ, yJ) at the pair's offset; l10[k] = (float)log10((double)k) for k <= the largest n.
-// Scratch at the pair's offset: pts (4 doubles), idx (the sampling list), logc (n + 1 floats each of logc_n and logc_k, at
+// corr: per correspondence P::kWidth doubles at the pair's offset, (xI, yI, xJ, yJ) or (xI, yI, zI, xJ, yJ, zJ); l10[k] =
+// (float)log10((double)k) for k <= the largest n.
+// Scratch at the pair's offset: pts (P::kWidth doubles), idx (the sampling list), logc (n + 1 floats each of logc_n and logc_k, at
 // 2 * (off + pair)), gkeys / gvals (pow2(n) at sort_off, pairs above kSmemSort only).  inliers: the result list at the offset.
 // mt_state: 625 words at p * mt_stride (mt_stride 0: one state for every pair); mt_out: NULL, or 625 words per pair receiving the
 // generator state after the pair's last draw.
@@ -164,16 +187,21 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
       for (int i = tid; i <= acr::kMtN; i += kThreads) mt_out[(long long)p * (acr::kMtN + 1) + i] = st_in[i];
     return;
   }
-  const acr::Norm n1 = acr::precondition(Q.w1, Q.h1), n2 = acr::precondition(Q.w2, Q.h2);
-  double* pts = pts_all + 4 * Q.off;
+  acr::Norm n1{1.0, 0.0, 0.0}, n2{1.0, 0.0, 0.0};   // identity for bearings (no image size)
+  if constexpr (P::kPlanar) { n1 = acr::precondition(Q.w1, Q.h1); n2 = acr::precondition(Q.w2, Q.h2); }
+  double* pts = pts_all + P::kWidth * Q.off;
   uint32_t* idx = idx_all + Q.off;
   uint32_t* inl = inliers_all + Q.off;
   float* lcn = logc_all + 2 * (Q.off + p);
   float* lck = lcn + n + 1;
-  const double* c = corr + 4 * Q.off;
+  const double* c = corr + P::kWidth * Q.off;
   for (int i = tid; i < n; i += kThreads) {
-    pts[4 * i] = acr::norm_x(n1, c[4 * i]); pts[4 * i + 1] = acr::norm_y(n1, c[4 * i + 1]);
-    pts[4 * i + 2] = acr::norm_x(n2, c[4 * i + 2]); pts[4 * i + 3] = acr::norm_y(n2, c[4 * i + 3]);
+    if constexpr (P::kPlanar) {
+      pts[4 * i] = acr::norm_x(n1, c[4 * i]); pts[4 * i + 1] = acr::norm_y(n1, c[4 * i + 1]);
+      pts[4 * i + 2] = acr::norm_x(n2, c[4 * i + 2]); pts[4 * i + 3] = acr::norm_y(n2, c[4 * i + 3]);
+    } else {
+      for (int t = 0; t < P::kWidth; ++t) pts[P::kWidth * i + t] = c[P::kWidth * i + t];
+    }
     idx[i] = i;
   }
   // makelogcombi: logcombi(k, n) is the float sum of the first min(k, n - k) terms l10[n - i + 1] - l10[i] in ascending i, so one
@@ -200,7 +228,9 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
   for (int i = tid; i < acr::kMtN; i += kThreads) g.x[i] = st_in[i];
   const double la0 = P::logalpha0(Q.w2, Q.h2, n2);
   const double loge0 = log10(acr::mul((double)P::kMaxModels, (double)(n - P::kSample)));
-  const double maxThr = precision == inf ? inf : acr::mul(acr::mul(acr::mul(precision, precision), n2.s), n2.s);
+  double maxThr;   // precision^2 thresholdNormalizer()^2; thresholdNormalizer() = 1 for bearings
+  if constexpr (P::kPlanar) maxThr = precision == inf ? inf : acr::mul(acr::mul(acr::mul(precision, precision), n2.s), n2.s);
+  else maxThr = precision == inf ? inf : acr::mul(precision, precision);
   if (tid == 0) {
     g.p = (int)st_in[acr::kMtN];
     nReserve = max_iter / 10; nIter = max_iter - nReserve; iter = 0;
@@ -217,12 +247,21 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
       } else {
         uint32_t s[P::kSample];
         acr::rand_sample<P::kSample>(g, (uint32_t)(mode ? n_idx : n), s);
-        double a[P::kSample], b[P::kSample], cc[P::kSample], d[P::kSample];
-        for (int i = 0; i < P::kSample; ++i) {
-          const uint32_t j = mode ? idx[s[i]] : s[i];
-          a[i] = pts[4 * j]; b[i] = pts[4 * j + 1]; cc[i] = pts[4 * j + 2]; d[i] = pts[4 * j + 3];
+        if constexpr (P::kPlanar) {
+          double a[P::kSample], b[P::kSample], cc[P::kSample], d[P::kSample];
+          for (int i = 0; i < P::kSample; ++i) {
+            const uint32_t j = mode ? idx[s[i]] : s[i];
+            a[i] = pts[4 * j]; b[i] = pts[4 * j + 1]; cc[i] = pts[4 * j + 2]; d[i] = pts[4 * j + 3];
+          }
+          nb = P::fit(a, b, cc, d, models);
+        } else {
+          double x1[3 * P::kSample], x2[3 * P::kSample];
+          for (int i = 0; i < P::kSample; ++i) {
+            const uint32_t j = mode ? idx[s[i]] : s[i];
+            for (int t = 0; t < 3; ++t) { x1[3 * i + t] = pts[6 * j + t]; x2[3 * i + t] = pts[6 * j + 3 + t]; }
+          }
+          nb = P::fit(x1, x2, models);
         }
-        nb = P::fit(a, b, cc, d, models);
         better = 0; copy_idx = 0;
       }
     }
@@ -325,7 +364,11 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
     double Fo[9];
     for (int t = 0; t < 9; ++t) Fo[t] = bestF[t];
     double em = errorMax;
-    if (valid) { P::unnormalize(n1, n2, Fo); em = sqrt(em) / n2.s; }
+    if (valid) {   // unormalizeError: sqrt(e) / s2 (planar), sqrt(e) (bearings)
+      P::unnormalize(n1, n2, Fo);
+      if constexpr (P::kPlanar) em = sqrt(em) / n2.s;
+      else em = sqrt(em);
+    }
     for (int t = 0; t < 9; ++t) out->model[t] = Fo[t];
     out->error_max = em; out->min_nfa = minNFA;
     out->evaluated = evaluated; out->skipped = skipped; out->exact = exact;

@@ -1,4 +1,5 @@
-// Host + device building blocks of the a-contrario fundamental-matrix and homography estimations (acransac.cuh):
+// Host + device building blocks of the a-contrario fundamental-matrix (planar and spherical) and homography estimations
+// (acransac.cuh):
 //   * std::mt19937 (libstdc++), std::uniform_int_distribution<int>(0, d) on it (GCC 13: Lemire's nearly-divisionless reduction
 //     of one 32-bit draw), and the sample of robustEstimation::randSample(g, 0, range, K) as ACRANSAC draws it: Floyd's algorithm
 //     with the iteration order of the std::unordered_set<std::size_t> it fills, or std::shuffle with its two-swaps-per-draw path
@@ -6,6 +7,8 @@
 //   * the F kernel of RelativePoseKernel<Fundamental7PSolver, FundamentalEpipolarDistanceError, UnnormalizerT>: image-size
 //     preconditioning, the 7-point solver (the 2-D null space of the epipolar rows, the cubic det(F1 + a F2) = 0 as written,
 //     SolveCubicPolynomial branch for branch), the point-to-line error and the unnormalisation N2^T F N1;
+//   * the spherical F kernel of RelativePoseSphericalKernel<Fundamental7PSphericalSolver, EpipolarSphericalDistanceError> for two
+//     equidistant cameras: the same 7-point null space and cubic on the rows of lifted unit vectors, the error (F x1 . x2)^2;
 //   * the H kernel of RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError, UnnormalizerI> (point-to-point): the same
 //     preconditioning, the 4-point DLT and its 1-D null space, the asymmetric transfer error and the unnormalisation N2^-1 H N1.
 // The same code runs in the engine (device) and in the oracle's restated kernels (host, -ffp-contract=off), so the two differ
@@ -257,14 +260,27 @@ ACR_HD void nullspace(const double A[R][9], double N[9 - R][9]) {
   }
 }
 
-// Fundamental7PSolver::solve on 7 normalised correspondences (x1[i], y1[i]) <-> (x2[i], y2[i]); returns the number of models
-// (0..3) written row-major to F[m * 9].
-ACR_HD int fit7(const double* x1, const double* y1, const double* x2, const double* y2, double* F) {
+// The 7-point solver of Fundamental7PSolver (kSpherical = false) and Fundamental7PSphericalSolver (true); returns the number of
+// models (0..3) written row-major to F[m * 9].  Only the epipolar rows differ:
+//   planar     encodeEpipolarEquation on 7 normalised correspondences (p0[i], p1[i]) <-> (p2[i], p3[i]);
+//   spherical  encodeEpipolarSphericalEquation on 7 bearing pairs x1 = p0[3 i + a] <-> x2 = p2[3 i + a], A(i, 3 a + b) = x2_a x1_b
+//              (p1, p3 unused);
+// then both take the 2-D null space F1, F2 of the rows, the cubic det(F1 + a F2) = 0 and its real roots.  One function rather than
+// a shared tail: the F kernel calls it at the depth fit7 had, which keeps its device code what it was before the spherical solver.
+template <bool kSpherical>
+ACR_HD int fit7_solve(const double* p0, const double* p1, const double* p2, const double* p3, double* F) {
   double A[kSample][9];
-  for (int i = 0; i < kSample; ++i) {   // encodeEpipolarEquation
-    A[i][0] = mul(x2[i], x1[i]); A[i][1] = mul(x2[i], y1[i]); A[i][2] = x2[i];
-    A[i][3] = mul(y2[i], x1[i]); A[i][4] = mul(y2[i], y1[i]); A[i][5] = y2[i];
-    A[i][6] = x1[i]; A[i][7] = y1[i]; A[i][8] = 1.0;
+  if constexpr (!kSpherical) {
+    const double *x1 = p0, *y1 = p1, *x2 = p2, *y2 = p3;
+    for (int i = 0; i < kSample; ++i) {   // encodeEpipolarEquation
+      A[i][0] = mul(x2[i], x1[i]); A[i][1] = mul(x2[i], y1[i]); A[i][2] = x2[i];
+      A[i][3] = mul(y2[i], x1[i]); A[i][4] = mul(y2[i], y1[i]); A[i][5] = y2[i];
+      A[i][6] = x1[i]; A[i][7] = y1[i]; A[i][8] = 1.0;
+    }
+  } else {
+    for (int i = 0; i < kSample; ++i)     // encodeEpipolarSphericalEquation
+      for (int a = 0; a < 3; ++a)
+        for (int b = 0; b < 3; ++b) A[i][3 * a + b] = mul(p2[3 * i + a], p0[3 * i + b]);
   }
   double f12[2][9];
   nullspace<kSample>(A, f12);
@@ -304,6 +320,28 @@ ACR_HD int fit7(const double* x1, const double* y1, const double* x2, const doub
   for (int kk = 0; kk < nb; ++kk)
     for (int t = 0; t < 9; ++t) F[kk * 9 + t] = add(f1[t], mul(roots[kk], f2[t]));
   return nb;
+}
+
+// Fundamental7PSolver::solve on 7 normalised correspondences (x1[i], y1[i]) <-> (x2[i], y2[i])
+ACR_HD int fit7(const double* x1, const double* y1, const double* x2, const double* y2, double* F) {
+  return fit7_solve<false>(x1, y1, x2, y2, F);
+}
+
+// ---------------------------------------------------------------------------------------------------------------- spherical F kernel
+// RelativePoseSphericalKernel<Fundamental7PSphericalSolver, EpipolarSphericalDistanceError>: correspondences are the lifted unit
+// vectors x1, x2 of two equidistant cameras (third component anywhere in [-1, 1]); no normalisation, logalpha0 = pi,
+// errorVectorDimension = 2, thresholdNormalizer = 1, unormalizeError = sqrt.
+
+// Fundamental7PSphericalSolver::solve on 7 bearing pairs x1[3 i + a] <-> x2[3 i + a]; returns the number of models (0..3)
+ACR_HD int fit7s(const double* x1, const double* x2, double* F) { return fit7_solve<true>(x1, nullptr, x2, nullptr, F); }
+
+// EpipolarSphericalDistanceError: (F x1 . x2)^2
+ACR_HD double spherical_error(const double* F, const double* x1, const double* x2) {
+  const double l0 = add(add(mul(F[0], x1[0]), mul(F[1], x1[1])), mul(F[2], x1[2]));
+  const double l1 = add(add(mul(F[3], x1[0]), mul(F[4], x1[1])), mul(F[5], x1[2]));
+  const double l2 = add(add(mul(F[6], x1[0]), mul(F[7], x1[1])), mul(F[8], x1[2]));
+  const double d = add(add(mul(l0, x2[0]), mul(l1, x2[1])), mul(l2, x2[2]));
+  return mul(d, d);
 }
 
 // UnnormalizerT: F <- N2^T F N1

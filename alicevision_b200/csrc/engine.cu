@@ -249,8 +249,8 @@ struct GuidedScratch {
   Event ev_k0, ev_k1;                         // search-kernel timing
 };
 
-// grow-only scratch of b200m_acransac_fundamental_pairs and b200m_acransac_homography_pairs (acransac.cuh); the last call's
-// instrumentation and trace, whichever model it estimated
+// grow-only scratch of b200m_acransac_fundamental_pairs, b200m_acransac_homography_pairs and
+// b200m_acransac_fundamental_spherical_pairs (acransac.cuh); the last call's instrumentation and trace, whichever model it estimated
 struct AcransacScratch {
   DeviceBuffer<char> d;
   bool skip = true;                                   // certified skip (b200m_ctx_set_acransac_skip)
@@ -1934,15 +1934,17 @@ int b200m_guided_match_positions_pairs(b200m_ctx* c, const uint32_t* pairs, int 
 
 }  // extern "C"
 
-// ---- K10: a-contrario RANSAC for a pair list, fundamental matrix or homography (acransac.cuh) ----------------------------
-// One launch of acransac_kernel<Policy> over the list; the two entry points differ in the model and in the generator contract.
+// ---- K10: a-contrario RANSAC for a pair list: fundamental matrix, homography, spherical fundamental matrix (acransac.cuh) ----
+// One launch of acransac_kernel<Policy> over the list; the entry points differ in the model, the correspondence width
+// (Policy::kWidth doubles) and the generator contract.  wh: image sizes of the planar policies (unused, may be NULL, for bearings).
 // mt_per_pair: 0 = mt_state is one 625-word state for every pair, 1 = n_pairs x 625.  mt_out: NULL or n_pairs x 625.
 template <class Policy>
 static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh, const uint32_t* mt_state,
                           int mt_per_pair, int64_t max_iteration, double precision, uint8_t* valid, int32_t* n_inliers, uint32_t* inliers,
                           double* model, double* error_max, double* min_nfa, int32_t* iterations, uint32_t* mt_out) {
   if (!c || n_pairs < 0 || max_iteration < 0 || max_iteration > INT32_MAX || !(precision > 0) || (mt_per_pair != 0 && mt_per_pair != 1) ||
-      (n_pairs > 0 && (!offsets || !wh || !mt_state || !valid || !n_inliers || !model || !error_max || !min_nfa || !iterations)))
+      (n_pairs > 0 && (!offsets || (Policy::kPlanar && !wh) || !mt_state || !valid || !n_inliers || !model || !error_max || !min_nfa ||
+                       !iterations)))
     return fail(B200M_ERR_ARG, "bad arguments");
   if (n_pairs > 0 && offsets[0] != 0) return fail(B200M_ERR_ARG, "offsets[0] must be 0");
   std::vector<acrk::Pair> pairs((size_t)n_pairs);
@@ -1950,13 +1952,16 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
   for (int k = 0; k < n_pairs; ++k) {
     const int64_t n = offsets[k + 1] - offsets[k];
     if (n < 0 || n > (1 << 24)) return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": offsets must ascend, at most 2^24 correspondences a pair");
-    for (int t = 0; t < 4; ++t)
-      if (wh[4 * k + t] < 1) return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": image sizes must be positive");
-    if ((int64_t)wh[4 * k] * wh[4 * k + 1] > INT32_MAX || (int64_t)wh[4 * k + 2] * wh[4 * k + 3] > INT32_MAX)
-      return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": width * height must fit an int, as in the reference");
+    int32_t s[4] = {0, 0, 0, 0};
+    if (Policy::kPlanar) {
+      for (int t = 0; t < 4; ++t)
+        if ((s[t] = wh[4 * k + t]) < 1) return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": image sizes must be positive");
+      if ((int64_t)s[0] * s[1] > INT32_MAX || (int64_t)s[2] * s[3] > INT32_MAX)
+        return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": width * height must fit an int, as in the reference");
+    }
     int64_t n2 = 1;
     while (n2 < n) n2 <<= 1;
-    pairs[k] = acrk::Pair{offsets[k], n2 > acrk::kSmemSort ? sort_total : 0, (int)n, wh[4 * k], wh[4 * k + 1], wh[4 * k + 2], wh[4 * k + 3]};
+    pairs[k] = acrk::Pair{offsets[k], n2 > acrk::kSmemSort ? sort_total : 0, (int)n, s[0], s[1], s[2], s[3]};
     if (n2 > acrk::kSmemSort) sort_total += n2;
     max_n = std::max(max_n, (int)n);
   }
@@ -1973,11 +1978,12 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
   std::vector<float> l10((size_t)max_n + 2);
   for (size_t k = 0; k < l10.size(); ++k) l10[k] = (float)log10((double)k);
   const size_t n_states = mt_per_pair ? (size_t)n_pairs : 1;
-  // one grow-only device buffer, shared by both models
+  // one grow-only device buffer, shared by every model
+  constexpr int W = Policy::kWidth;
   size_t at = 0;
   auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_pairs = take(sizeof(acrk::Pair) * n_pairs), o_corr = take(sizeof(double) * 4 * N), o_l10 = take(sizeof(float) * l10.size()),
-               o_mt = take(sizeof(uint32_t) * 625 * n_states), o_pts = take(sizeof(double) * 4 * N), o_idx = take(sizeof(uint32_t) * N),
+  const size_t o_pairs = take(sizeof(acrk::Pair) * n_pairs), o_corr = take(sizeof(double) * W * N), o_l10 = take(sizeof(float) * l10.size()),
+               o_mt = take(sizeof(uint32_t) * 625 * n_states), o_pts = take(sizeof(double) * W * N), o_idx = take(sizeof(uint32_t) * N),
                o_logc = take(sizeof(float) * 2 * (N + n_pairs)), o_gk = take(sizeof(unsigned long long) * sort_total),
                o_gv = take(sizeof(uint32_t) * sort_total), o_inl = take(sizeof(uint32_t) * N),
                o_tr = take(sizeof(int32_t) * acrk::kTraceCap * n_pairs),
@@ -1988,7 +1994,7 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
   char* d = c->acr.d;
   cudaStream_t st = c->stream;
   CK(cudaMemcpyAsync(d + o_pairs, pairs.data(), sizeof(acrk::Pair) * n_pairs, cudaMemcpyHostToDevice, st));
-  if (N) CK(cudaMemcpyAsync(d + o_corr, corr, sizeof(double) * 4 * N, cudaMemcpyHostToDevice, st));
+  if (N) CK(cudaMemcpyAsync(d + o_corr, corr, sizeof(double) * W * N, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d + o_l10, l10.data(), sizeof(float) * l10.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d + o_mt, mt_state, sizeof(uint32_t) * 625 * n_states, cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(c->acr.ev0, st));
@@ -2037,6 +2043,14 @@ int b200m_acransac_homography_pairs(b200m_ctx* c, int n_pairs, const int64_t* of
                                     uint32_t* mt_state_out) {
   return acransac_pairs<acrk::HPolicy>(c, n_pairs, offsets, corr, wh, mt_state, mt_state_per_pair, max_iteration, precision, valid, n_inliers,
                                        inliers, H, error_max, min_nfa, iterations, mt_state_out);
+}
+
+int b200m_acransac_fundamental_spherical_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* bearings,
+                                               const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision,
+                                               uint8_t* valid, int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max,
+                                               double* min_nfa, int32_t* iterations, uint32_t* mt_state_out) {
+  return acransac_pairs<acrk::SPolicy>(c, n_pairs, offsets, bearings, nullptr, mt_state, mt_state_per_pair, max_iteration, precision, valid,
+                                       n_inliers, inliers, F, error_max, min_nfa, iterations, mt_state_out);
 }
 
 double b200m_acransac_last_stats(const b200m_ctx* c, int64_t stats[4]) {

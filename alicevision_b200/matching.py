@@ -40,7 +40,7 @@ ABI_SYMBOLS = [
     "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model", "b200m_set_view_geometry", "b200m_guided_match_fast_pairs",
     "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
     "b200m_mt19937_seed", "b200m_debug_rand_sample", "b200m_acransac_homography_pairs", "b200m_debug_rand_sample_k", "b200m_guided_match_pairs",
-    "b200m_guided_match_positions_pairs",
+    "b200m_guided_match_positions_pairs", "b200m_acransac_fundamental_spherical_pairs",
 ]
 
 
@@ -232,7 +232,7 @@ class Context:
         mt_state: 625 words (mt19937_state), the same for every pair.  Returns per pair, in input order, {"valid", "inliers" (the
         reference's order), "F" (3 x 3, x_J^T F x_I = 0), "error_max", "min_nfa", "iterations", "trace" / "trace_nfa" (iterations at
         which a better model was found and its minNFA, the first 256), "n_trace"}."""
-        return self._acransac_pairs(False, corr_list, wh, np.ascontiguousarray(mt_state, np.uint32).reshape(625), maxIteration, precision)
+        return self._acransac_pairs("F", corr_list, wh, np.ascontiguousarray(mt_state, np.uint32).reshape(625), maxIteration, precision)
 
     def acransac_homography_pairs(self, corr_list, wh, mt_state_or_states, maxIteration: int = 50000, precision: float = np.inf) -> list[dict]:
         """b200m_acransac_homography_pairs: GeometricFilterMatrix_H_AC::geometricEstimation (ACRANSAC with Homography4PSolver and the
@@ -240,29 +240,39 @@ class Context:
         state for every pair, or an n_pairs x 625 array of per-pair start states.  Returns per pair the fields of
         acransac_fundamental_pairs with "H" (3 x 3, x_J ~ H x_I) in place of "F", and "mt_state_out": the generator state after the
         pair's estimation (the reference passes its generator on from pair to pair)."""
-        st = np.ascontiguousarray(mt_state_or_states, np.uint32)
-        if st.ndim == 1:
-            st = st.reshape(625)
-        elif st.shape != (len(corr_list), 625):
-            raise ValueError(f"mt_state_or_states: 625 words or n_pairs x 625, got {st.shape}")
-        return self._acransac_pairs(True, corr_list, wh, st, maxIteration, precision)
+        return self._acransac_pairs("H", corr_list, wh, _mt_states(mt_state_or_states, len(corr_list)), maxIteration, precision)
 
-    def _acransac_pairs(self, homography: bool, corr_list, wh, st, maxIteration, precision) -> list[dict]:
-        cs = [np.ascontiguousarray(c, np.float64).reshape(-1, 4) for c in corr_list]
+    def acransac_fundamental_spherical_pairs(self, corr_list, mt_state_or_states, maxIteration: int = 50000,
+                                             precision: float = np.inf) -> list[dict]:
+        """b200m_acransac_fundamental_spherical_pairs: GeometricFilterMatrix_F_AC::geometricEstimation_Spherical_Mat (ACRANSAC with
+        Fundamental7PSphericalSolver and EpipolarSphericalDistanceError, the branch for two equidistant cameras) for every pair.
+        corr_list: per pair an n x 6 array (xI, yI, zI, xJ, yJ, zJ) of lifted unit vectors; no image sizes.  mt_state_or_states as in
+        acransac_homography_pairs.  Returns per pair the fields of acransac_fundamental_pairs ("F": x_J^T F x_I = 0 on the bearings)
+        and "mt_state_out": the generator state after the pair's estimation (the reference passes this generator by reference)."""
+        return self._acransac_pairs("S", corr_list, None, _mt_states(mt_state_or_states, len(corr_list)), maxIteration, precision)
+
+    def _acransac_pairs(self, kind: str, corr_list, wh, st, maxIteration, precision) -> list[dict]:
+        width = 6 if kind == "S" else 4
+        cs = [np.ascontiguousarray(c, np.float64).reshape(-1, width) for c in corr_list]
         n = len(cs)
         offsets = np.zeros(n + 1, np.int64)
         offsets[1:] = np.cumsum([c.shape[0] for c in cs]) if n else []
-        corr = np.ascontiguousarray(np.concatenate(cs) if n and offsets[-1] else np.zeros((1, 4)), np.float64)
-        whm = np.ascontiguousarray(wh, np.int32).reshape(n, 4)
+        corr = np.ascontiguousarray(np.concatenate(cs) if n and offsets[-1] else np.zeros((1, width)), np.float64)
+        whm = np.ascontiguousarray(wh, np.int32).reshape(n, 4) if kind != "S" else None
         valid = np.zeros(max(n, 1), np.uint8); ninl = np.zeros(max(n, 1), np.int32); it = np.zeros(max(n, 1), np.int32)
         inl = np.zeros(max(int(offsets[-1]), 1), np.uint32); M = np.zeros((max(n, 1), 9)); em = np.zeros(max(n, 1)); nfa = np.zeros(max(n, 1))
         ptr = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-        if homography:
-            sto = np.zeros((max(n, 1), 625), np.uint32)
+        sto = np.zeros((max(n, 1), 625), np.uint32) if kind != "F" else None
+        if kind == "H":
             _check(self.lib.b200m_acransac_homography_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st), C.c_int(int(st.ndim == 2)),
                                                             C.c_int64(maxIteration), C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(M),
                                                             ptr(em), ptr(nfa), ptr(it), ptr(sto)),
                    "b200m_acransac_homography_pairs")
+        elif kind == "S":
+            _check(self.lib.b200m_acransac_fundamental_spherical_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(st), C.c_int(int(st.ndim == 2)),
+                                                                       C.c_int64(maxIteration), C.c_double(precision), ptr(valid), ptr(ninl),
+                                                                       ptr(inl), ptr(M), ptr(em), ptr(nfa), ptr(it), ptr(sto)),
+                   "b200m_acransac_fundamental_spherical_pairs")
         else:
             _check(self.lib.b200m_acransac_fundamental_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st), C.c_int64(maxIteration),
                                                              C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(M), ptr(em), ptr(nfa), ptr(it)),
@@ -271,19 +281,30 @@ class Context:
         tr = np.zeros(256, np.int32); trn = np.zeros(256, np.float64)
         for k in range(n):
             nt = self.lib.b200m_acransac_last_trace(self._h, C.c_int(k), ptr(tr), ptr(trn), C.c_int(tr.size))
-            r = {"valid": bool(valid[k]), "inliers": inl[offsets[k]:offsets[k] + ninl[k]].copy(), "H" if homography else "F": M[k].reshape(3, 3).copy(),
+            r = {"valid": bool(valid[k]), "inliers": inl[offsets[k]:offsets[k] + ninl[k]].copy(), "H" if kind == "H" else "F": M[k].reshape(3, 3).copy(),
                  "error_max": float(em[k]), "min_nfa": float(nfa[k]), "iterations": int(it[k]), "n_trace": int(nt),
                  "trace": tr[:min(nt, tr.size)].copy(), "trace_nfa": trn[:min(nt, trn.size)].copy()}
-            if homography:
+            if sto is not None:
                 r["mt_state_out"] = sto[k].copy()
             out.append(r)
         return out
 
     def acransac_last_stats(self) -> dict:
-        """Instrumentation of the last acransac_fundamental_pairs or acransac_homography_pairs call."""
+        """Instrumentation of the last acransac_fundamental_pairs, acransac_homography_pairs or acransac_fundamental_spherical_pairs
+        call."""
         st = np.zeros(4, np.int64)
         ms = self.lib.b200m_acransac_last_stats(self._h, st.ctypes.data_as(C.c_void_p))
         return {"gpu_ms": ms, "models_evaluated": int(st[0]), "models_skipped": int(st[1]), "models_exact": int(st[2]), "launches": int(st[3])}
+
+
+def _mt_states(mt_state_or_states, n: int) -> np.ndarray:
+    """One 625-word generator state (shape (625,)) or n per-pair states (n x 625)."""
+    st = np.ascontiguousarray(mt_state_or_states, np.uint32)
+    if st.ndim == 1:
+        return st.reshape(625)
+    if st.shape != (n, 625):
+        raise ValueError(f"mt_state_or_states: 625 words or n_pairs x 625, got {st.shape}")
+    return st
 
 
 def mt19937_state(seed: int) -> np.ndarray:
@@ -359,7 +380,8 @@ def hasStrongSupport(matches_per_type: dict, minimumSamples: int = 7) -> bool:
 
 def robustModelEstimation_F_AC(putatives: dict, regions_per_view: dict, image_sizes: dict, seed_or_state, maxIteration: int = 50000,
                                precision: float = np.inf, guidedMatching: bool = False, distanceRatio: float = 0.6, geometry: dict | None = None,
-                               guided_geometry: dict | None = None, desc_types=None, ctx: Context | None = None):
+                               guided_geometry: dict | None = None, desc_types=None, ctx: Context | None = None, bearings: dict | None = None,
+                               chain: bool = False):
     """matchingImageCollection::robustModelEstimation with GeometricFilterMatrix_F_AC (ACRANSAC, Fundamental7PSolver; GeometricFilter.hpp:40-88),
     the default `fundamental_matrix` filter of featureMatching, for a whole putative list: one a-contrario RANSAC call for every pair
     (b200m_acransac_fundamental_pairs), then, with guidedMatching, one guided-matching call for every kept pair and common descriptor
@@ -375,19 +397,56 @@ def robustModelEstimation_F_AC(putatives: dict, regions_per_view: dict, image_si
     guided_geometry  optional {view: {type: n x 2 double}}: getUndistortedPixel of every feature of a view whose camera isValid()
                      (guidedMatching.hpp:229-248), the positions guided matching uses
     desc_types       the describer types in EImageDescriberType order (default DESCRIBER_TYPES)
+    bearings         optional {view: {type: n x 3 double}}: for a view whose camera is camera::Equidistant, the unit vector
+                     toUnitSphere(removeDistortion(ima2cam(x))) of every feature, x its position as `geometry` gives it.  A pair whose
+                     two views have bearings for every common type is spherical: it is estimated by geometricEstimation_Spherical_Mat
+                     (GeometricFilterMatrix_F_AC.hpp:186-253, b200m_acransac_fundamental_spherical_pairs) on those vectors.  A view
+                     with bearings for some but not all of a pair's common types is a ValueError.
+    chain            the generator contract of spherical pairs, which take the std::mt19937 by reference:
+                       False  every pair starts from the caller's state: one planar and one spherical K10 call for the whole list;
+                       True   the single-threaded reference: a spherical pair starts where the previous spherical pair left the
+                              generator and hands it on; each run of planar pairs between two of them is one planar call from the
+                              current state.  Bit for bit the reference's run; meant for tests and short lists.
+                     Without spherical pairs both give today's single planar call.
 
     Returns (geometric matches {(I, J): {type: matches}} of the pairs with strong support, per-pair estimation
-    {(I, J): {"valid", "strong_support", "F", "error_max"}}).  Without guided matching the kept lists are the inlier putatives (ratio
-    and distance kept); with it, the guided lists of every common type (empty ones included) replace them, or nothing when error_max
-    is infinite (GeometricFilterMatrix_F_AC.hpp:363)."""
+    {(I, J): {"valid", "strong_support", "F", "error_max", "spherical"}, plus "mt_state_out" for the spherical pairs estimated}).
+    Without guided matching the kept lists are the inlier putatives (ratio and distance kept); with it, the guided lists of every
+    common type (empty ones included) replace them, or nothing when error_max is infinite (GeometricFilterMatrix_F_AC.hpp:363).  A
+    spherical pair's guided matching uses its F and error_max on the guided positions, as the reference does."""
     ctx = ctx or default_context()
     st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
     pairs, common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
-    res = ctx.acransac_fundamental_pairs(corrs, whs, st, maxIteration, precision) if est else []
-    info = {p: {"valid": False, "strong_support": False, "F": np.zeros((3, 3)), "error_max": np.inf} for p in pairs}
+    sph = _spherical_inputs(putatives, regions_per_view, bearings or {}, common, est)
+    planar = [k for k, p in enumerate(est) if p not in sph]
+    spherical = [k for k, p in enumerate(est) if p in sph]
+    res = [None] * len(est)
+
+    def run_planar(ks, state):
+        for k, r in zip(ks, ctx.acransac_fundamental_pairs([corrs[k] for k in ks], [whs[k] for k in ks], state, maxIteration, precision) if ks else []):
+            res[k] = r
+    if not chain or not spherical:
+        run_planar(planar, st)
+        rs = ctx.acransac_fundamental_spherical_pairs([sph[est[k]] for k in spherical], st, maxIteration, precision) if spherical else []
+        for k, r in zip(spherical, rs):
+            res[k] = r
+    else:
+        run = []
+        for k, p in enumerate(est):
+            if p not in sph:
+                run.append(k)
+                continue
+            run_planar(run, st)
+            run = []
+            res[k] = ctx.acransac_fundamental_spherical_pairs([sph[p]], st, maxIteration, precision)[0]
+            st = res[k]["mt_state_out"]
+        run_planar(run, st)
+    info = {p: {"valid": False, "strong_support": False, "F": np.zeros((3, 3)), "error_max": np.inf, "spherical": p in sph} for p in pairs}
     out = {}
     for p, r in zip(est, res):
         info[p].update(valid=r["valid"], F=r["F"], error_max=r["error_max"])
+        if p in sph:
+            info[p]["mt_state_out"] = r["mt_state_out"]
         if not r["valid"]:
             continue
         inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
@@ -425,6 +484,31 @@ def _estimation_inputs(putatives: dict, regions_per_view: dict, image_sizes: dic
         corrs.append(np.concatenate(parts))
         whs.append(tuple(image_sizes[I]) + tuple(image_sizes[J]))
     return pairs, common, est, corrs, whs
+
+
+def _spherical_inputs(putatives: dict, regions_per_view: dict, bearings: dict, common: dict, est) -> dict:
+    """{pair: n x 6 bearing pairs (xI, yI, zI, xJ, yJ, zJ), types concatenated in order} for the estimated pairs whose two views
+    have bearings for every common type (the rows of _estimation_inputs' correspondences, lifted)."""
+    out = {}
+    for I, J in est:
+        types = common[(I, J)]
+        have = [[t in bearings.get(v, {}) for t in types] for v in (I, J)]
+        for v, h in zip((I, J), have):
+            if any(h) and not all(h):
+                raise ValueError(f"bearings of view {v}: some but not all of the common types {types} of pair {(I, J)}")
+        if not all(have[0]) or not all(have[1]):
+            continue
+        parts = [np.zeros((0, 6))]
+        for t in types:
+            bI, bJ = (np.asarray(bearings[v][t], np.float64).reshape(-1, 3) for v in (I, J))
+            for v, b in ((I, bI), (J, bJ)):
+                if b.shape[0] != regions_per_view[v][t].RegionCount():
+                    raise ValueError(f"bearings of view {v}, type {t}: {b.shape[0]} vectors for {regions_per_view[v][t].RegionCount()} features")
+            m = putatives[(I, J)].get(t)
+            if m is not None and len(m):
+                parts.append(np.concatenate([bI[m["i"]], bJ[m["j"]]], axis=1))
+        out[(I, J)] = np.concatenate(parts)
+    return out
 
 
 def _guided_stage(ctx: Context, out: dict, info: dict, common: dict, regions_per_view: dict, guided_geometry: dict | None, run) -> None:

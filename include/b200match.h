@@ -248,15 +248,29 @@ int b200m_acransac_homography_pairs(b200m_ctx* ctx, int n_pairs, const int64_t* 
                                     const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision, uint8_t* valid,
                                     int32_t* n_inliers, uint32_t* inliers, double* H, double* error_max, double* min_nfa, int32_t* iterations,
                                     uint32_t* mt_state_out);
-/* instrumentation of the last a-contrario RANSAC call (b200m_acransac_fundamental_pairs or b200m_acransac_homography_pairs):
- * stats = {models evaluated in the a-contrario mode, of them skipped by the histogram bound, scored exactly, kernel launches};
- * returns its GPU time in ms */
+/* ---- geometric filtering: a-contrario RANSAC fundamental matrix of two equidistant cameras (K10, spherical) ------------- */
+/* GeometricFilterMatrix_F_AC::geometricEstimation_Spherical_Mat (ACRANSAC over RelativePoseSphericalKernel<Fundamental7PSphericalSolver,
+ * EpipolarSphericalDistanceError>), the branch the fundamental_matrix filter takes when both cameras of a pair are
+ * camera::Equidistant, for every pair of a list, results in input order.  No image size: the kernel works on unit vectors without
+ * normalisation, logalpha0 = pi, errorVectorDimension = 2, thresholdNormalizer = 1.
+ *   bearings   offsets[n_pairs] x 6 doubles (xI, yI, zI, xJ, yJ, zJ): the caller's lift of each correspondence,
+ *              toUnitSphere(removeDistortion(ima2cam(x))) of the xI / xJ columns the planar call would take
+ * Other arguments and outputs as in b200m_acransac_homography_pairs (the reference passes this generator by reference too), with
+ * F[9 * n_pairs] (row-major, x_J^T F x_I = 0 on the bearings; no unnormalisation) and error_max = sqrt of the largest inlier's
+ * squared residual when valid.  A pair with at most 7 correspondences returns (0, 0) and no iteration. */
+int b200m_acransac_fundamental_spherical_pairs(b200m_ctx* ctx, int n_pairs, const int64_t* offsets, const double* bearings,
+                                               const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision,
+                                               uint8_t* valid, int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max,
+                                               double* min_nfa, int32_t* iterations, uint32_t* mt_state_out);
+/* instrumentation of the last a-contrario RANSAC call (b200m_acransac_fundamental_pairs, b200m_acransac_homography_pairs or
+ * b200m_acransac_fundamental_spherical_pairs): stats = {models evaluated in the a-contrario mode, of them skipped by the histogram
+ * bound, scored exactly, kernel launches}; returns its GPU time in ms */
 double b200m_acransac_last_stats(const b200m_ctx* ctx, int64_t stats[4]);
-/* the `better` events of the last a-contrario RANSAC call's pair `pair` (F or H): the iterations at which a better model was found
+/* the `better` events of the last a-contrario RANSAC call's pair `pair` (F, H or spherical F): the iterations at which a better model was found
  * and the new minNFA of each (the first `cap`, at most 256; either pointer may be NULL); returns their number.  The getters of the
  * last call take the context's lock, so a concurrent call on the same context cannot rewrite what they read. */
 int b200m_acransac_last_trace(const b200m_ctx* ctx, int pair, int32_t* iters, double* nfa, int cap);
-/* debug, both models: 1 (default) = certified skip of models that cannot beat the running minNFA; 0 = score every model exactly */
+/* debug, every model: 1 (default) = certified skip of models that cannot beat the running minNFA; 0 = score every model exactly */
 int b200m_ctx_set_acransac_skip(b200m_ctx* ctx, int on);
 /* host only: std::mt19937(seed) as 625 words (see mt_state) */
 void b200m_mt19937_seed(uint32_t seed, uint32_t state[625]);
