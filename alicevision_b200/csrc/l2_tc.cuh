@@ -27,7 +27,8 @@
 //                runs through the tensor cores, so the match list is complete when the kernel ends
 //   warps 4-11   two consumer warpgroups of 64 query rows each: per tile 8 (AUG: 9) wgmma.m64n128k16 into 64 fp32 registers
 //                per thread, then the chunk-minimum epilogue on those registers.  The two warpgroups run independently, so
-//                one warpgroup's epilogue overlaps the other's MMAs.
+//                one warpgroup's epilogue overlaps the other's MMAs.  The u8 kernel (4 wgmma.m64n128k32 per tile) pipelines each
+//                warpgroup's tiles over two accumulators instead, so that its epilogue overlaps its own next MMAs.
 //   MODE_REAL adds six re-scoring warps (12-17).
 //
 // MODE (template): what the epilogue keeps per query row and what leaves the kernel
@@ -69,6 +70,11 @@ constexpr int AUG_BYTES = 128 * 16 * 2;   // 4 KB: 16 augmentation columns of 12
 constexpr int NB_BYTES = BN * 4;          // half-norms (u8: int32 norms) of one tile
 constexpr int U8_BYTES = 128 * 128;       // 16 KB: 128 uchar rows of 128 B = one TMA box of tmap_u8 (the whole K of a u8 query or database tile)
 constexpr int EPI_WARPS = 8;
+// u8 kernel: per-thread registers after set-up, warpgroup 0 (producer, exactness pass) and the two consumer warpgroups (two 64-register
+// accumulators).  setmaxnreg moves them inside the launch allocation of 384 x 128: 128 * U8_REGS_WG0 + 256 * U8_REGS_CONSUMER <= 49152.
+constexpr int U8_REGS_WG0 = 64;
+constexpr int U8_REGS_CONSUMER = 160;
+static_assert(128 * U8_REGS_WG0 + 256 * U8_REGS_CONSUMER <= 384 * 128, "the u8 kernel's register split exceeds its launch allocation");
 enum : int { MODE_MATCH = 0, MODE_KNN = 1, MODE_REAL = 2 };
 
 template <bool AUG, bool REAL = false, bool U8 = false> struct Lay {
@@ -180,6 +186,29 @@ __device__ __forceinline__ int32_t min16(const int32_t (&x)[16]) {
   return min(__vimin3_s32(a, b, c), __vimin3_s32(d, e, x[15]));
 }
 
+// The u8 epilogue of one tile, from the s32 accumulator acc = a.b (exact).  Per element s = ||b||^2 - 2 a.b = ||a - b||^2 - ||a||^2
+// (u8_elem), chunk minima in integers, and only the four minima per thread become h = s / 2: exactly the fp16 kernel's accumulator value
+// (|s| < 2^24), so everything from the folds on is shared.  Pad rows: a.b = 0 (TMA zero fill), ||b||^2 = 2^24 (prep.cuh) -> h = 2^23, as
+// in the fp16 kernel.  A chunk is the 16 columns THIS thread holds of a query row in one 64-column half of the tile (common.cuh chunk_row),
+// so its minimum needs no shuffle; pad rows of a partial last tile share chunks with real rows and lose to them.
+// Column 8j + 2 qlane + e of the tile (j = 0..15, e = 0, 1) is acc[4j + e] (row r0), acc[4j + 2 + e] (row r0 + 8); its norm is nb2[4j].
+// v2[r][h] = minimum h of chunk 4h + qlane of row r0 + 8r.
+__device__ __forceinline__ void u8_tile_minima(const int32_t (&acc)[64], const int2* nb2, float (&v2)[2][2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    int32_t x[2][16];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int2 n = nb2[4 * (8 * h + j)];
+      const int a = 32 * h + 4 * j;
+      x[0][2 * j] = u8_elem(n.x, acc[a + 0]); x[0][2 * j + 1] = u8_elem(n.y, acc[a + 1]);
+      x[1][2 * j] = u8_elem(n.x, acc[a + 2]); x[1][2 * j + 1] = u8_elem(n.y, acc[a + 3]);
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) v2[r][h] = u8_half_dist(min16(x[r]));
+  }
+}
+
 // The real-valued re-scoring reads 32 fp32 rows per candidate (16 KB, mostly from HBM) and is latency-bound: two warps cannot keep up with
 // the tensor cores, so MODE_REAL adds six re-scoring warps behind the epilogue warps.
 constexpr int REAL_EXTRA_VERIFY_WARPS = 6;
@@ -209,8 +238,10 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
   uint64_t* vq_full = db_empty + NS;        // [2]  4 arrivals (the epilogue quadrants that emit candidates)
   uint64_t* vq_empty = vq_full + 2;         // [2]  the exactness-pass warps
 
-  const int warp = threadIdx.x >> 5;
+  // U8: the role branches hold setmaxnreg and the wgmma pipeline, which ptxas only keeps on a path it can prove warp-uniform
+  const int warp = U8 ? __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0) : (int)(threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
+  // the roles take these as arguments: the u8 kernel computes them in each role (see the dispatch at the end)
   const int rank = (int)blockIdx.x % ctas_per_item;   // which 128 queries of the work item
   const int cl = (int)blockIdx.x / ctas_per_item;
   const int n_cl = (int)gridDim.x / ctas_per_item;
@@ -237,7 +268,7 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
   }
   __syncthreads();
 
-  if (warp == 0) {
+  auto producer = [&](int rank, int cl) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
       uint32_t qb = 0, qph = 0, st = 0, sph = 0, tt = 0;
@@ -279,7 +310,8 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
         }
       }
     }
-  } else if (warp == 2 || warp == 3 || warp >= 4 + EPI_WARPS) {
+  };
+  auto exactness_pass = [&](int cl) {
     // ------------------------------------------------------------------ exactness pass of the previous item
     // fused == 0 (short database images: an item lasts only a few tiles, two warps cannot hide the re-scoring latency):
     // the epilogue writes its candidates to global memory and the stand-alone exactness kernel handles them.
@@ -315,7 +347,8 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
       if (lane == 0) ptx::mbar_arrive(&vq_empty[par]);
       par ^= 1; if (par == 0) vph ^= 1;
     }
-  } else if (warp >= 4) {
+  };
+  auto consumers = [&](int rank, int cl) {
     // ------------------------------------------------------------------ consumers: MMA + epilogue (two warpgroups of 64 rows)
     const int wg = (warp - 4) >> 2;
     const int qlane = lane & 3;
@@ -334,58 +367,78 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
       constexpr uint32_t NONE = 0x7F800000u | REAL_IDMASK;                                               // MODE_REAL: +inf, id = none
       Top4 s4[2] = {{NONE, NONE, NONE, NONE}, {NONE, NONE, NONE, NONE}};
       ptx::mbar_wait(&q_full[qb], qph);
-      for (int t = 0; t < ntiles; ++t) {
-        ptx::trace_stamp(etrace, 1 + wg, tt, 0);
-        ptx::mbar_wait(&db_full[st], sph);
-        ptx::trace_stamp(etrace, 1 + wg, tt, 1);
-        const uint32_t b_base = db_addr + st * STAGE;
-        auto release_slot = [&] {
-          __syncwarp();
-          if (lane == 0) ptx::mbar_arrive(&db_empty[st]);             // this warp is done with the slot (operands and (half-)norms)
-          if (++st == NS) { st = 0; sph ^= 1; }
-        };
-        float v2[2][2];                        // chunk minima h of chunks 4h + qlane of rows r0, r0 + 8
-        if constexpr (U8) {
-          // acc = a.b, exact in s32.  Per element s = ||b||^2 - 2 a.b = ||a - b||^2 - ||a||^2 (u8_elem), chunk minima in integers, and only
-          // the four minima per thread become h = s / 2: exactly the fp16 kernel's accumulator value (|s| < 2^24), so everything
-          // from the folds on is shared.  Pad rows: a.b = 0 (TMA zero fill), ||b||^2 = 2^24 (prep.cuh) -> h = 2^23, as in the fp16 kernel.
-          // A chunk is the 16 columns THIS thread holds of a query row in one 64-column half of the tile (common.cuh chunk_row), so its
-          // minimum needs no shuffle; pad rows of a partial last tile share chunks with real rows and lose to them.
-          int32_t acc[64];
+      auto release_slot = [&] {
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&db_empty[st]);               // this warp is done with the slot (operands and (half-)norms)
+        if (++st == NS) { st = 0; sph ^= 1; }
+      };
+      // v2[r][h]: chunk minima h of chunks 4h + qlane of tile t, rows r0, r0 + 8
+      auto fold_tile = [&](int t, const float (&v2)[2][2]) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t gid = (uint32_t)t * (BN / CHUNK) + 4 * h + qlane;
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            if (REAL) fold_chunk_real(v2[r][h], gid, s4[r]);
+            else if (KNN) fold_chunk_knn(v2[r][h], gid, sk[r]);
+            else fold_chunk(v2[r][h], gid, s[r]);
+          }
+        }
+      };
+      if constexpr (U8) {
+        // Software pipeline over the item's tiles: the MMAs of tile t + 1 are issued into the other accumulator before the epilogue of
+        // tile t, and wgmma.wait_group 1 waits for tile t's group only, so each warpgroup's epilogue runs under its own next MMAs.  The
+        // pipeline fills and drains inside the work item: the item boundary (q_empty, the merge, the candidate hand-off) is unchanged.
+        // Slot t is released after its epilogue (its norms are read there), one MMA group later than without the pipeline.
+        const int nt = __shfl_sync(0xffffffffu, ntiles, 0);           // warp-uniform bounds keep the wgmma pipeline out of divergent paths
+        const uint32_t a_base = q_addr + qb * QT;
+        uint32_t ist = st, isph = sph;                                 // ring slot of the next tile to issue
+        auto issue = [&](int32_t (&acc)[64]) {
+          const uint32_t b_base = db_addr + ist * STAGE;
           ptx::wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t da = ptx::wgmma_desc_k_sw128(q_addr + qb * QT + k * 32);
-            const uint64_t db = ptx::wgmma_desc_k_sw128(b_base + k * 32);
-            ptx::wgmma_m64n128k32_u8(acc, da, db, k > 0 ? 1u : 0u);
-          }
+          for (int k = 0; k < 4; ++k)
+            ptx::wgmma_m64n128k32_u8(acc, ptx::wgmma_desc_k_sw128(a_base + k * 32), ptx::wgmma_desc_k_sw128(b_base + k * 32), k > 0 ? 1u : 0u);
           ptx::wgmma_commit();
-          // column 8j + 2 qlane + e of the tile (j = 0..15, e = 0, 1): acc[4j + e] (row r0), acc[4j + 2 + e] (row r0 + 8); norms nb2[4j]
-          const int2* nb2 = reinterpret_cast<const int2*>(smem + L::OFF_DB + st * STAGE + U8_BYTES) + qlane;
-          // half of the norms are loaded under the MMAs (they depend on db_full only); all 16 there would not fit in 128 registers
-          constexpr int U8_NB_EARLY = 8;
-          int2 nb[16];
-#pragma unroll
-          for (int j = 0; j < U8_NB_EARLY; ++j) nb[j] = nb2[4 * j];
-          ptx::wgmma_wait_all();
-          ptx::trace_stamp(etrace, 1 + wg, tt, 2);
-#pragma unroll
-          for (int j = U8_NB_EARLY; j < 16; ++j) nb[j] = nb2[4 * j];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            int32_t x[2][16];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int2 n = nb[8 * h + j];
-              const int a = 32 * h + 4 * j;
-              x[0][2 * j] = u8_elem(n.x, acc[a + 0]); x[0][2 * j + 1] = u8_elem(n.y, acc[a + 1]);
-              x[1][2 * j] = u8_elem(n.x, acc[a + 2]); x[1][2 * j + 1] = u8_elem(n.y, acc[a + 3]);
-            }
-#pragma unroll
-            for (int r = 0; r < 2; ++r) v2[r][h] = u8_half_dist(min16(x[r]));
+          if (++ist == NS) { ist = 0; isph ^= 1; }
+        };
+        // trace per tile: 0 start, 1 tile t + 1 landed (db_full), 2 tile t's MMAs complete (the wait_group 1), 3 tile t folded
+        // `last` is a constant after inlining: the wgmma sequence of each copy is branch-free, which ptxas needs to keep the pipeline
+        auto tile = [&](int t, const int32_t (&acc)[64], int32_t (&acc_next)[64], bool last) {
+          ptx::trace_stamp(etrace, 1 + wg, tt, 0);
+          if (!last) {
+            ptx::mbar_wait(&db_full[ist], isph);
+            ptx::trace_stamp(etrace, 1 + wg, tt, 1);
+            issue(acc_next);
+            ptx::wgmma_wait<1>();                                      // tile t's group has completed, tile t + 1's runs on
+          } else {
+            ptx::trace_stamp(etrace, 1 + wg, tt, 1);
+            ptx::wgmma_wait<0>();
           }
+          ptx::trace_stamp(etrace, 1 + wg, tt, 2);
+          float v2[2][2];
+          u8_tile_minima(acc, reinterpret_cast<const int2*>(smem + L::OFF_DB + st * STAGE + U8_BYTES) + qlane, v2);
           release_slot();
-        } else {
+          fold_tile(t, v2);
+          ptx::trace_stamp(etrace, 1 + wg, tt, 3); ++tt;
+        };
+        int32_t acc0[64], acc1[64];
+        if (nt > 0) {
+          ptx::mbar_wait(&db_full[ist], isph);
+          issue(acc0);
+          for (int t = 0;; t += 2) {                                   // unrolled by two: even tiles in acc0, odd tiles in acc1; the only
+            if (t + 1 == nt) { tile(t, acc0, acc1, true); break; }     // exits follow a drained last tile
+            tile(t, acc0, acc1, false);
+            if (t + 2 == nt) { tile(t + 1, acc1, acc0, true); break; }
+            tile(t + 1, acc1, acc0, false);
+          }
+        }
+      } else {
+        for (int t = 0; t < ntiles; ++t) {
+          ptx::trace_stamp(etrace, 1 + wg, tt, 0);
+          ptx::mbar_wait(&db_full[st], sph);
+          ptx::trace_stamp(etrace, 1 + wg, tt, 1);
+          const uint32_t b_base = db_addr + st * STAGE;
           float acc[64];
           ptx::wgmma_fence();
 #pragma unroll
@@ -418,19 +471,11 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
             pm[0][c] = fminf(fminf(acc[8 * c + 0], acc[8 * c + 1]), fminf(acc[8 * c + 4], acc[8 * c + 5]));
             pm[1][c] = fminf(fminf(acc[8 * c + 2], acc[8 * c + 3]), fminf(acc[8 * c + 6], acc[8 * c + 7]));
           }
+          float v2[2][2];
           quad_chunk_minima(pm, qlane, v2);
+          fold_tile(t, v2);
+          ptx::trace_stamp(etrace, 1 + wg, tt, 3); ++tt;
         }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t gid = (uint32_t)t * (BN / CHUNK) + 4 * h + qlane;
-#pragma unroll
-          for (int r = 0; r < 2; ++r) {
-            if (REAL) fold_chunk_real(v2[r][h], gid, s4[r]);
-            else if (KNN) fold_chunk_knn(v2[r][h], gid, sk[r]);
-            else fold_chunk(v2[r][h], gid, s[r]);
-          }
-        }
-        ptx::trace_stamp(etrace, 1 + wg, tt, 3); ++tt;
       }
       __syncwarp();
       if (lane == 0) ptx::mbar_arrive(&q_empty[qb]);                 // every MMA of this item has completed
@@ -518,6 +563,26 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
       }
       par ^= 1; if (par == 0) vqph ^= 1;
     }
+  };
+  if constexpr (U8) {
+    // Registers move from warpgroup 0 (producer, exactness pass: little state) to the consumers (two accumulators each).  One
+    // setmaxnreg per warpgroup, at the head of a branch that holds all of its code: ptxas compiles each region to its count, and code
+    // that both counts reach would have to fit the smaller one.  It spills a value that lives across setmaxnreg, so each role reads
+    // the block index itself.
+    if (warp < 4) {
+      ptx::setmaxnreg_dec<U8_REGS_WG0>();
+      const int b = ptx::block_index();
+      if (warp == 0) producer(b % ctas_per_item, b / ctas_per_item);
+      else if (warp >= 2) exactness_pass(b / ctas_per_item);
+    } else {
+      ptx::setmaxnreg_inc<U8_REGS_CONSUMER>();
+      const int b = ptx::block_index();
+      consumers(b % ctas_per_item, b / ctas_per_item);
+    }
+  } else {
+    if (warp == 0) producer(rank, cl);
+    else if (warp == 2 || warp == 3 || warp >= 4 + EPI_WARPS) exactness_pass(cl);
+    else if (warp >= 4) consumers(rank, cl);
   }
 }
 
@@ -529,9 +594,10 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
 template <bool AUG, int MODE = MODE_MATCH>
 __global__ void __launch_bounds__(block_threads<MODE>(), 1) l2_top2_tc_kernel(B200M_TC_PARAMS) { l2_top2_tc<AUG, MODE, false>(B200M_TC_ARGS); }
 
-// The u8 kernel is held to 128 registers per thread: the 512-thread, 32-register device finishing kernel (finish.cuh) of the previous batch
-// then still fits beside the persistent CTA of each SM, as it does beside the fp16 kernel.  At 130 registers it waited for the search
-// kernel to end, and consecutive batches' search kernels no longer ran back to back.
+// The u8 kernel is launched with 128 registers per thread: the 512-thread, 32-register device finishing kernel (finish.cuh) of the previous
+// batch then still fits beside the persistent CTA of each SM, as it does beside the fp16 kernel.  At 130 registers it waited for the search
+// kernel to end, and consecutive batches' search kernels no longer ran back to back.  Inside that allocation setmaxnreg gives the consumers
+// 160 (U8_REGS_CONSUMER) for their two accumulators.
 __global__ void __maxnreg__(128) l2_top2_tc_u8_kernel(B200M_TC_PARAMS) {
   l2_top2_tc<false, MODE_MATCH, true>(B200M_TC_ARGS);
 }

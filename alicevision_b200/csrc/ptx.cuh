@@ -9,6 +9,12 @@ namespace b200m {
 namespace ptx {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+// blockIdx.x, read where it is used: the compiler neither hoists nor merges the read (see the setmaxnreg roles of l2_tc.cuh)
+__device__ __forceinline__ int block_index() {
+  int b;
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(b));
+  return b;
+}
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -87,6 +93,19 @@ __device__ __forceinline__ uint64_t wgmma_desc_k_sw32(uint32_t smem_addr) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Wait until at most N committed groups of this warpgroup are still pending (N = 1: all but the most recent one have completed).
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// Move registers between the warpgroups of a CTA inside its launch allocation: every warp of a warpgroup executes the same instruction,
+// N is the new per-thread count (an immediate, a multiple of 8 in 24..256).  `inc` blocks until other warpgroups' `dec` freed enough.
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() {
+  static_assert(N % 8 == 0 && N >= 24 && N <= 256, "setmaxnreg count");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() {
+  static_assert(N % 8 == 0 && N >= 24 && N <= 256, "setmaxnreg count");
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
 
 // D[64 x 128] (+)= A[64 x 16] * (-B[128 x 16])^T, fp16 inputs from shared memory, fp32 accumulators in registers (the whole warpgroup
 // issues it).  Thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 + {0, 8}, columns 8*j + 2*(t%4) + {0, 1}, j = 0..15:

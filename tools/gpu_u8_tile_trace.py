@@ -1,11 +1,13 @@
 """Per-tile pipeline trace of the u8 search kernel (l2_tc.cuh, U8) on the GPU: where one tile's cycles go.
 
 Builds the library if needed, matches 20 x 8192 uchar SIFT images (190 pairs, every pair on the u8 kernel) with
-`Context.debug_trace` on, and prints one JSON line: the medians, in SM cycles, of what CTA 0 stamped per database tile
-  period         start of one tile's wait to the start of the next
-  wait           waiting for the tile's operands to land (db_full)
-  mma            MMAs issued -> complete (wgmma wait)
-  epilogue       MMAs complete -> chunk minima folded
+`Context.debug_trace` on, and prints one JSON line: the medians, in SM cycles, of what CTA 0 stamped per database tile t.
+Each warpgroup runs the tiles of a work item as a pipeline: it issues the MMAs of tile t + 1, then waits for tile t's and runs
+tile t's epilogue while tile t + 1's MMAs run.  The columns are
+  period         start of tile t's step to the start of tile t + 1's
+  wait           waiting for tile t + 1's operands to land (db_full; none on the last tile of an item)
+  mma            tile t + 1's MMAs issued, then blocked until tile t's have completed (wgmma.wait_group 1)
+  epilogue       tile t's MMAs complete -> its chunk minima folded (under tile t + 1's MMAs)
   producer_wait  the TMA producer waiting for a free ring slot
 for each of the two consumer warpgroups, over the traced tiles after the first two work items, and the card's name and power limit
 read in the same call.  There is no fallback: without a GPU the script fails.
