@@ -7,6 +7,8 @@
 // support rules, then one
 // guided-matching call for every kept pair and common descriptor type (b200m_guided_match_pairs, or for H with distanceRatio < 0
 // b200m_guided_match_positions_pairs).
+// GeometricFilterMatrix_HGrowing_Batch_b200 does the same for the `homography_growing` filter (GeometricFilterMatrix_HGrowing.hpp:176-266,
+// filterMatchesByHGrowing): one b200m_hgrowing_pairs call for every (pair, common describer type) of the list.
 // Header-only; compiled inside an AliceVision build and linked against libb200match.so.  The caller gathers xI / xJ with the
 // reference's fillMatricesWithUndistortFeaturesMatches and the guided positions with camera::IntrinsicBase::getUndistortedPixel.
 // Inside the AliceVision build (ALICEVISION_B200_REFERENCE_FILTER_UTILS defined) the library's own copyInlierMatches and
@@ -31,6 +33,7 @@
 #endif
 
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdint>
 #include <limits>
@@ -470,6 +473,141 @@ public:
 
 private:
     std::vector<Estimate> _estimates;
+};
+
+/// robustModelEstimation with GeometricFilterMatrix_HGrowing (the `homography_growing` filter: filterMatchesByHGrowing on the
+/// regions' raw PointFeatures, GeometricFilterMatrix_HGrowing.hpp:176-266, GeometricFilterMatrix_HGrowing.cpp:108-194) for the pairs
+/// added, then run().  No view is uploaded: each (pair, type) goes to the engine as its putatives' feature pairs.  The result is the
+/// reference's single-threaded seed loop, which is what featureMatching runs (its seed loop sits inside robustModelEstimation's OpenMP
+/// loop).
+class GeometricFilterMatrix_HGrowing_Batch_b200
+{
+public:
+    /// GrowParameters and HGrowingFilteringParam at the reference's defaults (GeometricFilterMatrix_HGrowing.hpp:23-106), which
+    /// featureMatching never changes
+    struct Param
+    {
+        double similarityTolerance = 20, affinityTolerance = 10, homographyTolerance = 5;
+        int minInliersToRefine = 6, nbRefiningIterations = 8, maxNbHomographies = 10, minNbMatchesPerH = 20;
+    };
+    /// per (pair, type): each homography (row-major, x_J ~ H x_I) with its matches, like the reference's _HsAndMatchesPerDesc
+    using HsAndMatches = std::vector<std::pair<std::array<double, 9>, matching::IndMatches>>;
+
+    explicit GeometricFilterMatrix_HGrowing_Batch_b200(b200m_ctx* ctx = matching::b200detail::sharedContext())
+      : _ctx(ctx)
+    {}
+    GeometricFilterMatrix_HGrowing_Batch_b200(b200m_ctx* ctx, const Param& param)
+      : _ctx(ctx),
+        _param(param)
+    {}
+
+    bool available() const { return _ctx != nullptr; }
+
+    /// One pair of the putative list: its common describer types (RegionsPerView::getCommonDescTypes), its putatives, and
+    /// featuresOf(view, type) -> const std::vector<feature::PointFeature>& (Regions::Features()).  A pair without a common type, or with
+    /// a CCTag or AprilTag type among them in builds that have those describers, gets no estimation; a type without a putative entry is
+    /// skipped.  The putatives are walked in their given order (featureMatching sorts them by Lowe ratio first).
+    template <class FeaturesOf>
+    void addPair(const Pair& pair, const matching::MatchesPerDescType& putatives, const std::vector<feature::EImageDescriberType>& descTypes,
+                 FeaturesOf featuresOf)
+    {
+        if (descTypes.empty())
+            return;
+        auto has = [&](feature::EImageDescriberType t) { return std::find(descTypes.begin(), descTypes.end(), t) != descTypes.end(); };
+        (void)has;
+#if ALICEVISION_IS_DEFINED(ALICEVISION_HAVE_CCTAG)
+        if (has(feature::EImageDescriberType::CCTAG3) || has(feature::EImageDescriberType::CCTAG4))
+            return;
+#endif
+#if ALICEVISION_IS_DEFINED(ALICEVISION_HAVE_APRILTAG)
+        if (has(feature::EImageDescriberType::APRILTAG16H5))
+            return;
+#endif
+        for (const feature::EImageDescriberType t : descTypes)
+        {
+            const auto it = putatives.find(t);
+            if (it == putatives.end())
+                continue;
+            const std::vector<feature::PointFeature>& fI = featuresOf(pair.first, t);
+            const std::vector<feature::PointFeature>& fJ = featuresOf(pair.second, t);
+            for (const matching::IndMatch& m : it->second)
+            {
+                const feature::PointFeature& a = fI.at(m._i);
+                const feature::PointFeature& b = fJ.at(m._j);
+                const float v[8] = {a.x(), a.y(), a.scale(), a.orientation(), b.x(), b.y(), b.scale(), b.orientation()};
+                _feat.insert(_feat.end(), v, v + 8);
+            }
+            _items.push_back(Item{pair, t, it->second});
+            _offsets.push_back(_offsets.back() + (int64_t)it->second.size());
+        }
+    }
+
+    /// filterMatchesByHGrowing for every (pair, type) added, in one engine call.  Every pair with at least one filtered type enters
+    /// out, with an entry per filtered type even when it is empty; with guidedMatching its lists are an empty map (the reference's
+    /// Geometry_guided_matching is an empty stub).  Returns false (out untouched) when the engine is unavailable or fails.
+    bool run(bool guidedMatching, matching::PairwiseMatches& out)
+    {
+        if (!available())
+            return false;
+        const int n = (int)_items.size();
+        const int mh = _param.maxNbHomographies;
+        std::vector<int32_t> nH(n), counts((std::size_t)n * std::max(mh, 1)), inl(std::max<int64_t>(_offsets.back(), 1));
+        std::vector<double> H((std::size_t)n * std::max(mh, 1) * 9);
+        if (n > 0 && b200m_hgrowing_pairs(_ctx, n, _offsets.data(), _feat.data(), _param.similarityTolerance, _param.affinityTolerance,
+                                          _param.homographyTolerance, _param.minInliersToRefine, _param.nbRefiningIterations, mh,
+                                          _param.minNbMatchesPerH, nH.data(), H.data(), counts.data(), inl.data(), nullptr, nullptr) != B200M_OK)
+            return false;
+        _hs.clear();
+        std::map<Pair, matching::MatchesPerDescType> result;
+        for (int k = 0; k < n; ++k)
+        {
+            const Item& item = _items[k];
+            HsAndMatches& hs = _hs[item.pair][item.type];
+            matching::IndMatches all;
+            int64_t at = _offsets[k];
+            for (int h = 0; h < nH[k]; ++h)
+            {
+                std::array<double, 9> M;
+                std::copy(H.begin() + ((std::size_t)k * mh + h) * 9, H.begin() + ((std::size_t)k * mh + h) * 9 + 9, M.begin());
+                matching::IndMatches ms;
+                for (int q = 0; q < counts[(std::size_t)k * mh + h]; ++q)
+                    ms.push_back(item.putatives[inl[at++]]);
+                all.insert(all.end(), ms.begin(), ms.end());
+                hs.emplace_back(M, std::move(ms));
+            }
+            matching::MatchesPerDescType& r = result[item.pair];
+            if (!guidedMatching)
+                r.emplace(item.type, std::move(all));
+        }
+        for (auto& x : result)
+            out[x.first] = std::move(x.second);
+        return true;
+    }
+
+    /// The homographies of one (pair, type) after run(); empty when it was not filtered.
+    const HsAndMatches& homographies(const Pair& pair, feature::EImageDescriberType type) const
+    {
+        static const HsAndMatches none;
+        const auto p = _hs.find(pair);
+        if (p == _hs.end())
+            return none;
+        const auto t = p->second.find(type);
+        return t == p->second.end() ? none : t->second;
+    }
+
+private:
+    struct Item
+    {
+        Pair pair;
+        feature::EImageDescriberType type;
+        matching::IndMatches putatives;
+    };
+    b200m_ctx* _ctx;
+    Param _param{};
+    std::vector<Item> _items;
+    std::vector<int64_t> _offsets{0};
+    std::vector<float> _feat;
+    std::map<Pair, std::map<feature::EImageDescriberType, HsAndMatches>> _hs;
 };
 
 }  // namespace matchingImageCollection

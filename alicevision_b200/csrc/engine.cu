@@ -10,6 +10,7 @@
 #include "finish.cuh"
 #include "guided.cuh"
 #include "acransac.cuh"
+#include "hgrowing.cuh"
 #include "guided_fast.cuh"
 #include "hamming.cuh"
 #include "l2_exact.cuh"
@@ -259,6 +260,15 @@ struct AcransacScratch {
   Event ev0, ev1;
 };
 
+// grow-only scratch of b200m_hgrowing_pairs (hgrowing.cuh): the call's features and outputs, and one batch's lists, bitsets, seed
+// slots and grow-warp bitsets; the last call's instrumentation
+struct HgrowingScratch {
+  DeviceBuffer<char> d;
+  int window = 256;                                   // seeds per item and window (b200m_ctx_set_hgrowing_window)
+  double last_ms = 0; int64_t stats[3] = {0, 0, 0};
+  Event ev0, ev1;
+};
+
 // What the last b200m_match_pairs, b200m_guided_match_pairs (and its one-pair forms), b200m_guided_match_positions_pairs, b200m_guided_match_fast_pairs
 // or b200m_knn measured (b200m_last_*);
 // a field the call does not measure is 0
@@ -275,6 +285,7 @@ struct b200m_ctx {
   int device = 0, num_sms = 148;
   Stream stream, copy_stream, up_stream, tab_stream, pack_stream;
   AcransacScratch acr;
+  HgrowingScratch hgr;
   KnnScratch knn;
   GuidedFastScratch gf;
   long gf_left_cap = 1l << 21;    // left features per internal batch of b200m_guided_match_fast_pairs (B200M_GUIDED_FAST_LEFT_CAP)
@@ -1929,6 +1940,181 @@ int b200m_guided_match_positions_pairs(b200m_ctx* c, const uint32_t* pairs, int 
   if (int rc = wait_uploads(c)) return rc;
   *out = guided_result(c, pairs, n_pairs, per_pair);
   c->last = LastCall{t.gpu_ms, t.search_ms, t.launches, 0, 0, 0, (*out)->offsets[n_pairs], 0};
+  return B200M_OK;
+}
+
+}  // extern "C"
+
+// ---- K12: homography growing for a list of work items (hgrowing.cuh) ----
+// Items go in batches, in input order: a batch holds at most kHgBatchPutatives putatives and kHgBatchSeeds / window items.  Per batch
+// and round: for each window w < ceil(n_max / window), one grow and one replay launch over the whole batch; then one finish launch.
+// The call's features and outputs stay on the device throughout, and the outputs come back in one copy at the end.
+constexpr long long kHgBatchPutatives = 1ll << 24;
+constexpr long long kHgBatchSeeds = 1ll << 21;
+
+static int hgrowing_pairs(b200m_ctx* c, int n_items, const int64_t* offsets, const float* feat, const hg::Param& p, int32_t* n_h_out,
+                          double* H_out, int32_t* counts_out, int32_t* inl_out, int32_t* trace_out, int32_t* rounds_out) {
+  const int mh = p.max_nb_homographies;
+  const long long N = n_items ? offsets[n_items] : 0;
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  CK(cudaSetDevice(c->device));
+  HgrowingScratch& S = c->hgr;
+  S.last_ms = 0; S.stats[0] = S.stats[1] = S.stats[2] = 0;
+  if (n_items == 0) return B200M_OK;
+  const int W = S.window;
+  // batches: [first item, last item + 1)
+  std::vector<std::pair<int, int>> batches;
+  for (int k = 0; k < n_items;) {
+    int e = k;
+    long long put = 0;
+    while (e < n_items && (e == k || (put + (offsets[e + 1] - offsets[e]) <= kHgBatchPutatives && (long long)(e - k + 1) * W <= kHgBatchSeeds))) {
+      put += offsets[e + 1] - offsets[e];
+      ++e;
+    }
+    batches.emplace_back(k, e);
+    k = e;
+  }
+  // the largest batch sizes the batch region
+  long long b_put = 0, b_words = 0, b_items = 0, n_max = 0;
+  for (auto& b : batches) {
+    long long put = 0, words = 0;
+    for (int k = b.first; k < b.second; ++k) {
+      const long long n = offsets[k + 1] - offsets[k];
+      put += n; words += (n + 31) / 32; n_max = std::max(n_max, n);
+    }
+    b_put = std::max(b_put, put); b_words = std::max(b_words, words); b_items = std::max(b_items, (long long)(b.second - b.first));
+  }
+  const int grow_blocks = (int)std::min<long long>((b_items * W + hgk::kWarps - 1) / hgk::kWarps, (long long)c->num_sms * 8);
+  const long long scratch_words = std::max<long long>(1, (n_max + 31) / 32);
+  const size_t rows = (size_t)n_items * std::max(mh, 1);
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
+  // output region first: one contiguous read-back
+  const size_t o_H = take(sizeof(double) * 9 * rows), o_stats = take(sizeof(unsigned long long) * 2), o_cnt = take(sizeof(int) * rows),
+               o_tr = take(sizeof(int) * 3 * rows), o_nh = take(sizeof(int) * n_items), o_rounds = take(sizeof(int) * n_items),
+               o_inl = take(sizeof(int) * std::max<long long>(N, 1));
+  const size_t out_bytes = at;
+  const size_t o_feat = take(sizeof(float) * hg::kFeat * std::max<long long>(N, 1)), o_items = take(sizeof(hgk::Item) * b_items),
+               o_rem = take(sizeof(int) * std::max<long long>(b_put, 1)), o_used = take(sizeof(uint32_t) * std::max<long long>(b_words, 1)),
+               o_seeds = take(sizeof(hgk::Seed) * b_items * W),
+               o_scr = take(sizeof(uint32_t) * (size_t)scratch_words * grow_blocks * hgk::kWarps);
+  int rc;
+  if ((rc = S.d.reserve(at)) || (rc = S.ev0.create()) || (rc = S.ev1.create())) return rc;
+  char* d = S.d;
+  cudaStream_t st = c->stream;
+  CK(cudaMemsetAsync(d, 0, out_bytes, st));
+  if (N) CK(cudaMemcpyAsync(d + o_feat, feat, sizeof(float) * hg::kFeat * N, cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(S.ev0, st));
+  hgk::Ctl ctl{};
+  ctl.feat = (const float*)(d + o_feat);
+  ctl.items = (hgk::Item*)(d + o_items);
+  ctl.rem = (int*)(d + o_rem); ctl.used = (uint32_t*)(d + o_used); ctl.seeds = (hgk::Seed*)(d + o_seeds);
+  ctl.window = W; ctl.scratch = (uint32_t*)(d + o_scr); ctl.scratch_words = (int)scratch_words; ctl.p = p;
+  ctl.H = (double*)(d + o_H); ctl.counts = (int*)(d + o_cnt); ctl.trace = (int*)(d + o_tr); ctl.inl = (int*)(d + o_inl);
+  ctl.n_h = (int*)(d + o_nh); ctl.rounds = (int*)(d + o_rounds); ctl.stats = (unsigned long long*)(d + o_stats);
+  std::vector<hgk::Item> items;
+  std::vector<int> rem;
+  for (auto& b : batches) {
+    items.clear(); rem.clear();
+    long long words = 0, bmax = 0;
+    for (int k = b.first; k < b.second; ++k) {
+      hgk::Item it{};
+      it.off = offsets[k]; it.n = it.n_r = (int)(offsets[k + 1] - offsets[k]);
+      it.rem_off = (long long)rem.size(); it.used_off = words;
+      it.done = mh == 0; it.best_seed = -1; it.row = k;
+      for (int j = 0; j < it.n; ++j) rem.push_back(j);
+      words += (it.n + 31) / 32; bmax = std::max(bmax, (long long)it.n);
+      items.push_back(it);
+    }
+    const int nb = (int)items.size();
+    ctl.n_items = nb;
+    // the host vectors stay alive until the synchronise below (the copies read pageable memory when they run)
+    CK(cudaMemcpyAsync(ctl.items, items.data(), sizeof(hgk::Item) * nb, cudaMemcpyHostToDevice, st));
+    if (!rem.empty()) CK(cudaMemcpyAsync(ctl.rem, rem.data(), sizeof(int) * rem.size(), cudaMemcpyHostToDevice, st));
+    if (words) CK(cudaMemsetAsync(ctl.used, 0, sizeof(uint32_t) * words, st));
+    const int n_win = (int)((bmax + W - 1) / W);
+    const int item_blocks = (nb + hgk::kWarps - 1) / hgk::kWarps;
+    const int gb = (int)std::min<long long>(((long long)nb * W + hgk::kWarps - 1) / hgk::kWarps, grow_blocks);
+    for (int r = 0; r < mh; ++r) {
+      for (int w = 0; w < n_win; ++w) {
+        hgk::hg_grow_kernel<<<gb, 32 * hgk::kWarps, 0, st>>>(ctl, w);
+        hgk::hg_replay_kernel<<<item_blocks, 32 * hgk::kWarps, 0, st>>>(ctl, w);
+      }
+      hgk::hg_finish_kernel<<<item_blocks, 32 * hgk::kWarps, 0, st>>>(ctl);
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));   // `items` and `rem` are rewritten for the next batch
+  }
+  CK(cudaEventRecord(S.ev1, st));
+  std::vector<char> out(out_bytes);
+  CK(cudaMemcpyAsync(out.data(), d, out_bytes, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0;
+  CK(cudaEventElapsedTime(&ms, S.ev0, S.ev1));
+  S.last_ms = ms;
+  const unsigned long long* stats = (const unsigned long long*)(out.data() + o_stats);
+  const int* nh = (const int*)(out.data() + o_nh);
+  const int* rounds = (const int*)(out.data() + o_rounds);
+  const int* cnt = (const int*)(out.data() + o_cnt);
+  const int* inl = (const int*)(out.data() + o_inl);
+  S.stats[0] = (int64_t)stats[0]; S.stats[1] = (int64_t)stats[1];
+  for (int k = 0; k < n_items; ++k) {
+    n_h_out[k] = nh[k];
+    S.stats[2] += rounds[k];
+    if (rounds_out) rounds_out[k] = rounds[k];
+    long long stored = 0;
+    for (int h = 0; h < nh[k]; ++h) stored += cnt[(size_t)k * mh + h];
+    if (stored) std::memcpy(inl_out + offsets[k], inl + offsets[k], sizeof(int) * stored);
+  }
+  if (mh) {
+    std::memcpy(H_out, out.data() + o_H, sizeof(double) * 9 * rows);
+    std::memcpy(counts_out, cnt, sizeof(int) * rows);
+    if (trace_out) std::memcpy(trace_out, out.data() + o_tr, sizeof(int) * 3 * rows);
+  }
+  return B200M_OK;
+}
+
+extern "C" {
+
+int b200m_hgrowing_pairs(b200m_ctx* c, int n_items, const int64_t* offsets, const float* feat, double similarity_tolerance,
+                         double affinity_tolerance, double homography_tolerance, int min_inliers_to_refine, int nb_refining_iterations,
+                         int max_nb_homographies, int min_nb_matches_per_h, int32_t* n_homographies, double* H, int32_t* counts,
+                         int32_t* inliers, int32_t* trace, int32_t* rounds) {
+  auto tol_ok = [](double t) { return t >= 0 && t <= 1e150; };
+  if (!c || n_items < 0 || (n_items > 0 && (!offsets || !n_homographies || (max_nb_homographies > 0 && (!H || !counts)))))
+    return fail(B200M_ERR_ARG, "bad arguments");
+  if (!tol_ok(similarity_tolerance) || !tol_ok(affinity_tolerance) || !tol_ok(homography_tolerance))
+    return fail(B200M_ERR_ARG, "tolerances must be finite and non-negative");
+  if (min_inliers_to_refine < 1 || nb_refining_iterations < 0 || nb_refining_iterations > 64 || max_nb_homographies < 0 ||
+      max_nb_homographies > hgk::kMaxH || min_nb_matches_per_h < 0)
+    return fail(B200M_ERR_ARG, "parameters out of range: min_inliers_to_refine >= 1, nb_refining_iterations 0..64, max_nb_homographies 0..64, "
+                               "min_nb_matches_per_h >= 0");
+  if (n_items > 0 && offsets[0] != 0) return fail(B200M_ERR_ARG, "offsets[0] must be 0");
+  for (int k = 0; k < n_items; ++k) {
+    const int64_t n = offsets[k + 1] - offsets[k];
+    if (n < 0 || n > hgk::kMaxItem)
+      return fail(B200M_ERR_ARG, "item " + std::to_string(k) + ": offsets must ascend, at most " + std::to_string(hgk::kMaxItem) +
+                                     " putatives an item");
+  }
+  if (n_items > 0 && offsets[n_items] > 0 && (!feat || !inliers)) return fail(B200M_ERR_ARG, "bad arguments");
+  hg::Param p;
+  p.tol_similarity = similarity_tolerance; p.tol_affinity = affinity_tolerance; p.tol_homography = homography_tolerance;
+  p.min_inliers_to_refine = min_inliers_to_refine; p.nb_refining_iterations = nb_refining_iterations;
+  p.max_nb_homographies = max_nb_homographies; p.min_nb_matches_per_h = min_nb_matches_per_h;
+  return hgrowing_pairs(c, n_items, offsets, feat, p, n_homographies, H, counts, inliers, trace, rounds);
+}
+
+double b200m_hgrowing_last_stats(const b200m_ctx* c, int64_t stats[3]) {
+  if (!c) return 0;
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  if (stats) for (int t = 0; t < 3; ++t) stats[t] = c->hgr.stats[t];
+  return c->hgr.last_ms;
+}
+
+int b200m_ctx_set_hgrowing_window(b200m_ctx* c, int window) {
+  if (!c || window < 1 || window > 4096) return fail(B200M_ERR_ARG, "bad arguments: window 1..4096");
+  std::lock_guard<std::recursive_mutex> api_lock(c->api_mu);
+  c->hgr.window = window;
   return B200M_OK;
 }
 

@@ -40,7 +40,8 @@ ABI_SYMBOLS = [
     "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model", "b200m_set_view_geometry", "b200m_guided_match_fast_pairs",
     "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
     "b200m_mt19937_seed", "b200m_debug_rand_sample", "b200m_acransac_homography_pairs", "b200m_debug_rand_sample_k", "b200m_guided_match_pairs",
-    "b200m_guided_match_positions_pairs", "b200m_acransac_fundamental_spherical_pairs",
+    "b200m_guided_match_positions_pairs", "b200m_acransac_fundamental_spherical_pairs", "b200m_hgrowing_pairs", "b200m_hgrowing_last_stats",
+    "b200m_ctx_set_hgrowing_window",
 ]
 
 
@@ -79,6 +80,7 @@ def load_library() -> C.CDLL:
     lib.b200m_multi_last_gpu_ms.restype = C.c_double
     lib.b200m_multi_ctx.restype = C.c_void_p
     lib.b200m_acransac_last_stats.restype = C.c_double
+    lib.b200m_hgrowing_last_stats.restype = C.c_double
     for name in ("b200m_ctx_destroy", "b200m_db_destroy", "b200m_result_free", "b200m_multi_destroy", "b200m_mt19937_seed"):
         getattr(lib, name).restype = None
     _lib = lib
@@ -295,6 +297,47 @@ class Context:
         st = np.zeros(4, np.int64)
         ms = self.lib.b200m_acransac_last_stats(self._h, st.ctypes.data_as(C.c_void_p))
         return {"gpu_ms": ms, "models_evaluated": int(st[0]), "models_skipped": int(st[1]), "models_exact": int(st[2]), "launches": int(st[3])}
+
+    def set_hgrowing_window(self, window: int) -> None:
+        """Debug: seeds per item grown speculatively per window by hgrowing_pairs (default 256); 1 is the reference's loop.  Results
+        do not depend on it."""
+        _check(self.lib.b200m_ctx_set_hgrowing_window(self._h, C.c_int(int(window))), "b200m_ctx_set_hgrowing_window")
+
+    def hgrowing_pairs(self, items, param: dict | None = None) -> list[dict]:
+        """b200m_hgrowing_pairs: filterMatchesByHGrowing for every work item, one (pair, describer type) each: an n x 8 float32 array of
+        its putatives (xI, yI, scaleI, orientationI, xJ, yJ, scaleJ, orientationJ), in the caller's order.  param: HGrowingParam fields
+        (HGROWING_DEFAULTS).  Returns per item {"H": (n_h, 3, 3), "counts": (n_h,), "inliers": putative indices in outGeometricInliers
+        order, "trace": (rounds, 3): per round the chosen seed's position in the remaining list (-1: none grew) and the best set's size
+        before and after the refine}."""
+        q = dict(HGROWING_DEFAULTS, **(param or {}))
+        feats = [np.ascontiguousarray(f, np.float32).reshape(-1, 8) for f in items]
+        n = len(feats)
+        offsets = np.zeros(n + 1, np.int64)
+        offsets[1:] = np.cumsum([len(f) for f in feats])
+        feat = np.ascontiguousarray(np.concatenate(feats) if n else np.zeros((0, 8), np.float32), np.float32)
+        mh = int(q["maxNbHomographies"])
+        nh = np.zeros(max(n, 1), np.int32); rounds = np.zeros(max(n, 1), np.int32)
+        H = np.zeros((max(n, 1), max(mh, 1), 9)); counts = np.zeros((max(n, 1), max(mh, 1)), np.int32)
+        trace = np.zeros((max(n, 1), max(mh, 1), 3), np.int32); inl = np.zeros(max(int(offsets[-1]), 1), np.int32)
+        ptr = lambda a: a.ctypes.data_as(C.c_void_p)
+        _check(self.lib.b200m_hgrowing_pairs(self._h, C.c_int(n), ptr(offsets), ptr(feat), C.c_double(q["similarityTolerance"]),
+                                             C.c_double(q["affinityTolerance"]), C.c_double(q["homographyTolerance"]),
+                                             C.c_int(int(q["minInliersToRefine"])), C.c_int(int(q["nbRefiningIterations"])), C.c_int(mh),
+                                             C.c_int(int(q["minNbMatchesPerH"])), ptr(nh), ptr(H), ptr(counts), ptr(inl), ptr(trace), ptr(rounds)),
+               "b200m_hgrowing_pairs")
+        out = []
+        for k in range(n):
+            h = int(nh[k])
+            c = counts[k, :h].copy()
+            out.append({"H": H[k, :h].reshape(h, 3, 3).copy(), "counts": c, "inliers": inl[offsets[k]:offsets[k] + int(c.sum())].copy(),
+                        "trace": trace[k, :int(rounds[k])].copy()})
+        return out
+
+    def hgrowing_last_stats(self) -> dict:
+        """Instrumentation of the last hgrowing_pairs call."""
+        st = np.zeros(3, np.int64)
+        ms = self.lib.b200m_hgrowing_last_stats(self._h, st.ctypes.data_as(C.c_void_p))
+        return {"gpu_ms": ms, "seeds_grown": int(st[0]), "seeds_skipped": int(st[1]), "rounds": int(st[2])}
 
 
 def _mt_states(mt_state_or_states, n: int) -> np.ndarray:
@@ -589,6 +632,67 @@ def robustModelEstimation_H_AC(putatives: dict, regions_per_view: dict, image_si
             return ctx.guided_match_pairs(vp, Hs, th, distanceRatio * distanceRatio, MODEL_HOMOGRAPHY)
         _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry, run)
     return out, info
+
+
+# GrowParameters / HGrowingFilteringParam defaults (GeometricFilterMatrix_HGrowing.hpp:23-106); featureMatching never changes them
+HGROWING_DEFAULTS = dict(similarityTolerance=20.0, affinityTolerance=10.0, homographyTolerance=5.0, minInliersToRefine=6,
+                         nbRefiningIterations=8, maxNbHomographies=10, minNbMatchesPerH=20)
+# describer types whose presence among a pair's common types drops the pair (GeometricFilterMatrix_HGrowing.hpp, CCTag / AprilTag builds)
+HGROWING_TAG_TYPES = ("cctag3", "cctag4", "tag16h5")
+
+
+def _hgrowing_item(featuresI, featuresJ, matches) -> np.ndarray:
+    fi = np.asarray(featuresI, np.float32).reshape(-1, 4)
+    fj = np.asarray(featuresJ, np.float32).reshape(-1, 4)
+    return np.ascontiguousarray(np.concatenate([fi[matches["i"]], fj[matches["j"]]], axis=1), np.float32)
+
+
+def _hgrowing_split(r: dict, matches: np.ndarray):
+    bounds = np.concatenate([[0], np.cumsum(r["counts"])]).astype(np.int64)
+    return [(r["H"][k], matches[r["inliers"][bounds[k]:bounds[k + 1]]]) for k in range(len(r["counts"]))], matches[r["inliers"]]
+
+
+def filterMatchesByHGrowing(featuresI, featuresJ, putatives, param: dict | None = None, ctx: Context | None = None):
+    """filterMatchesByHGrowing (GeometricFilterMatrix_HGrowing.cpp:108-194) of one putative list on the GPU.  featuresI / featuresJ:
+    n x 4 float32 PointFeatures (x, y, scale, orientation); putatives: matches[MATCH_DTYPE] (or any array with "i" and "j" fields) in
+    the order the filter walks them.  Returns (homographiesAndMatches: [(H 3 x 3, matches)], outGeometricInliers)."""
+    ctx = ctx or default_context()
+    r = ctx.hgrowing_pairs([_hgrowing_item(featuresI, featuresJ, putatives)], param)[0]
+    return _hgrowing_split(r, putatives)
+
+
+def robustModelEstimation_HGrowing(putatives: dict, features_per_view: dict, guidedMatching: bool = False, param: dict | None = None,
+                                   desc_types=None, ctx: Context | None = None):
+    """matchingImageCollection::robustModelEstimation with GeometricFilterMatrix_HGrowing (the `homography_growing` filter of
+    featureMatching) for a whole putative list, with one engine call for every (pair, describer type):
+      putatives          {(I, J): {describer type: matches[MATCH_DTYPE]}}, used in the caller's order (featureMatching sorts each list
+                         by Lowe ratio first: matches_filtering.sortMatches_byDistanceRatio)
+      features_per_view  {view: {describer type: n x 4 float32 (x, y, scale, orientation)}}, as regions_io.loadFeatsFromFile returns them
+    The stage rules of geometricEstimation (GeometricFilterMatrix_HGrowing.hpp:176-266): every common type with a putative entry is
+    filtered and gets an entry, even an empty one, and such a pair is kept; a pair with a CCTag or AprilTag type among its common types
+    is dropped; with guidedMatching the kept pair's lists become an empty map (Geometry_guided_matching is an empty stub).
+    Returns (geometric matches {(I, J): {type: matches}}, {(I, J): {type: [(H, matches)]}} like the reference's _HsAndMatchesPerDesc)."""
+    ctx = ctx or default_context()
+    order = list(desc_types) if desc_types is not None else DESCRIBER_TYPES
+    work, items = [], []
+    for (I, J), per_type in putatives.items():
+        common = [t for t in order if t in features_per_view[I] and t in features_per_view[J]]
+        if any(t in HGROWING_TAG_TYPES for t in common):
+            continue
+        for t in common:
+            if t in per_type:
+                work.append(((I, J), t))
+                items.append(_hgrowing_item(features_per_view[I][t], features_per_view[J][t], per_type[t]))
+    res = ctx.hgrowing_pairs(items, param) if items else []
+    out, hs = {}, {}
+    for (p, t), r in zip(work, res):
+        m = putatives[p][t]
+        h_list, inl = _hgrowing_split(r, m)
+        hs.setdefault(p, {})[t] = h_list
+        out.setdefault(p, {})
+        if not guidedMatching:
+            out[p][t] = inl
+    return out, hs
 
 
 _default_ctx: dict[int, Context] = {}

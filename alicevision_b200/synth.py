@@ -170,3 +170,46 @@ def vocabulary_tree(k: int = 8, levels: int = 3, seed: int = 4, pool: np.ndarray
                 valid[start + g * k + k - invalid_tail:start + (g + 1) * k] = 0
             start += cnt
     return centers, valid
+
+
+def planar_views(n_views: int, n_points: int, planes: int = 2, dtype=np.uint8, seed: int = SEED_DATA, visible: float = 1.0,
+                 fresh: float = 0.3, noise: int = 4, ring: bool = False):
+    """A multi-plane scene seen by n_views cameras, for the homography-growing filter.  Returns (descs, feats): per view an (m,128)
+    ``dtype`` array and an (m,4) float32 array of PointFeatures (x, y, scale, orientation).  Each world point lies on one of `planes`
+    planes; view v maps plane p by its own homography, so every pair of views relates each plane by a homography, and each feature's
+    scale and orientation follow that homography's local affinity.  A view sees a seeded `visible` fraction of the points (descriptor
+    +-noise per component) and adds a `fresh` fraction of unrelated features.  ring=True: the points and the views lie on a circle and
+    a view sees the points within a `visible` fraction of the circle around it, so only nearby views share points."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    pool = sift_pool(n_points, rng)
+    plane = rng.integers(0, planes, n_points)
+    base = np.c_[rng.uniform(0, 2000, (n_points, 2)), rng.uniform(1.5, 8, n_points), rng.uniform(-np.pi, np.pi, n_points)]
+    angle = rng.uniform(0, 1, n_points)
+    descs, feats = [], []
+    for v in range(n_views):
+        Hs = []
+        for _ in range(planes):
+            th, s = rng.uniform(-0.2, 0.2), rng.uniform(0.85, 1.15)
+            Hs.append(np.array([[s * np.cos(th), -s * np.sin(th), rng.uniform(-150, 150)], [s * np.sin(th), s * np.cos(th), rng.uniform(-150, 150)],
+                                [rng.uniform(-5e-5, 5e-5), rng.uniform(-5e-5, 5e-5), 1.0]]))
+        if ring:
+            d_ang = np.abs((angle - v / n_views + 0.5) % 1.0 - 0.5)
+            sel = np.flatnonzero(d_ang < visible / 2)
+        else:
+            sel = np.flatnonzero(rng.uniform(0, 1, n_points) < visible)
+        f = np.zeros((len(sel), 4))
+        for r, i in enumerate(sel):
+            H = Hs[plane[i]]
+            x = np.array([base[i, 0], base[i, 1], 1.0])
+            X = H @ x
+            A = (H[:2, :2] * X[2] - np.outer(X[:2], H[2, :2])) / X[2] ** 2
+            F = A @ (base[i, 2] * np.array([[np.cos(base[i, 3]), -np.sin(base[i, 3])], [np.sin(base[i, 3]), np.cos(base[i, 3])]]))
+            f[r] = [X[0] / X[2], X[1] / X[2], np.sqrt(abs(np.linalg.det(F))), np.arctan2(F[1, 0] - F[0, 1], F[0, 0] + F[1, 1])]
+        d = np.clip(pool[sel].astype(np.int16) + rng.integers(-noise, noise + 1, size=(len(sel), 128), dtype=np.int16), 0, 255)
+        k = int(len(sel) * fresh)
+        d = np.concatenate([d, np.clip(sift_pool(k, rng), 0, 255)])
+        f = np.concatenate([f, np.c_[rng.uniform(0, 2000, (k, 2)), rng.uniform(1.5, 8, k), rng.uniform(-np.pi, np.pi, k)]])
+        order = rng.permutation(len(d))
+        descs.append(np.ascontiguousarray(d[order].astype(dtype)))
+        feats.append(np.ascontiguousarray(f[order].astype(np.float32)))
+    return descs, feats

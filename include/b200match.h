@@ -272,6 +272,32 @@ double b200m_acransac_last_stats(const b200m_ctx* ctx, int64_t stats[4]);
 int b200m_acransac_last_trace(const b200m_ctx* ctx, int pair, int32_t* iters, double* nfa, int cap);
 /* debug, every model: 1 (default) = certified skip of models that cannot beat the running minNFA; 0 = score every model exactly */
 int b200m_ctx_set_acransac_skip(b200m_ctx* ctx, int on);
+/* ---- geometric filtering: homography growing (K12) ------------------------------------------------------------------ */
+/* filterMatchesByHGrowing (GeometricFilterMatrix_HGrowing.cpp:108-194, the homography_growing filter) for every work item of a list,
+ * results in input order.  A work item is one (pair, describer type) with its putatives in the caller's order:
+ *   offsets    n_items + 1 ascending, offsets[0] = 0; item k owns putatives offsets[k] .. offsets[k + 1] - 1, at most 262144
+ *   feat       offsets[n_items] x 8 floats: xI, yI, scaleI, orientationI, xJ, yJ, scaleJ, orientationJ (the two PointFeatures)
+ *   parameters GrowParameters (tolerances >= 0 and finite, min_inliers_to_refine >= 1, nb_refining_iterations 0..64) and
+ *              HGrowingFilteringParam (max_nb_homographies 0..64, min_nb_matches_per_h >= 0); the reference's defaults are
+ *              20, 10, 5, 6, 8, 10, 20
+ * Outputs (max_h = max_nb_homographies):
+ *   n_homographies[n_items]; H[n_items x max_h x 9] (row-major, x_J ~ H x_I); counts[n_items x max_h];
+ *   inliers[offsets[n_items]]: item k's stored matches as putative indices (0-based within the item) from inliers[offsets[k]] on, in
+ *              outGeometricInliers order (homography by homography, each in putative order); the rest of its range is left as is
+ *   trace[n_items x max_h x 3] or NULL: per round, the chosen seed's position in that round's remaining list (-1: no seed grew, which
+ *              ends the item) and the best set's size before and after refineHomography
+ *   rounds[n_items] or NULL: the rounds each item ran
+ * The whole list is checked before anything runs; a bad argument returns B200M_ERR_ARG and queues nothing. */
+int b200m_hgrowing_pairs(b200m_ctx* ctx, int n_items, const int64_t* offsets, const float* feat, double similarity_tolerance,
+                         double affinity_tolerance, double homography_tolerance, int min_inliers_to_refine, int nb_refining_iterations,
+                         int max_nb_homographies, int min_nb_matches_per_h, int32_t* n_homographies, double* H, int32_t* counts,
+                         int32_t* inliers, int32_t* trace, int32_t* rounds);
+/* instrumentation of the last b200m_hgrowing_pairs: stats = {seeds grown (speculative grows included), seeds the reference skips as
+ * already used, rounds over all items}; returns its GPU time in ms */
+double b200m_hgrowing_last_stats(const b200m_ctx* ctx, int64_t stats[3]);
+/* debug: seeds per item grown speculatively per window (default 256, 1..4096); 1 is the reference's sequential loop.  Results do not
+ * depend on it. */
+int b200m_ctx_set_hgrowing_window(b200m_ctx* ctx, int window);
 /* host only: std::mt19937(seed) as 625 words (see mt_state) */
 void b200m_mt19937_seed(uint32_t seed, uint32_t state[625]);
 /* host only (debug): the engine's sampler on the CPU.  `draws` consecutive randSample(g, 0, range, 7) from `state`: the samples in
