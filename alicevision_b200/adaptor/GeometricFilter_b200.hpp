@@ -7,6 +7,8 @@
 // support rules, then one
 // guided-matching call for every kept pair and common descriptor type (b200m_guided_match_pairs, or for H with distanceRatio < 0
 // b200m_guided_match_positions_pairs).
+// GeometricFilterMatrix_E_AC_Batch_b200 does the same for the `essential_matrix` filter (GeometricFilterMatrix_E_AC.hpp, pinhole pairs):
+// one b200m_acransac_essential_pairs call, then guided matching with F = K_J^-T E K_I^-1.
 // GeometricFilterMatrix_HGrowing_Batch_b200 does the same for the `homography_growing` filter (GeometricFilterMatrix_HGrowing.hpp:176-266,
 // filterMatchesByHGrowing): one b200m_hgrowing_pairs call for every (pair, common describer type) of the list.
 // Header-only; compiled inside an AliceVision build and linked against libb200match.so.  The caller gathers xI / xJ with the
@@ -473,6 +475,132 @@ public:
 
 private:
     std::vector<Estimate> _estimates;
+};
+
+/// robustModelEstimation with GeometricFilterMatrix_E_AC (ACRANSAC, Essential5PSolver on K^-1 x, FundamentalEpipolarDistanceError of
+/// F = K_J^-T E K_I^-1 on the pixels; GeometricFilterMatrix_E_AC.hpp) for the pairs added (addView of the base, addPairCalibrated),
+/// then run().
+class GeometricFilterMatrix_E_AC_Batch_b200 : public GeometricFilterBatchBase_b200
+{
+public:
+    /// What the estimation of one pair gave (in addPairCalibrated order): ACRANSAC's validity, E (row-major), errorMax
+    /// (m_dPrecision_robust, in pixels; infinite when not valid) and the support decision.
+    struct Estimate
+    {
+        bool valid = false, strongSupport = false;
+        double E[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        double errorMax = std::numeric_limits<double>::infinity();
+    };
+
+    explicit GeometricFilterMatrix_E_AC_Batch_b200(b200m_ctx* ctx = matching::b200detail::sharedContext())
+      : GeometricFilterBatchBase_b200(ctx)
+    {}
+
+    /// addPair with the pair's two camera::Pinhole::K() (row-major, 9 doubles each).  A pair the reference does not estimate (no
+    /// common describer type, a missing or non-pinhole intrinsic) is simply not added.
+    template<class MatT>
+    void addPairCalibrated(const Pair& pair,
+                           const matching::MatchesPerDescType& putatives,
+                           const std::vector<feature::EImageDescriberType>& descTypes,
+                           const MatT& xI,
+                           const MatT& xJ,
+                           const std::pair<std::size_t, std::size_t>& sizeI,
+                           const std::pair<std::size_t, std::size_t>& sizeJ,
+                           const double KI[9],
+                           const double KJ[9])
+    {
+        addPair(pair, putatives, descTypes, xI, xJ, sizeI, sizeJ);
+        _K.insert(_K.end(), KI, KI + 9);
+        _K.insert(_K.end(), KJ, KJ + 9);
+    }
+
+    /// robustModelEstimation over every pair added so far.  ACRANSAC's precision is Square(precision), as the filter passes
+    /// upperBoundPrecision = Square(m_dPrecision) (the residual threshold is then precision^4).  Every pair starts from `rng`: the
+    /// reference hands one generator from pair to pair by reference, shared by featureMatching's OpenMP threads in no fixed order, so
+    /// no run of it is reproducible.  Pairs with strong support (hasStrongSupport(.., 5)) enter out; with guidedMatching their lists
+    /// are guidedMatching's with F = K_J^-T E K_I^-1, errorTh = errorMax^2 and distRatio = distanceRatio^2 (every common type, empty
+    /// lists included; nothing when errorMax is infinite).  Returns false (out untouched) when the engine is unavailable or fails.
+    bool run(const std::mt19937& rng, std::size_t maxIteration, double precision, bool guidedMatching, double distanceRatio,
+             matching::PairwiseMatches& out)
+    {
+        if (!available())
+            return false;
+        const int n = (int)_pairs.size();
+        uint32_t state[625];
+        b200detail::mtState(rng, state);
+        K10Out r(_pairs, _corr.size() / 4);
+        if (n > 0 && b200m_acransac_essential_pairs(_ctx, n, r.offsets.data(), corrData(), _wh.data(), _K.data(), state, 0, (int64_t)maxIteration,
+                                                    precision * precision, r.valid.data(), r.nInl.data(), r.inl.data(), r.M.data(),
+                                                    r.errMax.data(), r.nfa.data(), r.iters.data(), nullptr) != B200M_OK)
+            return false;
+        _estimates.assign(n, Estimate());
+        _F.assign(9 * n, 0.0);
+        std::map<Pair, matching::MatchesPerDescType> result;
+        std::vector<int> kept;
+        std::vector<double> errorMax(n, std::numeric_limits<double>::infinity());
+        for (int k = 0; k < n; ++k)
+        {
+            Estimate& e = _estimates[k];
+            e.valid = r.valid[k] != 0;
+            std::copy(r.M.begin() + 9 * k, r.M.begin() + 9 * k + 9, e.E);
+            if (!e.valid)
+                continue;
+            e.errorMax = errorMax[k] = r.errMax[k];
+            fundamentalFromEssential(e.E, &_K[18 * k], &_K[18 * k + 9], &_F[9 * k]);
+            e.strongSupport = keepInliers(k, r, k, 5, result);             // Essential5PSolver::getMinimumNbRequiredSamples
+            if (e.strongSupport)
+                kept.push_back(k);
+        }
+        if (guidedMatching &&
+            !guided(kept, errorMax, [&](int k) { return &_F[9 * k]; },
+                    [&](const uint32_t* ids, int np, const double* M, const double* th, b200m_result** res) {
+                        return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distanceRatio * distanceRatio, res);
+                    },
+                    result))
+            return false;
+        for (auto& x : result)
+            out[x.first] = std::move(x.second);
+        return true;
+    }
+
+    /// The estimation of the k-th pair added, after run().
+    const Estimate& estimate(std::size_t k) const { return _estimates.at(k); }
+
+    /// fundamentalFromEssential (multiview/essential.cpp): F = K_J^-T E K_I^-1, formed as (K_J^-T E) K_I^-1 with the engine's cofactor
+    /// inverse; all row-major.
+    static void fundamentalFromEssential(const double E[9], const double KI[9], const double KJ[9], double F[9])
+    {
+        double iI[9], iJ[9], T[9];
+        inverse3(KI, iI);
+        inverse3(KJ, iJ);
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c)
+                T[3 * r + c] = (iJ[r] * E[c] + iJ[3 + r] * E[3 + c]) + iJ[6 + r] * E[6 + c];
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c)
+                F[3 * r + c] = (T[3 * r] * iI[c] + T[3 * r + 1] * iI[3 + c]) + T[3 * r + 2] * iI[6 + c];
+    }
+
+private:
+    /// M^-1 by cofactors over the determinant expanded along the first column
+    static void inverse3(const double M[9], double R[9])
+    {
+        double C[9];
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j)
+            {
+                const int i1 = (i + 1) % 3, i2 = (i + 2) % 3, j1 = (j + 1) % 3, j2 = (j + 2) % 3;
+                C[3 * i + j] = M[3 * i1 + j1] * M[3 * i2 + j2] - M[3 * i1 + j2] * M[3 * i2 + j1];
+            }
+        const double inv = 1.0 / ((C[0] * M[0] + C[3] * M[3]) + C[6] * M[6]);
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j)
+                R[3 * i + j] = C[3 * j + i] * inv;
+    }
+
+    std::vector<Estimate> _estimates;
+    std::vector<double> _K;   // 18 per pair: K_I, K_J
+    std::vector<double> _F;   // 9 per pair: the guided step's F
 };
 
 /// robustModelEstimation with GeometricFilterMatrix_HGrowing (the `homography_growing` filter: filterMatchesByHGrowing on the

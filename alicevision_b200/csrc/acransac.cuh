@@ -1,11 +1,12 @@
 // K10: a-contrario RANSAC estimation for a list of pairs, sm_90a: the fundamental matrix (b200m_acransac_fundamental_pairs,
 // FPolicy), the homography (b200m_acransac_homography_pairs, HPolicy) and the fundamental matrix of two equidistant cameras on
-// lifted unit vectors (b200m_acransac_fundamental_spherical_pairs, SPolicy).  The kernel is one template over the model policy.
+// lifted unit vectors (b200m_acransac_fundamental_spherical_pairs, SPolicy) and the essential matrix of two pinhole cameras
+// (b200m_acransac_essential_pairs, EPolicy).  The kernel is one template over the model policy.
 //
 // One CTA runs one pair's robustEstimation::ACRANSAC loop (robustEstimation/ACRansac.hpp:186-272) iteration by iteration, with the
 // reference's control flow (10 % reserve, strict `<` on minNFA, the switch to sampling among the inliers, the "no model at all"
 // extension, the precision mode and its early exit).  Per iteration thread 0 draws the sample from the pair's own copy of the
-// caller's std::mt19937 (shared memory) and fits the models (7-point F or 4-point H, acransac_math.h); then the whole CTA scores
+// caller's std::mt19937 (shared memory) and fits the models (7-point F, 4-point H or 5-point E, acransac_math.h); then the whole CTA scores
 // each model:
 //   * n residuals (F: point-to-line error, H: point-to-point transfer error, on normalised points; S: (F x_I . x_J)^2 on bearings);
 //   * certified skip: a shared-memory histogram of the residuals over quarter-binade bins gives, for every k, a lower bound of the
@@ -32,6 +33,7 @@ constexpr int kBins = 2 + 4 * 128; // ... up to 2^28; the last bin holds everyth
 constexpr int kTraceCap = 256;      // `better` events (iteration, new minNFA) kept per pair (b200m_acransac_last_trace)
 
 struct Pair { long long off, sort_off; int n, w1, h1, w2, h2; };
+struct PairE { Pair q; double kinv[18]; };   // EPolicy's pair: K_I^-1 then K_J^-1, row-major
 struct Out {
   double model[9]; double error_max, min_nfa;
   long long evaluated, skipped, exact;
@@ -52,11 +54,12 @@ __device__ __forceinline__ double bin_low(int b) {
 }
 
 // Model policies: sample size, maximum number of models, fit, residual, logalpha0, errorVectorDimension, unnormaliser, and the
-// correspondence layout: kPlanar = pixel pairs (xI, yI, xJ, yJ) preconditioned by the image sizes, else lifted unit vectors
-// (xI, yI, zI, xJ, yJ, zJ) used as given; kWidth doubles per correspondence.
+// correspondence layout: kPlanar = pixel pairs (xI, yI, xJ, yJ) preconditioned by the image sizes; kCalibrated = pixel pairs
+// followed by their K^-1-normalised copies (xI, yI, xJ, yJ, uI, vI, uJ, vJ), fitted on the copies, scored on the pixels; else
+// lifted unit vectors (xI, yI, zI, xJ, yJ, zJ) used as given; kWidth doubles per correspondence.
 struct FPolicy {   // RelativePoseKernel<Fundamental7PSolver, FundamentalEpipolarDistanceError, UnnormalizerT>
   static constexpr int kSample = acr::kSample, kMaxModels = acr::kMaxModels, kErrDim = 1, kWidth = 4;
-  static constexpr bool kPlanar = true;
+  static constexpr bool kPlanar = true, kCalibrated = false;
   __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) {
     return acr::fit7_solve<false>(a, b, c, d, m);   // = acr::fit7, one inlining level shallower
   }
@@ -68,7 +71,7 @@ struct FPolicy {   // RelativePoseKernel<Fundamental7PSolver, FundamentalEpipola
 };
 struct HPolicy {   // RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError, UnnormalizerI>, point to point
   static constexpr int kSample = acr::kSampleH, kMaxModels = acr::kMaxModelsH, kErrDim = 2, kWidth = 4;
-  static constexpr bool kPlanar = true;
+  static constexpr bool kPlanar = true, kCalibrated = false;
   __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) { return acr::fit4(a, b, c, d, m); }
   __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::homography_error(m, x1, y1, x2, y2); }
   __device__ static double logalpha0(int w2, int h2, const acr::Norm& n2) { return acr::logalpha0_h(w2, h2, n2); }
@@ -76,19 +79,36 @@ struct HPolicy {   // RelativePoseKernel<Homography4PSolver, HomographyAsymmetri
 };
 struct SPolicy {   // RelativePoseSphericalKernel<Fundamental7PSphericalSolver, EpipolarSphericalDistanceError>
   static constexpr int kSample = acr::kSample, kMaxModels = acr::kMaxModels, kErrDim = 2, kWidth = 6;
-  static constexpr bool kPlanar = false;
+  static constexpr bool kPlanar = false, kCalibrated = false;
   __device__ static int fit(const double* x1, const double* x2, double* m) { return acr::fit7s(x1, x2, m); }
   __device__ static double error(const double* m, const double* x1, const double* x2) { return acr::spherical_error(m, x1, x2); }
   __device__ static double logalpha0(int, int, const acr::Norm&) { return M_PI; }   // the value itself, not its log10
   __device__ static void unnormalize(const acr::Norm&, const acr::Norm&, double*) {}
 };
+struct EPolicy {   // RelativePoseKernel_K<Essential5PSolver, FundamentalEpipolarDistanceError, Mat3Model>
+  // models[] holds F = K_J^-T E K_I^-1 of each model for the residuals, then the Es.  errorVectorDimension is 0.5, which the int
+  // kErrDim of the other policies cannot hold: nfa_of applies it under `if constexpr (P::kCalibrated)`, and kErrDim = 0 is unused.
+  static constexpr int kSample = acr::kSampleE, kMaxModels = acr::kMaxModelsE, kErrDim = 0, kWidth = 8;
+  static constexpr bool kPlanar = false, kCalibrated = true;
+  __device__ static int fit(const double* a, const double* b, const double* c, const double* d, const double* kinv, double* m) {
+    double* E = m + 9 * kMaxModels;
+    const int nb = acr::fit5(a, b, c, d, E);
+    for (int k = 0; k < nb; ++k) acr::fundamental_from_essential(E + 9 * k, kinv, kinv + 9, m + 9 * k);
+    return nb;
+  }
+  __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::epipolar_error(m, x1, y1, x2, y2); }
+  __device__ static double logalpha0(int w2, int h2, const acr::Norm&) { return acr::logalpha0_e(w2, h2); }
+  __device__ static void unnormalize(const acr::Norm&, const acr::Norm&, double*) {}
+};
 
 // NFA(k) of bestNFA for the squared residual e of rank k: loge0 + (la0 + d log10(sqrt(e) + FLT_EPSILON)) (k - kSample) + logc_n[k]
-// + logc_k[k], d = errorVectorDimension (1: F, 2: H and S; the product by 2 is exact)
+// + logc_k[k], d = errorVectorDimension (1: F, 2: H and S, 0.5: E; the products are exact)
 template <class P>
 __device__ __forceinline__ double nfa_of(double e, int k, double la0, double loge0, const float* lcn, const float* lck) {
   const double l = log10(acr::add(sqrt(e), (double)FLT_EPSILON));
-  const double la = acr::add(la0, P::kErrDim == 1 ? l : acr::mul((double)P::kErrDim, l));
+  double la;
+  if constexpr (P::kCalibrated) la = acr::add(la0, acr::mul(0.5, l));
+  else la = acr::add(la0, P::kErrDim == 1 ? l : acr::mul((double)P::kErrDim, l));
   return acr::add(acr::add(acr::add(loge0, acr::mul(la, (double)(k - P::kSample))), (double)lcn[k]), (double)lck[k]);
 }
 
@@ -139,6 +159,9 @@ __device__ __forceinline__ double residual(const double* M, const double* pts, i
   if constexpr (P::kPlanar) {
     const double2 a = reinterpret_cast<const double2*>(pts)[2 * i], b = reinterpret_cast<const double2*>(pts)[2 * i + 1];
     return P::error(M, a.x, a.y, b.x, b.y);
+  } else if constexpr (P::kCalibrated) {   // the pixel half of the correspondence
+    const double2 a = reinterpret_cast<const double2*>(pts)[4 * i], b = reinterpret_cast<const double2*>(pts)[4 * i + 1];
+    return P::error(M, a.x, a.y, b.x, b.y);
   } else {   // 48 bytes a correspondence: three aligned 16-byte loads
     const double2* q = reinterpret_cast<const double2*>(pts) + 3 * i;
     const double2 a = q[0], b = q[1], c = q[2];
@@ -147,8 +170,8 @@ __device__ __forceinline__ double residual(const double* M, const double* pts, i
   }
 }
 
-// corr: per correspondence P::kWidth doubles at the pair's offset, (xI, yI, xJ, yJ) or (xI, yI, zI, xJ, yJ, zJ); l10[k] =
-// (float)log10((double)k) for k <= the largest n.
+// corr: per correspondence P::kWidth doubles at the pair's offset, (xI, yI, xJ, yJ) or (xI, yI, zI, xJ, yJ, zJ); 4 doubles
+// (xI, yI, xJ, yJ) for EPolicy, whose pairs are PairE; l10[k] = (float)log10((double)k) for k <= the largest n.
 // Scratch at the pair's offset: pts (P::kWidth doubles), idx (the sampling list), logc (n + 1 floats each of logc_n and logc_k, at
 // 2 * (off + pair)), gkeys / gvals (pow2(n) at sort_off, pairs above kSmemSort only).  inliers: the result list at the offset.
 // mt_state: 625 words at p * mt_stride (mt_stride 0: one state for every pair); mt_out: NULL, or 625 words per pair receiving the
@@ -161,7 +184,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
                                                              uint32_t* gvals, uint32_t* inliers_all, int* trace_all, double* trace_nfa_all,
                                                              Out* out_all, uint32_t* mt_out) {
   __shared__ acr::Mt19937 g;
-  __shared__ double models[9 * P::kMaxModels], bestF[9];
+  __shared__ double models[9 * P::kMaxModels * (P::kCalibrated ? 2 : 1)], bestF[9];
   __shared__ int hist[kBins];
   __shared__ unsigned long long skeys[kSmemSort];
   __shared__ uint32_t svals[kSmemSort];
@@ -172,7 +195,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
   __shared__ double minNFA, errorMax;
 
   const int p = blockIdx.x, tid = threadIdx.x;
-  const Pair Q = pairs[p];
+  const Pair Q = P::kCalibrated ? reinterpret_cast<const PairE*>(pairs)[p].q : pairs[p];
   const int n = Q.n;
   Out* out = out_all + p;
   const double inf = __longlong_as_double(0x7ff0000000000000ll);
@@ -194,9 +217,14 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
   uint32_t* inl = inliers_all + Q.off;
   float* lcn = logc_all + 2 * (Q.off + p);
   float* lck = lcn + n + 1;
-  const double* c = corr + P::kWidth * Q.off;
+  const double* c = corr + (P::kCalibrated ? 4 : P::kWidth) * Q.off;
+  const double* kinv = P::kCalibrated ? reinterpret_cast<const PairE*>(pairs)[p].kinv : nullptr;
   for (int i = tid; i < n; i += kThreads) {
-    if constexpr (P::kPlanar) {
+    if constexpr (P::kCalibrated) {   // RelativePoseKernel_K's constructor: the pixels, and K^-1 applied to them
+      for (int t = 0; t < 4; ++t) pts[8 * i + t] = c[4 * i + t];
+      acr::transform_point(kinv, c[4 * i], c[4 * i + 1], pts[8 * i + 4], pts[8 * i + 5]);
+      acr::transform_point(kinv + 9, c[4 * i + 2], c[4 * i + 3], pts[8 * i + 6], pts[8 * i + 7]);
+    } else if constexpr (P::kPlanar) {
       pts[4 * i] = acr::norm_x(n1, c[4 * i]); pts[4 * i + 1] = acr::norm_y(n1, c[4 * i + 1]);
       pts[4 * i + 2] = acr::norm_x(n2, c[4 * i + 2]); pts[4 * i + 3] = acr::norm_y(n2, c[4 * i + 3]);
     } else {
@@ -254,6 +282,13 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
             a[i] = pts[4 * j]; b[i] = pts[4 * j + 1]; cc[i] = pts[4 * j + 2]; d[i] = pts[4 * j + 3];
           }
           nb = P::fit(a, b, cc, d, models);
+        } else if constexpr (P::kCalibrated) {
+          double a[P::kSample], b[P::kSample], cc[P::kSample], d[P::kSample];
+          for (int i = 0; i < P::kSample; ++i) {
+            const uint32_t j = mode ? idx[s[i]] : s[i];
+            a[i] = pts[8 * j + 4]; b[i] = pts[8 * j + 5]; cc[i] = pts[8 * j + 6]; d[i] = pts[8 * j + 7];
+          }
+          nb = P::fit(a, b, cc, d, kinv, models);
         } else {
           double x1[3 * P::kSample], x2[3 * P::kSample];
           for (int i = 0; i < P::kSample; ++i) {
@@ -331,7 +366,8 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
         if (tid == 0) {
           better = 1; minNFA = bv; n_inl = bk;
           errorMax = __longlong_as_double((long long)K[bk - 1]);
-          for (int t = 0; t < 9; ++t) bestF[t] = F[t];
+          const double* Mo = P::kCalibrated ? models + 9 * (P::kMaxModels + m) : F;   // E: the fitted model, not its F
+          for (int t = 0; t < 9; ++t) bestF[t] = Mo[t];
           if (n_trace < kTraceCap) {
             trace_all[(long long)p * kTraceCap + n_trace] = (int)iter;
             trace_nfa_all[(long long)p * kTraceCap + n_trace] = bv;
@@ -364,7 +400,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
     double Fo[9];
     for (int t = 0; t < 9; ++t) Fo[t] = bestF[t];
     double em = errorMax;
-    if (valid) {   // unormalizeError: sqrt(e) / s2 (planar), sqrt(e) (bearings)
+    if (valid) {   // unormalizeError: sqrt(e) / s2 (planar), sqrt(e) (bearings, calibrated)
       P::unnormalize(n1, n2, Fo);
       if constexpr (P::kPlanar) em = sqrt(em) / n2.s;
       else em = sqrt(em);

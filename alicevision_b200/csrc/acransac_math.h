@@ -10,7 +10,10 @@
 //   * the spherical F kernel of RelativePoseSphericalKernel<Fundamental7PSphericalSolver, EpipolarSphericalDistanceError> for two
 //     equidistant cameras: the same 7-point null space and cubic on the rows of lifted unit vectors, the error (F x1 . x2)^2;
 //   * the H kernel of RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError, UnnormalizerI> (point-to-point): the same
-//     preconditioning, the 4-point DLT and its 1-D null space, the asymmetric transfer error and the unnormalisation N2^-1 H N1.
+//     preconditioning, the 4-point DLT and its 1-D null space, the asymmetric transfer error and the unnormalisation N2^-1 H N1;
+//   * the E kernel of RelativePoseKernel_K<Essential5PSolver, FundamentalEpipolarDistanceError> for two pinhole cameras: the 5-point
+//     solver (null space, constraint matrix, full-pivot LU, action matrix, and Eigen's RealSchur / EigenSolver restated for it)
+//     on K^-1 x, and F = K_J^-T E K_I^-1 for the point-to-line error on pixels.
 // The same code runs in the engine (device) and in the oracle's restated kernels (host, -ffp-contract=off), so the two differ
 // only through acos / cos / pow / log10.  Device double arithmetic goes through __dmul_rn / __dadd_rn / __dsub_rn so that no
 // product is contracted into an FMA.
@@ -418,5 +421,504 @@ ACR_HD void unnormalize_h(const Norm& n1, const Norm& n2, double H[9]) {
 
 // logalpha0 of the point-to-point error: log10(pi / (w2 h2) / s2^2), the unit circle over the image area in normalised units
 ACR_HD double logalpha0_h(int w2, int h2, const Norm& n2) { return log10(M_PI / mul((double)w2, (double)h2) / mul(n2.s, n2.s)); }
+
+// ---------------------------------------------------------------------------------------------------------------- E kernel
+// RelativePoseKernel_K<Essential5PSolver, FundamentalEpipolarDistanceError, Mat3Model> of two pinhole cameras: the fit runs on
+// K^-1 x (applyTransformationToPoints, once per pair), the residual is the point-to-line error of F = K_J^-T E K_I^-1 on the pixel
+// points; no normaliser (thresholdNormalizer = 1, unormalizeError = sqrt), errorVectorDimension = 0.5,
+// logalpha0 = log10(2 D / A * .5) of the raw w_J, h_J.
+constexpr int kSampleE = 5;       // Essential5PSolver::getMinimumNbRequiredSamples
+constexpr int kMaxModelsE = 10;   // Essential5PSolver::getMaximumNbModels
+
+ACR_HD double logalpha0_e(int w2, int h2) {
+  const double D = sqrt(add(mul((double)w2, (double)w2), mul((double)h2, (double)h2)));
+  const double A = mul((double)w2, (double)h2);
+  return log10(mul(mul(2.0, D) / A, .5));
+}
+
+// applyTransformationToPoints(x, T): (T (x, y, 1))_{0,1} / (T (x, y, 1))_2
+ACR_HD void transform_point(const double T[9], double x, double y, double& u, double& v) {
+  const double a = add(add(mul(T[0], x), mul(T[1], y)), T[2]);
+  const double b = add(add(mul(T[3], x), mul(T[4], y)), T[5]);
+  const double c = add(add(mul(T[6], x), mul(T[7], y)), T[8]);
+  u = a / c;
+  v = b / c;
+}
+
+// fundamentalFromEssential: F = K_J^-T E K_I^-1, formed as (K_J^-T E) K_I^-1; all three row-major
+ACR_HD void fundamental_from_essential(const double E[9], const double KIinv[9], const double KJinv[9], double F[9]) {
+  double T[9];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) T[r * 3 + c] = add(add(mul(KJinv[r], E[c]), mul(KJinv[3 + r], E[3 + c])), mul(KJinv[6 + r], E[6 + c]));
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) F[r * 3 + c] = add(add(mul(T[r * 3], KIinv[c]), mul(T[r * 3 + 1], KIinv[3 + c])), mul(T[r * 3 + 2], KIinv[6 + c]));
+}
+
+namespace e5 {
+constexpr int N = 10;   // the action matrix is 10 x 10
+constexpr double kEps = 2.220446049250313e-16;       // NumTraits<double>::epsilon()
+constexpr double kMin = 2.2250738585072014e-308;     // std::numeric_limits<double>::min()
+
+// Essential5PSolver's monomials (Pc::coef_*): cubic 0..9, then xx xy yy xz yz zz x y z 1 (10..19).  Degree-1 polynomials (the
+// entries of E) are kept as their (x, y, z, 1) coefficients and degree-2 ones as their coefficients 10..19: o1 and o2 read nothing
+// else, so this is the reference's arithmetic on its non-zero entries.
+enum { XXX, XXY, XYY, YYY, XXZ, XYZ, YYZ, XZZ, YZZ, ZZZ };
+enum { XX, XY, YY, XZ, YZ, ZZ, X1, Y1, Z1, ONE };   // degree 2, offset 10
+enum { X, Y, Z, W };                                 // degree 1
+
+// o1: degree 1 x degree 1
+ACR_HD void o1(const double* a, const double* b, double* r) {
+  r[XX] = mul(a[X], b[X]);
+  r[XY] = add(mul(a[X], b[Y]), mul(a[Y], b[X]));
+  r[XZ] = add(mul(a[X], b[Z]), mul(a[Z], b[X]));
+  r[YY] = mul(a[Y], b[Y]);
+  r[YZ] = add(mul(a[Y], b[Z]), mul(a[Z], b[Y]));
+  r[ZZ] = mul(a[Z], b[Z]);
+  r[X1] = add(mul(a[X], b[W]), mul(a[W], b[X]));
+  r[Y1] = add(mul(a[Y], b[W]), mul(a[W], b[Y]));
+  r[Z1] = add(mul(a[Z], b[W]), mul(a[W], b[Z]));
+  r[ONE] = mul(a[W], b[W]);
+}
+
+// o2: degree 2 x degree 1, all 20 coefficients
+ACR_HD void o2(const double* a, const double* b, double* r) {
+  r[XXX] = mul(a[XX], b[X]);
+  r[XXY] = add(mul(a[XX], b[Y]), mul(a[XY], b[X]));
+  r[XXZ] = add(mul(a[XX], b[Z]), mul(a[XZ], b[X]));
+  r[XYY] = add(mul(a[XY], b[Y]), mul(a[YY], b[X]));
+  r[XYZ] = add(add(mul(a[XY], b[Z]), mul(a[YZ], b[X])), mul(a[XZ], b[Y]));
+  r[XZZ] = add(mul(a[XZ], b[Z]), mul(a[ZZ], b[X]));
+  r[YYY] = mul(a[YY], b[Y]);
+  r[YYZ] = add(mul(a[YY], b[Z]), mul(a[YZ], b[Y]));
+  r[YZZ] = add(mul(a[YZ], b[Z]), mul(a[ZZ], b[Y]));
+  r[ZZZ] = mul(a[ZZ], b[Z]);
+  r[10 + XX] = add(mul(a[XX], b[W]), mul(a[X1], b[X]));
+  r[10 + XY] = add(add(mul(a[XY], b[W]), mul(a[X1], b[Y])), mul(a[Y1], b[X]));
+  r[10 + XZ] = add(add(mul(a[XZ], b[W]), mul(a[X1], b[Z])), mul(a[Z1], b[X]));
+  r[10 + YY] = add(mul(a[YY], b[W]), mul(a[Y1], b[Y]));
+  r[10 + YZ] = add(add(mul(a[YZ], b[W]), mul(a[Y1], b[Z])), mul(a[Z1], b[Y]));
+  r[10 + ZZ] = add(mul(a[ZZ], b[W]), mul(a[Z1], b[Z]));
+  r[10 + X1] = add(mul(a[X1], b[W]), mul(a[ONE], b[X]));
+  r[10 + Y1] = add(mul(a[Y1], b[W]), mul(a[ONE], b[Y]));
+  r[10 + Z1] = add(mul(a[Z1], b[W]), mul(a[ONE], b[Z]));
+  r[10 + ONE] = mul(a[ONE], b[W]);
+}
+
+// fivePointsPolynomialConstraints: the 10 x 20 matrix of det(E) = 0 (row 0) and 2 E E^T E - tr(E E^T) E = 0 (rows 1..9, (i, j)
+// row-major), E = x B0 + y B1 + z B2 + B3 with B_c the basis columns (Eb[t][c], t = 3 i + j)
+ACR_HD void constraints(const double Eb[9][4], double M[N][20]) {
+  double a[10], b[10], r0[20], r1[20], r2[20];
+  const int det[3][5] = {{1, 5, 2, 4, 6}, {2, 3, 0, 5, 7}, {0, 4, 1, 3, 8}};   // o2(o1(E_p, E_q) - o1(E_r, E_s), E_t)
+  double* r[3] = {r0, r1, r2};
+  for (int u = 0; u < 3; ++u) {
+    o1(Eb[det[u][0]], Eb[det[u][1]], a);
+    o1(Eb[det[u][2]], Eb[det[u][3]], b);
+    for (int t = 0; t < 10; ++t) a[t] = sub(a[t], b[t]);
+    o2(a, Eb[det[u][4]], r[u]);
+  }
+  for (int t = 0; t < 20; ++t) M[0][t] = add(add(r0[t], r1[t]), r2[t]);
+  double L[3][3][10];   // E E^T (upper triangle computed, mirrored), then its diagonal less half its trace
+  for (int i = 0; i < 3; ++i)
+    for (int j = i; j < 3; ++j) {
+      o1(Eb[3 * i], Eb[3 * j], L[i][j]);
+      o1(Eb[3 * i + 1], Eb[3 * j + 1], a);
+      o1(Eb[3 * i + 2], Eb[3 * j + 2], b);
+      for (int t = 0; t < 10; ++t) L[i][j][t] = add(add(L[i][j][t], a[t]), b[t]);
+    }
+  for (int i = 1; i < 3; ++i)
+    for (int j = 0; j < i; ++j)
+      for (int t = 0; t < 10; ++t) L[i][j][t] = L[j][i][t];
+  for (int t = 0; t < 10; ++t) {
+    const double tr = mul(0.5, add(add(L[0][0][t], L[1][1][t]), L[2][2][t]));
+    for (int i = 0; i < 3; ++i) L[i][i][t] = sub(L[i][i][t], tr);
+  }
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      o2(L[i][0], Eb[j], r0);
+      o2(L[i][1], Eb[3 + j], r1);
+      o2(L[i][2], Eb[6 + j], r2);
+      for (int t = 0; t < 20; ++t) M[1 + 3 * i + j][t] = add(add(r0[t], r1[t]), r2[t]);
+    }
+}
+
+// FullPivLU<Mat10>(M[:, 0:10]).solve(M[:, 10:20]) into X: complete pivoting on the largest |entry| of the remaining corner (the first
+// in column-major order on a tie), a zero corner ends the factorisation, the rank counts the pivots above |max pivot| * 10 eps, and
+// the unknowns of the columns past the rank are 0.  The substitutions accumulate in index order.
+ACR_HD void lu_solve(double M[N][20], double X[N][N]) {
+  int colT[N], nz = N;
+  double maxpivot = 0;
+  for (int k = 0; k < N; ++k) {
+    int br = k, bc = k;
+    double big = fabs(M[k][k]);
+    for (int c = k; c < N; ++c)
+      for (int r = k; r < N; ++r)
+        if (fabs(M[r][c]) > big) { big = fabs(M[r][c]); br = r; bc = c; }
+    if (big == 0) {
+      nz = k;
+      for (int i = k; i < N; ++i) colT[i] = i;
+      break;
+    }
+    if (big > maxpivot) maxpivot = big;
+    colT[k] = bc;
+    if (br != k)
+      for (int c = 0; c < 20; ++c) { const double t = M[k][c]; M[k][c] = M[br][c]; M[br][c] = t; }   // the right side moves with P
+    if (bc != k)
+      for (int r = 0; r < N; ++r) { const double t = M[r][k]; M[r][k] = M[r][bc]; M[r][bc] = t; }
+    for (int r = k + 1; r < N; ++r) M[r][k] = M[r][k] / M[k][k];
+    for (int r = k + 1; r < N; ++r)
+      for (int c = k + 1; c < N; ++c) M[r][c] = sub(M[r][c], mul(M[r][k], M[k][c]));
+  }
+  const double thr = mul(maxpivot, mul((double)N, kEps));
+  int rank = 0;
+  for (int i = 0; i < nz; ++i) rank += fabs(M[i][i]) > thr;
+  int q[N];   // permutationQ().indices()
+  for (int i = 0; i < N; ++i) q[i] = i;
+  for (int k = 0; k < N; ++k) { const int t = q[k]; q[k] = q[colT[k]]; q[colT[k]] = t; }
+  for (int j = 0; j < N; ++j) {
+    double c[N];
+    for (int i = 0; i < N; ++i) c[i] = M[i][10 + j];
+    for (int i = 1; i < N; ++i)   // unit lower
+      for (int k = 0; k < i; ++k) c[i] = sub(c[i], mul(M[i][k], c[k]));
+    for (int i = rank - 1; i >= 0; --i) {   // upper, on the leading rank x rank block
+      for (int k = i + 1; k < rank; ++k) c[i] = sub(c[i], mul(M[i][k], c[k]));
+      c[i] = c[i] / M[i][i];
+    }
+    for (int i = 0; i < N; ++i) X[q[i]][j] = i < rank ? c[i] : 0.0;
+  }
+}
+
+// Householder::makeHouseholder of the real n-vector v: essential part ess[n - 1], tau, beta
+ACR_HD void make_householder(const double* v, int n, double* ess, double& tau, double& beta) {
+  double tail = 0;
+  for (int i = 1; i < n; ++i) tail = add(tail, mul(v[i], v[i]));
+  const double c0 = v[0];
+  if (tail <= kMin) {
+    tau = 0; beta = c0;
+    for (int i = 1; i < n; ++i) ess[i - 1] = 0;
+  } else {
+    beta = sqrt(add(mul(c0, c0), tail));
+    if (c0 >= 0) beta = -beta;
+    for (int i = 1; i < n; ++i) ess[i - 1] = v[i] / sub(c0, beta);
+    tau = sub(beta, c0) / beta;
+  }
+}
+
+// applyHouseholderOnTheLeft / OnTheRight of (ess (length m - 1), tau) to the rows r0..r0+m-1, columns c0..c1 (left) or the columns
+// c0..c0+m-1, rows r0..r1 (right) of A
+ACR_HD void house_left(double A[N][N], int r0, int m, int c0, int c1, const double* ess, double tau) {
+  if (m == 1) {
+    for (int c = c0; c <= c1; ++c) A[r0][c] = mul(A[r0][c], sub(1.0, tau));
+    return;
+  }
+  if (tau == 0) return;
+  for (int c = c0; c <= c1; ++c) {
+    double t = mul(ess[0], A[r0 + 1][c]);
+    for (int i = 1; i < m - 1; ++i) t = add(t, mul(ess[i], A[r0 + 1 + i][c]));
+    t = add(t, A[r0][c]);
+    A[r0][c] = sub(A[r0][c], mul(tau, t));
+    for (int i = 0; i < m - 1; ++i) A[r0 + 1 + i][c] = sub(A[r0 + 1 + i][c], mul(mul(tau, ess[i]), t));
+  }
+}
+ACR_HD void house_right(double A[N][N], int c0, int m, int r0, int r1, const double* ess, double tau) {
+  if (m == 1) {
+    for (int r = r0; r <= r1; ++r) A[r][c0] = mul(A[r][c0], sub(1.0, tau));
+    return;
+  }
+  if (tau == 0) return;
+  for (int r = r0; r <= r1; ++r) {
+    double t = mul(A[r][c0 + 1], ess[0]);
+    for (int j = 1; j < m - 1; ++j) t = add(t, mul(A[r][c0 + 1 + j], ess[j]));
+    t = add(t, A[r][c0]);
+    A[r][c0] = sub(A[r][c0], mul(tau, t));
+    const double tt = mul(tau, t);
+    for (int j = 0; j < m - 1; ++j) A[r][c0 + 1 + j] = sub(A[r][c0 + 1 + j], mul(tt, ess[j]));
+  }
+}
+
+// JacobiRotation::makeGivens(p, q) (real, no r)
+ACR_HD void make_givens(double p, double q, double& c, double& s) {
+  if (q == 0) {
+    c = p < 0 ? -1.0 : 1.0; s = 0;
+  } else if (p == 0) {
+    c = 0; s = q < 0 ? 1.0 : -1.0;
+  } else if (fabs(p) > fabs(q)) {
+    const double t = q / p;
+    double u = sqrt(add(1.0, mul(t, t)));
+    if (p < 0) u = -u;
+    c = 1.0 / u; s = mul(-t, c);
+  } else {
+    const double t = p / q;
+    double u = sqrt(add(1.0, mul(t, t)));
+    if (q < 0) u = -u;
+    s = -1.0 / u; c = mul(-t, s);
+  }
+}
+
+// apply_rotation_in_the_plane(x, y, (c, s')) with s' = -s, as applyOnTheLeft(rot.adjoint()) and applyOnTheRight(rot) both reduce to
+// for a real rotation: x <- c x - s y, y <- s x + c y
+ACR_HD void rotate(double& x, double& y, double c, double s) {
+  const double xi = x, yi = y;
+  x = add(mul(c, xi), mul(-s, yi));
+  y = add(mul(s, xi), mul(c, yi));
+}
+
+// RealSchur<Mat10>::compute(A, computeU = true) on the action matrix: scale by max |A|, Householder Hessenberg reduction (and its Q
+// accumulated as HouseholderSequence::evalTo does), then computeFromHessenberg: Francis double-shift QR steps with Eigen's deflation
+// test (findSmallSubdiagEntry), exceptional shifts at iterations 10 and 30 (computeShift), splitOffTwoRows for converged 2 x 2 blocks
+// and at most 40 N iterations in all.  T is quasi-triangular on return; false when the iteration limit was reached (NoConvergence).
+ACR_HD bool real_schur(const double A[N][N], double T[N][N], double U[N][N]) {
+  double scale = 0;
+  for (int r = 0; r < N; ++r)
+    for (int c = 0; c < N; ++c) scale = fmax(scale, fabs(A[r][c]));
+  for (int r = 0; r < N; ++r)
+    for (int c = 0; c < N; ++c) { T[r][c] = scale < kMin ? 0.0 : A[r][c] / scale; U[r][c] = r == c ? 1.0 : 0.0; }
+  if (scale < kMin) return true;
+  // HessenbergDecomposition::_compute: the essential parts stay below the subdiagonal of T
+  double h[N - 1];
+  for (int i = 0; i < N - 1; ++i) {
+    const int rem = N - i - 1;
+    double v[N], ess[N], beta;
+    for (int t = 0; t < rem; ++t) v[t] = T[i + 1 + t][i];
+    make_householder(v, rem, ess, h[i], beta);
+    for (int t = 0; t < rem - 1; ++t) T[i + 2 + t][i] = ess[t];
+    T[i + 1][i] = beta;
+    house_left(T, i + 1, rem, i + 1, N - 1, ess, h[i]);
+    house_right(T, i + 1, rem, 0, N - 1, ess, h[i]);
+  }
+  for (int k = N - 2; k >= 0; --k) {   // Q = H_0 ... H_{N-2}, applied from the last
+    const int m = N - k - 1;
+    double ess[N];
+    for (int t = 0; t < m - 1; ++t) ess[t] = T[k + 2 + t][k];
+    house_left(U, k + 1, m, k + 1, N - 1, ess, h[k]);
+  }
+  for (int r = 2; r < N; ++r)
+    for (int c = 0; c < r - 1; ++c) T[r][c] = 0;
+
+  int iu = N - 1, iter = 0, total = 0;
+  double exshift = 0, norm = 0;
+  for (int j = 0; j < N; ++j)
+    for (int r = 0; r < (j + 2 < N ? j + 2 : N); ++r) norm = add(norm, fabs(T[r][j]));
+  const double zero = fmax(mul(norm, mul(kEps, kEps)), kMin);
+  if (norm != 0) {
+    while (iu >= 0) {
+      int il = iu;   // findSmallSubdiagEntry
+      while (il > 0) {
+        double s = add(fabs(T[il - 1][il - 1]), fabs(T[il][il]));
+        s = fmax(mul(s, kEps), zero);
+        if (fabs(T[il][il - 1]) <= s) break;
+        --il;
+      }
+      if (il == iu) {   // one root
+        T[iu][iu] = add(T[iu][iu], exshift);
+        if (iu > 0) T[iu][iu - 1] = 0;
+        --iu; iter = 0;
+      } else if (il == iu - 1) {   // two roots: splitOffTwoRows
+        const double p = mul(0.5, sub(T[iu - 1][iu - 1], T[iu][iu]));
+        const double q = add(mul(p, p), mul(T[iu][iu - 1], T[iu - 1][iu]));
+        T[iu][iu] = add(T[iu][iu], exshift);
+        T[iu - 1][iu - 1] = add(T[iu - 1][iu - 1], exshift);
+        if (q >= 0) {
+          const double z = sqrt(fabs(q));
+          double c, s;
+          make_givens(p >= 0 ? add(p, z) : sub(p, z), T[iu][iu - 1], c, s);
+          for (int k = iu - 1; k < N; ++k) rotate(T[iu - 1][k], T[iu][k], c, s);
+          for (int k = 0; k <= iu; ++k) rotate(T[k][iu - 1], T[k][iu], c, s);
+          T[iu][iu - 1] = 0;
+          for (int k = 0; k < N; ++k) rotate(U[k][iu - 1], U[k][iu], c, s);
+        }
+        if (iu > 1) T[iu - 1][iu - 2] = 0;
+        iu -= 2; iter = 0;
+      } else {
+        double sh[3] = {T[iu][iu], T[iu - 1][iu - 1], mul(T[iu][iu - 1], T[iu - 1][iu])};   // computeShift
+        if (iter == 10) {   // Wilkinson's original ad hoc shift
+          exshift = add(exshift, sh[0]);
+          for (int i = 0; i <= iu; ++i) T[i][i] = sub(T[i][i], sh[0]);
+          const double s = add(fabs(T[iu][iu - 1]), fabs(T[iu - 1][iu - 2]));
+          sh[0] = mul(0.75, s); sh[1] = mul(0.75, s); sh[2] = mul(mul(-0.4375, s), s);
+        }
+        if (iter == 30) {   // MATLAB's ad hoc shift
+          double s = sub(sh[1], sh[0]) / 2.0;
+          s = add(mul(s, s), sh[2]);
+          if (s > 0) {
+            s = sqrt(s);
+            if (sh[1] < sh[0]) s = -s;
+            s = add(s, sub(sh[1], sh[0]) / 2.0);
+            s = sub(sh[0], sh[2] / s);
+            exshift = add(exshift, s);
+            for (int i = 0; i <= iu; ++i) T[i][i] = sub(T[i][i], s);
+            sh[0] = sh[1] = sh[2] = 0.964;
+          }
+        }
+        ++iter; ++total;
+        if (total > 40 * N) return false;
+        double v[3] = {0, 0, 0};   // initFrancisQRStep
+        int im;
+        for (im = iu - 2; im >= il; --im) {
+          const double Tmm = T[im][im], r = sub(sh[0], Tmm), s = sub(sh[1], Tmm);
+          v[0] = add(sub(mul(r, s), sh[2]) / T[im + 1][im], T[im][im + 1]);
+          v[1] = sub(sub(sub(T[im + 1][im + 1], Tmm), r), s);
+          v[2] = T[im + 2][im + 1];
+          if (im == il) break;
+          const double lhs = mul(T[im][im - 1], add(fabs(v[1]), fabs(v[2])));
+          const double rhs = mul(v[0], add(add(fabs(T[im - 1][im - 1]), fabs(Tmm)), fabs(T[im + 1][im + 1])));
+          if (fabs(lhs) < mul(kEps, rhs)) break;
+        }
+        for (int k = im; k <= iu - 2; ++k) {   // performFrancisQRStep
+          const bool first = k == im;
+          double w[3], ess[2], tau, beta;
+          for (int t = 0; t < 3; ++t) w[t] = first ? v[t] : T[k + t][k - 1];
+          make_householder(w, 3, ess, tau, beta);
+          if (beta != 0) {
+            if (first && k > il) T[k][k - 1] = -T[k][k - 1];
+            else if (!first) T[k][k - 1] = beta;
+            house_left(T, k, 3, k, N - 1, ess, tau);
+            house_right(T, k, 3, 0, (iu < k + 3 ? iu : k + 3), ess, tau);
+            house_right(U, k, 3, 0, N - 1, ess, tau);
+          }
+        }
+        {
+          double w[2] = {T[iu - 1][iu - 2], T[iu][iu - 2]}, ess[1], tau, beta;
+          make_householder(w, 2, ess, tau, beta);
+          if (beta != 0) {
+            T[iu - 1][iu - 2] = beta;
+            house_left(T, iu - 1, 2, iu - 1, N - 1, ess, tau);
+            house_right(T, iu - 1, 2, 0, iu, ess, tau);
+            house_right(U, iu - 1, 2, 0, N - 1, ess, tau);
+          }
+        }
+        for (int i = im + 2; i <= iu; ++i) {   // clean up pollution due to round-off errors
+          T[i][i - 2] = 0;
+          if (i > im + 2) T[i][i - 3] = 0;
+        }
+      }
+    }
+  }
+  for (int r = 0; r < N; ++r)
+    for (int c = 0; c < N; ++c) T[r][c] = mul(T[r][c], scale);
+  return true;
+}
+
+// EigenSolver<Mat10>(A): the real Schur form, its eigenvalues (a 2 x 2 block gives (T(i+1, i+1) + p) +- z i, z computed without
+// overflow), and the normalised eigenvectors of the real ones (imag() exactly 0), by doComputeEigenvectors' back-substitution
+// and back-transformation.  re[i], im[i]: the eigenvalues in Schur order; V[i][*]: the eigenvector of eigenvalue i when im[i] == 0.
+// Returns false where Eigen reports NoConvergence or NumericalIssue (no eigenvector computed).
+ACR_HD bool eigen_solve(const double A[N][N], double re[N], double im[N], double V[N][N]) {
+  double T[N][N], U[N][N];
+  if (!real_schur(A, T, U)) return false;
+  for (int i = 0; i < N;) {
+    if (i == N - 1 || T[i + 1][i] == 0) {
+      re[i] = T[i][i]; im[i] = 0;
+      if (!(fabs(re[i]) <= 1.7976931348623157e308)) return false;   // not finite
+      ++i;
+    } else {
+      const double p = mul(0.5, sub(T[i][i], T[i + 1][i + 1]));
+      double t0 = T[i + 1][i], t1 = T[i][i + 1];
+      const double mx = fmax(fabs(p), fmax(fabs(t0), fabs(t1)));
+      t0 = t0 / mx; t1 = t1 / mx;
+      const double p0 = p / mx;
+      const double z = mul(mx, sqrt(fabs(add(mul(p0, p0), mul(t0, t1)))));
+      re[i] = re[i + 1] = add(T[i + 1][i + 1], p);
+      im[i] = z; im[i + 1] = -z;
+      i += 2;
+    }
+  }
+  double norm = 0;
+  for (int j = 0; j < N; ++j)
+    for (int c = (j > 0 ? j - 1 : 0); c < N; ++c) norm = add(norm, fabs(T[j][c]));
+  if (norm != 0) {
+    for (int n = N - 1; n >= 0; --n) {   // back-substitution, real eigenvalues only (the complex ones touch no column used here)
+      if (im[n] != 0) continue;
+      const double p = re[n];
+      double lastr = 0, lastw = 0;
+      int l = n;
+      T[n][n] = 1.0;
+      for (int i = n - 1; i >= 0; --i) {
+        const double w = sub(T[i][i], p);
+        double r = 0;
+        for (int k = l; k <= n; ++k) r = add(r, mul(T[i][k], T[k][n]));
+        if (im[i] < 0) {
+          lastw = w; lastr = r;
+        } else {
+          l = i;
+          if (im[i] == 0) {
+            T[i][n] = w != 0 ? -r / w : -r / mul(kEps, norm);
+          } else {   // a complex pair above: solve the real 2 x 2 equations
+            const double x = T[i][i + 1], y = T[i + 1][i];
+            const double dr = sub(re[i], p);
+            const double denom = add(mul(dr, dr), mul(im[i], im[i]));
+            const double t = sub(mul(x, lastr), mul(lastw, r)) / denom;
+            T[i][n] = t;
+            T[i + 1][n] = fabs(x) > fabs(lastw) ? sub(-r, mul(w, t)) / x : sub(-lastr, mul(y, t)) / lastw;
+          }
+          const double t = fabs(T[i][n]);   // overflow control
+          if (mul(mul(kEps, t), t) > 1)
+            for (int k = i; k < N; ++k) T[k][n] = T[k][n] / t;
+        }
+      }
+    }
+    for (int j = N - 1; j >= 0; --j) {   // back-transformation: column j <- U[:, 0..j] T[0..j, j]
+      if (im[j] != 0) continue;
+      double col[N];
+      for (int r = 0; r < N; ++r) {
+        double s = mul(U[r][0], T[0][j]);
+        for (int k = 1; k <= j; ++k) s = add(s, mul(U[r][k], T[k][j]));
+        col[r] = s;
+      }
+      for (int r = 0; r < N; ++r) U[r][j] = col[r];
+    }
+  }
+  for (int j = 0; j < N; ++j) {
+    if (im[j] != 0) continue;
+    double s = 0;
+    for (int r = 0; r < N; ++r) s = add(s, mul(U[r][j], U[r][j]));
+    const double nr = sqrt(s);
+    for (int r = 0; r < N; ++r) V[j][r] = s > 0 ? U[r][j] / nr : U[r][j];
+  }
+  return true;
+}
+// Steps 1-4 of Essential5PSolver::solve on the 5 epipolar rows A: the null-space basis Eb (column c = N[c] of nullspace<5>), the
+// constraint matrix, its full-pivot LU solve and the action matrix At
+ACR_HD void action_matrix(const double A[5][9], double Eb[9][4], double At[N][N]) {
+  double Nb[4][9];
+  nullspace<5>(A, Nb);
+  for (int t = 0; t < 9; ++t)
+    for (int c = 0; c < 4; ++c) Eb[t][c] = Nb[c][t];
+  double M[N][20], X[N][N];
+  constraints(Eb, M);
+  lu_solve(M, X);
+  for (int r = 0; r < N; ++r)
+    for (int c = 0; c < N; ++c) At[r][c] = 0;
+  const int from[6] = {0, 1, 2, 4, 5, 7};
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < N; ++c) At[r][c] = X[from[r]][c];
+  At[6][0] = At[7][1] = At[8][3] = At[9][6] = -1;
+}
+}  // namespace e5
+
+// Essential5PSolver::solve on 5 K^-1-normalised correspondences (x1[i], y1[i]) <-> (x2[i], y2[i]): the 4-D null space of the
+// epipolar rows (nullspace<5>; basis column c = N[c]), the 10 x 20 constraint matrix, its full-pivot LU solve, the action matrix,
+// and E = (EBasis v.tail<4>())^T in Eigen's column-major map for every eigenvalue whose imaginary part is exactly 0, in Schur
+// order.  Returns the number of models (0..10) written row-major to E[m * 9] (x_J^T E x_I = 0 on normalised points).
+ACR_HD int fit5(const double* x1, const double* y1, const double* x2, const double* y2, double* E) {
+  double A[kSampleE][9];
+  for (int i = 0; i < kSampleE; ++i) {   // encodeEpipolarEquation
+    A[i][0] = mul(x2[i], x1[i]); A[i][1] = mul(x2[i], y1[i]); A[i][2] = x2[i];
+    A[i][3] = mul(y2[i], x1[i]); A[i][4] = mul(y2[i], y1[i]); A[i][5] = y2[i];
+    A[i][6] = x1[i]; A[i][7] = y1[i]; A[i][8] = 1.0;
+  }
+  double Eb[9][4], At[e5::N][e5::N];
+  e5::action_matrix(A, Eb, At);
+  double re[e5::N], im[e5::N], V[e5::N][e5::N];
+  if (!e5::eigen_solve(At, re, im, V)) return 0;
+  int nb = 0;
+  for (int s = 0; s < e5::N; ++s) {
+    if (im[s] != 0) continue;
+    const double* v = V[s] + 6;
+    for (int t = 0; t < 9; ++t)
+      E[nb * 9 + t] = add(add(add(mul(Eb[t][0], v[0]), mul(Eb[t][1], v[1])), mul(Eb[t][2], v[2])), mul(Eb[t][3], v[3]));
+    ++nb;
+  }
+  return nb;
+}
 
 }  // namespace acr

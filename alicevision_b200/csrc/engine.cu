@@ -2120,35 +2120,49 @@ int b200m_ctx_set_hgrowing_window(b200m_ctx* c, int window) {
 
 }  // extern "C"
 
-// ---- K10: a-contrario RANSAC for a pair list: fundamental matrix, homography, spherical fundamental matrix (acransac.cuh) ----
+// ---- K10: a-contrario RANSAC for a pair list: fundamental matrix, homography, spherical fundamental matrix, essential matrix
+// (acransac.cuh) ----
 // One launch of acransac_kernel<Policy> over the list; the entry points differ in the model, the correspondence width
-// (Policy::kWidth doubles) and the generator contract.  wh: image sizes of the planar policies (unused, may be NULL, for bearings).
-// mt_per_pair: 0 = mt_state is one 625-word state for every pair, 1 = n_pairs x 625.  mt_out: NULL or n_pairs x 625.
+// (Policy::kWidth doubles; 4 pixel doubles in for the calibrated policy) and the generator contract.  wh: image sizes of the planar
+// and calibrated policies (unused, may be NULL, for bearings).  K: n_pairs x 18 (K_I, K_J row-major) for the calibrated policy, else
+// unused.  mt_per_pair: 0 = mt_state is one 625-word state for every pair, 1 = n_pairs x 625.  mt_out: NULL or n_pairs x 625.
 template <class Policy>
-static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh, const uint32_t* mt_state,
-                          int mt_per_pair, int64_t max_iteration, double precision, uint8_t* valid, int32_t* n_inliers, uint32_t* inliers,
-                          double* model, double* error_max, double* min_nfa, int32_t* iterations, uint32_t* mt_out) {
+static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh, const double* K,
+                          const uint32_t* mt_state, int mt_per_pair, int64_t max_iteration, double precision, uint8_t* valid, int32_t* n_inliers,
+                          uint32_t* inliers, double* model, double* error_max, double* min_nfa, int32_t* iterations, uint32_t* mt_out) {
+  constexpr bool kSized = Policy::kPlanar || Policy::kCalibrated;
   if (!c || n_pairs < 0 || max_iteration < 0 || max_iteration > INT32_MAX || !(precision > 0) || (mt_per_pair != 0 && mt_per_pair != 1) ||
-      (n_pairs > 0 && (!offsets || (Policy::kPlanar && !wh) || !mt_state || !valid || !n_inliers || !model || !error_max || !min_nfa ||
-                       !iterations)))
+      (n_pairs > 0 && (!offsets || (kSized && !wh) || (Policy::kCalibrated && !K) || !mt_state || !valid || !n_inliers || !model ||
+                       !error_max || !min_nfa || !iterations)))
     return fail(B200M_ERR_ARG, "bad arguments");
   if (n_pairs > 0 && offsets[0] != 0) return fail(B200M_ERR_ARG, "offsets[0] must be 0");
   std::vector<acrk::Pair> pairs((size_t)n_pairs);
+  std::vector<acrk::PairE> pairs_e(Policy::kCalibrated ? (size_t)n_pairs : 0);
   int64_t sort_total = 0; int max_n = 0;
   for (int k = 0; k < n_pairs; ++k) {
     const int64_t n = offsets[k + 1] - offsets[k];
     if (n < 0 || n > (1 << 24)) return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": offsets must ascend, at most 2^24 correspondences a pair");
     int32_t s[4] = {0, 0, 0, 0};
-    if (Policy::kPlanar) {
+    if (kSized)
       for (int t = 0; t < 4; ++t)
         if ((s[t] = wh[4 * k + t]) < 1) return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": image sizes must be positive");
-      if ((int64_t)s[0] * s[1] > INT32_MAX || (int64_t)s[2] * s[3] > INT32_MAX)
-        return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": width * height must fit an int, as in the reference");
+    if (Policy::kPlanar && ((int64_t)s[0] * s[1] > INT32_MAX || (int64_t)s[2] * s[3] > INT32_MAX))
+      return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": width * height must fit an int, as in the reference");
+    if (Policy::kCalibrated) {   // K^-1 as RelativePoseKernel_K's constructor takes it; a singular K gives a non-finite inverse
+      bool ok = true;
+      for (int t = 0; t < 18; ++t) ok &= std::isfinite(K[18 * k + t]);
+      if (ok) {
+        acr::inverse3(K + 18 * k, pairs_e[k].kinv);
+        acr::inverse3(K + 18 * k + 9, pairs_e[k].kinv + 9);
+        for (int t = 0; t < 18; ++t) ok &= std::isfinite(pairs_e[k].kinv[t]);
+      }
+      if (!ok) return fail(B200M_ERR_ARG, "pair " + std::to_string(k) + ": K must be finite and invertible");
     }
     int64_t n2 = 1;
     while (n2 < n) n2 <<= 1;
     pairs[k] = acrk::Pair{offsets[k], n2 > acrk::kSmemSort ? sort_total : 0, (int)n, s[0], s[1], s[2], s[3]};
     if (n2 > acrk::kSmemSort) sort_total += n2;
+    if (Policy::kCalibrated) pairs_e[k].q = pairs[k];
     max_n = std::max(max_n, (int)n);
   }
   const int64_t N = n_pairs ? offsets[n_pairs] : 0;
@@ -2165,10 +2179,12 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
   for (size_t k = 0; k < l10.size(); ++k) l10[k] = (float)log10((double)k);
   const size_t n_states = mt_per_pair ? (size_t)n_pairs : 1;
   // one grow-only device buffer, shared by every model
-  constexpr int W = Policy::kWidth;
+  constexpr int W = Policy::kWidth, W_in = Policy::kCalibrated ? 4 : W;
+  const size_t pair_bytes = Policy::kCalibrated ? sizeof(acrk::PairE) : sizeof(acrk::Pair);
+  const void* pair_src = Policy::kCalibrated ? (const void*)pairs_e.data() : (const void*)pairs.data();
   size_t at = 0;
   auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
-  const size_t o_pairs = take(sizeof(acrk::Pair) * n_pairs), o_corr = take(sizeof(double) * W * N), o_l10 = take(sizeof(float) * l10.size()),
+  const size_t o_pairs = take(pair_bytes * n_pairs), o_corr = take(sizeof(double) * W_in * N), o_l10 = take(sizeof(float) * l10.size()),
                o_mt = take(sizeof(uint32_t) * 625 * n_states), o_pts = take(sizeof(double) * W * N), o_idx = take(sizeof(uint32_t) * N),
                o_logc = take(sizeof(float) * 2 * (N + n_pairs)), o_gk = take(sizeof(unsigned long long) * sort_total),
                o_gv = take(sizeof(uint32_t) * sort_total), o_inl = take(sizeof(uint32_t) * N),
@@ -2179,8 +2195,8 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
   if ((rc = c->acr.d.reserve(at)) || (rc = c->acr.ev0.create()) || (rc = c->acr.ev1.create())) return rc;
   char* d = c->acr.d;
   cudaStream_t st = c->stream;
-  CK(cudaMemcpyAsync(d + o_pairs, pairs.data(), sizeof(acrk::Pair) * n_pairs, cudaMemcpyHostToDevice, st));
-  if (N) CK(cudaMemcpyAsync(d + o_corr, corr, sizeof(double) * W * N, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d + o_pairs, pair_src, pair_bytes * n_pairs, cudaMemcpyHostToDevice, st));
+  if (N) CK(cudaMemcpyAsync(d + o_corr, corr, sizeof(double) * W_in * N, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d + o_l10, l10.data(), sizeof(float) * l10.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d + o_mt, mt_state, sizeof(uint32_t) * 625 * n_states, cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(c->acr.ev0, st));
@@ -2219,7 +2235,7 @@ int b200m_acransac_fundamental_pairs(b200m_ctx* c, int n_pairs, const int64_t* o
                                      const uint32_t* mt_state, int64_t max_iteration, double precision, uint8_t* valid,
                                      int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max, double* min_nfa,
                                      int32_t* iterations) {
-  return acransac_pairs<acrk::FPolicy>(c, n_pairs, offsets, corr, wh, mt_state, 0, max_iteration, precision, valid, n_inliers, inliers, F,
+  return acransac_pairs<acrk::FPolicy>(c, n_pairs, offsets, corr, wh, nullptr, mt_state, 0, max_iteration, precision, valid, n_inliers, inliers, F,
                                        error_max, min_nfa, iterations, nullptr);
 }
 
@@ -2227,7 +2243,7 @@ int b200m_acransac_homography_pairs(b200m_ctx* c, int n_pairs, const int64_t* of
                                     const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision, uint8_t* valid,
                                     int32_t* n_inliers, uint32_t* inliers, double* H, double* error_max, double* min_nfa, int32_t* iterations,
                                     uint32_t* mt_state_out) {
-  return acransac_pairs<acrk::HPolicy>(c, n_pairs, offsets, corr, wh, mt_state, mt_state_per_pair, max_iteration, precision, valid, n_inliers,
+  return acransac_pairs<acrk::HPolicy>(c, n_pairs, offsets, corr, wh, nullptr, mt_state, mt_state_per_pair, max_iteration, precision, valid, n_inliers,
                                        inliers, H, error_max, min_nfa, iterations, mt_state_out);
 }
 
@@ -2235,8 +2251,16 @@ int b200m_acransac_fundamental_spherical_pairs(b200m_ctx* c, int n_pairs, const 
                                                const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision,
                                                uint8_t* valid, int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max,
                                                double* min_nfa, int32_t* iterations, uint32_t* mt_state_out) {
-  return acransac_pairs<acrk::SPolicy>(c, n_pairs, offsets, bearings, nullptr, mt_state, mt_state_per_pair, max_iteration, precision, valid,
+  return acransac_pairs<acrk::SPolicy>(c, n_pairs, offsets, bearings, nullptr, nullptr, mt_state, mt_state_per_pair, max_iteration, precision, valid,
                                        n_inliers, inliers, F, error_max, min_nfa, iterations, mt_state_out);
+}
+
+int b200m_acransac_essential_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh, const double* K,
+                                   const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision, uint8_t* valid,
+                                   int32_t* n_inliers, uint32_t* inliers, double* E, double* error_max, double* min_nfa, int32_t* iterations,
+                                   uint32_t* mt_state_out) {
+  return acransac_pairs<acrk::EPolicy>(c, n_pairs, offsets, corr, wh, K, mt_state, mt_state_per_pair, max_iteration, precision, valid,
+                                       n_inliers, inliers, E, error_max, min_nfa, iterations, mt_state_out);
 }
 
 double b200m_acransac_last_stats(const b200m_ctx* c, int64_t stats[4]) {

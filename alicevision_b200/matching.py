@@ -41,7 +41,7 @@ ABI_SYMBOLS = [
     "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
     "b200m_mt19937_seed", "b200m_debug_rand_sample", "b200m_acransac_homography_pairs", "b200m_debug_rand_sample_k", "b200m_guided_match_pairs",
     "b200m_guided_match_positions_pairs", "b200m_acransac_fundamental_spherical_pairs", "b200m_hgrowing_pairs", "b200m_hgrowing_last_stats",
-    "b200m_ctx_set_hgrowing_window",
+    "b200m_ctx_set_hgrowing_window", "b200m_acransac_essential_pairs",
 ]
 
 
@@ -253,7 +253,16 @@ class Context:
         and "mt_state_out": the generator state after the pair's estimation (the reference passes this generator by reference)."""
         return self._acransac_pairs("S", corr_list, None, _mt_states(mt_state_or_states, len(corr_list)), maxIteration, precision)
 
-    def _acransac_pairs(self, kind: str, corr_list, wh, st, maxIteration, precision) -> list[dict]:
+    def acransac_essential_pairs(self, corr_list, wh, K, mt_state_or_states, maxIteration: int = 50000, precision: float = np.inf) -> list[dict]:
+        """b200m_acransac_essential_pairs: GeometricFilterMatrix_E_AC::geometricEstimation (ACRANSAC with Essential5PSolver on K^-1 x
+        and the point-to-line error of K_J^-T E K_I^-1 on the pixels) for every pair.  corr_list and wh as in
+        acransac_fundamental_pairs; K: per pair (K_I, K_J), two 3 x 3 camera matrices; mt_state_or_states as in
+        acransac_homography_pairs.  `precision` is ACRANSAC's own argument (the filter passes it squared).  Returns per pair the fields
+        of acransac_fundamental_pairs with "E" (3 x 3) in place of "F", and "mt_state_out"."""
+        Km = np.ascontiguousarray(K, np.float64).reshape(len(corr_list), 18)
+        return self._acransac_pairs("E", corr_list, wh, _mt_states(mt_state_or_states, len(corr_list)), maxIteration, precision, Km)
+
+    def _acransac_pairs(self, kind: str, corr_list, wh, st, maxIteration, precision, K=None) -> list[dict]:
         width = 6 if kind == "S" else 4
         cs = [np.ascontiguousarray(c, np.float64).reshape(-1, width) for c in corr_list]
         n = len(cs)
@@ -270,6 +279,11 @@ class Context:
                                                             C.c_int64(maxIteration), C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(M),
                                                             ptr(em), ptr(nfa), ptr(it), ptr(sto)),
                    "b200m_acransac_homography_pairs")
+        elif kind == "E":
+            _check(self.lib.b200m_acransac_essential_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(K if n else np.zeros(18)),
+                                                           ptr(st), C.c_int(int(st.ndim == 2)), C.c_int64(maxIteration), C.c_double(precision),
+                                                           ptr(valid), ptr(ninl), ptr(inl), ptr(M), ptr(em), ptr(nfa), ptr(it), ptr(sto)),
+                   "b200m_acransac_essential_pairs")
         elif kind == "S":
             _check(self.lib.b200m_acransac_fundamental_spherical_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(st), C.c_int(int(st.ndim == 2)),
                                                                        C.c_int64(maxIteration), C.c_double(precision), ptr(valid), ptr(ninl),
@@ -283,7 +297,7 @@ class Context:
         tr = np.zeros(256, np.int32); trn = np.zeros(256, np.float64)
         for k in range(n):
             nt = self.lib.b200m_acransac_last_trace(self._h, C.c_int(k), ptr(tr), ptr(trn), C.c_int(tr.size))
-            r = {"valid": bool(valid[k]), "inliers": inl[offsets[k]:offsets[k] + ninl[k]].copy(), "H" if kind == "H" else "F": M[k].reshape(3, 3).copy(),
+            r = {"valid": bool(valid[k]), "inliers": inl[offsets[k]:offsets[k] + ninl[k]].copy(), kind if kind in "HE" else "F": M[k].reshape(3, 3).copy(),
                  "error_max": float(em[k]), "min_nfa": float(nfa[k]), "iterations": int(it[k]), "n_trace": int(nt),
                  "trace": tr[:min(nt, tr.size)].copy(), "trace_nfa": trn[:min(nt, trn.size)].copy()}
             if sto is not None:
@@ -292,8 +306,8 @@ class Context:
         return out
 
     def acransac_last_stats(self) -> dict:
-        """Instrumentation of the last acransac_fundamental_pairs, acransac_homography_pairs or acransac_fundamental_spherical_pairs
-        call."""
+        """Instrumentation of the last acransac_fundamental_pairs, acransac_homography_pairs, acransac_fundamental_spherical_pairs or
+        acransac_essential_pairs call."""
         st = np.zeros(4, np.int64)
         ms = self.lib.b200m_acransac_last_stats(self._h, st.ctypes.data_as(C.c_void_p))
         return {"gpu_ms": ms, "models_evaluated": int(st[0]), "models_skipped": int(st[1]), "models_exact": int(st[2]), "launches": int(st[3])}
@@ -632,6 +646,108 @@ def robustModelEstimation_H_AC(putatives: dict, regions_per_view: dict, image_si
             return ctx.guided_match_pairs(vp, Hs, th, distanceRatio * distanceRatio, MODEL_HOMOGRAPHY)
         _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry, run)
     return out, info
+
+
+def geometricEstimation_E_AC(xI, xJ, sizeI, sizeJ, KI, KJ, seed_or_state, maxIteration: int = 50000, precision: float = np.inf,
+                             ctx: Context | None = None) -> dict:
+    """GeometricFilterMatrix_E_AC::geometricEstimation's ACRANSAC of one pair on the GPU: arguments as geometricEstimation_F_AC plus
+    the two pinhole matrices K (3 x 3); `precision` is what the filter passes to ACRANSAC, Square(m_dPrecision).  Returns the dict of
+    Context.acransac_essential_pairs ("E", "mt_state_out")."""
+    ctx = ctx or default_context()
+    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else seed_or_state
+    corr = np.concatenate([np.asarray(xI, np.float64).reshape(-1, 2), np.asarray(xJ, np.float64).reshape(-1, 2)], axis=1)
+    K = np.concatenate([np.asarray(KI, np.float64).reshape(9), np.asarray(KJ, np.float64).reshape(9)])
+    return ctx.acransac_essential_pairs([corr], [tuple(sizeI) + tuple(sizeJ)], [K], st, maxIteration, precision)[0]
+
+
+def _inverse3(M) -> np.ndarray:
+    """The engine's 3 x 3 inverse (acr::inverse3): cofactors over the determinant expanded along the first column."""
+    M = np.asarray(M, np.float64).reshape(3, 3)
+    C_ = np.empty((3, 3))
+    for i in range(3):
+        for j in range(3):
+            i1, i2, j1, j2 = (i + 1) % 3, (i + 2) % 3, (j + 1) % 3, (j + 2) % 3
+            C_[i, j] = M[i1, j1] * M[i2, j2] - M[i1, j2] * M[i2, j1]
+    inv = 1.0 / ((C_[0, 0] * M[0, 0] + C_[1, 0] * M[1, 0]) + C_[2, 0] * M[2, 0])
+    return C_.T * inv
+
+
+def fundamentalFromEssential(E, KI, KJ) -> np.ndarray:
+    """multiview::fundamentalFromEssential: F = K_J^-T E K_I^-1, formed as (K_J^-T E) K_I^-1 with the engine's inverses, each entry
+    summed in index order (the C++ adaptor's and acr::fundamental_from_essential's arithmetic)."""
+    E, iI, iJ = np.asarray(E, np.float64).reshape(3, 3), _inverse3(KI), _inverse3(KJ)
+    T = (iJ[0][:, None] * E[0] + iJ[1][:, None] * E[1]) + iJ[2][:, None] * E[2]      # T[r, c] = sum_k iJ[k, r] E[k, c], k in order
+    return (T[:, 0:1] * iI[0] + T[:, 1:2] * iI[1]) + T[:, 2:3] * iI[2]
+
+
+def robustModelEstimation_E_AC(putatives: dict, regions_per_view: dict, image_sizes: dict, intrinsics: dict, seed_or_state,
+                               maxIteration: int = 50000, precision: float = np.inf, guidedMatching: bool = False, distanceRatio: float = 0.6,
+                               geometry: dict | None = None, guided_geometry: dict | None = None, desc_types=None, chain: bool = False,
+                               ctx: Context | None = None):
+    """matchingImageCollection::robustModelEstimation with GeometricFilterMatrix_E_AC (ACRANSAC, Essential5PSolver;
+    GeometricFilterMatrix_E_AC.hpp), the `essential_matrix` filter of featureMatching, for a whole putative list: a-contrario RANSAC
+    for every estimated pair (b200m_acransac_essential_pairs), copyInlierMatches and hasStrongSupport(.., 5); then, with guidedMatching,
+    one guided-matching call (b200m_guided_match_pairs) for every kept pair with a finite error_max and every common type, with
+    F = K_J^-T E K_I^-1, errorTh = error_max^2 and distRatio = distanceRatio^2.  featureMatching then applies
+    removePoorlyOverlappingImagePairs to the result.
+
+    intrinsics  {view: 3 x 3 K of its camera::Pinhole (equidistant cameras included), or None for a missing or non-pinhole intrinsic}.
+                A pair is not estimated (EstimationStatus(false, false)) without a common describer type, or when either view has no
+                pinhole K.
+    precision   the filter's m_dPrecision (geometricErrorMax; +inf = none): the filter passes Square(precision) to ACRANSAC, which
+                squares it again, so the residual threshold is precision^4, as in the reference.
+    Other arguments as robustModelEstimation_H_AC, the generator contract (chain) included.
+
+    Returns (geometric matches {(I, J): {type: matches}} of the pairs with strong support, per-pair estimation
+    {(I, J): {"valid", "strong_support", "E", "error_max"}, plus "mt_state_out" for the estimated pairs})."""
+    ctx = ctx or default_context()
+    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
+    pairs, common, est_all, corrs_all, whs_all = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
+    Ks = lambda p: [intrinsics.get(v) for v in p]  # noqa: E731
+    keep = [k for k, p in enumerate(est_all) if all(K is not None for K in Ks(p))]
+    est = [est_all[k] for k in keep]
+    corrs, whs = [corrs_all[k] for k in keep], [whs_all[k] for k in keep]
+    Kp = [np.concatenate([np.asarray(K, np.float64).reshape(9) for K in Ks(p)]) for p in est]
+    upper = precision * precision   # upperBoundPrecision = Square(m_dPrecision)
+    if not est:
+        res = []
+    elif chain:
+        res = []
+        for c, wh, K in zip(corrs, whs, Kp):
+            res.append(ctx.acransac_essential_pairs([c], [wh], [K], st, maxIteration, upper)[0])
+            st = res[-1]["mt_state_out"]
+    else:
+        res = ctx.acransac_essential_pairs(corrs, whs, Kp, st, maxIteration, upper)
+    info = {p: {"valid": False, "strong_support": False, "E": np.zeros((3, 3)), "error_max": np.inf} for p in pairs}
+    out = {}
+    for p, r in zip(est, res):
+        info[p].update(valid=r["valid"], E=r["E"], error_max=r["error_max"], mt_state_out=r["mt_state_out"])
+        if not r["valid"]:
+            continue
+        inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
+        info[p]["strong_support"] = hasStrongSupport(inl, 5)          # Essential5PSolver::getMinimumNbRequiredSamples
+        if info[p]["strong_support"]:
+            out[p] = inl
+    if guidedMatching and out:
+        _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry,
+                      lambda vp, items: ctx.guided_match_pairs(vp, [fundamentalFromEssential(info[p]["E"], *Ks(p)) for p, _ in items],
+                                                               [info[p]["error_max"] * info[p]["error_max"] for p, _ in items],
+                                                               distanceRatio * distanceRatio))
+    return out, info
+
+
+def removePoorlyOverlappingImagePairs(geometric: dict, putatives: dict, minimumRatio: float = 0.3, minimumGeometricCount: int = 50) -> dict:
+    """matchingImageCollection::removePoorlyOverlappingImagePairs (GeometricFilter.cpp:12-34): a pair of `geometric` is removed when
+    its match count (all types) is below minimumGeometricCount, or when that count over its putative count, divided in float, is below
+    minimumRatio (a float).  Returns the kept pairs."""
+    out = {}
+    for p, m in geometric.items():
+        g = sum(len(v) for v in m.values())
+        n = sum(len(v) for v in putatives[p].values())
+        if g < minimumGeometricCount or np.float32(g) / np.float32(n) < np.float32(minimumRatio):
+            continue
+        out[p] = m
+    return out
 
 
 # GrowParameters / HGrowingFilteringParam defaults (GeometricFilterMatrix_HGrowing.hpp:23-106); featureMatching never changes them

@@ -262,11 +262,26 @@ int b200m_acransac_fundamental_spherical_pairs(b200m_ctx* ctx, int n_pairs, cons
                                                const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision,
                                                uint8_t* valid, int32_t* n_inliers, uint32_t* inliers, double* F, double* error_max,
                                                double* min_nfa, int32_t* iterations, uint32_t* mt_state_out);
-/* instrumentation of the last a-contrario RANSAC call (b200m_acransac_fundamental_pairs, b200m_acransac_homography_pairs or
- * b200m_acransac_fundamental_spherical_pairs): stats = {models evaluated in the a-contrario mode, of them skipped by the histogram
+/* ---- geometric filtering: a-contrario RANSAC essential matrix of two pinhole cameras (K10, essential_matrix filter) ------ */
+/* GeometricFilterMatrix_E_AC::geometricEstimation (ACRANSAC over RelativePoseKernel_K<Essential5PSolver,
+ * FundamentalEpipolarDistanceError, Mat3Model>) for every pair of a list, results in input order.  The 5-point solver runs on
+ * K^-1 x; the residual is the point-to-line error of F = K_J^-T E K_I^-1 on the pixels; no normalisation, errorVectorDimension = 0.5,
+ * logalpha0 = log10(2 D / A * .5) of (widthJ, heightJ), maxThreshold = precision^2.
+ *   corr       offsets[n_pairs] x 4 doubles (xI, yI, xJ, yJ), as for b200m_acransac_fundamental_pairs
+ *   wh         n_pairs x 4 = (widthI, heightI, widthJ, heightJ), each >= 1
+ *   K          n_pairs x 18 doubles: K_I then K_J, row-major (camera::Pinhole::K()); finite and invertible
+ * Other arguments and outputs as in b200m_acransac_homography_pairs (the reference passes this generator by reference too), with
+ * E[9 * n_pairs] (row-major, x_J^T F x_I = 0 with F as above) and error_max = sqrt of the largest inlier's squared residual, in
+ * pixels, when valid.  A pair with at most 5 correspondences returns (0, 0) and no iteration. */
+int b200m_acransac_essential_pairs(b200m_ctx* ctx, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh, const double* K,
+                                   const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision, uint8_t* valid,
+                                   int32_t* n_inliers, uint32_t* inliers, double* E, double* error_max, double* min_nfa, int32_t* iterations,
+                                   uint32_t* mt_state_out);
+/* instrumentation of the last a-contrario RANSAC call (b200m_acransac_fundamental_pairs, b200m_acransac_homography_pairs,
+ * b200m_acransac_fundamental_spherical_pairs or b200m_acransac_essential_pairs): stats = {models evaluated in the a-contrario mode, of them skipped by the histogram
  * bound, scored exactly, kernel launches}; returns its GPU time in ms */
 double b200m_acransac_last_stats(const b200m_ctx* ctx, int64_t stats[4]);
-/* the `better` events of the last a-contrario RANSAC call's pair `pair` (F, H or spherical F): the iterations at which a better model was found
+/* the `better` events of the last a-contrario RANSAC call's pair `pair` (F, H, spherical F or E): the iterations at which a better model was found
  * and the new minNFA of each (the first `cap`, at most 256; either pointer may be NULL); returns their number.  The getters of the
  * last call take the context's lock, so a concurrent call on the same context cannot rewrite what they read. */
 int b200m_acransac_last_trace(const b200m_ctx* ctx, int pair, int32_t* iters, double* nfa, int cap);
