@@ -276,6 +276,7 @@ struct LastCall {
   double gpu_ms, search_ms;
   int launches, tc_pairs, real_pairs, u8_pairs;
   int64_t records, fallback_rows;
+  int batches;                // b200m_match_pairs only
 };
 
 // Members are released in reverse order of declaration, after ~b200m_ctx has stopped the uploader and the pool and freed the views:
@@ -1434,7 +1435,7 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
   }
   if (timing) fprintf(stderr, "[b200m] match_pairs n=%d stage=%d: setup %.2f ms, batches %.2f ms (gpu %.2f), tail (cross+assemble) %.2f ms, total %.2f ms\n",
                       n_pairs, stage, t_setup - t_begin, t_gpu_done - t_setup, ms, now() - t_gpu_done, now() - t_begin);
-  c->last = LastCall{ms, sk, launches, tc_pairs, real_pairs, u8_pairs, total_records, fallback_rows};
+  c->last = LastCall{ms, sk, launches, tc_pairs, real_pairs, u8_pairs, total_records, fallback_rows, (int)batches.size()};
   *out = res.release();
   return B200M_OK;
 }
@@ -1463,6 +1464,7 @@ int64_t b200m_last_records(const b200m_ctx* c) { return last_call(c).records; }
 int b200m_last_real_tc_pairs(const b200m_ctx* c) { return last_call(c).real_pairs; }
 int b200m_last_u8_tc_pairs(const b200m_ctx* c) { return last_call(c).u8_pairs; }
 int64_t b200m_last_fallback_rows(const b200m_ctx* c) { return last_call(c).fallback_rows; }
+int b200m_last_batches(const b200m_ctx* c) { return last_call(c).batches; }
 
 // ---- guided matching (after the path: GeometricFilterMatrix_F_AC.hpp:363-390 -> matching/guidedMatching.hpp:206-268) ----------------
 int b200m_guided_match(b200m_ctx* c, uint32_t view_left, uint32_t view_right, const double* F, double errorTh, double distRatio, b200m_result** out) {
