@@ -18,6 +18,9 @@ enum : uint32_t {
   VF_NORM = 4u,         // some squared norm >= 2^22 (distances would leave the exact-fp32 range)
   VF_EXACT_MASK = 7u,   // the bits above: any of them set -> the view cannot take the (integer) tensor-core path
   VF_POS_NONGENERIC = 8u,   // feature positions: two features share an x or a y (or a NaN): coordinate de-duplication stays on the host
+  // uchar-stored views only (prep.cuh), outside VF_EXACT_MASK: which side of the u8 norm-GEMM kernel (l2_tc.cuh NG) a view may take
+  VF_U8_WIDE = 16u,     // some component > 127: 2a would not fit in u8, so the view is no QUERY of the norm-GEMM kernel
+  VF_U8_NORMCAP = 32u,  // some squared norm > U8_LIMB_CAP: its limbs cannot hold it, so the view is no DATABASE of the norm-GEMM kernel
 };
 
 // One uploaded view (image) resident in HBM.
@@ -26,6 +29,7 @@ struct alignas(128) ViewDev {
   CUtensorMap tmap_aug; // fp16 [m_pad x 16] half-norm limbs, box {16 x 128 rows}, SWIZZLE_32B (9th K-step of the AUG kernel)
   CUtensorMap tmap_augq; // the same for augq16 (the view as QUERY of the real-valued kernel: its own half-norm limbs as A columns)
   CUtensorMap tmap_u8;  // uchar-stored views only: `raw` as u8 [m x 128], box {128 B x 128 rows}, SWIZZLE_128B (the u8 kernel's operand tile)
+  CUtensorMap tmap_limb; // uchar-stored views only: limb8 as u8 [m_pad x 32], box {32 B x 128 rows}, SWIZZLE_32B (the norm-GEMM kernel's 5th K-step)
   const int32_t* nb32;  // uchar-stored views only: ||row||^2 + U8_NORM_BIAS as int32, padded to a multiple of 256 rows with 2^24 + U8_NORM_BIAS (prep.cuh), else nullptr
   const void* raw;      // descriptors as STORED, row-major m x dim: f32 / u8 / 64-byte binary; `dtype` is the storage type (integer-valued
                         // fp32 descriptors are staged and stored as u8: same values, a quarter of the bytes)
@@ -72,6 +76,19 @@ struct Cand { uint32_t q, b; float d1, d2; };
 // ViewDev::nb32 holds ||row||^2 + U8_NORM_BIAS: with it the u8 kernel's per-element value ||b||^2 - 2 a.b > -||a||^2 > -2^22 is positive, and
 // positive values order the same as integers and as float bit patterns (l2_tc.cuh u8_elem)
 constexpr int32_t U8_NORM_BIAS = 1 << 22;
+
+// The u8 norm-GEMM kernel (l2_tc.cuh NG) folds the database norm into its s32 accumulator with one extra K32 step: per database row 32 u8
+// limbs l_k with ||b||^2 = l_0 + 128 * (l_1 + ... + l_31), l_0 < 128, each limb <= 255, against the constant s8 weights
+// w_0 = -1, w_1..31 = -128 (U8_LIMB_W0, U8_LIMB_W).  Capacity: 127 + 128 * 31 * 255.  Pad rows carry all limbs 255, whose norm
+// U8_LIMB_PAD exceeds every real row's.
+constexpr int32_t U8_LIMB_W0 = -1, U8_LIMB_W = -128;
+constexpr int32_t U8_LIMB_CAP = 127 + 128 * 31 * 255;          // 1,011,967
+constexpr int32_t U8_LIMB_PAD = 255 + 128 * 31 * 255;          // 1,012,095
+__host__ __device__ __forceinline__ uint32_t u8_limb(int32_t nrm2, int k) {
+  if (k == 0) return (uint32_t)(nrm2 & 127);
+  const int32_t q = (nrm2 >> 7) - 255 * (k - 1);                // limbs 1..31 fill up to 255 each, in order
+  return (uint32_t)(q < 0 ? 0 : q > 255 ? 255 : q);
+}
 
 // Database row r (0..15, ascending) of 16-row chunk g of a tensor-core candidate.  The fp16 kernels' chunks are contiguous rows.  The u8
 // kernel's chunk g = 8t + 4h + q is what ONE thread (lane % 4 = q) holds of a query row in the 64-column half h of tile t:

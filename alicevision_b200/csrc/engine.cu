@@ -179,6 +179,7 @@ struct ViewHost {
   void* arena = nullptr; void* raw_own = nullptr;     // the one allocation all device buffers of the view live in; a separately owned `raw`
   bool stored_u8 = false;     // dtype == DT_F32 whose values are integers in 0..255: staged and kept on the device as uchar (hostconv.hpp)
   int32_t* nb32 = nullptr;    // uchar-stored tensor-core views: int32 squared norms of the u8 kernel (prep.cuh)
+  uint8_t* limb8 = nullptr;   // ... and the 32 norm limbs per row of the u8 norm-GEMM kernel (prep.cuh)
   float* d_xy = nullptr; uint32_t* d_yrank = nullptr;   // positions + rank of y on the device (device finishing stage, finish.cuh)
   double2* d_geom = nullptr;  // b200m_set_view_geometry: the (undistorted) positions guided matching uses instead of xy; own allocation
   bool failed = false;       // its upload job failed: the device buffers were never filled
@@ -195,6 +196,11 @@ struct ViewHost {
   bool tc_ok() const { return tc_capable() && (flags & VF_EXACT_MASK) == 0; }
   // real-valued rows may take the tensor-core FILTER path (MODE_REAL): fp16 range and the half-norm limbs must hold, integers need not
   bool real_ok() const { return tc_capable() && (flags & (VF_RANGE | VF_NORM)) == 0 && m <= REAL_MAX_ROWS; }
+  // uchar-stored tensor-core view as the query / the database of the u8 norm-GEMM kernel (l2_tc.cuh NG).  A database needs one full tile of
+  // rows: then at least two chunks hold real rows, and a chunk of padding (whose value the limbs set lower than the u8 kernel's) can never
+  // be one of the two smallest chunk minima the pre-test reads.
+  bool ng_query_ok() const { return limb8 && store_dtype() == DT_U8 && (flags & VF_U8_WIDE) == 0; }
+  bool ng_db_ok() const { return limb8 && store_dtype() == DT_U8 && (flags & VF_U8_NORMCAP) == 0 && m >= tc::BN; }
 };
 
 struct UploadJob {
@@ -277,6 +283,7 @@ struct LastCall {
   int launches, tc_pairs, real_pairs, u8_pairs;
   int64_t records, fallback_rows;
   int batches;                // b200m_match_pairs only
+  int u8_norm_gemm_pairs;     // b200m_match_pairs only: the u8 pairs on the norm-GEMM kernel
 };
 
 // Members are released in reverse order of declaration, after ~b200m_ctx has stopped the uploader and the pool and freed the views:
@@ -325,6 +332,7 @@ struct b200m_ctx {
   std::shared_ptr<Recycler> recycler = std::make_shared<Recycler>();
   bool force_exact = false;
   bool real_tc = true;            // real-valued fp32 pairs on the tensor-core filter kernel (B200M_REAL_TC=0: exact CUDA-core kernel as in round 1)
+  bool u8_norm_gemm = true;       // u8 pairs whose views pass its gates on the norm-GEMM kernel (B200M_U8_NORM_GEMM=0: all on the u8 kernel)
   int first_batch_pairs = 16;     // while uploads are in flight: pairs of the first batch (then 2x per batch): how soon the GPU starts (B200M_FIRST_BATCH)
   long real_fused_rows = 6144;    // average database rows per item from which the real-valued re-scoring runs inside the filter kernel
   int tc_variant = 4;             // tensor-core kernel (l2_tc.cuh): 4 (default) = half-norms folded into the GEMM (AUG), 256-query work items;
@@ -346,9 +354,10 @@ struct b200m_result {
 // ------------------------------------------------------------------------------------------------ helpers
 // Device buffers of one view (stream-ordered allocations out of the default pool).
 // ONE stream-ordered allocation per view, carved into its buffers (a view of 1024 features paid more for its ten allocations and ten
-// frees than for its copy): raw | h16 | nbh | nrm | aug16 | augq16 | err | nb32 | stats | yrank | xy, each 256-byte aligned; stats and yrank are
-// adjacent so that one memset zeroes both.
-// u8_norms: the int32 norms of the u8 search kernel for a uchar-stored view (not for b200m_db_create's databases, which only MODE_KNN reads).
+// frees than for its copy): raw | h16 | nbh | nrm | aug16 | augq16 | err | nb32 | limb8 | stats | yrank | xy, each 256-byte aligned; stats and
+// yrank are adjacent so that one memset zeroes both.
+// u8_norms: the int32 norms and the norm limbs of the u8 search kernels for a uchar-stored view (not for b200m_db_create's databases, which
+// only MODE_KNN reads).
 static int alloc_view_buffers(b200m_ctx* c, ViewHost& v, bool u8_norms = true) {
   const size_t esz = v.store_dtype() == DT_F32 ? 4 : 1;
   auto al = [](size_t x) { return (x + 255) / 256 * 256; };
@@ -360,7 +369,7 @@ static int alloc_view_buffers(b200m_ctx* c, ViewHost& v, bool u8_norms = true) {
   const size_t o_h16 = tcv ? take((size_t)v.m * 128 * 2) : 0, o_nbh = tcv ? take((size_t)v.m_pad * 4) : 0, o_nrm = tcv ? take((size_t)v.m_pad * 4) : 0;
   const size_t o_aug = tcv ? take((size_t)v.m_pad * 32) : 0, o_augq = tcv ? take((size_t)v.m_pad * 32) : 0, o_err = tcv ? take((size_t)v.m_pad * 4) : 0;
   const bool nb32 = tcv && u8_norms && v.store_dtype() == DT_U8;
-  const size_t o_nb32 = nb32 ? take((size_t)v.m_pad * 4) : 0;
+  const size_t o_nb32 = nb32 ? take((size_t)v.m_pad * 4) : 0, o_limb = nb32 ? take((size_t)v.m_pad * 32) : 0;
   const size_t o_stats = tcv ? take(16) : 0;
   const size_t o_yrank = pos ? take((size_t)v.m * 4) : 0, o_xy = pos ? take((size_t)v.m * 8) : 0;
   char* base = nullptr;
@@ -371,6 +380,7 @@ static int alloc_view_buffers(b200m_ctx* c, ViewHost& v, bool u8_norms = true) {
     v.h16 = (__half*)(base + o_h16); v.nbh = (float*)(base + o_nbh); v.nrm = (float*)(base + o_nrm); v.aug16 = (__half*)(base + o_aug);
     v.augq16 = (__half*)(base + o_augq); v.err = (float*)(base + o_err); v.stats = (uint32_t*)(base + o_stats);
     v.nb32 = nb32 ? (int32_t*)(base + o_nb32) : nullptr;
+    v.limb8 = nb32 ? (uint8_t*)(base + o_limb) : nullptr;
   }
   if (pos) { v.d_yrank = (uint32_t*)(base + o_yrank); v.d_xy = (float*)(base + o_xy); }
   return B200M_OK;
@@ -381,7 +391,7 @@ static void free_view_buffers(b200m_ctx* c, ViewHost& v) {
   if (v.d_geom) cudaFreeAsync(v.d_geom, c->stream);        // re-uploading or removing a view drops its geometry positions
   v.arena = nullptr; v.raw_own = nullptr; v.d_geom = nullptr;
   v.raw = nullptr; v.h16 = nullptr; v.nbh = nullptr; v.nrm = nullptr; v.aug16 = nullptr; v.d_xy = nullptr; v.d_yrank = nullptr;
-  v.augq16 = nullptr; v.err = nullptr; v.stats = nullptr; v.nb32 = nullptr;
+  v.augq16 = nullptr; v.err = nullptr; v.stats = nullptr; v.nb32 = nullptr; v.limb8 = nullptr;
 }
 
 // The shutdown that has to stay in this order; the owners among the members release the rest.  Also runs on the partly built
@@ -435,6 +445,13 @@ static int make_view_dev(b200m_ctx* c, const ViewHost& v, ViewDev& d) {
       CUresult r = c->encode(&d.tmap_u8, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void*)v.raw, gdim, ustr, ubox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) return fail(B200M_ERR_CUDA, "cuTensorMapEncodeTiled(u8) failed: " + std::to_string((int)r));
+      // the norm limbs of the norm-GEMM kernel: 32-byte rows in the 32-byte-swizzled layout of the fp16 augmentation columns
+      const cuuint64_t ldim[2] = {32, (cuuint64_t)v.m_pad};
+      const cuuint64_t lstr[1] = {32};
+      const cuuint32_t lbox[2] = {32, 128};
+      r = c->encode(&d.tmap_limb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void*)v.limb8, ldim, lstr, lbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                    CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) return fail(B200M_ERR_CUDA, "cuTensorMapEncodeTiled(limb) failed: " + std::to_string((int)r));
     }
   }
   return B200M_OK;
@@ -445,8 +462,8 @@ static int run_prep(b200m_ctx* c, const ViewHost& v, uint32_t* d_flag, cudaStrea
   if (!v.tc_capable()) return B200M_OK;
   const int grid = (v.m_pad + 7) / 8;
   if (zero_stats) CK(cudaMemsetAsync(v.stats, 0, 16, st));
-  if (v.store_dtype() == DT_F32) prep_view_kernel<float><<<grid, 256, 0, st>>>((const float*)v.raw, v.m, v.h16, v.nbh, v.nrm, v.m_pad, d_flag, v.aug16, v.augq16, v.err, v.stats, nullptr);
-  else prep_view_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)v.raw, v.m, v.h16, v.nbh, v.nrm, v.m_pad, d_flag, v.aug16, v.augq16, v.err, v.stats, v.nb32);
+  if (v.store_dtype() == DT_F32) prep_view_kernel<float><<<grid, 256, 0, st>>>((const float*)v.raw, v.m, v.h16, v.nbh, v.nrm, v.m_pad, d_flag, v.aug16, v.augq16, v.err, v.stats, nullptr, nullptr);
+  else prep_view_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)v.raw, v.m, v.h16, v.nbh, v.nrm, v.m_pad, d_flag, v.aug16, v.augq16, v.err, v.stats, v.nb32, v.limb8);
   CK(cudaGetLastError());
   return B200M_OK;
 }
@@ -511,6 +528,7 @@ static int ensure_batch_buffers(b200m_ctx* c) {
   CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true, tc::MODE_REAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true, true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tc::l2_top2_tc_kernel<true, tc::MODE_KNN>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tc::l2_top2_tc_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<false, false, true>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tc::l2_top2_tc_u8ng_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::Lay<false, false, true, true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(exact_rows_pairs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XP_SMEM));
   CK(cudaFuncSetAttribute(exact_top2_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, EX_SMEM));
   CK(cudaFuncSetAttribute(exact_top2_kernel<uint8_t, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, EX_SMEM));
@@ -639,6 +657,7 @@ int b200m_ctx_create(int device, void* stream, b200m_ctx** out) {
   if (const char* e = getenv("B200M_DEVICE_FINISH")) c->device_finish = atoi(e) != 0;
   if (const char* e = getenv("B200M_FIRST_BATCH")) c->first_batch_pairs = std::max(1, atoi(e));
   if (const char* e = getenv("B200M_REAL_TC")) c->real_tc = atoi(e) != 0;
+  if (const char* e = getenv("B200M_U8_NORM_GEMM")) c->u8_norm_gemm = atoi(e) != 0;
   if (const char* e = getenv("B200M_REAL_FUSED_ROWS")) c->real_fused_rows = std::max(0l, atol(e));
   if (const char* e = getenv("B200M_GUIDED_FAST_LEFT_CAP")) c->gf_left_cap = std::max(1l, atol(e));
   if (const char* e = getenv("B200M_GUIDED_LEFT_CAP")) c->gm_left_cap = std::max(1l, atol(e));
@@ -1137,19 +1156,24 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> kernel_events;
   int launches = 0;
   int64_t total_records = 0, fallback_rows = 0;
-  int real_pairs = 0, u8_pairs = 0;
+  int real_pairs = 0, u8_pairs = 0, ng_pairs = 0;
   const bool real_tc = !c->force_exact && c->real_tc && c->tc_variant == 4;
   // integer-valued pairs whose views are both stored as uchar run the u8 kernel (8-bit tensor cores, exact int32 distances) under the
   // default variant; the other tensor-core pairs run the fp16 kernel
   auto u8_pair = [&](const Directed& d) {
     return d.mode == PM_TC && c->tc_variant == 4 && c->views[d.slot_i].store_dtype() == DT_U8 && c->views[d.slot_j].store_dtype() == DT_U8;
   };
+  // ... and of those, the pairs whose query view has no component above 127 and whose database view's norms fit the limbs run the u8
+  // norm-GEMM kernel (the norms folded into the 8-bit GEMM); the others stay on the u8 kernel
+  auto ng_pair = [&](const Directed& d) {
+    return c->u8_norm_gemm && u8_pair(d) && c->views[d.slot_i].ng_db_ok() && c->views[d.slot_j].ng_query_ok();
+  };
 
   auto enqueue = [&](size_t bi) -> int {
     const Batch& B = batches[bi];
     BatchBuf& bb = c->buf[bi & 1];
     const int np = (int)(B.end - B.begin);
-    uint32_t cbase = 0, sbase = 0; int n_items = 0, n_items_real = 0, n_items_u8 = 0; int max_qblk_exact = 0, max_qblk_ham = 0;
+    uint32_t cbase = 0, sbase = 0; int n_items = 0, n_items_real = 0, n_items_u8 = 0, n_items_ng = 0; int max_qblk_exact = 0, max_qblk_ham = 0;
     // In-kernel exactness pass only when a work item lasts long enough (>= 24 database tiles on average) for two warps to
     // re-score the previous item's candidates behind it; shorter images use the stand-alone exactness kernel.
     // the views of this batch must be complete on the device; their exactness flags decide tensor-core vs exact kernel
@@ -1160,20 +1184,22 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       if ((r2 = ensure_view_ready(c, d.slot_i)) || (r2 = ensure_view_ready(c, d.slot_j))) return r2;
       if (d.mode == PM_TC) {
         const ViewHost& vi = c->views[d.slot_i]; const ViewHost& vj = c->views[d.slot_j];
-        if (!c->force_exact && vi.tc_ok() && vj.tc_ok()) { ++tc_pairs; u8_pairs += u8_pair(d); }
+        if (!c->force_exact && vi.tc_ok() && vj.tc_ok()) { ++tc_pairs; u8_pairs += u8_pair(d); ng_pairs += ng_pair(d); }
         else if (real_tc && vi.real_ok() && vj.real_ok()) { d.mode = PM_TC_REAL; ++real_pairs; }   // real-valued fp32: tensor-core filter + exact re-scoring
         else d.mode = vi.dtype == DT_F32 ? PM_EXACT_F32 : PM_EXACT_U8;
       }
     }
-    long tc_rows = 0, tc_n = 0, real_rows = 0, real_n = 0, u8_rows = 0, u8_n = 0;
+    long tc_rows = 0, tc_n = 0, real_rows = 0, real_n = 0, u8_rows = 0, u8_n = 0, ng_rows = 0, ng_n = 0;
     for (int p = 0; p < np; ++p) {
       const Directed& d = dir[seqv[B.begin + p]];
-      if (u8_pair(d)) { u8_rows += c->views[d.slot_i].m; ++u8_n; }
+      if (ng_pair(d)) { ng_rows += c->views[d.slot_i].m; ++ng_n; }
+      else if (u8_pair(d)) { u8_rows += c->views[d.slot_i].m; ++u8_n; }
       else if (d.mode == PM_TC) { tc_rows += c->views[d.slot_i].m; ++tc_n; }
       if (d.mode == PM_TC_REAL) { real_rows += c->views[d.slot_i].m; ++real_n; }
     }
     const bool fused = c->tc_variant >= 2 && tc_n > 0 && tc_rows / tc_n >= 6144;
     const bool fused_u8 = u8_n > 0 && u8_rows / u8_n >= 6144;
+    const bool fused_ng = ng_n > 0 && ng_rows / ng_n >= 6144;
     const int tc_ctas_per_item = (c->tc_variant == 2 || c->tc_variant == 4) ? 2 : 1;
     const bool fused_real = real_n > 0 && real_rows / real_n >= c->real_fused_rows;
     bool any_f32 = false, any_u8 = false, any_ham = false, any_gf32 = false, any_gu8 = false; int max_qblk_gen = 0;
@@ -1182,7 +1208,7 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       const ViewHost& vi = c->views[d.slot_i]; const ViewHost& vj = c->views[d.slot_j];
       // the CTA-pair kernel runs the exactness pass itself: its candidates are final records
       const bool u8 = u8_pair(d);
-      const uint32_t dev_mode = (d.mode == PM_TC && (u8 ? fused_u8 : fused)) ? (uint32_t)PM_TC_FUSED : d.mode;
+      const uint32_t dev_mode = (d.mode == PM_TC && (ng_pair(d) ? fused_ng : u8 ? fused_u8 : fused)) ? (uint32_t)PM_TC_FUSED : d.mode;
       bb.h_pairs[p] = PairDev{(uint32_t)d.slot_i, (uint32_t)d.slot_j, (uint32_t)vi.m, (uint32_t)vj.m, cbase, dev_mode, sbase, u8 ? 1u : 0u};
       cbase += (uint32_t)vj.m; sbase += (uint32_t)vi.m;
       const int qrows = tc_ctas_per_item * tc::BM;   // queries per work item
@@ -1193,17 +1219,22 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
       if (d.mode == PM_HAMMING) { any_ham = true; max_qblk_ham = std::max(max_qblk_ham, (vj.m + HM_TQ - 1) / HM_TQ); }
       if (d.mode == PM_GENERIC_F32 || d.mode == PM_GENERIC_U8) { (d.mode == PM_GENERIC_F32 ? any_gf32 : any_gu8) = true; max_qblk_gen = std::max(max_qblk_gen, (vj.m + 3) / 4); }
     }
-    // the u8 kernel's work items (256 queries each) follow the fp16 kernel's in the same table
+    // the u8 kernel's work items (256 queries each) follow the fp16 kernel's in the same table, and the norm-GEMM kernel's follow those
     for (int p = 0; p < np; ++p) {
       const Directed& d = dir[seqv[B.begin + p]];
-      if (u8_pair(d)) for (int qt = 0; qt < (c->views[d.slot_j].m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items[n_items + n_items_u8++] = WorkItem{(uint32_t)p, (uint32_t)qt};
+      if (u8_pair(d) && !ng_pair(d)) for (int qt = 0; qt < (c->views[d.slot_j].m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items[n_items + n_items_u8++] = WorkItem{(uint32_t)p, (uint32_t)qt};
     }
+    for (int p = 0; p < np; ++p) {
+      const Directed& d = dir[seqv[B.begin + p]];
+      if (ng_pair(d)) for (int qt = 0; qt < (c->views[d.slot_j].m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items[n_items + n_items_u8 + n_items_ng++] = WorkItem{(uint32_t)p, (uint32_t)qt};
+    }
+    const int n_items_tab = n_items + n_items_u8 + n_items_ng;
     // Three streams so that consecutive batches' search kernels run back to back: the pair / work-item tables of this batch travel on
     // `tab_stream` (issued while the previous batch is still searching), the packing / finishing kernels and the meta read-back of this
     // batch run on `pack_stream` beside the next batch's search kernel.  Buffer set (bi & 1) is free: the host has seen ev_meta of batch bi-2.
     cudaStream_t ts = c->pipe_streams ? c->tab_stream : c->stream, ps = c->pipe_streams ? c->pack_stream : c->stream;
     CK(cudaMemcpyAsync(bb.d_pairs, bb.h_pairs, sizeof(PairDev) * np, cudaMemcpyHostToDevice, ts));
-    if (n_items + n_items_u8) CK(cudaMemcpyAsync(bb.d_items, bb.h_items, sizeof(WorkItem) * (n_items + n_items_u8), cudaMemcpyHostToDevice, ts));
+    if (n_items_tab) CK(cudaMemcpyAsync(bb.d_items, bb.h_items, sizeof(WorkItem) * n_items_tab, cudaMemcpyHostToDevice, ts));
     if (n_items_real) CK(cudaMemcpyAsync(bb.d_items_real, bb.h_items_real, sizeof(WorkItem) * n_items_real, cudaMemcpyHostToDevice, ts));
     CK(cudaMemsetAsync(bb.d_count, 0, sizeof(int) * np, ts));
     CK(cudaMemsetAsync(bb.d_fb_count, 0, 2 * sizeof(int), ts));
@@ -1211,8 +1242,11 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
     if (c->pipe_streams) { CK(cudaEventRecord(bb.ev_tab, ts)); CK(cudaStreamWaitEvent(c->stream, bb.ev_tab, 0)); }
     cudaEvent_t k0 = timing_event(c, tev_used), k1 = timing_event(c, tev_used);
     CK(cudaEventRecord(k0, c->stream));
-    // the debug trace (one kernel's CTA 0) shows the u8 kernel when the batch has u8 pairs, else the fp16 kernel
-    long long* fp16_trace = n_items_u8 ? nullptr : (long long*)c->d_trace;
+    // the debug trace (one kernel's CTA 0) shows the norm-GEMM kernel when the batch has pairs on it, else the u8 kernel when it has u8
+    // pairs, else the fp16 kernel
+    long long* ng_trace = c->d_trace;
+    long long* u8_trace = n_items_ng ? nullptr : ng_trace;
+    long long* fp16_trace = (n_items_ng || n_items_u8) ? nullptr : ng_trace;
     if (n_items) {
       const int grid = tc_ctas_per_item * std::min(n_items, c->num_sms / tc_ctas_per_item);   // one CTA per SM, whole work items per CTA group
       if (c->tc_variant == 4)
@@ -1224,7 +1258,14 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
     if (n_items_u8) {
       const int grid = 2 * std::min(n_items_u8, c->num_sms / 2);
       tc::l2_top2_tc_u8_kernel<<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false, false, true>::SMEM_BYTES, c->stream>>>(
-          c->d_views, bb.d_pairs, bb.d_items + n_items, n_items_u8, 2, bb.d_cands, bb.d_count, ratio_sq, c->d_trace, c->d_err, (int)fused_u8, nullptr, FbSink{});
+          c->d_views, bb.d_pairs, bb.d_items + n_items, n_items_u8, 2, bb.d_cands, bb.d_count, ratio_sq, u8_trace, c->d_err, (int)fused_u8, nullptr, FbSink{});
+      ++launches;
+    }
+    if (n_items_ng) {
+      const int grid = 2 * std::min(n_items_ng, c->num_sms / 2);
+      tc::l2_top2_tc_u8ng_kernel<<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false, false, true, true>::SMEM_BYTES, c->stream>>>(
+          c->d_views, bb.d_pairs, bb.d_items + n_items + n_items_u8, n_items_ng, 2, bb.d_cands, bb.d_count, ratio_sq, ng_trace, c->d_err, (int)fused_ng,
+          nullptr, FbSink{});
       ++launches;
     }
     if (n_items_real) {
@@ -1435,7 +1476,7 @@ static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, fl
   }
   if (timing) fprintf(stderr, "[b200m] match_pairs n=%d stage=%d: setup %.2f ms, batches %.2f ms (gpu %.2f), tail (cross+assemble) %.2f ms, total %.2f ms\n",
                       n_pairs, stage, t_setup - t_begin, t_gpu_done - t_setup, ms, now() - t_gpu_done, now() - t_begin);
-  c->last = LastCall{ms, sk, launches, tc_pairs, real_pairs, u8_pairs, total_records, fallback_rows, (int)batches.size()};
+  c->last = LastCall{ms, sk, launches, tc_pairs, real_pairs, u8_pairs, total_records, fallback_rows, (int)batches.size(), ng_pairs};
   *out = res.release();
   return B200M_OK;
 }
@@ -1463,6 +1504,7 @@ unsigned b200m_exactness_errors(const b200m_ctx* c) { return c ? c->err_total : 
 int64_t b200m_last_records(const b200m_ctx* c) { return last_call(c).records; }
 int b200m_last_real_tc_pairs(const b200m_ctx* c) { return last_call(c).real_pairs; }
 int b200m_last_u8_tc_pairs(const b200m_ctx* c) { return last_call(c).u8_pairs; }
+int b200m_last_u8_norm_gemm_pairs(const b200m_ctx* c) { return last_call(c).u8_norm_gemm_pairs; }
 int64_t b200m_last_fallback_rows(const b200m_ctx* c) { return last_call(c).fallback_rows; }
 int b200m_last_batches(const b200m_ctx* c) { return last_call(c).batches; }
 

@@ -29,7 +29,14 @@
 //                per thread, then the chunk-minimum epilogue on those registers.  The two warpgroups run independently, so
 //                one warpgroup's epilogue overlaps the other's MMAs.  The u8 kernel (4 wgmma.m64n128k32 per tile) pipelines each
 //                warpgroup's tiles over two accumulators instead, so that its epilogue overlaps its own next MMAs.
+//                The u8 norm-GEMM kernel (NG) adds a 5th K32 step that puts the database norm into the accumulator as well (below).
 //   MODE_REAL adds six re-scoring warps (12-17).
+//
+// NG (u8 norm-GEMM kernel, template flag of the u8 body): for query views with every component <= 127, the query tile is doubled in
+// shared memory (2a fits in u8) and a 5th K-step, m64n128k32 s8 x u8, multiplies constant weights [-1, -128 x 31] by the database row's 32
+// norm limbs (common.cuh u8_limb), so the exact s32 accumulator is 2 a.b - ||b||^2 = -s: the epilogue is an integer max per chunk with no
+// shared-memory reads and no per-element arithmetic.  Views with a component above 127 (as queries) or a norm above the limbs' capacity
+// (as databases) stay on the u8 kernel (VF_U8_WIDE, VF_U8_NORMCAP).
 //
 // MODE (template): what the epilogue keeps per query row and what leaves the kernel
 //   MODE_MATCH  integer-valued descriptors (exact accumulators): two smallest chunk minima + chunk of the best, ratio pre-test,
@@ -69,6 +76,7 @@ constexpr int DB_BYTES = 2 * KB_BYTES;    // 32 KB
 constexpr int AUG_BYTES = 128 * 16 * 2;   // 4 KB: 16 augmentation columns of 128 rows
 constexpr int NB_BYTES = BN * 4;          // half-norms (u8: int32 norms) of one tile
 constexpr int U8_BYTES = 128 * 128;       // 16 KB: 128 uchar rows of 128 B = one TMA box of tmap_u8 (the whole K of a u8 query or database tile)
+constexpr int LIMB_BYTES = BN * 32;       // 4 KB: the 32 norm limbs of 128 database rows (NG), or the constant weight tile of 128 query rows
 constexpr int EPI_WARPS = 8;
 // u8 kernel: per-thread registers after set-up, warpgroup 0 (producer, exactness pass) and the two consumer warpgroups (two 64-register
 // accumulators).  setmaxnreg moves them inside the launch allocation of 384 x 128: 128 * U8_REGS_WG0 + 256 * U8_REGS_CONSUMER <= 49152.
@@ -77,16 +85,17 @@ constexpr int U8_REGS_CONSUMER = 160;
 static_assert(128 * U8_REGS_WG0 + 256 * U8_REGS_CONSUMER <= 384 * 128, "the u8 kernel's register split exceeds its launch allocation");
 enum : int { MODE_MATCH = 0, MODE_KNN = 1, MODE_REAL = 2 };
 
-template <bool AUG, bool REAL = false, bool U8 = false> struct Lay {
+template <bool AUG, bool REAL = false, bool U8 = false, bool NG = false> struct Lay {
   // database ring slots (AUG: leaves shared memory to L1 for the re-scoring warps; U8: half-size stages, twice as many in about the same bytes)
   static constexpr int NS = U8 ? 8 : AUG ? 3 : 4;
   static constexpr int QT = U8 ? U8_BYTES : Q_BYTES;                 // one query tile buffer
-  // + augmentation columns, or the (half-)norms (padded: tiles stay 1024-B aligned)
-  static constexpr int STAGE = U8 ? U8_BYTES + 1024 : DB_BYTES + (AUG ? AUG_BYTES : 1024);
+  // + augmentation columns, the (half-)norms (padded: tiles stay 1024-B aligned) or (NG) the norm limbs
+  static constexpr int STAGE = U8 ? U8_BYTES + (NG ? LIMB_BYTES : 1024) : DB_BYTES + (AUG ? AUG_BYTES : 1024);
   static constexpr int OFF_Q = 0;
   static constexpr int OFF_DB = OFF_Q + 2 * QT;
-  static constexpr int OFF_A = OFF_DB + NS * STAGE;                  // AUG: the constant A tile of the 9th K-step; REAL: the query's own limb tile, 2 buffers
-  static constexpr int OFF_MRG = OFF_A + (AUG ? (REAL ? 2 : 1) * AUG_BYTES : 0);   // per-row merged state, 2 buffers x 128 x 16 B
+  // AUG: the constant A tile of the 9th K-step; REAL: the query's own limb tile, 2 buffers; NG: the constant weight tile of the 5th K-step
+  static constexpr int OFF_A = OFF_DB + NS * STAGE;
+  static constexpr int OFF_MRG = OFF_A + (AUG ? (REAL ? 2 : 1) * AUG_BYTES : NG ? LIMB_BYTES : 0);   // per-row merged state, 2 buffers x 128 x 16 B
   static constexpr int OFF_VQ = OFF_MRG + 2 * BM * 16;               // candidate queue: 2 buffers x 128 Cand (32 slots per row quadrant)
   static constexpr int OFF_VQX = OFF_VQ + 2 * BM * 16;               // REAL: 5th word of the queued candidates (p4), 2 x 128 x 4 B
   static constexpr int OFF_VQN = OFF_VQX + (REAL ? 2 * BM * 4 : 0);  // 2 x (4 per-quadrant counts + pair index), 32 B each
@@ -185,6 +194,11 @@ __device__ __forceinline__ int32_t min16(const int32_t (&x)[16]) {
   const int32_t d = __vimin3_s32(x[9], x[10], x[11]), e = __vimin3_s32(x[12], x[13], x[14]);
   return min(__vimin3_s32(a, b, c), __vimin3_s32(d, e, x[15]));
 }
+__device__ __forceinline__ int32_t max16(const int32_t (&x)[16]) {
+  const int32_t a = __vimax3_s32(x[0], x[1], x[2]), b = __vimax3_s32(x[3], x[4], x[5]), c = __vimax3_s32(x[6], x[7], x[8]);
+  const int32_t d = __vimax3_s32(x[9], x[10], x[11]), e = __vimax3_s32(x[12], x[13], x[14]);
+  return max(__vimax3_s32(a, b, c), __vimax3_s32(d, e, x[15]));
+}
 
 // The u8 epilogue of one tile, from the s32 accumulator acc = a.b (exact).  Per element s = ||b||^2 - 2 a.b = ||a - b||^2 - ||a||^2
 // (u8_elem), chunk minima in integers, and only the four minima per thread become h = s / 2: exactly the fp16 kernel's accumulator value
@@ -209,14 +223,32 @@ __device__ __forceinline__ void u8_tile_minima(const int32_t (&acc)[64], const i
   }
 }
 
+// The norm-GEMM (NG) epilogue of one tile: the accumulator already holds acc = 2 a.b - ||b||^2 = -s (exact s32), so a chunk minimum of s is
+// minus the chunk maximum of acc, and h = s / 2 is exactly what u8_tile_minima computes.  Same chunks and v2 layout as there.  Pad rows:
+// a.b = 0 (TMA zero fill) and all limbs 255 -> s = U8_LIMB_PAD, above every real row's s <= ||b||^2 <= U8_LIMB_CAP.
+__device__ __forceinline__ void u8ng_tile_minima(const int32_t (&acc)[64], float (&v2)[2][2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    int32_t x[2][16];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int a = 32 * h + 4 * j;
+      x[0][2 * j] = acc[a + 0]; x[0][2 * j + 1] = acc[a + 1];
+      x[1][2 * j] = acc[a + 2]; x[1][2 * j + 1] = acc[a + 3];
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) v2[r][h] = 0.5f * (float)(-max16(x[r]));   // |s| < 2^24: exact, and +0 for s = 0 as in u8_half_dist
+  }
+}
+
 // The real-valued re-scoring reads 32 fp32 rows per candidate (16 KB, mostly from HBM) and is latency-bound: two warps cannot keep up with
 // the tensor cores, so MODE_REAL adds six re-scoring warps behind the epilogue warps.
 constexpr int REAL_EXTRA_VERIFY_WARPS = 6;
 template <int MODE> constexpr int block_threads() { return 128 + EPI_WARPS * 32 + (MODE == MODE_REAL ? REAL_EXTRA_VERIFY_WARPS * 32 : 0); }
 
 // The kernel body (entry points at the end of the file).  U8: the operands are the views' uchar rows (tmap_u8) on the 8-bit tensor cores,
-// MODE_MATCH only; see the consumer loop.
-template <bool AUG, int MODE, bool U8>
+// MODE_MATCH only; see the consumer loop.  NG (with U8): the norm-GEMM kernel (header comment).
+template <bool AUG, int MODE, bool U8, bool NG = false>
 __device__ __forceinline__ void
 l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs, const WorkItem* __restrict__ items, int n_items,
            int ctas_per_item, Cand* __restrict__ cands, int* __restrict__ cand_count, float ratio_sq, long long* __restrict__ trace_buf,
@@ -226,7 +258,8 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
   constexpr int VERIFY_WARPS_K = REAL ? 2 + REAL_EXTRA_VERIFY_WARPS : 2;   // warps 2, 3 (+ the warps behind the epilogue warps)
   static_assert(!(REAL || KNN) || AUG, "MODE_REAL / MODE_KNN exist for the AUG layout only");
   static_assert(!U8 || (MODE == MODE_MATCH && !AUG), "the u8 kernel is MODE_MATCH with its norms in the database ring");
-  using L = Lay<AUG, REAL, U8>;
+  static_assert(!NG || U8, "the norm-GEMM kernel is a form of the u8 kernel");
+  using L = Lay<AUG, REAL, U8, NG>;
   constexpr int NS = L::NS, STAGE = L::STAGE, QT = L::QT;
   extern __shared__ __align__(1024) uint8_t smem[];   // SWIZZLE_128B operand tiles need 1024-B alignment
   if ((ptx::smem_u32(smem) & 1023u) != 0) { asm volatile("trap;"); }
@@ -266,6 +299,17 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
     rowp[sw ^ 1] = make_uint4(0u, 0u, 0u, 0u);
     ptx::fence_proxy_async();          // generic-proxy stores -> visible to the tensor core (async proxy)
   }
+  if (NG && warp >= 4 && warp < 8) {
+    // the constant s8 weight tile of the 5th K-step: 128 rows x 32 B in the 32-byte-swizzled K-major layout (16-byte chunk index XOR
+    // ((row >> 2) & 1)); logical chunk 0 = [-1, -128 x 15], chunk 1 = [-128 x 16] (U8_LIMB_W0, U8_LIMB_W)
+    static_assert(U8_LIMB_W0 == -1 && U8_LIMB_W == -128, "the weight bytes below");
+    const int r = (warp - 4) * 32 + lane;
+    uint4* rowp = reinterpret_cast<uint4*>(smem + L::OFF_A + r * 32);
+    const int sw = (r >> 2) & 1;
+    rowp[sw] = make_uint4(0x808080FFu, 0x80808080u, 0x80808080u, 0x80808080u);
+    rowp[sw ^ 1] = make_uint4(0x80808080u, 0x80808080u, 0x80808080u, 0x80808080u);
+    ptx::fence_proxy_async();
+  }
   __syncthreads();
 
   auto producer = [&](int rank, int cl) {
@@ -294,7 +338,11 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
           ptx::mbar_wait(&db_empty[st], sph ^ 1);
           ptx::trace_stamp(trace, 0, tt, 0);
           uint8_t* ds = smem + L::OFF_DB + st * STAGE;
-          if (U8) {
+          if (NG) {
+            ptx::mbar_arrive_expect_tx(&db_full[st], U8_BYTES + LIMB_BYTES);
+            ptx::tma_load_2d(ds, &vi->tmap_u8, &db_full[st], 0, t * BN);
+            ptx::tma_load_2d(ds + U8_BYTES, &vi->tmap_limb, &db_full[st], 0, t * BN);
+          } else if (U8) {
             ptx::mbar_arrive_expect_tx(&db_full[st], U8_BYTES + NB_BYTES);
             ptx::tma_load_2d(ds, &vi->tmap_u8, &db_full[st], 0, t * BN);
             ptx::bulk_load_1d(ds + U8_BYTES, vi->nb32 + (size_t)t * BN, NB_BYTES, &db_full[st]);
@@ -389,9 +437,24 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
         // Software pipeline over the item's tiles: the MMAs of tile t + 1 are issued into the other accumulator before the epilogue of
         // tile t, and wgmma.wait_group 1 waits for tile t's group only, so each warpgroup's epilogue runs under its own next MMAs.  The
         // pipeline fills and drains inside the work item: the item boundary (q_empty, the merge, the candidate hand-off) is unchanged.
-        // Slot t is released after its epilogue (its norms are read there), one MMA group later than without the pipeline.
+        // Slot t is released after its epilogue (its norms are read there), one MMA group later than without the pipeline; NG reads nothing
+        // from the slot in its epilogue and releases it as soon as tile t's MMAs have completed.
         const int nt = __shfl_sync(0xffffffffu, ntiles, 0);           // warp-uniform bounds keep the wgmma pipeline out of divergent paths
         const uint32_t a_base = q_addr + qb * QT;
+        if constexpr (NG) {
+          // 2a in place: this warpgroup's 64 query rows (8 KB, contiguous whatever the swizzle).  Every byte is <= 127 (VF_U8_WIDE), so a
+          // left shift of each 32-bit word doubles its four bytes without carries.  The exactness pass reads the queries from global memory.
+          uint4* qw = reinterpret_cast<uint4*>(smem + L::OFF_Q + qb * QT + wg * 64 * 128);
+          const int tid = (warp & 3) * 32 + lane;
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            uint4 x = qw[tid + 128 * k];
+            x.x <<= 1; x.y <<= 1; x.z <<= 1; x.w <<= 1;
+            qw[tid + 128 * k] = x;
+          }
+          ptx::fence_proxy_async();                                    // generic-proxy stores -> visible to this warpgroup's wgmma
+          if (wg == 0) ptx::named_bar_sync(2, 128); else ptx::named_bar_sync(3, 128);   // immediate ids: ptxas reserves all 16 for a register id
+        }
         uint32_t ist = st, isph = sph;                                 // ring slot of the next tile to issue
         auto issue = [&](int32_t (&acc)[64]) {
           const uint32_t b_base = db_addr + ist * STAGE;
@@ -399,6 +462,7 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
 #pragma unroll
           for (int k = 0; k < 4; ++k)
             ptx::wgmma_m64n128k32_u8(acc, ptx::wgmma_desc_k_sw128(a_base + k * 32), ptx::wgmma_desc_k_sw128(b_base + k * 32), k > 0 ? 1u : 0u);
+          if (NG) ptx::wgmma_m64n128k32_s8u8(acc, ptx::wgmma_desc_k_sw32(a_aug), ptx::wgmma_desc_k_sw32(b_base + U8_BYTES), 1u);   // - ||b||^2
           ptx::wgmma_commit();
           if (++ist == NS) { ist = 0; isph ^= 1; }
         };
@@ -417,8 +481,13 @@ l2_top2_tc(const ViewDev* __restrict__ views, const PairDev* __restrict__ pairs,
           }
           ptx::trace_stamp(etrace, 1 + wg, tt, 2);
           float v2[2][2];
-          u8_tile_minima(acc, reinterpret_cast<const int2*>(smem + L::OFF_DB + st * STAGE + U8_BYTES) + qlane, v2);
-          release_slot();
+          if (NG) {
+            release_slot();
+            u8ng_tile_minima(acc, v2);
+          } else {
+            u8_tile_minima(acc, reinterpret_cast<const int2*>(smem + L::OFF_DB + st * STAGE + U8_BYTES) + qlane, v2);
+            release_slot();
+          }
           fold_tile(t, v2);
           ptx::trace_stamp(etrace, 1 + wg, tt, 3); ++tt;
         };
@@ -600,6 +669,10 @@ __global__ void __launch_bounds__(block_threads<MODE>(), 1) l2_top2_tc_kernel(B2
 // 160 (U8_REGS_CONSUMER) for their two accumulators.
 __global__ void __maxnreg__(128) l2_top2_tc_u8_kernel(B200M_TC_PARAMS) {
   l2_top2_tc<false, MODE_MATCH, true>(B200M_TC_ARGS);
+}
+// The u8 norm-GEMM kernel: the same launch shape and register split.
+__global__ void __maxnreg__(128) l2_top2_tc_u8ng_kernel(B200M_TC_PARAMS) {
+  l2_top2_tc<false, MODE_MATCH, true, true>(B200M_TC_ARGS);
 }
 
 #undef B200M_TC_PARAMS

@@ -38,11 +38,14 @@ __device__ __forceinline__ void halfnorm_limbs(float s, bool integer_valued, flo
 //   err   ||row - fp16(row)||_2 inflated by 2^-9 (upper bound of the rounding error norm), 0 for integer-valued rows
 //   stats [0] = max err over the view, [1] = max nrm  (float bits, atomicMax on the non-negative patterns)
 //   nb32  (uchar-stored views, else nullptr) m_pad x int32 ||row||^2 + U8_NORM_BIAS for the u8 kernel; pad rows 2^24 + U8_NORM_BIAS (see below)
+//   limb8 (uchar-stored views, else nullptr) m_pad x 32 u8 norm limbs of the norm-GEMM kernel (common.cuh u8_limb); pad rows all 255, and the
+//         flags VF_U8_WIDE / VF_U8_NORMCAP that gate it
 template <typename T>
 __global__ void __launch_bounds__(256)
 prep_view_kernel(const T* __restrict__ raw, int m, __half* __restrict__ h16, float* __restrict__ nbh, float* __restrict__ nrm,
                  int m_pad, uint32_t* __restrict__ flags, __half* __restrict__ aug16, __half* __restrict__ augq16,
-                 float* __restrict__ err, uint32_t* __restrict__ stats, int32_t* __restrict__ nb32) {
+                 float* __restrict__ err, uint32_t* __restrict__ stats, int32_t* __restrict__ nb32,
+                 uint8_t* __restrict__ limb8) {
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= m_pad) return;
@@ -54,6 +57,7 @@ prep_view_kernel(const T* __restrict__ raw, int m, __half* __restrict__ h16, flo
     // exactness pass re-scores the one real chunk.  (A pad half-norm below 2^21 + 2^22 lost to anti-correlated queries.)
     // The u8 kernel's pad rows (zero-filled by TMA, a.b = 0) get s = ||b||^2 - 2 a.b = 2^24 and h = s/2 = 2^23: the same value as here.
     if (lane == 0) { nbh[row] = 1e30f; err[row] = 0.f; if (nb32) nb32[row] = (1 << 24) + U8_NORM_BIAS; }
+    if (limb8) limb8[(size_t)row * 32 + lane] = 255;     // U8_LIMB_PAD: above every real row's norm, so s = U8_LIMB_PAD - 0 never wins
     if (lane < 16) {
       aug16[(size_t)row * 16 + lane] = __float2half_rn(lane == 2 ? 4096.f : (lane >= 3 && lane < 6) ? (lane == 3 ? -0.5f : lane == 4 ? -1.f : -2048.f) : 0.f);
       augq16[(size_t)row * 16 + lane] = __float2half_rn(cst);
@@ -66,6 +70,7 @@ prep_view_kernel(const T* __restrict__ raw, int m, __half* __restrict__ h16, flo
     const float v = (float)raw[(size_t)row * 128 + lane + 32 * k];
     if (v != rintf(v)) f |= VF_NONINTEGER;
     if (!(fabsf(v) <= 1024.f)) f |= VF_RANGE;
+    if (limb8 && v > 127.f) f |= VF_U8_WIDE;
     const __half hv = __float2half_rn(v);
     h16[(size_t)row * 128 + lane + 32 * k] = hv;
     const float r = __half2float(hv);
@@ -78,6 +83,10 @@ prep_view_kernel(const T* __restrict__ raw, int m, __half* __restrict__ h16, flo
     s += __shfl_xor_sync(0xffffffffu, s, o); e2 += __shfl_xor_sync(0xffffffffu, e2, o); f |= __shfl_xor_sync(0xffffffffu, f, o);
   }
   if (!(s < 4194304.f)) f |= VF_NORM;
+  if (limb8) {
+    if (s > (float)U8_LIMB_CAP) f |= VF_U8_NORMCAP;     // s is an exact integer here (uchar rows)
+    limb8[(size_t)row * 32 + lane] = (uint8_t)u8_limb((int32_t)s, lane);
+  }
   const float er = (f & VF_NONINTEGER) ? sqrtf(e2) * (1.f + 1.f / 512.f) + 1e-30f : 0.f;
   if (lane == 0) {
     nrm[row] = s;

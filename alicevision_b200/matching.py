@@ -36,6 +36,7 @@ ABI_SYMBOLS = [
     "b200m_ctx_set_force_exact", "b200m_ctx_set_tc_variant", "b200m_debug_trace", "b200m_debug_convert_f32_u8", "b200m_db_create", "b200m_db_destroy", "b200m_knn", "b200m_upload_view", "b200m_upload_views", "b200m_upload_views_async", "b200m_wait_uploads", "b200m_clear_views", "b200m_remove_view",
     "b200m_match_pairs", "b200m_result_num_pairs", "b200m_result_get", "b200m_result_free", "b200m_last_gpu_ms",
     "b200m_last_search_kernel_ms", "b200m_last_launches", "b200m_last_tc_pairs", "b200m_exactness_errors", "b200m_last_records", "b200m_last_real_tc_pairs", "b200m_last_fallback_rows", "b200m_last_u8_tc_pairs", "b200m_last_batches",
+    "b200m_last_u8_norm_gemm_pairs",
     "b200m_shard_pairs", "b200m_shard_pairs_2d", "b200m_multi_create", "b200m_multi_destroy", "b200m_multi_num_devices", "b200m_multi_ctx", "b200m_multi_match",
     "b200m_multi_last_gpu_ms", "b200m_guided_match", "b200m_guided_match_model", "b200m_set_view_geometry", "b200m_guided_match_fast_pairs",
     "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
@@ -159,6 +160,7 @@ class Context:
     def last_real_tc_pairs(self) -> int: return self.lib.b200m_last_real_tc_pairs(self._h)
     def last_fallback_rows(self) -> int: return self.lib.b200m_last_fallback_rows(self._h)
     def last_u8_tc_pairs(self) -> int: return self.lib.b200m_last_u8_tc_pairs(self._h)
+    def last_u8_norm_gemm_pairs(self) -> int: return self.lib.b200m_last_u8_norm_gemm_pairs(self._h)
     def last_batches(self) -> int: return self.lib.b200m_last_batches(self._h)
 
     def set_view_geometry(self, view_id: int, xy) -> None:

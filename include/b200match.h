@@ -348,6 +348,10 @@ int64_t b200m_last_fallback_rows(const b200m_ctx* ctx);
 /* the tensor-core pairs of the last call (counted in b200m_last_tc_pairs too) whose two views are stored as uchar and ran on the 8-bit
  * tensor cores (exact int32 distances) */
 int b200m_last_u8_tc_pairs(const b200m_ctx* ctx);
+/* the u8 pairs of the last b200m_match_pairs (counted in b200m_last_u8_tc_pairs too) that ran on the u8 norm-GEMM kernel: query view
+ * without a component above 127, database view of at least 128 rows whose squared norms fit its limbs (<= 1,011,967), and
+ * B200M_U8_NORM_GEMM not set to 0 */
+int b200m_last_u8_norm_gemm_pairs(const b200m_ctx* ctx);
 /* batches the last b200m_match_pairs split its directed pairs into (skipped pairs included); 0 after the other calls */
 int b200m_last_batches(const b200m_ctx* ctx);
 

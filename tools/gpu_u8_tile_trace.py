@@ -1,6 +1,7 @@
-"""Per-tile pipeline trace of the u8 search kernel (l2_tc.cuh, U8) on the GPU: where one tile's cycles go.
+"""Per-tile pipeline trace of the u8 search kernels (l2_tc.cuh, U8 and its norm-GEMM form NG) on the GPU: where one tile's cycles go.
 
-Builds the library if needed, matches 20 x 8192 uchar SIFT images (190 pairs, every pair on the u8 kernel) with
+Builds the library if needed, matches 20 x 8192 uchar SIFT images (190 pairs, every pair on the norm-GEMM kernel, or on the u8 kernel
+under B200M_U8_NORM_GEMM=0) with
 `Context.debug_trace` on, and prints one JSON line: the medians, in SM cycles, of what CTA 0 stamped per database tile t.
 Each warpgroup runs the tiles of a work item as a pipeline: it issues the MMAs of tile t + 1, then waits for tile t's and runs
 tile t's epilogue while tile t + 1's MMAs run.  The columns are
@@ -79,7 +80,8 @@ def main():
     ctx.debug_trace(False)
     if ctx.last_u8_tc_pairs() != len(pairs) or ctx.exactness_errors() != 0:
         raise SystemExit(f"u8 pairs {ctx.last_u8_tc_pairs()} of {len(pairs)}, exactness errors {ctx.exactness_errors()}")
-    out = {"workload": f"{args.images} x {args.features} uchar SIFT, {len(pairs)} pairs, CTA 0 of l2_top2_tc_u8_kernel", "unit": "SM cycles (median per tile)",
+    kernel = "l2_top2_tc_u8ng_kernel" if ctx.last_u8_norm_gemm_pairs() == len(pairs) else "l2_top2_tc_u8_kernel"
+    out = {"workload": f"{args.images} x {args.features} uchar SIFT, {len(pairs)} pairs, CTA 0 of {kernel}", "unit": "SM cycles (median per tile)",
            "search_kernel_ms": ctx.last_search_kernel_ms(), "gpu": gpu_info(args.device)}
     out.update(medians(trace))
     print(json.dumps(out))
