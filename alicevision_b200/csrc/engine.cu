@@ -209,22 +209,27 @@ struct UploadJob {
   std::shared_ptr<std::vector<int>> bad = std::make_shared<std::vector<int>>();   // per view: the checked f32 -> u8 conversion hit a value it cannot hold
 };
 
-struct BatchBuf {
-  DeviceBuffer<PairDev> d_pairs; DeviceBuffer<WorkItem> d_items; DeviceBuffer<Cand> d_cands; DeviceBuffer<int> d_count, d_off;
-  DeviceBuffer<Rec> d_out;
-  DeviceBuffer<FinMatch> d_fin; DeviceBuffer<int> d_fin_count; DeviceBuffer<uint32_t> d_scratch;   // device finishing stage (finish.cuh)
-  DeviceBuffer<WorkItem> d_items_real; PinnedBuffer<WorkItem> h_items_real;                     // work items of the real-valued pairs (own launch)
-  DeviceBuffer<uint32_t> d_candx; DeviceBuffer<uint4> d_fb; DeviceBuffer<int> d_fb_count;      // fallback lists: d_fb_count = [overflow count, total]
-  DeviceBuffer<uint4> d_fb_pair; DeviceBuffer<int> d_fb_pair_cnt;    // real-valued path: 5th candidate word, fallback list (pair, query)
-  PinnedBuffer<PairDev> h_pairs; PinnedBuffer<WorkItem> h_items; PinnedBuffer<int> h_meta; PinnedBuffer<Rec> h_out;
-  Event ev_meta, ev_copy, ev_tab;
-};
-
 constexpr int PAIR_CAP = 4096;            // directed pairs per batch
 constexpr long CAND_CAP = 4l << 20;       // candidate slots per batch (sum of m_j)
 constexpr long ITEM_CAP = CAND_CAP / 64 + PAIR_CAP;
 constexpr long SLOT_CAP = 8l << 20;       // database rows per batch (sum of m_i): scratch of the device finishing stage
 constexpr int META_INTS = 3 * PAIR_CAP + 3;   // pinned per-batch read-back: counts | offsets (+1) | finishing counts | fallback rows of the real-valued path
+
+struct BatchBuf {
+  DeviceBuffer<PairDev> d_pairs; DeviceBuffer<WorkItem> d_items; DeviceBuffer<Cand> d_cands; DeviceBuffer<int> d_count, d_off;
+  DeviceBuffer<Rec> d_out;
+  DeviceBuffer<FinMatch> d_fin; DeviceBuffer<int> d_fin_count; DeviceBuffer<uint32_t> d_scratch;   // device finishing stage (finish.cuh)
+  DeviceBuffer<uint32_t> d_candx; DeviceBuffer<uint4> d_fb; DeviceBuffer<int> d_fb_count;      // fallback lists: d_fb_count = [overflow count, total]
+  DeviceBuffer<uint4> d_fb_pair; DeviceBuffer<int> d_fb_pair_cnt;    // real-valued path: 5th candidate word, fallback list (pair, query)
+  PinnedBuffer<PairDev> h_pairs; PinnedBuffer<WorkItem> h_items; PinnedBuffer<int> h_meta; PinnedBuffer<Rec> h_out;
+  Event ev_meta, ev_copy, ev_tab;
+  // the regions of the meta block (META_INTS): per-pair record counts, record offsets (np + 1, the last one the batch's total),
+  // per-pair counts of the device finishing stage, and the fallback rows of the real-valued path
+  int* meta_counts() const { return h_meta; }
+  int* meta_offsets() const { return h_meta + PAIR_CAP; }
+  int* meta_fin_counts() const { return h_meta + 2 * PAIR_CAP + 2; }
+  int* meta_fallback_rows() const { return h_meta + 3 * PAIR_CAP + 2; }
+};
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -513,10 +518,10 @@ static int ensure_batch_buffers(b200m_ctx* c) {
         (rc = b.d_cands.reserve(sizeof(Cand) * CAND_CAP)) || (rc = b.d_count.reserve(sizeof(int) * PAIR_CAP)) ||
         (rc = b.d_off.reserve(sizeof(int) * (PAIR_CAP + 1))) || (rc = b.d_out.reserve(sizeof(Rec) * CAND_CAP)) ||
         (rc = b.d_fin.reserve(sizeof(FinMatch) * CAND_CAP)) || (rc = b.d_fin_count.reserve(sizeof(int) * PAIR_CAP)) ||
-        (rc = b.d_scratch.reserve(sizeof(uint32_t) * 2 * SLOT_CAP)) || (rc = b.d_items_real.reserve(sizeof(WorkItem) * ITEM_CAP)) ||
+        (rc = b.d_scratch.reserve(sizeof(uint32_t) * 2 * SLOT_CAP)) ||
         (rc = b.d_candx.reserve(sizeof(uint32_t) * CAND_CAP)) || (rc = b.d_fb.reserve(sizeof(uint4) * CAND_CAP)) ||
         (rc = b.d_fb_count.reserve(2 * sizeof(int))) || (rc = b.d_fb_pair.reserve(sizeof(uint4) * (size_t)PAIR_CAP * FB_PER_PAIR)) ||
-        (rc = b.d_fb_pair_cnt.reserve(sizeof(int) * PAIR_CAP)) || (rc = b.h_items_real.reserve(sizeof(WorkItem) * ITEM_CAP)) ||
+        (rc = b.d_fb_pair_cnt.reserve(sizeof(int) * PAIR_CAP)) ||
         (rc = b.h_pairs.reserve(sizeof(PairDev) * PAIR_CAP)) || (rc = b.h_items.reserve(sizeof(WorkItem) * ITEM_CAP)) ||
         (rc = b.h_meta.reserve(sizeof(int) * META_INTS)) || (rc = b.h_out.reserve(sizeof(Rec) * CAND_CAP)) ||
         (rc = b.ev_meta.create(cudaEventDisableTiming)) || (rc = b.ev_copy.create(cudaEventDisableTiming)) ||
@@ -1033,9 +1038,486 @@ int b200m_remove_view(b200m_ctx* c, uint32_t view_id) {
 }
 
 // ---- Surface 2: pairs -------------------------------------------------------------------------------------------
-struct Directed { int slot_i, slot_j; uint32_t mode; int fwd_index; bool reverse; };
+// The search-kernel class of a directed pair, decided once, when its batch is enqueued (pair_class).  The tensor-core classes come
+// first, in the order of their work items in the batch's table; the kernels launch in class order.
+enum : int { K_FP16, K_U8, K_NG, K_REAL, K_EXACT_F32, K_EXACT_U8, K_HAMMING, K_GENERIC_F32, K_GENERIC_U8, K_SKIP, K_COUNT };
+constexpr int K_TC_COUNT = K_REAL + 1;
+// PairDev::mode of each class (the fp16, u8 and norm-GEMM classes: PM_TC_FUSED when their kernel runs the exactness pass itself)
+static const uint32_t kClassMode[K_COUNT] = {PM_TC, PM_TC, PM_TC, PM_TC_REAL, PM_EXACT_F32, PM_EXACT_U8, PM_HAMMING, PM_GENERIC_F32,
+                                              PM_GENERIC_U8, PM_SKIP};
 
-static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, float dist_ratio, int cross, int stage, b200m_result** out);
+struct Directed { int slot_i, slot_j; bool skip; };   // slot_i = database, slot_j = query; skip: nothing to search (plan_pairs)
+struct Batch { size_t begin, end; };                  // a range of the processing order
+
+// The state of one b200m_match_pairs call, shared by its steps.  The destructor runs on every exit path (CUDA error, failed upload
+// ...): the finishing tasks already submitted write into `arena` and `dir_len` and signal `groups`, so they are waited for first.
+struct MatchCall {
+  MatchCall(b200m_ctx* c_, int stage_, int cross, float dist_ratio_)
+      : c(c_), stage(stage_), do_cross(cross != 0 && stage_ == B200M_STAGE_FULL), dev_fin(c_->device_finish && stage_ == B200M_STAGE_FULL),
+        step(do_cross ? 2 : 1), tc_ctas_per_item((c_->tc_variant == 2 || c_->tc_variant == 4) ? 2 : 1), dist_ratio(dist_ratio_),
+        ratio_sq(dist_ratio_ * dist_ratio_) {}   // Square(f_dist_ratio) in float, RegionsMatcher.hpp:150 / numeric.hpp:130
+  ~MatchCall() { for (auto& g : groups) g->wait(); for (auto& b : arena) c->recycler->give(b); }
+
+  b200m_ctx* c;
+  int stage; bool do_cross, dev_fin;
+  size_t step;                                  // directed pairs per pair: 2 when cross matching
+  int tc_ctas_per_item;                         // CTAs per work item of the fp16 kernel
+  float dist_ratio, ratio_sq;
+  std::vector<std::pair<uint32_t, uint32_t>> fwd;   // the PairSet
+  std::vector<Directed> dir;                    // fwd[k]: dir[k * step] = (i, j), then dir[k * step + 1] = (j, i) when cross matching
+  std::vector<uint32_t> seqv;                   // directed-pair indices in processing order
+  bool pending = false;                         // views still arriving: arrival order and short first batches
+  std::vector<Batch> batches;
+  std::vector<uint8_t> cls;                     // per directed pair: its class (K_*), set when its batch is enqueued
+  // the batch being enqueued, per class: pairs, database rows, work items (tensor-core classes, from item0 in the table) or query
+  // blocks of its largest pair (the grid of the exact, Hamming and generic kernels), and whether its kernel runs the exactness pass
+  struct Tally { int n; long rows; int items, item0, qblk; bool fused; } tally[K_COUNT];
+  // finishing output: one slot per directed pair in a flat arena per batch (capacity = its record count), filled by pool tasks
+  std::vector<Recycler::Block> arena;
+  std::vector<b200m_match*> dir_ptr; std::vector<int> dir_len;
+  std::vector<std::unique_ptr<TaskGroup>> groups;   // per batch: its finishing tasks
+  size_t tev_used = 0; std::vector<std::pair<cudaEvent_t, cudaEvent_t>> kernel_events;
+  int launches = 0, tc_pairs = 0, u8_pairs = 0, ng_pairs = 0, real_pairs = 0;
+  int64_t total_records = 0, fallback_rows = 0;
+};
+
+static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+// PairSet semantics (types.hpp:23): unique, lexicographically ordered; then the directed pairs of each pair and the argument errors.
+static int plan_pairs(MatchCall& s, const uint32_t* pairs, int n_pairs) {
+  b200m_ctx* c = s.c;
+  s.fwd.resize((size_t)n_pairs);
+  for (int k = 0; k < n_pairs; ++k) s.fwd[k] = {pairs[2 * k], pairs[2 * k + 1]};
+  if (!std::is_sorted(s.fwd.begin(), s.fwd.end())) std::sort(s.fwd.begin(), s.fwd.end());
+  s.fwd.erase(std::unique(s.fwd.begin(), s.fwd.end()), s.fwd.end());
+  s.dir.reserve(s.fwd.size() * s.step);
+  for (const auto& f : s.fwd) {
+    auto si = c->slot_of.find(f.first), sj = c->slot_of.find(f.second);
+    if (si == c->slot_of.end() || sj == c->slot_of.end())
+      return fail(B200M_ERR_ARG, "pair references a view that was never uploaded (RegionsPerView::getRegions would throw std::out_of_range)");
+    for (size_t rev = 0; rev < s.step; ++rev) {
+      const int a = rev ? sj->second : si->second, b = rev ? si->second : sj->second;   // a = database, b = query
+      const ViewHost& vi = c->views[a]; const ViewHost& vj = c->views[b];
+      const bool skip = vi.m == 0 || vj.m == 0 || vi.dtype != vj.dtype || vi.dim != vj.dim     // generic.cpp:59-63,74-78
+                        || vi.m < 2;                                                          // NN=2 > rows: bruteForce.hpp:105
+      if (!skip && vi.dtype == DT_BIN && vi.dim != 64) return fail(B200M_ERR_UNSUPPORTED, "binary descriptors must be 64 bytes (AKAZE_BinaryRegions)");
+      if (s.stage == B200M_STAGE_FULL && !skip && (vi.xy.empty() || vj.xy.empty()))
+        return fail(B200M_ERR_ARG, "B200M_STAGE_FULL needs feature positions for every matched view");
+      s.dir.push_back(Directed{a, b, skip});
+    }
+  }
+  return B200M_OK;
+}
+
+// Processing order: PairSet order, or - while uploads are in flight - the order in which the pairs' views arrive.  Arrival order (with
+// short first batches) only while copies are really in flight, not for views that are merely not yet marked ready after a completed
+// upload.
+static void order_pairs(MatchCall& s) {
+  b200m_ctx* c = s.c;
+  std::vector<uint32_t> ord(s.fwd.size());
+  for (size_t k = 0; k < s.fwd.size(); ++k) ord[k] = (uint32_t)k;
+  bool uploading;
+  { std::lock_guard<std::mutex> l(c->up_mu); uploading = c->up_active > 0; }
+  if (uploading) for (const Directed& d : s.dir) if (!d.skip) s.pending |= !c->views[d.slot_i].ready || !c->views[d.slot_j].ready;
+  if (s.pending) {
+    std::vector<uint64_t> key(s.fwd.size());
+    for (size_t k = 0; k < s.fwd.size(); ++k) key[k] = std::max(c->views[s.dir[k * s.step].slot_i].seq, c->views[s.dir[k * s.step].slot_j].seq);
+    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return key[a] < key[b]; });
+  }
+  s.seqv.reserve(s.dir.size());
+  for (uint32_t k : ord) for (size_t u = 0; u < s.step; ++u) s.seqv.push_back((uint32_t)(k * s.step + u));
+}
+
+// Batches over the processing order, each within PAIR_CAP, CAND_CAP, ITEM_CAP and SLOT_CAP; both directions of a pair go into the
+// same batch.  While views are still arriving the first batches are short (B200M_FIRST_BATCH pairs, doubled per batch) so the GPU
+// starts early.
+static int split_batches(MatchCall& s) {
+  b200m_ctx* c = s.c;
+  size_t b0 = 0; long cand = 0, items = 0, slots = 0;
+  size_t pair_cap = s.pending ? (size_t)c->first_batch_pairs : (size_t)PAIR_CAP;
+  for (size_t k = 0; k < s.seqv.size(); k += s.step) {
+    long need_c = 0, need_i = 0, need_s = 0;
+    for (size_t u = k; u < k + s.step; ++u) {
+      const int mj = c->views[s.dir[s.seqv[u]].slot_j].m, mi = c->views[s.dir[s.seqv[u]].slot_i].m;
+      if (mj > CAND_CAP || mi > SLOT_CAP / 2) return fail(B200M_ERR_UNSUPPORTED, "view too large for one batch");
+      need_c += mj; need_i += (mj + tc::BM - 1) / tc::BM; need_s += mi;
+    }
+    if (k > b0 && (cand + need_c > CAND_CAP || items + need_i > ITEM_CAP || slots + need_s > SLOT_CAP || k - b0 + s.step > pair_cap)) {
+      s.batches.push_back({b0, k}); b0 = k; cand = 0; items = 0; slots = 0;
+      pair_cap = std::min<size_t>(PAIR_CAP, pair_cap * 2);
+    }
+    cand += need_c; items += need_i; slots += need_s;
+  }
+  if (s.seqv.size() > b0) s.batches.push_back({b0, s.seqv.size()});
+  return B200M_OK;
+}
+
+// The class of a directed pair, from both views' exactness flags: they are known once the views are ready on the device.
+static int pair_class(const b200m_ctx* c, const Directed& d) {
+  if (d.skip) return K_SKIP;
+  const ViewHost& vi = c->views[d.slot_i]; const ViewHost& vj = c->views[d.slot_j];
+  if (vi.dtype == DT_BIN) return K_HAMMING;
+  if (vi.dim != 128) return vi.dtype == DT_F32 ? K_GENERIC_F32 : K_GENERIC_U8;   // AKAZE float (64), LIOP (144), ...: generic exact path
+  if (!c->force_exact && vi.tc_ok() && vj.tc_ok()) {
+    // integer-valued pairs whose views are both stored as uchar run the u8 kernel (8-bit tensor cores, exact int32 distances) under
+    // the default variant; the other tensor-core pairs run the fp16 kernel
+    if (c->tc_variant != 4 || vi.store_dtype() != DT_U8 || vj.store_dtype() != DT_U8) return K_FP16;
+    // ... and of those, the pairs whose query view has no component above 127 and whose database view's norms fit the limbs run the
+    // u8 norm-GEMM kernel (the norms folded into the 8-bit GEMM)
+    return c->u8_norm_gemm && vi.ng_db_ok() && vj.ng_query_ok() ? K_NG : K_U8;
+  }
+  // real-valued fp32: tensor-core filter + exact re-scoring
+  if (!c->force_exact && c->real_tc && c->tc_variant == 4 && vi.real_ok() && vj.real_ok()) return K_REAL;
+  return vi.dtype == DT_F32 ? K_EXACT_F32 : K_EXACT_U8;
+}
+
+// The search kernels of one batch on the search stream, in class order: each tensor-core kernel over its range of the work-item
+// table, the real-valued path's re-scoring and fallbacks, then the exact, Hamming and generic kernels, each over all pairs of the
+// batch (a kernel searches the pairs of its mode).
+static void launch_search(MatchCall& s, const BatchBuf& bb, int np) {
+  b200m_ctx* c = s.c;
+  const MatchCall::Tally* t = s.tally;
+  const cudaStream_t st = c->stream;
+  const float r2 = s.ratio_sq;
+  // the debug trace (one kernel's CTA 0) shows the norm-GEMM kernel when the batch has pairs on it, else the u8 kernel when it has u8
+  // pairs, else the fp16 kernel
+  const int traced = t[K_NG].n ? K_NG : t[K_U8].n ? K_U8 : K_FP16;
+  auto trace = [&](int k) { return k == traced ? static_cast<long long*>(c->d_trace) : nullptr; };
+  // one CTA per SM, whole work items per CTA group
+  auto grid = [&](int k, int ctas) { return ctas * std::min(t[k].items, c->num_sms / ctas); };
+  if (t[K_FP16].items) {
+    const bool aug = c->tc_variant == 4;
+    const int ctas = s.tc_ctas_per_item;
+    auto* kernel = aug ? tc::l2_top2_tc_kernel<true> : tc::l2_top2_tc_kernel<false>;
+    kernel<<<grid(K_FP16, ctas), tc::block_threads<tc::MODE_MATCH>(), aug ? tc::Lay<true>::SMEM_BYTES : tc::Lay<false>::SMEM_BYTES, st>>>(
+        c->d_views, bb.d_pairs, bb.d_items + t[K_FP16].item0, t[K_FP16].items, ctas, bb.d_cands, bb.d_count, r2, trace(K_FP16), c->d_err,
+        (int)t[K_FP16].fused, nullptr, FbSink{});
+    ++s.launches;
+  }
+  if (t[K_U8].items) {
+    tc::l2_top2_tc_u8_kernel<<<grid(K_U8, 2), tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false, false, true>::SMEM_BYTES, st>>>(
+        c->d_views, bb.d_pairs, bb.d_items + t[K_U8].item0, t[K_U8].items, 2, bb.d_cands, bb.d_count, r2, trace(K_U8), c->d_err,
+        (int)t[K_U8].fused, nullptr, FbSink{});
+    ++s.launches;
+  }
+  if (t[K_NG].items) {
+    tc::l2_top2_tc_u8ng_kernel<<<grid(K_NG, 2), tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false, false, true, true>::SMEM_BYTES, st>>>(
+        c->d_views, bb.d_pairs, bb.d_items + t[K_NG].item0, t[K_NG].items, 2, bb.d_cands, bb.d_count, r2, trace(K_NG), c->d_err,
+        (int)t[K_NG].fused, nullptr, FbSink{});
+    ++s.launches;
+  }
+  if (t[K_REAL].items) {
+    // real-valued pairs: filter kernel (re-scoring in-kernel when the items are long enough), stand-alone re-scoring otherwise, then the
+    // exact search of the few queries the error bound could not decide; after that their candidates are final like everyone else's
+    const FbSink fbs{bb.d_fb_pair, bb.d_fb_pair_cnt, bb.d_fb, bb.d_fb_count, (int)CAND_CAP, bb.d_fb_count + 1};
+    tc::l2_top2_tc_kernel<true, tc::MODE_REAL><<<grid(K_REAL, 2), tc::block_threads<tc::MODE_REAL>(), tc::Lay<true, true>::SMEM_BYTES, st>>>(
+        c->d_views, bb.d_pairs, bb.d_items + t[K_REAL].item0, t[K_REAL].items, 2, bb.d_cands, bb.d_count, r2, nullptr, c->d_err,
+        (int)t[K_REAL].fused, bb.d_candx, fbs);
+    ++s.launches;
+    if (!t[K_REAL].fused) {
+      rescore_real_kernel<<<dim3(np, 4), VERIFY_WARPS_REAL * 32, 0, st>>>(c->d_views, bb.d_pairs, bb.d_cands, bb.d_candx, bb.d_count, r2, c->d_err, fbs);
+      ++s.launches;
+    }
+    exact_rows_pairs_kernel<<<dim3(np, FB_PER_PAIR / XP_MAXQ), XP_THREADS, XP_SMEM, st>>>(c->d_views, bb.d_pairs, bb.d_fb_pair, bb.d_fb_pair_cnt, bb.d_cands, bb.d_count, r2);
+    exact_rows_kernel<<<c->num_sms, XR_THREADS, 0, st>>>(c->d_views, bb.d_pairs, bb.d_fb, bb.d_fb_count, (int)CAND_CAP, bb.d_cands, bb.d_count, r2);   // overflow list: normally empty
+    s.launches += 2;
+  }
+  // the two exact kernels share one grid, as do the two generic ones
+  const int qblk_exact = std::max(t[K_EXACT_F32].qblk, t[K_EXACT_U8].qblk), qblk_gen = std::max(t[K_GENERIC_F32].qblk, t[K_GENERIC_U8].qblk);
+  if (t[K_EXACT_F32].n) {
+    exact_top2_kernel<float, false><<<dim3(qblk_exact, np), 256, EX_SMEM, st>>>(c->d_views, bb.d_pairs, PM_EXACT_F32, bb.d_cands, bb.d_count, r2, nullptr, nullptr);
+    ++s.launches;
+  }
+  if (t[K_EXACT_U8].n) {
+    exact_top2_kernel<uint8_t, false><<<dim3(qblk_exact, np), 256, EX_SMEM, st>>>(c->d_views, bb.d_pairs, PM_EXACT_U8, bb.d_cands, bb.d_count, r2, nullptr, nullptr);
+    ++s.launches;
+  }
+  if (t[K_HAMMING].n) {
+    hamming_top2_kernel<false><<<dim3(t[K_HAMMING].qblk, np), HM_TQ, 0, st>>>(c->d_views, bb.d_pairs, bb.d_cands, bb.d_count, s.dist_ratio, nullptr, nullptr);
+    ++s.launches;
+  }
+  if (t[K_GENERIC_F32].n) {
+    generic_top2_pairs_kernel<float><<<dim3(qblk_gen, np), 128, 0, st>>>(c->d_views, bb.d_pairs, PM_GENERIC_F32, bb.d_cands, bb.d_count, r2);
+    ++s.launches;
+  }
+  if (t[K_GENERIC_U8].n) {
+    generic_top2_pairs_kernel<uint8_t><<<dim3(qblk_gen, np), 128, 0, st>>>(c->d_views, bb.d_pairs, PM_GENERIC_U8, bb.d_cands, bb.d_count, r2);
+    ++s.launches;
+  }
+}
+
+// Batch bi: the class of each pair, the per-class tally, the pair and work-item tables, the search, packing and finishing kernels and
+// the meta read-back.  Three streams so that consecutive batches' search kernels run back to back: the tables of this batch travel on
+// `tab_stream` (issued while the previous batch is still searching), the packing / finishing kernels and the meta read-back of this
+// batch run on `pack_stream` beside the next batch's search kernel.  Buffer set (bi & 1) is free: the host has seen ev_meta of batch
+// bi-2.
+static int enqueue_batch(MatchCall& s, size_t bi) {
+  b200m_ctx* c = s.c;
+  const Batch& B = s.batches[bi];
+  BatchBuf& bb = c->buf[bi & 1];
+  const int np = (int)(B.end - B.begin);
+  // queries per work item (tensor-core classes) or per block of the grid (the others)
+  const int qrows[K_COUNT] = {s.tc_ctas_per_item * tc::BM, 2 * tc::BM, 2 * tc::BM, 2 * tc::BM, EX_TQ, EX_TQ, HM_TQ, 4, 4, 1};
+  for (MatchCall::Tally& t : s.tally) t = MatchCall::Tally{};
+  for (int p = 0; p < np; ++p) {
+    const uint32_t di = s.seqv[B.begin + p];
+    const Directed& d = s.dir[di];
+    int rc;
+    if (!d.skip && ((rc = ensure_view_ready(c, d.slot_i)) || (rc = ensure_view_ready(c, d.slot_j)))) return rc;
+    const int k = s.cls[di] = (uint8_t)pair_class(c, d);
+    const int blocks = (c->views[d.slot_j].m + qrows[k] - 1) / qrows[k];
+    MatchCall::Tally& t = s.tally[k];
+    ++t.n; t.rows += c->views[d.slot_i].m; t.items += blocks; t.qblk = std::max(t.qblk, blocks);
+  }
+  // In-kernel exactness pass only when a work item lasts long enough (>= 24 database tiles on average) for two warps to re-score the
+  // previous item's candidates behind it; shorter images use the stand-alone exactness kernel.
+  int n_items = 0, next[K_TC_COUNT];
+  for (int k = 0; k < K_TC_COUNT; ++k) {
+    MatchCall::Tally& t = s.tally[k];
+    t.fused = t.n > 0 && t.rows / t.n >= (k == K_REAL ? c->real_fused_rows : 6144) && (k != K_FP16 || c->tc_variant >= 2);
+    t.item0 = next[k] = n_items;
+    n_items += t.items;
+  }
+  uint32_t cbase = 0, sbase = 0;
+  for (int p = 0; p < np; ++p) {
+    const uint32_t di = s.seqv[B.begin + p];
+    const Directed& d = s.dir[di];
+    const int k = s.cls[di];
+    const ViewHost& vi = c->views[d.slot_i]; const ViewHost& vj = c->views[d.slot_j];
+    const uint32_t mode = k < K_REAL && s.tally[k].fused ? (uint32_t)PM_TC_FUSED : kClassMode[k];
+    bb.h_pairs[p] = PairDev{(uint32_t)d.slot_i, (uint32_t)d.slot_j, (uint32_t)vi.m, (uint32_t)vj.m, cbase, mode, sbase, k == K_U8 || k == K_NG ? 1u : 0u};
+    cbase += (uint32_t)vj.m; sbase += (uint32_t)vi.m;
+    if (k < K_TC_COUNT) for (int qt = 0; qt < (vj.m + qrows[k] - 1) / qrows[k]; ++qt) bb.h_items[next[k]++] = WorkItem{(uint32_t)p, (uint32_t)qt};
+  }
+  s.tc_pairs += s.tally[K_FP16].n + s.tally[K_U8].n + s.tally[K_NG].n;
+  s.u8_pairs += s.tally[K_U8].n + s.tally[K_NG].n;
+  s.ng_pairs += s.tally[K_NG].n;
+  s.real_pairs += s.tally[K_REAL].n;
+
+  cudaStream_t ts = c->pipe_streams ? c->tab_stream : c->stream, ps = c->pipe_streams ? c->pack_stream : c->stream;
+  CK(cudaMemcpyAsync(bb.d_pairs, bb.h_pairs, sizeof(PairDev) * np, cudaMemcpyHostToDevice, ts));
+  if (n_items) CK(cudaMemcpyAsync(bb.d_items, bb.h_items, sizeof(WorkItem) * n_items, cudaMemcpyHostToDevice, ts));
+  CK(cudaMemsetAsync(bb.d_count, 0, sizeof(int) * np, ts));
+  CK(cudaMemsetAsync(bb.d_fb_count, 0, 2 * sizeof(int), ts));
+  if (s.tally[K_REAL].items) CK(cudaMemsetAsync(bb.d_fb_pair_cnt, 0, sizeof(int) * np, ts));
+  if (c->pipe_streams) { CK(cudaEventRecord(bb.ev_tab, ts)); CK(cudaStreamWaitEvent(c->stream, bb.ev_tab, 0)); }
+  cudaEvent_t k0 = timing_event(c, s.tev_used), k1 = timing_event(c, s.tev_used);
+  CK(cudaEventRecord(k0, c->stream));
+  launch_search(s, bb, np);
+  CK(cudaEventRecord(k1, c->stream));
+  if (c->pipe_streams) CK(cudaStreamWaitEvent(ps, k1, 0));
+  s.kernel_events.push_back({k0, k1});
+  scan_counts_kernel<<<1, 256, 0, ps>>>(bb.d_count, np, bb.d_off);
+  verify_pack_kernel<<<dim3(np, VERIFY_BLOCKS_PER_PAIR), VERIFY_WARPS * 32, 0, ps>>>(c->d_views, bb.d_pairs, bb.d_cands, bb.d_count, bb.d_off, bb.d_out, s.ratio_sq, c->d_err);
+  s.launches += 2;
+  if (s.dev_fin) {
+    finish_pairs_kernel<<<np, FIN_THREADS, 0, ps>>>(c->d_views, bb.d_pairs, c->d_flags, bb.d_out, bb.d_count, bb.d_off, bb.d_scratch, bb.d_fin, bb.d_fin_count);
+    ++s.launches;
+    CK(cudaMemcpyAsync(bb.meta_fin_counts(), bb.d_fin_count, sizeof(int) * np, cudaMemcpyDeviceToHost, ps));
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(bb.meta_fallback_rows(), bb.d_fb_count + 1, sizeof(int), cudaMemcpyDeviceToHost, ps));
+  CK(cudaMemcpyAsync(bb.meta_counts(), bb.d_count, sizeof(int) * np, cudaMemcpyDeviceToHost, ps));
+  CK(cudaMemcpyAsync(bb.meta_offsets(), bb.d_off, sizeof(int) * (np + 1), cudaMemcpyDeviceToHost, ps));
+  CK(cudaEventRecord(bb.ev_meta, ps));
+  return B200M_OK;
+}
+
+// RAW / FULL: batch bi's records, copied to pinned memory once its meta block is in, and its finishing tasks.  The tasks run behind
+// the GPU: they only have to be done before batch bi+2's records are copied into the same pinned buffer.  They take the per-pair
+// counts and offsets out of the meta block here, because enqueue_batch(bi+2) overwrites it.
+static int finish_batch(MatchCall& s, size_t bi) {
+  b200m_ctx* c = s.c;
+  const Batch& B = s.batches[bi];
+  const BatchBuf& bb = c->buf[bi & 1];
+  const int np = (int)(B.end - B.begin);
+  const int total = bb.meta_offsets()[np];
+  if (bi >= 2) s.groups[bi - 2]->wait();       // the tasks of batch bi-2 read this pinned record buffer
+  if (total > 0) {
+    CK(cudaStreamWaitEvent(c->copy_stream, bb.ev_meta, 0));
+    CK(cudaMemcpyAsync(bb.h_out, s.dev_fin ? (const void*)bb.d_fin : (const void*)bb.d_out, sizeof(Rec) * (size_t)total, cudaMemcpyDeviceToHost, c->copy_stream));
+    CK(cudaEventRecord(bb.ev_copy, c->copy_stream));
+    CK(cudaEventSynchronize(bb.ev_copy));
+  }
+  if (bi + 1 == s.batches.size()) {
+    // end of the device work of this call = the last match list has landed in pinned host memory (SURVEY 8d)
+    CK(cudaStreamWaitEvent(c->copy_stream, bb.ev_meta, 0));
+    CK(cudaEventRecord(c->ev_end, c->copy_stream));
+  }
+  s.arena[bi] = c->recycler->take((size_t)std::max(total, 1));
+  TaskGroup* grp = s.groups[bi].get();
+  // one pool task per ~4096 records (or 64 pairs): for small images the task hand-off would otherwise cost more than the work
+  // cnt >= 0: raw records, finished here (finish_directed); done >= 0: `done` final matches from the device finishing stage, copied
+  struct Job { const Rec* recs; int cnt; int done; b200m_match* dst; int* len; const ViewHost* vi; const ViewHost* vj; bool ham; };
+  auto jobs = std::make_shared<std::vector<Job>>();
+  long job_records = 0;
+  const bool full = s.stage == B200M_STAGE_FULL;
+  auto flush = [&] {
+    if (jobs->empty()) return;
+    grp->add(1);
+    std::shared_ptr<std::vector<Job>> mine = std::move(jobs);
+    c->pool->submit([mine, grp, full] {
+      for (const Job& j : *mine) {
+        if (j.done >= 0) { std::memcpy(j.dst, j.recs, sizeof(b200m_match) * (size_t)j.done); *j.len = j.done; }
+        else *j.len = finish_directed(j.recs, j.cnt, j.ham, full, *j.vi, *j.vj, j.dst);
+      }
+      grp->done();
+    });
+    jobs = std::make_shared<std::vector<Job>>();
+    job_records = 0;
+  };
+  for (int p = 0; p < np; ++p) {
+    const size_t di = s.seqv[B.begin + p];
+    const Directed& d = s.dir[di];
+    s.dir_ptr[di] = s.arena[bi].p + bb.meta_offsets()[p];
+    int cnt = bb.meta_counts()[p], done = -1;
+    if (d.skip || cnt == 0) continue;
+    if (s.dev_fin) {                                 // >= 0: final matches; < 0: -(records + 1) left for the host (view not in general position)
+      const int f = bb.meta_fin_counts()[p];
+      if (f >= 0) done = f; else cnt = -(f + 1);
+      if (done == 0) continue;
+    }
+    jobs->push_back(Job{bb.h_out + bb.meta_offsets()[p], cnt, done, s.dir_ptr[di], &s.dir_len[di], &c->views[d.slot_i], &c->views[d.slot_j],
+                        s.cls[di] == K_HAMMING});
+    job_records += cnt;
+    if (job_records >= 4096 || jobs->size() >= 64) flush();
+  }
+  flush();
+  return B200M_OK;
+}
+
+// Every stage runs the same pipeline: batch j is enqueued while the host waits for the meta block of batch j-1 (which also frees
+// buffer set j+1 & 1 for the next enqueue), then RAW / FULL copy batch j-1's records and submit its finishing tasks.  The device work
+// of the call ends with the last batch's kernels (DEVICE) or with its records in pinned host memory (RAW / FULL, finish_batch).
+static int batch_loop(MatchCall& s, bool timing) {
+  b200m_ctx* c = s.c;
+  const double t0 = now_ms();
+  const size_t nb = s.batches.size();
+  CK(cudaEventRecord(c->ev_start, c->stream));
+  if (nb == 0) CK(cudaEventRecord(c->ev_end, c->stream));
+  for (size_t j = 0; j <= nb; ++j) {
+    int rc;
+    if (j < nb) {
+      if ((rc = enqueue_batch(s, j))) return rc;
+      if (j + 1 == nb && s.stage == B200M_STAGE_DEVICE) CK(cudaEventRecord(c->ev_end, c->stream));
+    }
+    if (j == 0) continue;
+    const size_t bi = j - 1;
+    const BatchBuf& bb = c->buf[bi & 1];
+    CK(cudaEventSynchronize(bb.ev_meta));
+    s.total_records += bb.meta_offsets()[s.batches[bi].end - s.batches[bi].begin];
+    s.fallback_rows += *bb.meta_fallback_rows();
+    if (s.stage != B200M_STAGE_DEVICE && (rc = finish_batch(s, bi))) return rc;
+  }
+  const double t_loop = now_ms();
+  for (auto& g : s.groups) g->wait();
+  if (timing) fprintf(stderr, "[b200m] match_pairs: batch loop %.2f ms, last finishing groups +%.2f ms\n", t_loop - t0, now_ms() - t_loop);
+  return B200M_OK;
+}
+
+// Cross matching: keep m iff (m.j, m.i) is in the reverse list (ImageCollectionMatcher_generic.cpp:92-109); filtered in place, in
+// parallel.
+static void cross_filter(MatchCall& s) {
+  TaskGroup g; g.add((int)s.fwd.size());
+  for (size_t k = 0; k < s.fwd.size(); ++k) {
+    b200m_match* f = s.dir_ptr[k * s.step]; int* nf = &s.dir_len[k * s.step];
+    const b200m_match* r = s.dir_ptr[k * s.step + 1]; const int nr = s.dir_len[k * s.step + 1];
+    TaskGroup* gp = &g;
+    s.c->pool->submit([=] {
+      std::vector<std::pair<uint32_t, uint32_t>> rv; rv.reserve(nr);
+      for (int e = 0; e < nr; ++e) rv.push_back({r[e].i, r[e].j});
+      std::sort(rv.begin(), rv.end());
+      int w = 0;
+      for (int e = 0; e < *nf; ++e)
+        if (std::binary_search(rv.begin(), rv.end(), std::make_pair(f[e].j, f[e].i))) f[w++] = f[e];
+      *nf = w;
+      gp->done();
+    });
+  }
+  g.wait();
+}
+
+// The result: offsets first, then the per-pair copies into one contiguous block in parallel on the pool.
+static b200m_result* assemble_result(MatchCall& s) {
+  b200m_ctx* c = s.c;
+  const size_t n = s.fwd.size(), step = s.step;
+  std::unique_ptr<b200m_result> res(new b200m_result());
+  res->pair_ids.reserve(2 * n);
+  res->offsets.assign(n + 1, 0);
+  for (size_t k = 0; k < n; ++k) {
+    res->pair_ids.push_back(s.fwd[k].first); res->pair_ids.push_back(s.fwd[k].second);
+    res->offsets[k + 1] = res->offsets[k] + (s.stage != B200M_STAGE_DEVICE ? s.dir_len[k * step] : 0);
+  }
+  const size_t total_matches = (size_t)res->offsets[n];
+  res->recycler = c->recycler;
+  res->matches = c->recycler->take(total_matches);
+  if (total_matches) {
+    const size_t CHUNK_PAIRS = 64;
+    TaskGroup g; g.add((int)((n + CHUNK_PAIRS - 1) / CHUNK_PAIRS));
+    for (size_t k0 = 0; k0 < n; k0 += CHUNK_PAIRS) {
+      const size_t k1 = std::min(n, k0 + CHUNK_PAIRS);
+      b200m_match* base = res->matches.p; const int64_t* offs = res->offsets.data();
+      b200m_match* const* dp = s.dir_ptr.data(); const int* dl = s.dir_len.data(); TaskGroup* gp = &g;
+      c->pool->submit([=] {
+        for (size_t k = k0; k < k1; ++k) if (dl[k * step] > 0) std::memcpy(base + offs[k], dp[k * step], sizeof(b200m_match) * (size_t)dl[k * step]);
+        gp->done();
+      });
+    }
+    g.wait();
+  }
+  return res.release();
+}
+
+static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, float dist_ratio, int cross, int stage, b200m_result** out) {
+  if (!c || !out || n_pairs < 0 || (n_pairs > 0 && !pairs) || stage < 0 || stage > 2) return fail(B200M_ERR_ARG, "bad arguments");
+  *out = nullptr;
+  CK(cudaSetDevice(c->device));
+  int rc = ensure_batch_buffers(c);
+  if (rc) return rc;
+  const bool timing = getenv("B200M_TIMING") != nullptr;
+  const double t_begin = now_ms();
+  MatchCall s(c, stage, cross, dist_ratio);
+  if ((rc = plan_pairs(s, pairs, n_pairs))) return rc;
+  order_pairs(s);
+  if ((rc = split_batches(s))) return rc;
+  s.cls.assign(s.dir.size(), K_SKIP);
+  s.dir_ptr.assign(s.dir.size(), nullptr);
+  s.dir_len.assign(s.dir.size(), 0);
+  s.arena.resize(s.batches.size());
+  for (size_t b = 0; b < s.batches.size(); ++b) s.groups.emplace_back(new TaskGroup());
+
+  const double t_setup = now_ms();
+  if ((rc = batch_loop(s, timing))) return rc;
+  const double t_gpu_done = now_ms();
+  CK(cudaStreamSynchronize(c->stream));
+  CK(cudaStreamSynchronize(c->pack_stream));
+  float ms = 0.f;
+  CK(cudaEventSynchronize(c->ev_end));
+  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
+  double sk = 0;
+  const auto& kev = s.kernel_events;
+  for (auto& e : kev) { float t = 0.f; CK(cudaEventElapsedTime(&t, e.first, e.second)); sk += t; }
+  if (timing && !kev.empty()) {
+    // device timeline of the call: search kernels back to back?  gap = end of one batch's search kernels -> start of the next one's
+    // (packing / finishing kernels, meta copies, the next batch's pair-table copies, and any wait for the host)
+    float lead = 0.f, gaps = 0.f, gmax = 0.f, tail = 0.f;
+    CK(cudaEventElapsedTime(&lead, c->ev_start, kev.front().first));
+    for (size_t k = 0; k + 1 < kev.size(); ++k) { float t = 0.f; CK(cudaEventElapsedTime(&t, kev[k].second, kev[k + 1].first)); gaps += t; gmax = std::max(gmax, t); }
+    CK(cudaEventElapsedTime(&tail, kev.back().second, c->ev_end));
+    fprintf(stderr, "[b200m] device timeline: %zu batches, search kernels %.2f ms, lead-in %.2f, gaps between batches %.2f (max %.2f), tail after the last search kernel %.2f ms\n",
+            kev.size(), sk, lead, gaps, gmax, tail);
+  }
+  unsigned errs = 0;
+  CK(cudaMemcpy(&errs, c->d_err, sizeof(unsigned), cudaMemcpyDeviceToHost));
+  c->err_total = errs;
+
+  if (s.do_cross) cross_filter(s);
+  *out = assemble_result(s);
+  if (timing) fprintf(stderr, "[b200m] match_pairs n=%d stage=%d: setup %.2f ms, batches %.2f ms (gpu %.2f), tail (cross+assemble) %.2f ms, total %.2f ms\n",
+                      n_pairs, stage, t_setup - t_begin, t_gpu_done - t_setup, ms, now_ms() - t_gpu_done, now_ms() - t_begin);
+  c->last = LastCall{ms, sk, s.launches, s.tc_pairs, s.real_pairs, s.u8_pairs, s.total_records, s.fallback_rows, (int)s.batches.size(), s.ng_pairs};
+  return B200M_OK;
+}
 
 int b200m_match_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, float dist_ratio, int cross, int stage, b200m_result** out) {
   if (!c) return fail(B200M_ERR_ARG, "ctx is null");
@@ -1049,436 +1531,6 @@ int b200m_match_pairs(b200m_ctx* c, const uint32_t* pairs, int n_pairs, float di
     if (rcu) { if (out && *out) { b200m_result_free(*out); *out = nullptr; } return rcu; }
   }
   return rc;
-}
-
-static int match_pairs_impl(b200m_ctx* c, const uint32_t* pairs, int n_pairs, float dist_ratio, int cross, int stage, b200m_result** out) {
-  if (!c || !out || n_pairs < 0 || (n_pairs > 0 && !pairs) || stage < 0 || stage > 2) return fail(B200M_ERR_ARG, "bad arguments");
-  *out = nullptr;
-  CK(cudaSetDevice(c->device));
-  int rc = ensure_batch_buffers(c);
-  if (rc) return rc;
-  const bool timing = getenv("B200M_TIMING") != nullptr;
-  auto now = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  const double t_begin = now();
-
-  // PairSet semantics (types.hpp:23): unique, lexicographically ordered.
-  std::vector<std::pair<uint32_t, uint32_t>> fwd((size_t)n_pairs);
-  for (int k = 0; k < n_pairs; ++k) fwd[k] = {pairs[2 * k], pairs[2 * k + 1]};
-  if (!std::is_sorted(fwd.begin(), fwd.end())) std::sort(fwd.begin(), fwd.end());
-  fwd.erase(std::unique(fwd.begin(), fwd.end()), fwd.end());
-
-  const bool do_cross = cross != 0 && stage == B200M_STAGE_FULL;
-  std::vector<Directed> dir;
-  dir.reserve(fwd.size() * (do_cross ? 2 : 1));
-  int tc_pairs = 0;
-  for (size_t k = 0; k < fwd.size(); ++k) {
-    auto si = c->slot_of.find(fwd[k].first), sj = c->slot_of.find(fwd[k].second);
-    if (si == c->slot_of.end() || sj == c->slot_of.end())
-      return fail(B200M_ERR_ARG, "pair references a view that was never uploaded (RegionsPerView::getRegions would throw std::out_of_range)");
-    for (int rev = 0; rev < (do_cross ? 2 : 1); ++rev) {
-      const int a = rev ? sj->second : si->second, b = rev ? si->second : sj->second;   // a = database, b = query
-      const ViewHost& vi = c->views[a]; const ViewHost& vj = c->views[b];
-      uint32_t mode;
-      if (vi.m == 0 || vj.m == 0 || vi.dtype != vj.dtype || vi.dim != vj.dim) mode = PM_SKIP;           // generic.cpp:59-63,74-78
-      else if (vi.m < 2) mode = PM_SKIP;                                                                 // NN=2 > rows: bruteForce.hpp:105
-      else if (vi.dtype == DT_BIN) {
-        if (vi.dim != 64) return fail(B200M_ERR_UNSUPPORTED, "binary descriptors must be 64 bytes (AKAZE_BinaryRegions)");
-        mode = PM_HAMMING;
-      } else {
-        if (vi.dim != 128) mode = vi.dtype == DT_F32 ? PM_GENERIC_F32 : PM_GENERIC_U8;   // AKAZE float (64), LIOP (144), ...: generic exact path
-        else mode = PM_TC;      // provisional: resolved to the tensor-core or an exact kernel once both views' exactness flags are known (enqueue)
-      }
-      if (stage == B200M_STAGE_FULL && mode != PM_SKIP && (vi.xy.empty() || vj.xy.empty()))
-        return fail(B200M_ERR_ARG, "B200M_STAGE_FULL needs feature positions for every matched view");
-      dir.push_back(Directed{a, b, mode, (int)k, rev != 0});
-    }
-  }
-
-  // ---- processing order: PairSet order, or - while uploads are in flight - the order in which the pairs' views arrive
-  const size_t step = do_cross ? 2 : 1;
-  std::vector<uint32_t> seqv;                      // directed-pair indices in processing order
-  bool pending = false;
-  {
-    std::vector<uint32_t> ord(fwd.size());
-    for (size_t k = 0; k < fwd.size(); ++k) ord[k] = (uint32_t)k;
-    bool uploading;
-    { std::lock_guard<std::mutex> l(c->up_mu); uploading = c->up_active > 0; }
-    // arrival-order processing with short first batches only while copies are really in flight (not for views that are merely not yet
-    // marked ready after a completed upload)
-    if (uploading) for (const Directed& d : dir) if (d.mode != PM_SKIP) pending |= !c->views[d.slot_i].ready || !c->views[d.slot_j].ready;
-    if (pending) {
-      std::vector<uint64_t> key(fwd.size());
-      for (size_t k = 0; k < fwd.size(); ++k) key[k] = std::max(c->views[dir[k * step].slot_i].seq, c->views[dir[k * step].slot_j].seq);
-      std::stable_sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return key[a] < key[b]; });
-    }
-    seqv.reserve(dir.size());
-    for (uint32_t k : ord) for (size_t u = 0; u < step; ++u) seqv.push_back((uint32_t)(k * step + u));
-  }
-
-  // ---- batching (over the processing order); while views are still arriving the first batches are short so the GPU starts early
-  struct Batch { size_t begin, end; };
-  std::vector<Batch> batches;
-  {
-    size_t b0 = 0; long cand = 0, items = 0, slots = 0;
-    size_t pair_cap = pending ? (size_t)c->first_batch_pairs : (size_t)PAIR_CAP;
-    for (size_t k = 0; k < seqv.size(); k += step) {
-      long need_c = 0, need_i = 0, need_s = 0;
-      for (size_t u = k; u < k + step; ++u) {
-        const int mj = c->views[dir[seqv[u]].slot_j].m, mi = c->views[dir[seqv[u]].slot_i].m;
-        if (mj > CAND_CAP || mi > SLOT_CAP / 2) return fail(B200M_ERR_UNSUPPORTED, "view too large for one batch");
-        need_c += mj; need_i += (mj + tc::BM - 1) / tc::BM; need_s += mi;
-      }
-      if (k > b0 && (cand + need_c > CAND_CAP || items + need_i > ITEM_CAP || slots + need_s > SLOT_CAP || k - b0 + step > pair_cap)) {
-        batches.push_back({b0, k}); b0 = k; cand = 0; items = 0; slots = 0;
-        pair_cap = std::min<size_t>(PAIR_CAP, pair_cap * 2);
-      }
-      cand += need_c; items += need_i; slots += need_s;
-    }
-    if (seqv.size() > b0) batches.push_back({b0, seqv.size()});
-  }
-
-  const float ratio_sq = dist_ratio * dist_ratio;   // Square(f_dist_ratio) in float, RegionsMatcher.hpp:150 / numeric.hpp:130
-  // finishing output: one slot per directed pair in a flat arena (capacity = its record count), filled by pool tasks
-  struct ArenaSet {                                                     // uninitialised blocks, one per batch, recycled on exit
-    std::vector<Recycler::Block> b; Recycler* r;
-    ~ArenaSet() { for (auto& x : b) r->give(x); }
-  } arena{std::vector<Recycler::Block>(batches.size()), c->recycler.get()};
-  std::vector<b200m_match*> dir_ptr(dir.size(), nullptr);
-  std::vector<int> dir_len(dir.size(), 0);
-  std::vector<std::unique_ptr<TaskGroup>> groups;
-  for (size_t b = 0; b < batches.size(); ++b) groups.emplace_back(new TaskGroup());
-  struct WaitGroups {       // every exit path (CUDA error, failed upload ...): the finishing tasks already submitted write into `arena`, `dir_len`
-    std::vector<std::unique_ptr<TaskGroup>>& g;             // and signal `groups`; they must be done before those locals are destroyed
-    ~WaitGroups() { for (auto& x : g) x->wait(); }
-  } wait_groups{groups};
-  const bool dev_fin = c->device_finish && stage == B200M_STAGE_FULL;
-  size_t tev_used = 0;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> kernel_events;
-  int launches = 0;
-  int64_t total_records = 0, fallback_rows = 0;
-  int real_pairs = 0, u8_pairs = 0, ng_pairs = 0;
-  const bool real_tc = !c->force_exact && c->real_tc && c->tc_variant == 4;
-  // integer-valued pairs whose views are both stored as uchar run the u8 kernel (8-bit tensor cores, exact int32 distances) under the
-  // default variant; the other tensor-core pairs run the fp16 kernel
-  auto u8_pair = [&](const Directed& d) {
-    return d.mode == PM_TC && c->tc_variant == 4 && c->views[d.slot_i].store_dtype() == DT_U8 && c->views[d.slot_j].store_dtype() == DT_U8;
-  };
-  // ... and of those, the pairs whose query view has no component above 127 and whose database view's norms fit the limbs run the u8
-  // norm-GEMM kernel (the norms folded into the 8-bit GEMM); the others stay on the u8 kernel
-  auto ng_pair = [&](const Directed& d) {
-    return c->u8_norm_gemm && u8_pair(d) && c->views[d.slot_i].ng_db_ok() && c->views[d.slot_j].ng_query_ok();
-  };
-
-  auto enqueue = [&](size_t bi) -> int {
-    const Batch& B = batches[bi];
-    BatchBuf& bb = c->buf[bi & 1];
-    const int np = (int)(B.end - B.begin);
-    uint32_t cbase = 0, sbase = 0; int n_items = 0, n_items_real = 0, n_items_u8 = 0, n_items_ng = 0; int max_qblk_exact = 0, max_qblk_ham = 0;
-    // In-kernel exactness pass only when a work item lasts long enough (>= 24 database tiles on average) for two warps to
-    // re-score the previous item's candidates behind it; shorter images use the stand-alone exactness kernel.
-    // the views of this batch must be complete on the device; their exactness flags decide tensor-core vs exact kernel
-    for (int p = 0; p < np; ++p) {
-      Directed& d = dir[seqv[B.begin + p]];
-      if (d.mode == PM_SKIP) continue;
-      int r2;
-      if ((r2 = ensure_view_ready(c, d.slot_i)) || (r2 = ensure_view_ready(c, d.slot_j))) return r2;
-      if (d.mode == PM_TC) {
-        const ViewHost& vi = c->views[d.slot_i]; const ViewHost& vj = c->views[d.slot_j];
-        if (!c->force_exact && vi.tc_ok() && vj.tc_ok()) { ++tc_pairs; u8_pairs += u8_pair(d); ng_pairs += ng_pair(d); }
-        else if (real_tc && vi.real_ok() && vj.real_ok()) { d.mode = PM_TC_REAL; ++real_pairs; }   // real-valued fp32: tensor-core filter + exact re-scoring
-        else d.mode = vi.dtype == DT_F32 ? PM_EXACT_F32 : PM_EXACT_U8;
-      }
-    }
-    long tc_rows = 0, tc_n = 0, real_rows = 0, real_n = 0, u8_rows = 0, u8_n = 0, ng_rows = 0, ng_n = 0;
-    for (int p = 0; p < np; ++p) {
-      const Directed& d = dir[seqv[B.begin + p]];
-      if (ng_pair(d)) { ng_rows += c->views[d.slot_i].m; ++ng_n; }
-      else if (u8_pair(d)) { u8_rows += c->views[d.slot_i].m; ++u8_n; }
-      else if (d.mode == PM_TC) { tc_rows += c->views[d.slot_i].m; ++tc_n; }
-      if (d.mode == PM_TC_REAL) { real_rows += c->views[d.slot_i].m; ++real_n; }
-    }
-    const bool fused = c->tc_variant >= 2 && tc_n > 0 && tc_rows / tc_n >= 6144;
-    const bool fused_u8 = u8_n > 0 && u8_rows / u8_n >= 6144;
-    const bool fused_ng = ng_n > 0 && ng_rows / ng_n >= 6144;
-    const int tc_ctas_per_item = (c->tc_variant == 2 || c->tc_variant == 4) ? 2 : 1;
-    const bool fused_real = real_n > 0 && real_rows / real_n >= c->real_fused_rows;
-    bool any_f32 = false, any_u8 = false, any_ham = false, any_gf32 = false, any_gu8 = false; int max_qblk_gen = 0;
-    for (int p = 0; p < np; ++p) {
-      const Directed& d = dir[seqv[B.begin + p]];
-      const ViewHost& vi = c->views[d.slot_i]; const ViewHost& vj = c->views[d.slot_j];
-      // the CTA-pair kernel runs the exactness pass itself: its candidates are final records
-      const bool u8 = u8_pair(d);
-      const uint32_t dev_mode = (d.mode == PM_TC && (ng_pair(d) ? fused_ng : u8 ? fused_u8 : fused)) ? (uint32_t)PM_TC_FUSED : d.mode;
-      bb.h_pairs[p] = PairDev{(uint32_t)d.slot_i, (uint32_t)d.slot_j, (uint32_t)vi.m, (uint32_t)vj.m, cbase, dev_mode, sbase, u8 ? 1u : 0u};
-      cbase += (uint32_t)vj.m; sbase += (uint32_t)vi.m;
-      const int qrows = tc_ctas_per_item * tc::BM;   // queries per work item
-      if (d.mode == PM_TC && !u8) for (int qt = 0; qt < (vj.m + qrows - 1) / qrows; ++qt) bb.h_items[n_items++] = WorkItem{(uint32_t)p, (uint32_t)qt};
-      if (d.mode == PM_TC_REAL) for (int qt = 0; qt < (vj.m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items_real[n_items_real++] = WorkItem{(uint32_t)p, (uint32_t)qt};
-      if (d.mode == PM_EXACT_F32) { any_f32 = true; max_qblk_exact = std::max(max_qblk_exact, (vj.m + EX_TQ - 1) / EX_TQ); }
-      if (d.mode == PM_EXACT_U8) { any_u8 = true; max_qblk_exact = std::max(max_qblk_exact, (vj.m + EX_TQ - 1) / EX_TQ); }
-      if (d.mode == PM_HAMMING) { any_ham = true; max_qblk_ham = std::max(max_qblk_ham, (vj.m + HM_TQ - 1) / HM_TQ); }
-      if (d.mode == PM_GENERIC_F32 || d.mode == PM_GENERIC_U8) { (d.mode == PM_GENERIC_F32 ? any_gf32 : any_gu8) = true; max_qblk_gen = std::max(max_qblk_gen, (vj.m + 3) / 4); }
-    }
-    // the u8 kernel's work items (256 queries each) follow the fp16 kernel's in the same table, and the norm-GEMM kernel's follow those
-    for (int p = 0; p < np; ++p) {
-      const Directed& d = dir[seqv[B.begin + p]];
-      if (u8_pair(d) && !ng_pair(d)) for (int qt = 0; qt < (c->views[d.slot_j].m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items[n_items + n_items_u8++] = WorkItem{(uint32_t)p, (uint32_t)qt};
-    }
-    for (int p = 0; p < np; ++p) {
-      const Directed& d = dir[seqv[B.begin + p]];
-      if (ng_pair(d)) for (int qt = 0; qt < (c->views[d.slot_j].m + 2 * tc::BM - 1) / (2 * tc::BM); ++qt) bb.h_items[n_items + n_items_u8 + n_items_ng++] = WorkItem{(uint32_t)p, (uint32_t)qt};
-    }
-    const int n_items_tab = n_items + n_items_u8 + n_items_ng;
-    // Three streams so that consecutive batches' search kernels run back to back: the pair / work-item tables of this batch travel on
-    // `tab_stream` (issued while the previous batch is still searching), the packing / finishing kernels and the meta read-back of this
-    // batch run on `pack_stream` beside the next batch's search kernel.  Buffer set (bi & 1) is free: the host has seen ev_meta of batch bi-2.
-    cudaStream_t ts = c->pipe_streams ? c->tab_stream : c->stream, ps = c->pipe_streams ? c->pack_stream : c->stream;
-    CK(cudaMemcpyAsync(bb.d_pairs, bb.h_pairs, sizeof(PairDev) * np, cudaMemcpyHostToDevice, ts));
-    if (n_items_tab) CK(cudaMemcpyAsync(bb.d_items, bb.h_items, sizeof(WorkItem) * n_items_tab, cudaMemcpyHostToDevice, ts));
-    if (n_items_real) CK(cudaMemcpyAsync(bb.d_items_real, bb.h_items_real, sizeof(WorkItem) * n_items_real, cudaMemcpyHostToDevice, ts));
-    CK(cudaMemsetAsync(bb.d_count, 0, sizeof(int) * np, ts));
-    CK(cudaMemsetAsync(bb.d_fb_count, 0, 2 * sizeof(int), ts));
-    if (n_items_real) CK(cudaMemsetAsync(bb.d_fb_pair_cnt, 0, sizeof(int) * np, ts));
-    if (c->pipe_streams) { CK(cudaEventRecord(bb.ev_tab, ts)); CK(cudaStreamWaitEvent(c->stream, bb.ev_tab, 0)); }
-    cudaEvent_t k0 = timing_event(c, tev_used), k1 = timing_event(c, tev_used);
-    CK(cudaEventRecord(k0, c->stream));
-    // the debug trace (one kernel's CTA 0) shows the norm-GEMM kernel when the batch has pairs on it, else the u8 kernel when it has u8
-    // pairs, else the fp16 kernel
-    long long* ng_trace = c->d_trace;
-    long long* u8_trace = n_items_ng ? nullptr : ng_trace;
-    long long* fp16_trace = (n_items_ng || n_items_u8) ? nullptr : ng_trace;
-    if (n_items) {
-      const int grid = tc_ctas_per_item * std::min(n_items, c->num_sms / tc_ctas_per_item);   // one CTA per SM, whole work items per CTA group
-      if (c->tc_variant == 4)
-        tc::l2_top2_tc_kernel<true><<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<true>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, tc_ctas_per_item, bb.d_cands, bb.d_count, ratio_sq, fp16_trace, c->d_err, (int)fused, nullptr, FbSink{});
-      else
-        tc::l2_top2_tc_kernel<false><<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false>::SMEM_BYTES, c->stream>>>(c->d_views, bb.d_pairs, bb.d_items, n_items, tc_ctas_per_item, bb.d_cands, bb.d_count, ratio_sq, fp16_trace, c->d_err, (int)fused, nullptr, FbSink{});
-      ++launches;
-    }
-    if (n_items_u8) {
-      const int grid = 2 * std::min(n_items_u8, c->num_sms / 2);
-      tc::l2_top2_tc_u8_kernel<<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false, false, true>::SMEM_BYTES, c->stream>>>(
-          c->d_views, bb.d_pairs, bb.d_items + n_items, n_items_u8, 2, bb.d_cands, bb.d_count, ratio_sq, u8_trace, c->d_err, (int)fused_u8, nullptr, FbSink{});
-      ++launches;
-    }
-    if (n_items_ng) {
-      const int grid = 2 * std::min(n_items_ng, c->num_sms / 2);
-      tc::l2_top2_tc_u8ng_kernel<<<grid, tc::block_threads<tc::MODE_MATCH>(), tc::Lay<false, false, true, true>::SMEM_BYTES, c->stream>>>(
-          c->d_views, bb.d_pairs, bb.d_items + n_items + n_items_u8, n_items_ng, 2, bb.d_cands, bb.d_count, ratio_sq, ng_trace, c->d_err, (int)fused_ng,
-          nullptr, FbSink{});
-      ++launches;
-    }
-    if (n_items_real) {
-      // real-valued pairs: filter kernel (re-scoring in-kernel when the items are long enough), stand-alone re-scoring otherwise, then the
-      // exact search of the few queries the error bound could not decide; after that their candidates are final like everyone else's
-      const int grid = 2 * std::min(n_items_real, c->num_sms / 2);
-      const FbSink fbs{bb.d_fb_pair, bb.d_fb_pair_cnt, bb.d_fb, bb.d_fb_count, (int)CAND_CAP, bb.d_fb_count + 1};
-      tc::l2_top2_tc_kernel<true, tc::MODE_REAL><<<grid, tc::block_threads<tc::MODE_REAL>(), tc::Lay<true, true>::SMEM_BYTES, c->stream>>>(
-          c->d_views, bb.d_pairs, bb.d_items_real, n_items_real, 2, bb.d_cands, bb.d_count, ratio_sq, nullptr, c->d_err, (int)fused_real, bb.d_candx, fbs);
-      ++launches;
-      if (!fused_real) {
-        rescore_real_kernel<<<dim3(np, 4), VERIFY_WARPS_REAL * 32, 0, c->stream>>>(c->d_views, bb.d_pairs, bb.d_cands, bb.d_candx, bb.d_count, ratio_sq, c->d_err, fbs);
-        ++launches;
-      }
-      exact_rows_pairs_kernel<<<dim3(np, FB_PER_PAIR / XP_MAXQ), XP_THREADS, XP_SMEM, c->stream>>>(c->d_views, bb.d_pairs, bb.d_fb_pair, bb.d_fb_pair_cnt, bb.d_cands, bb.d_count, ratio_sq);
-      exact_rows_kernel<<<c->num_sms, XR_THREADS, 0, c->stream>>>(c->d_views, bb.d_pairs, bb.d_fb, bb.d_fb_count, (int)CAND_CAP, bb.d_cands, bb.d_count, ratio_sq);   // overflow list: normally empty
-      launches += 2;
-    }
-    if (any_f32) {
-      exact_top2_kernel<float, false><<<dim3(max_qblk_exact, np), 256, EX_SMEM, c->stream>>>(c->d_views, bb.d_pairs, PM_EXACT_F32, bb.d_cands, bb.d_count, ratio_sq, nullptr, nullptr);
-      ++launches;
-    }
-    if (any_u8) {
-      exact_top2_kernel<uint8_t, false><<<dim3(max_qblk_exact, np), 256, EX_SMEM, c->stream>>>(c->d_views, bb.d_pairs, PM_EXACT_U8, bb.d_cands, bb.d_count, ratio_sq, nullptr, nullptr);
-      ++launches;
-    }
-    if (any_ham) {
-      hamming_top2_kernel<false><<<dim3(max_qblk_ham, np), HM_TQ, 0, c->stream>>>(c->d_views, bb.d_pairs, bb.d_cands, bb.d_count, dist_ratio, nullptr, nullptr);
-      ++launches;
-    }
-    if (any_gf32) {
-      generic_top2_pairs_kernel<float><<<dim3(max_qblk_gen, np), 128, 0, c->stream>>>(c->d_views, bb.d_pairs, PM_GENERIC_F32, bb.d_cands, bb.d_count, ratio_sq);
-      ++launches;
-    }
-    if (any_gu8) {
-      generic_top2_pairs_kernel<uint8_t><<<dim3(max_qblk_gen, np), 128, 0, c->stream>>>(c->d_views, bb.d_pairs, PM_GENERIC_U8, bb.d_cands, bb.d_count, ratio_sq);
-      ++launches;
-    }
-    CK(cudaEventRecord(k1, c->stream));
-    if (c->pipe_streams) CK(cudaStreamWaitEvent(ps, k1, 0));
-    kernel_events.push_back({k0, k1});
-    scan_counts_kernel<<<1, 256, 0, ps>>>(bb.d_count, np, bb.d_off);
-    verify_pack_kernel<<<dim3(np, VERIFY_BLOCKS_PER_PAIR), VERIFY_WARPS * 32, 0, ps>>>(c->d_views, bb.d_pairs, bb.d_cands, bb.d_count, bb.d_off, bb.d_out, ratio_sq, c->d_err);
-    launches += 2;
-    if (dev_fin) {
-      finish_pairs_kernel<<<np, FIN_THREADS, 0, ps>>>(c->d_views, bb.d_pairs, c->d_flags, bb.d_out, bb.d_count, bb.d_off, bb.d_scratch, bb.d_fin, bb.d_fin_count);
-      ++launches;
-      CK(cudaMemcpyAsync(bb.h_meta + 2 * PAIR_CAP + 2, bb.d_fin_count, sizeof(int) * np, cudaMemcpyDeviceToHost, ps));
-    }
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(bb.h_meta + 3 * PAIR_CAP + 2, bb.d_fb_count + 1, sizeof(int), cudaMemcpyDeviceToHost, ps));
-    CK(cudaMemcpyAsync(bb.h_meta, bb.d_count, sizeof(int) * np, cudaMemcpyDeviceToHost, ps));
-    CK(cudaMemcpyAsync(bb.h_meta + PAIR_CAP, bb.d_off, sizeof(int) * (np + 1), cudaMemcpyDeviceToHost, ps));
-    CK(cudaEventRecord(bb.ev_meta, ps));
-    return B200M_OK;
-  };
-
-  const double t_setup = now();
-  CK(cudaEventRecord(c->ev_start, c->stream));
-  if (stage == B200M_STAGE_DEVICE) {
-    for (size_t bi = 0; bi < batches.size(); ++bi) {
-      if (bi >= 2) CK(cudaEventSynchronize(c->buf[bi & 1].ev_meta));   // pinned staging of batch bi-2 consumed by its H2D copies
-      if ((rc = enqueue(bi))) return rc;
-      // totals are read from the pinned meta buffer once the batch is done; accumulate lazily below
-      if (bi >= 1) { CK(cudaEventSynchronize(c->buf[(bi - 1) & 1].ev_meta)); const Batch& P = batches[bi - 1]; total_records += c->buf[(bi - 1) & 1].h_meta[PAIR_CAP + (P.end - P.begin)]; fallback_rows += c->buf[(bi - 1) & 1].h_meta[3 * PAIR_CAP + 2]; }
-    }
-    CK(cudaEventRecord(c->ev_end, c->stream));
-    if (!batches.empty()) { const size_t l = batches.size() - 1; CK(cudaEventSynchronize(c->buf[l & 1].ev_meta)); total_records += c->buf[l & 1].h_meta[PAIR_CAP + (batches[l].end - batches[l].begin)]; fallback_rows += c->buf[l & 1].h_meta[3 * PAIR_CAP + 2]; }
-  } else {
-    if (!batches.empty() && (rc = enqueue(0))) return rc;
-    for (size_t bi = 0; bi < batches.size(); ++bi) {
-      const Batch& B = batches[bi];
-      BatchBuf& bb = c->buf[bi & 1];
-      const int np = (int)(B.end - B.begin);
-      if (bi + 1 < batches.size()) {
-        // buffer set (bi+1)&1 was last used by batch bi-1: its records have been consumed (pool wait below)
-        if ((rc = enqueue(bi + 1))) return rc;
-      }
-      CK(cudaEventSynchronize(bb.ev_meta));
-      const int total = bb.h_meta[PAIR_CAP + np];
-      fallback_rows += bb.h_meta[3 * PAIR_CAP + 2];
-      if (bi >= 2) groups[bi - 2]->wait();       // the tasks of batch bi-2 read this pinned record buffer
-      if (total > 0) {
-        CK(cudaStreamWaitEvent(c->copy_stream, bb.ev_meta, 0));
-        CK(cudaMemcpyAsync(bb.h_out, dev_fin ? (const void*)bb.d_fin : (const void*)bb.d_out, sizeof(Rec) * (size_t)total, cudaMemcpyDeviceToHost, c->copy_stream));
-        CK(cudaEventRecord(bb.ev_copy, c->copy_stream));
-        CK(cudaEventSynchronize(bb.ev_copy));
-      }
-      if (bi + 1 == batches.size()) {
-        // end of the device work of this call = the last match list has landed in pinned host memory (SURVEY 8d)
-        CK(cudaStreamWaitEvent(c->copy_stream, bb.ev_meta, 0));
-        CK(cudaEventRecord(c->ev_end, c->copy_stream));
-      }
-      total_records += total;
-      // finishing tasks (one per directed pair) run behind the GPU: they only have to be done before batch bi+2's records
-      // are copied into the same pinned buffer.  The per-pair counts/offsets are copied out of the pinned meta block first,
-      // because enqueue(bi+2) overwrites it.
-      arena.b[bi] = c->recycler->take((size_t)std::max(total, 1));
-      TaskGroup* grp = groups[bi].get();
-      // one pool task per ~4096 records (or 64 pairs): for small images the task hand-off would otherwise cost more than the work
-      // cnt >= 0: raw records, finished here (finish_directed); done >= 0: `done` final matches from the device finishing stage, copied
-      struct Job { const Rec* recs; int cnt; int done; b200m_match* dst; int* len; const ViewHost* vi; const ViewHost* vj; bool ham; };
-      auto jobs = std::make_shared<std::vector<Job>>();
-      long job_records = 0;
-      const bool full = stage == B200M_STAGE_FULL;
-      auto flush = [&] {
-        if (jobs->empty()) return;
-        grp->add(1);
-        std::shared_ptr<std::vector<Job>> mine = std::move(jobs);
-        c->pool->submit([mine, grp, full] {
-          for (const Job& j : *mine) {
-            if (j.done >= 0) { std::memcpy(j.dst, j.recs, sizeof(b200m_match) * (size_t)j.done); *j.len = j.done; }
-            else *j.len = finish_directed(j.recs, j.cnt, j.ham, full, *j.vi, *j.vj, j.dst);
-          }
-          grp->done();
-        });
-        jobs = std::make_shared<std::vector<Job>>();
-        job_records = 0;
-      };
-      for (int p = 0; p < np; ++p) {
-        const size_t di = seqv[B.begin + p];
-        const Directed d = dir[di];
-        dir_ptr[di] = arena.b[bi].p + bb.h_meta[PAIR_CAP + p];
-        int cnt = bb.h_meta[p], done = -1;
-        if (d.mode == PM_SKIP || cnt == 0) continue;
-        if (dev_fin) {                                   // >= 0: final matches; < 0: -(records + 1) left for the host (view not in general position)
-          const int f = bb.h_meta[2 * PAIR_CAP + 2 + p];
-          if (f >= 0) done = f; else cnt = -(f + 1);
-          if (done == 0) continue;
-        }
-        jobs->push_back(Job{bb.h_out + bb.h_meta[PAIR_CAP + p], cnt, done, dir_ptr[di], &dir_len[di], &c->views[d.slot_i], &c->views[d.slot_j], d.mode == PM_HAMMING});
-        job_records += cnt;
-        if (job_records >= 4096 || jobs->size() >= 64) flush();
-      }
-      flush();
-    }
-    const double t_loop = now();
-    for (auto& g : groups) g->wait();
-    if (timing) fprintf(stderr, "[b200m] match_pairs: batch loop %.2f ms, last finishing groups +%.2f ms\n", t_loop - t_setup, now() - t_loop);
-    if (batches.empty()) CK(cudaEventRecord(c->ev_end, c->stream));
-  }
-  const double t_gpu_done = now();
-  CK(cudaStreamSynchronize(c->stream));
-  CK(cudaStreamSynchronize(c->pack_stream));
-  float ms = 0.f;
-  CK(cudaEventSynchronize(c->ev_end));
-  CK(cudaEventElapsedTime(&ms, c->ev_start, c->ev_end));
-  double sk = 0;
-  for (auto& e : kernel_events) { float t = 0.f; CK(cudaEventElapsedTime(&t, e.first, e.second)); sk += t; }
-  if (timing && !kernel_events.empty()) {
-    // device timeline of the call: search kernels back to back?  gap = end of one batch's search kernels -> start of the next one's
-    // (packing / finishing kernels, meta copies, the next batch's pair-table copies, and any wait for the host)
-    float lead = 0.f, gaps = 0.f, gmax = 0.f, tail = 0.f;
-    CK(cudaEventElapsedTime(&lead, c->ev_start, kernel_events.front().first));
-    for (size_t k = 0; k + 1 < kernel_events.size(); ++k) { float t = 0.f; CK(cudaEventElapsedTime(&t, kernel_events[k].second, kernel_events[k + 1].first)); gaps += t; gmax = std::max(gmax, t); }
-    CK(cudaEventElapsedTime(&tail, kernel_events.back().second, c->ev_end));
-    fprintf(stderr, "[b200m] device timeline: %zu batches, search kernels %.2f ms, lead-in %.2f, gaps between batches %.2f (max %.2f), tail after the last search kernel %.2f ms\n",
-            kernel_events.size(), sk, lead, gaps, gmax, tail);
-  }
-  unsigned errs = 0;
-  CK(cudaMemcpy(&errs, c->d_err, sizeof(unsigned), cudaMemcpyDeviceToHost));
-  c->err_total = errs;
-
-  // ---- assemble: offsets first, then the per-pair copies into one contiguous block in parallel on the pool
-  std::unique_ptr<b200m_result> res(new b200m_result());
-  res->pair_ids.reserve(2 * fwd.size());
-  res->offsets.assign(fwd.size() + 1, 0);
-  if (stage != B200M_STAGE_DEVICE && do_cross) {
-    // keep m iff (m.j, m.i) is in the reverse list (ImageCollectionMatcher_generic.cpp:92-109); filtered in place, in parallel
-    TaskGroup g; g.add((int)fwd.size());
-    for (size_t k = 0; k < fwd.size(); ++k) {
-      b200m_match* f = dir_ptr[k * step]; int* nf = &dir_len[k * step];
-      const b200m_match* r = dir_ptr[k * step + 1]; const int nr = dir_len[k * step + 1];
-      TaskGroup* gp = &g;
-      c->pool->submit([=] {
-        std::vector<std::pair<uint32_t, uint32_t>> rv; rv.reserve(nr);
-        for (int e = 0; e < nr; ++e) rv.push_back({r[e].i, r[e].j});
-        std::sort(rv.begin(), rv.end());
-        int w = 0;
-        for (int e = 0; e < *nf; ++e)
-          if (std::binary_search(rv.begin(), rv.end(), std::make_pair(f[e].j, f[e].i))) f[w++] = f[e];
-        *nf = w;
-        gp->done();
-      });
-    }
-    g.wait();
-  }
-  for (size_t k = 0; k < fwd.size(); ++k) {
-    res->pair_ids.push_back(fwd[k].first); res->pair_ids.push_back(fwd[k].second);
-    res->offsets[k + 1] = res->offsets[k] + (stage != B200M_STAGE_DEVICE ? dir_len[k * step] : 0);
-  }
-  const size_t total_matches = (size_t)res->offsets[fwd.size()];
-  res->recycler = c->recycler;
-  res->matches = c->recycler->take(total_matches);
-  if (total_matches) {
-    const size_t CHUNK_PAIRS = 64;
-    TaskGroup g; g.add((int)((fwd.size() + CHUNK_PAIRS - 1) / CHUNK_PAIRS));
-    for (size_t k0 = 0; k0 < fwd.size(); k0 += CHUNK_PAIRS) {
-      const size_t k1 = std::min(fwd.size(), k0 + CHUNK_PAIRS);
-      b200m_match* base = res->matches.p; const int64_t* offs = res->offsets.data();
-      b200m_match* const* dp = dir_ptr.data(); const int* dl = dir_len.data(); TaskGroup* gp = &g;
-      c->pool->submit([=] {
-        for (size_t k = k0; k < k1; ++k) if (dl[k * step] > 0) std::memcpy(base + offs[k], dp[k * step], sizeof(b200m_match) * (size_t)dl[k * step]);
-        gp->done();
-      });
-    }
-    g.wait();
-  }
-  if (timing) fprintf(stderr, "[b200m] match_pairs n=%d stage=%d: setup %.2f ms, batches %.2f ms (gpu %.2f), tail (cross+assemble) %.2f ms, total %.2f ms\n",
-                      n_pairs, stage, t_setup - t_begin, t_gpu_done - t_setup, ms, now() - t_gpu_done, now() - t_begin);
-  c->last = LastCall{ms, sk, launches, tc_pairs, real_pairs, u8_pairs, total_records, fallback_rows, (int)batches.size(), ng_pairs};
-  *out = res.release();
-  return B200M_OK;
 }
 
 int b200m_result_num_pairs(const b200m_result* r) { return r ? (int)(r->offsets.size() - 1) : 0; }

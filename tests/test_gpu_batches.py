@@ -287,6 +287,7 @@ class Run:
         self.bytes = pid.tobytes() + off.tobytes() + mat.tobytes()
         self.got = as_dict((pid, off, mat))
         self.batches, self.tc, self.u8 = ctx.last_batches(), ctx.last_tc_pairs(), ctx.last_u8_tc_pairs()
+        self.ng = ctx.last_u8_norm_gemm_pairs()
         self.real, self.fallback, self.errors = ctx.last_real_tc_pairs(), ctx.last_fallback_rows(), ctx.exactness_errors()
 
 
@@ -442,8 +443,8 @@ def test_reused_context_equals_fresh(world, answers):
 
 
 # ---------------------------------------------------------------------------------------------- every kernel class in every batch
-CLASSES = ["u8", "fp16", "real", "exact_f32", "exact_u8", "generic"]
-K_DB, L_Q = 30, 50          # database / query views per class: 9000 directed pairs, three batches
+CLASSES = ["u8", "ng", "fp16", "real", "exact_f32", "exact_u8", "generic"]
+K_DB, L_Q = 30, 50          # database / query views per class: 10500 directed pairs, three batches
 
 
 def noise_rows(rng, n):
@@ -458,6 +459,8 @@ def class_view(rng, pool, gpool, cls, m):
     d = sift_view(rng, pool, m, m)
     if cls == "u8":                                        # integer-valued fp32 in 0..255: staged as uchar, u8 kernel
         return d.astype(np.float32)
+    if cls == "ng":                                        # ... in 0..127 (databases of >= 128 rows): u8 norm-GEMM kernel
+        return np.minimum(d, 127).astype(np.float32)
     if cls == "fp16":                                      # signed integers: fp16 kernel
         return d.astype(np.float32) - np.float32(64)
     if cls == "real":                                      # real-valued: filter kernel; noise rows in all four chunks fall back
@@ -474,14 +477,16 @@ def class_view(rng, pool, gpool, cls, m):
 
 
 def class_scene(seed=8201):
-    """Database view k of class c has id 6k + c, so PairSet order cycles through the classes every 6 database views (300 pairs)."""
+    """Database view k of class c has id 7k + c, so PairSet order cycles through the classes every 7 database views (350 pairs).
+    The norm-GEMM class's database views have 128 to 160 rows (one full tile at least), every other class's at most 50."""
     rng = np.random.default_rng(seed)
     pool, gpool = synth.sift_pool(48, rng), rng.gamma(2.0, 20.0, (48, 64))
     descs, cls_of, pairs = {}, {}, []
     for k in range(K_DB):
         for c, cls in enumerate(CLASSES):
             v = len(CLASSES) * k + c
-            descs[v] = class_view(rng, pool, gpool, cls, 50 if cls == "real" else int(rng.integers(2, 41)))
+            m = 50 if cls == "real" else int(rng.integers(128, 161)) if cls == "ng" else int(rng.integers(2, 41))
+            descs[v] = class_view(rng, pool, gpool, cls, m)
             cls_of[v] = cls
     q0 = len(CLASSES) * K_DB
     for c, cls in enumerate(CLASSES):
@@ -512,14 +517,15 @@ def oracle_view_list(descs, xys, keep, dim, dtype):
 
 @pytest.mark.gpu
 def test_every_kernel_class_in_every_batch(ora):
-    """One L2 list across three batches (PAIR_CAP) whose every batch launches the u8, fp16, real-valued (filter, re-scoring and
-    per-pair fallback), exact f32 / u8 and generic kernels into one candidate array."""
+    """One L2 list across three batches (PAIR_CAP) whose every batch launches the u8, u8 norm-GEMM, fp16, real-valued (filter,
+    re-scoring and per-pair fallback), exact f32 / u8 and generic kernels into one candidate array; the work items of all four
+    tensor-core classes share each batch's item table."""
     descs, xys, cls_of, pairs = class_scene()
     sizes = {v: len(d) for v, d in descs.items()}
     plan = plan_of(sizes, pairs)
     per = {c: sum(cls_of[a] == c for a, _ in pairs) for c in CLASSES}
     want = {}
-    groups = {"f32": ({"u8", "fp16", "real", "exact_f32"}, 128, np.float32, ora), "u8": ({"exact_u8"}, 128, np.uint8, ora),
+    groups = {"f32": ({"u8", "ng", "fp16", "real", "exact_f32"}, 128, np.float32, ora), "u8": ({"exact_u8"}, 128, np.uint8, ora),
               "generic": ({"generic"}, 64, np.float32, oracle.Oracle("port"))}
     for keep_cls, dim, dt, checker in groups.values():
         keep = {v for v, c in cls_of.items() if c in keep_cls}
@@ -534,7 +540,7 @@ def test_every_kernel_class_in_every_batch(ora):
     finally:
         ctx.close()
     assert r.batches == len(plan) >= 3
-    assert (r.tc, r.u8, r.real) == (per["u8"] + per["fp16"], per["u8"], per["real"])
+    assert (r.tc, r.u8, r.ng, r.real) == (per["u8"] + per["ng"] + per["fp16"], per["u8"] + per["ng"], per["ng"], per["real"])
     assert r.errors == 0 and r.fallback > 0
     assert_same(r.got, want, "classes")
 

@@ -132,7 +132,7 @@ def directed(descs, pairs, cross):
 
 
 def ng_eligible(descs, i, j):
-    """Directed pair (database i, query j) on the norm-GEMM kernel: the engine's gates (engine.cu ng_pair)."""
+    """Directed pair (database i, query j) on the norm-GEMM kernel: the engine's gates (engine.cu pair_class)."""
     db, q = np.asarray(descs[i], np.int64), np.asarray(descs[j], np.int64)
     return len(db) >= BN and len(q) >= 1 and q.max() <= 127 and (db * db).sum(1).max() <= LIMB_CAP
 
