@@ -37,11 +37,14 @@
 #include <algorithm>
 #include <array>
 #include <cmath>
+#include <cstddef>
 #include <cstdint>
 #include <limits>
 #include <map>
+#include <numeric>
 #include <random>
 #include <sstream>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -97,9 +100,9 @@ inline void mtState(const std::mt19937& g, uint32_t state[625])
 }
 }  // namespace b200detail
 
-/// The bookkeeping both batch adaptors share: a putative list over views that are uploaded ONCE per descriptor type.  addView every
-/// (view, type) with its guided positions, addPair every pair, then the derived class's run().  The views are removed from the engine
-/// when the batch is destroyed.
+/// The bookkeeping the a-contrario batch adaptors share: a putative list over views that are uploaded ONCE per descriptor type.
+/// addView every (view, type) with its guided positions, addPair every pair, then the derived class's run(), which makes its engine
+/// call(s) and hands them to finish().  The views are removed from the engine when the batch is destroyed.
 class GeometricFilterBatchBase_b200
 {
 public:
@@ -171,23 +174,23 @@ protected:
         std::size_t offset;
     };
 
-    /// What one K10 call over the list returned, per pair in addPair order.
+    /// What one K10 call returned for its pairs (indices in addPair order, ascending), entry q for pairs[q].
     struct K10Out
     {
+        std::vector<int> pairs;
         std::vector<int64_t> offsets;
         std::vector<uint8_t> valid;
         std::vector<int32_t> nInl, iters;
         std::vector<uint32_t> inl;
         std::vector<double> M, errMax, nfa;
-        explicit K10Out(const std::vector<PairIn>& pairs, std::size_t nCorr)
-          : K10Out(offsetsOf(pairs, nCorr))
-        {}
-        /// offs: the n + 1 correspondence offsets of the call's pairs
-        explicit K10Out(std::vector<int64_t> offs)
-          : offsets(std::move(offs))
+        /// nCorr: the size, in correspondences, of the buffer the pairs' offsets index
+        K10Out(const std::vector<PairIn>& added, std::vector<int> ks, std::size_t nCorr)
+          : pairs(std::move(ks))
         {
-            const int n = (int)offsets.size() - 1;
-            const std::size_t nCorr = (std::size_t)offsets.back();
+            const int n = (int)pairs.size();
+            for (const int k : pairs)
+                offsets.push_back((int64_t)added[k].offset);
+            offsets.push_back((int64_t)nCorr);
             valid.resize(std::max(n, 1));
             nInl.resize(std::max(n, 1));
             iters.resize(std::max(n, 1));
@@ -196,14 +199,15 @@ protected:
             errMax.resize(std::max(n, 1));
             nfa.resize(std::max(n, 1));
         }
-        static std::vector<int64_t> offsetsOf(const std::vector<PairIn>& pairs, std::size_t nCorr)
-        {
-            std::vector<int64_t> o(pairs.size() + 1, 0);
-            for (std::size_t k = 0; k < pairs.size(); ++k)
-                o[k + 1] = (k + 1 < pairs.size() ? (int64_t)pairs[k + 1].offset : (int64_t)nCorr);
-            return o;
-        }
     };
+
+    /// 0 .. n-1: every pair added
+    std::vector<int> allPairs() const
+    {
+        std::vector<int> ks(_pairs.size());
+        std::iota(ks.begin(), ks.end(), 0);
+        return ks;
+    }
 
     const double* corrData() const
     {
@@ -211,23 +215,58 @@ protected:
         return _corr.empty() ? dummy : _corr.data();
     }
 
-    /// copyInlierMatches and hasStrongSupport(minimumSamples) of pair k, entry q of the call r that estimated it; returns whether it
-    /// has strong support (then result[pair] holds its inliers).
-    bool keepInliers(int k, const K10Out& r, int q, std::size_t minimumSamples, std::map<Pair, matching::MatchesPerDescType>& result) const
+    /// What every stage does after its engine call(s), each call's entries given with their pairs: fills estimates (the model into
+    /// the field `model`; errorMax and support only for a pair ACRANSAC found valid), keeps the pairs whose copied inliers pass
+    /// hasStrongSupport(.., minimumSamples), minimumSamples the solver's getMinimumNbRequiredSamples, and with guidedMatching
+    /// replaces their lists by the guided ones (see guided) over pair k's model, or over modelOf(k) when the guided step needs
+    /// another matrix.  Then moves the kept lists into out.
+    template<class Estimate, class Call, class ModelOf = std::nullptr_t>
+    bool finish(std::initializer_list<const K10Out*> calls, std::vector<Estimate>& estimates, double (Estimate::*model)[9],
+                std::size_t minimumSamples, bool guidedMatching, double distanceRatio, Call call, matching::PairwiseMatches& out,
+                ModelOf modelOf = nullptr) const
     {
-        const std::vector<std::size_t> inliers(r.inl.begin() + r.offsets[q], r.inl.begin() + r.offsets[q] + r.nInl[q]);
-        matching::MatchesPerDescType perType;
-        b200detail::copyInlierMatches(inliers, _pairs[k].putatives, _pairs[k].descTypes, perType);
-        if (!b200detail::hasStrongSupport(perType, minimumSamples))
+        estimates.assign(_pairs.size(), Estimate());
+        std::map<Pair, matching::MatchesPerDescType> result;
+        std::vector<int> kept;
+        for (const K10Out* r : calls)
+            for (int q = 0; q < (int)r->pairs.size(); ++q)
+            {
+                const int k = r->pairs[q];
+                Estimate& e = estimates[k];
+                e.valid = r->valid[q] != 0;
+                std::copy(r->M.begin() + 9 * q, r->M.begin() + 9 * q + 9, e.*model);
+                if (!e.valid)
+                    continue;
+                e.errorMax = r->errMax[q];
+                const std::vector<std::size_t> inliers(r->inl.begin() + r->offsets[q], r->inl.begin() + r->offsets[q] + r->nInl[q]);
+                matching::MatchesPerDescType perType;
+                b200detail::copyInlierMatches(inliers, _pairs[k].putatives, _pairs[k].descTypes, perType);
+                e.strongSupport = b200detail::hasStrongSupport(perType, minimumSamples);
+                if (e.strongSupport)
+                {
+                    result[_pairs[k].pair] = std::move(perType);
+                    kept.push_back(k);
+                }
+            }
+        std::sort(kept.begin(), kept.end());
+        const auto guidedModel = [&](int k) -> const double* {
+            if constexpr (std::is_null_pointer_v<ModelOf>)
+                return estimates[k].*model;
+            else
+                return modelOf(k);
+        };
+        if (guidedMatching && !guided(kept, estimates, guidedModel, call, distanceRatio * distanceRatio, result))
             return false;
-        result[_pairs[k].pair] = std::move(perType);
+        for (auto& x : result)
+            out[x.first] = std::move(x.second);
         return true;
     }
 
     /// The guided step of the kept pairs: their lists are replaced by one entry per common type (empty ones included) when errorMax
-    /// is finite, else by nothing.  M(k) is pair k's 9 model coefficients; call(ids, n, M, errorTh, &res) makes the one batched call.
-    template<class ModelOf, class Call>
-    bool guided(const std::vector<int>& kept, const std::vector<double>& errorMax, ModelOf M_of, Call call,
+    /// is finite, else by nothing.  M(k) is pair k's 9 model coefficients; call(ids, n, M, errorTh, distRatio, &res) makes the one
+    /// batched call, with errorTh = errorMax^2 per item and distRatio = distanceRatio^2.
+    template<class Estimate, class ModelOf, class Call>
+    bool guided(const std::vector<int>& kept, const std::vector<Estimate>& estimates, ModelOf M_of, Call call, double distRatio,
                 std::map<Pair, matching::MatchesPerDescType>& result) const
     {
         std::vector<uint32_t> ids;
@@ -236,8 +275,10 @@ protected:
         for (const int k : kept)
         {
             result[_pairs[k].pair] = matching::MatchesPerDescType();       // the guided result replaces the inliers, even when empty
-            if (errorMax[k] == std::numeric_limits<double>::infinity())
+            const double errorMax = estimates[k].errorMax;
+            if (errorMax == std::numeric_limits<double>::infinity())
                 continue;                                                  // Geometry_guided_matching: m_dPrecision_robust infinite
+            const double* m = M_of(k);
             for (const feature::EImageDescriberType t : _pairs[k].descTypes)
             {
                 const auto l = _views.find(std::make_pair(_pairs[k].pair.first, t)), r = _views.find(std::make_pair(_pairs[k].pair.second, t));
@@ -245,16 +286,15 @@ protected:
                     return false;
                 ids.push_back(l->second);
                 ids.push_back(r->second);
-                const double* m = M_of(k);
                 M.insert(M.end(), m, m + 9);
-                th.push_back(errorMax[k] * errorMax[k]);
+                th.push_back(errorMax * errorMax);
                 items.emplace_back(_pairs[k].pair, t);
             }
         }
         if (items.empty())
             return true;
         b200m_result* res = nullptr;
-        if (call(ids.data(), (int)items.size(), M.data(), th.data(), &res) != B200M_OK)
+        if (call(ids.data(), (int)items.size(), M.data(), th.data(), distRatio, &res) != B200M_OK)
         {
             b200m_result_free(res);
             return false;
@@ -341,55 +381,24 @@ public:
         std::vector<int> sub[2];                                        // in addPair order: the planar pairs, the spherical pairs
         for (int k = 0; k < n; ++k)
             sub[(int)_spherical[k]].push_back(k);
-        std::vector<int64_t> offs[2];
-        for (int s = 0; s < 2; ++s)
-        {
-            for (const int k : sub[s])
-                offs[s].push_back((int64_t)_pairs[k].offset);
-            offs[s].push_back(s == 0 ? (int64_t)(_corr.size() / 4) : (int64_t)(_bear.size() / 6));
-        }
         std::vector<int32_t> wh;
         for (const int k : sub[0])
             wh.insert(wh.end(), _wh.begin() + 4 * k, _wh.begin() + 4 * k + 4);
-        K10Out r[2] = {K10Out(offs[0]), K10Out(offs[1])};
+        K10Out r0(_pairs, sub[0], _corr.size() / 4), r1(_pairs, sub[1], _bear.size() / 6);
         const int n0 = (int)sub[0].size(), n1 = (int)sub[1].size();
-        if (n0 > 0 && b200m_acransac_fundamental_pairs(_ctx, n0, r[0].offsets.data(), corrData(), wh.data(), state, (int64_t)maxIteration,
-                                                       precision, r[0].valid.data(), r[0].nInl.data(), r[0].inl.data(), r[0].M.data(),
-                                                       r[0].errMax.data(), r[0].nfa.data(), r[0].iters.data()) != B200M_OK)
+        if (n0 > 0 && b200m_acransac_fundamental_pairs(_ctx, n0, r0.offsets.data(), corrData(), wh.data(), state, (int64_t)maxIteration,
+                                                       precision, r0.valid.data(), r0.nInl.data(), r0.inl.data(), r0.M.data(),
+                                                       r0.errMax.data(), r0.nfa.data(), r0.iters.data()) != B200M_OK)
             return false;
-        if (n1 > 0 && b200m_acransac_fundamental_spherical_pairs(_ctx, n1, r[1].offsets.data(), _bear.data(), state, 0, (int64_t)maxIteration,
-                                                                 precision, r[1].valid.data(), r[1].nInl.data(), r[1].inl.data(), r[1].M.data(),
-                                                                 r[1].errMax.data(), r[1].nfa.data(), r[1].iters.data(), nullptr) != B200M_OK)
+        if (n1 > 0 && b200m_acransac_fundamental_spherical_pairs(_ctx, n1, r1.offsets.data(), _bear.data(), state, 0, (int64_t)maxIteration,
+                                                                 precision, r1.valid.data(), r1.nInl.data(), r1.inl.data(), r1.M.data(),
+                                                                 r1.errMax.data(), r1.nfa.data(), r1.iters.data(), nullptr) != B200M_OK)
             return false;
-        _estimates.assign(n, Estimate());
-        std::map<Pair, matching::MatchesPerDescType> result;
-        std::vector<int> kept;
-        std::vector<double> errorMax(n, std::numeric_limits<double>::infinity());
-        for (int s = 0; s < 2; ++s)
-            for (int q = 0; q < (int)sub[s].size(); ++q)
-            {
-                const int k = sub[s][q];
-                Estimate& e = _estimates[k];
-                e.valid = r[s].valid[q] != 0;
-                std::copy(r[s].M.begin() + 9 * q, r[s].M.begin() + 9 * q + 9, e.F);
-                if (!e.valid)
-                    continue;
-                e.errorMax = errorMax[k] = r[s].errMax[q];
-                e.strongSupport = keepInliers(k, r[s], q, 7, result);   // getMinimumNbRequiredSamples of both 7-point solvers
-                if (e.strongSupport)
-                    kept.push_back(k);
-            }
-        std::sort(kept.begin(), kept.end());
-        if (guidedMatching &&
-            !guided(kept, errorMax, [&](int k) { return _estimates[k].F; },
-                    [&](const uint32_t* ids, int np, const double* M, const double* th, b200m_result** res) {
-                        return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distanceRatio * distanceRatio, res);
-                    },
-                    result))
-            return false;
-        for (auto& x : result)
-            out[x.first] = std::move(x.second);
-        return true;
+        return finish({&r0, &r1}, _estimates, &Estimate::F, 7, guidedMatching, distanceRatio,   // 7: both 7-point solvers
+                      [&](const uint32_t* ids, int np, const double* M, const double* th, double distRatio, b200m_result** res) {
+                          return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distRatio, res);
+                      },
+                      out);
     }
 
     /// The estimation of the k-th pair added, after run().
@@ -435,39 +444,18 @@ public:
         const int n = (int)_pairs.size();
         uint32_t state[625];
         b200detail::mtState(rng, state);
-        K10Out r(_pairs, _corr.size() / 4);
+        K10Out r(_pairs, allPairs(), _corr.size() / 4);
         if (n > 0 && b200m_acransac_homography_pairs(_ctx, n, r.offsets.data(), corrData(), _wh.data(), state, 0, (int64_t)maxIteration, precision,
                                                      r.valid.data(), r.nInl.data(), r.inl.data(), r.M.data(), r.errMax.data(), r.nfa.data(),
                                                      r.iters.data(), nullptr) != B200M_OK)
             return false;
-        _estimates.assign(n, Estimate());
-        std::map<Pair, matching::MatchesPerDescType> result;
-        std::vector<int> kept;
-        std::vector<double> errorMax(n, std::numeric_limits<double>::infinity());
-        for (int k = 0; k < n; ++k)
-        {
-            Estimate& e = _estimates[k];
-            e.valid = r.valid[k] != 0;
-            std::copy(r.M.begin() + 9 * k, r.M.begin() + 9 * k + 9, e.H);
-            if (!e.valid)
-                continue;
-            e.errorMax = errorMax[k] = r.errMax[k];
-            e.strongSupport = keepInliers(k, r, k, 4, result);             // Homography4PSolver::getMinimumNbRequiredSamples
-            if (e.strongSupport)
-                kept.push_back(k);
-        }
-        if (guidedMatching &&
-            !guided(kept, errorMax, [&](int k) { return _estimates[k].H; },
-                    [&](const uint32_t* ids, int np, const double* M, const double* th, b200m_result** res) {
-                        if (distanceRatio < 0)
-                            return b200m_guided_match_positions_pairs(_ctx, ids, np, B200M_MODEL_HOMOGRAPHY, M, th, 1, res);
-                        return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_HOMOGRAPHY, M, th, distanceRatio * distanceRatio, res);
-                    },
-                    result))
-            return false;
-        for (auto& x : result)
-            out[x.first] = std::move(x.second);
-        return true;
+        return finish({&r}, _estimates, &Estimate::H, 4, guidedMatching, distanceRatio,   // 4: Homography4PSolver
+                      [&](const uint32_t* ids, int np, const double* M, const double* th, double distRatio, b200m_result** res) {
+                          if (distanceRatio < 0)
+                              return b200m_guided_match_positions_pairs(_ctx, ids, np, B200M_MODEL_HOMOGRAPHY, M, th, 1, res);
+                          return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_HOMOGRAPHY, M, th, distRatio, res);
+                      },
+                      out);
     }
 
     /// The estimation of the k-th pair added, after run().
@@ -528,39 +516,21 @@ public:
         const int n = (int)_pairs.size();
         uint32_t state[625];
         b200detail::mtState(rng, state);
-        K10Out r(_pairs, _corr.size() / 4);
+        K10Out r(_pairs, allPairs(), _corr.size() / 4);
         if (n > 0 && b200m_acransac_essential_pairs(_ctx, n, r.offsets.data(), corrData(), _wh.data(), _K.data(), state, 0, (int64_t)maxIteration,
                                                     precision * precision, r.valid.data(), r.nInl.data(), r.inl.data(), r.M.data(),
                                                     r.errMax.data(), r.nfa.data(), r.iters.data(), nullptr) != B200M_OK)
             return false;
-        _estimates.assign(n, Estimate());
-        _F.assign(9 * n, 0.0);
-        std::map<Pair, matching::MatchesPerDescType> result;
-        std::vector<int> kept;
-        std::vector<double> errorMax(n, std::numeric_limits<double>::infinity());
-        for (int k = 0; k < n; ++k)
-        {
-            Estimate& e = _estimates[k];
-            e.valid = r.valid[k] != 0;
-            std::copy(r.M.begin() + 9 * k, r.M.begin() + 9 * k + 9, e.E);
-            if (!e.valid)
-                continue;
-            e.errorMax = errorMax[k] = r.errMax[k];
-            fundamentalFromEssential(e.E, &_K[18 * k], &_K[18 * k + 9], &_F[9 * k]);
-            e.strongSupport = keepInliers(k, r, k, 5, result);             // Essential5PSolver::getMinimumNbRequiredSamples
-            if (e.strongSupport)
-                kept.push_back(k);
-        }
-        if (guidedMatching &&
-            !guided(kept, errorMax, [&](int k) { return &_F[9 * k]; },
-                    [&](const uint32_t* ids, int np, const double* M, const double* th, b200m_result** res) {
-                        return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distanceRatio * distanceRatio, res);
-                    },
-                    result))
-            return false;
-        for (auto& x : result)
-            out[x.first] = std::move(x.second);
-        return true;
+        std::vector<double> F(9 * n);   // the guided step's F of each kept pair
+        return finish({&r}, _estimates, &Estimate::E, 5, guidedMatching, distanceRatio,   // 5: Essential5PSolver
+                      [&](const uint32_t* ids, int np, const double* M, const double* th, double distRatio, b200m_result** res) {
+                          return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distRatio, res);
+                      },
+                      out,
+                      [&](int k) {
+                          fundamentalFromEssential(_estimates[k].E, &_K[18 * k], &_K[18 * k + 9], &F[9 * k]);
+                          return &F[9 * k];
+                      });
     }
 
     /// The estimation of the k-th pair added, after run().
@@ -600,7 +570,6 @@ private:
 
     std::vector<Estimate> _estimates;
     std::vector<double> _K;   // 18 per pair: K_I, K_J
-    std::vector<double> _F;   // 9 per pair: the guided step's F
 };
 
 /// robustModelEstimation with GeometricFilterMatrix_HGrowing (the `homography_growing` filter: filterMatchesByHGrowing on the

@@ -14,6 +14,7 @@ from __future__ import annotations
 
 import atexit
 import ctypes as C
+import itertools
 import os
 import weakref
 from enum import IntEnum
@@ -391,9 +392,7 @@ def geometricEstimation_F_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: 
     xI, xJ: n x 2 positions (the 2 x n matrices of fillMatricesWithUndistortFeaturesMatches, transposed); sizeI / sizeJ: (width,
     height); seed_or_state: a std::mt19937 seed or its 625-word state.  Returns the dict of Context.acransac_fundamental_pairs."""
     ctx = ctx or default_context()
-    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else seed_or_state
-    corr = np.concatenate([np.asarray(xI, np.float64).reshape(-1, 2), np.asarray(xJ, np.float64).reshape(-1, 2)], axis=1)
-    return ctx.acransac_fundamental_pairs([corr], [tuple(sizeI) + tuple(sizeJ)], st, maxIteration, precision)[0]
+    return ctx.acransac_fundamental_pairs(*_one_pair(xI, xJ, sizeI, sizeJ), _start_state(seed_or_state), maxIteration, precision)[0]
 
 
 def geometricEstimation_H_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: int = 50000, precision: float = np.inf,
@@ -402,9 +401,18 @@ def geometricEstimation_H_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: 
     dict of Context.acransac_homography_pairs: "H" and "mt_state_out", the generator advanced past this pair's draws, which the
     reference's single-threaded filter hands to the next pair."""
     ctx = ctx or default_context()
-    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else seed_or_state
+    return ctx.acransac_homography_pairs(*_one_pair(xI, xJ, sizeI, sizeJ), _start_state(seed_or_state), maxIteration, precision)[0]
+
+
+def _start_state(seed_or_state) -> np.ndarray:
+    """The caller's std::mt19937, given as a seed or as its 625-word state."""
+    return mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
+
+
+def _one_pair(xI, xJ, sizeI, sizeJ):
+    """The correspondence list (one n x 4 array: xI, yI, xJ, yJ) and size list of a single pair's K10 call."""
     corr = np.concatenate([np.asarray(xI, np.float64).reshape(-1, 2), np.asarray(xJ, np.float64).reshape(-1, 2)], axis=1)
-    return ctx.acransac_homography_pairs([corr], [tuple(sizeI) + tuple(sizeJ)], st, maxIteration, precision)[0]
+    return [corr], [tuple(sizeI) + tuple(sizeJ)]
 
 
 # EImageDescriberType in enum order (feature/imageDescriberCommon.hpp:19-55): getCommonDescTypes returns the common types in this order
@@ -475,65 +483,30 @@ def robustModelEstimation_F_AC(putatives: dict, regions_per_view: dict, image_si
     common type (empty ones included) replace them, or nothing when error_max is infinite (GeometricFilterMatrix_F_AC.hpp:363).  A
     spherical pair's guided matching uses its F and error_max on the guided positions, as the reference does."""
     ctx = ctx or default_context()
-    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
-    pairs, common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
+    common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
     sph = _spherical_inputs(putatives, regions_per_view, bearings or {}, common, est)
-    planar = [k for k, p in enumerate(est) if p not in sph]
-    spherical = [k for k, p in enumerate(est) if p in sph]
-    res = [None] * len(est)
-
-    def run_planar(ks, state):
-        for k, r in zip(ks, ctx.acransac_fundamental_pairs([corrs[k] for k in ks], [whs[k] for k in ks], state, maxIteration, precision) if ks else []):
-            res[k] = r
-    if not chain or not spherical:
-        run_planar(planar, st)
-        rs = ctx.acransac_fundamental_spherical_pairs([sph[est[k]] for k in spherical], st, maxIteration, precision) if spherical else []
-        for k, r in zip(spherical, rs):
-            res[k] = r
-    else:
-        run = []
-        for k, p in enumerate(est):
-            if p not in sph:
-                run.append(k)
-                continue
-            run_planar(run, st)
-            run = []
-            res[k] = ctx.acransac_fundamental_spherical_pairs([sph[p]], st, maxIteration, precision)[0]
-            st = res[k]["mt_state_out"]
-        run_planar(run, st)
-    info = {p: {"valid": False, "strong_support": False, "F": np.zeros((3, 3)), "error_max": np.inf, "spherical": p in sph} for p in pairs}
-    out = {}
-    for p, r in zip(est, res):
-        info[p].update(valid=r["valid"], F=r["F"], error_max=r["error_max"])
-        if p in sph:
-            info[p]["mt_state_out"] = r["mt_state_out"]
-        if not r["valid"]:
-            continue
-        inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
-        info[p]["strong_support"] = hasStrongSupport(inl)
-        if info[p]["strong_support"]:
-            out[p] = inl
-    if guidedMatching and out:
-        _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry,
-                      lambda vp, items: ctx.guided_match_pairs(vp, [info[p]["F"] for p, _ in items],
-                                                               [info[p]["error_max"] * info[p]["error_max"] for p, _ in items],
-                                                               distanceRatio * distanceRatio))
+    calls = [(lambda ks, st: ctx.acransac_fundamental_pairs([corrs[k] for k in ks], [whs[k] for k in ks], st, maxIteration, precision), False),
+             (lambda ks, st: ctx.acransac_fundamental_spherical_pairs([sph[est[k]] for k in ks], st, maxIteration, precision), True)]
+    out, info = _acransac_stage(ctx, putatives, regions_per_view, guided_geometry, common, est, [int(p in sph) for p in est], calls, "F", 7,
+                                seed_or_state, chain, guidedMatching, distanceRatio,
+                                lambda vp, items, Fs, th, ratio: ctx.guided_match_pairs(vp, Fs, th, ratio))
+    for p, d in info.items():
+        d["spherical"] = p in sph
     return out, info
 
 
 def _estimation_inputs(putatives: dict, regions_per_view: dict, image_sizes: dict, geometry: dict | None, desc_types):
-    """The pair list, each pair's common describer types (EImageDescriberType order), the pairs that have one, and for those the
-    correspondences of fillMatricesWithUndistortFeaturesMatches (n x 4: xI, yI, xJ, yJ, types concatenated in order) and image sizes."""
+    """Each pair's common describer types (EImageDescriberType order), the pairs that have one, and for those the correspondences of
+    fillMatricesWithUndistortFeaturesMatches (n x 4: xI, yI, xJ, yJ, types concatenated in order) and image sizes."""
     order = list(desc_types) if desc_types is not None else DESCRIBER_TYPES
     geometry = geometry or {}
-    pairs = list(putatives)
-    common = {p: [t for t in order if t in regions_per_view[p[0]] and t in regions_per_view[p[1]]] for p in pairs}
+    common = {p: [t for t in order if t in regions_per_view[p[0]] and t in regions_per_view[p[1]]] for p in putatives}
 
     def positions(v, t):
         g = geometry.get(v, {}).get(t)
         return np.asarray(g, np.float64).reshape(-1, 2) if g is not None else regions_per_view[v][t].positions.astype(np.float64)
 
-    est = [p for p in pairs if common[p]]                     # no common type: EstimationStatus(false, false)
+    est = [p for p in putatives if common[p]]                 # no common type: EstimationStatus(false, false)
     corrs, whs = [], []
     for I, J in est:
         parts = [np.zeros((0, 4))]
@@ -543,7 +516,7 @@ def _estimation_inputs(putatives: dict, regions_per_view: dict, image_sizes: dic
                 parts.append(np.concatenate([positions(I, t)[m["i"]], positions(J, t)[m["j"]]], axis=1))
         corrs.append(np.concatenate(parts))
         whs.append(tuple(image_sizes[I]) + tuple(image_sizes[J]))
-    return pairs, common, est, corrs, whs
+    return common, est, corrs, whs
 
 
 def _spherical_inputs(putatives: dict, regions_per_view: dict, bearings: dict, common: dict, est) -> dict:
@@ -596,6 +569,50 @@ def _guided_stage(ctx: Context, out: dict, info: dict, common: dict, regions_per
             ctx.lib.b200m_remove_view(ctx._h, C.c_uint32(vid))
 
 
+def _acransac_stage(ctx: Context, putatives: dict, regions_per_view: dict, guided_geometry: dict | None, common: dict, est: list, groups: list,
+                    calls: list, key: str, min_samples: int, seed_or_state, chain: bool, guidedMatching: bool, distanceRatio: float, guided):
+    """The stage rules the a-contrario filters share (robustModelEstimation around GeometricFilterMatrix_F_AC, _H_AC and _E_AC), over
+    the estimated pairs `est` in putative-list order.
+      groups, calls  pair k goes through calls[groups[k]] = (run(ks, state) -> the results of pairs ks, by_reference), by_reference
+                     the generator contract of its geometricEstimation.  chain=False: one call per group from the caller's state, in
+                     `calls` order.  chain=True: in list order, a by-reference pair alone, handing its mt_state_out to the next call,
+                     and each run of by-value pairs of one group in one call from the current state.
+      key            the model's name in the results and in info; min_samples: the solver's getMinimumNbRequiredSamples
+      guided         guided(view_pairs, items, models, errorTh, distRatio): the batched guided call over items = [(pair, type)],
+                     with errorTh = error_max^2 and distRatio = distanceRatio^2
+    ACRANSAC's validity comes before support.  Returns (out, info) as robustModelEstimation_H_AC describes them, "mt_state_out"
+    on the pairs whose call returned one."""
+    st = _start_state(seed_or_state)
+    if chain:
+        segments = [list(ks) for _, ks in itertools.groupby(range(len(est)), lambda k: (groups[k], k if calls[groups[k]][1] else -1))]
+    else:
+        segments = [ks for g in range(len(calls)) if (ks := [k for k, h in enumerate(groups) if h == g])]
+    res = [None] * len(est)
+    for ks in segments:
+        run, by_reference = calls[groups[ks[0]]]
+        for k, r in zip(ks, run(ks, st)):
+            res[k] = r
+        if chain and by_reference:
+            st = res[ks[0]]["mt_state_out"]
+    info = {p: {"valid": False, "strong_support": False, key: np.zeros((3, 3)), "error_max": np.inf} for p in putatives}
+    out = {}
+    for p, r in zip(est, res):
+        info[p].update({"valid": r["valid"], key: r[key], "error_max": r["error_max"]})
+        if "mt_state_out" in r:
+            info[p]["mt_state_out"] = r["mt_state_out"]
+        if not r["valid"]:
+            continue
+        inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
+        info[p]["strong_support"] = hasStrongSupport(inl, min_samples)
+        if info[p]["strong_support"]:
+            out[p] = inl
+    if guidedMatching and out:
+        _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry,
+                      lambda vp, items: guided(vp, items, [info[p][key] for p, _ in items],
+                                               [info[p]["error_max"] * info[p]["error_max"] for p, _ in items], distanceRatio * distanceRatio))
+    return out, info
+
+
 def robustModelEstimation_H_AC(putatives: dict, regions_per_view: dict, image_sizes: dict, seed_or_state, maxIteration: int = 50000,
                                precision: float = np.inf, guidedMatching: bool = False, distanceRatio: float = -1.0, geometry: dict | None = None,
                                guided_geometry: dict | None = None, desc_types=None, chain: bool = False, ctx: Context | None = None):
@@ -619,36 +636,15 @@ def robustModelEstimation_H_AC(putatives: dict, regions_per_view: dict, image_si
     {(I, J): {"valid", "strong_support", "H", "error_max"}, plus "mt_state_out" for the estimated pairs}).  The kept lists are as in
     robustModelEstimation_F_AC; the position-only guided lists are in the decorator's order (ratio and distance 0)."""
     ctx = ctx or default_context()
-    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
-    pairs, common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
-    if not est:
-        res = []
-    elif chain:
-        res = []
-        for c, wh in zip(corrs, whs):
-            res.append(ctx.acransac_homography_pairs([c], [wh], st, maxIteration, precision)[0])
-            st = res[-1]["mt_state_out"]
-    else:
-        res = ctx.acransac_homography_pairs(corrs, whs, st, maxIteration, precision)
-    info = {p: {"valid": False, "strong_support": False, "H": np.zeros((3, 3)), "error_max": np.inf} for p in pairs}
-    out = {}
-    for p, r in zip(est, res):
-        info[p].update(valid=r["valid"], H=r["H"], error_max=r["error_max"], mt_state_out=r["mt_state_out"])
-        if not r["valid"]:
-            continue
-        inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
-        info[p]["strong_support"] = hasStrongSupport(inl, 4)          # Homography4PSolver::getMinimumNbRequiredSamples
-        if info[p]["strong_support"]:
-            out[p] = inl
-    if guidedMatching and out:
-        def run(vp, items):
-            Hs = [info[p]["H"] for p, _ in items]
-            th = [info[p]["error_max"] * info[p]["error_max"] for p, _ in items]
-            if distanceRatio < 0:
-                return ctx.guided_match_positions_pairs(vp, Hs, th, MODEL_HOMOGRAPHY, decorate=True)
-            return ctx.guided_match_pairs(vp, Hs, th, distanceRatio * distanceRatio, MODEL_HOMOGRAPHY)
-        _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry, run)
-    return out, info
+    common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
+
+    def guided(vp, items, Hs, th, ratio):
+        if distanceRatio < 0:
+            return ctx.guided_match_positions_pairs(vp, Hs, th, MODEL_HOMOGRAPHY, decorate=True)
+        return ctx.guided_match_pairs(vp, Hs, th, ratio, MODEL_HOMOGRAPHY)
+    calls = [(lambda ks, st: ctx.acransac_homography_pairs([corrs[k] for k in ks], [whs[k] for k in ks], st, maxIteration, precision), True)]
+    return _acransac_stage(ctx, putatives, regions_per_view, guided_geometry, common, est, [0] * len(est), calls, "H", 4, seed_or_state,
+                           chain, guidedMatching, distanceRatio, guided)
 
 
 def geometricEstimation_E_AC(xI, xJ, sizeI, sizeJ, KI, KJ, seed_or_state, maxIteration: int = 50000, precision: float = np.inf,
@@ -657,10 +653,8 @@ def geometricEstimation_E_AC(xI, xJ, sizeI, sizeJ, KI, KJ, seed_or_state, maxIte
     the two pinhole matrices K (3 x 3); `precision` is what the filter passes to ACRANSAC, Square(m_dPrecision).  Returns the dict of
     Context.acransac_essential_pairs ("E", "mt_state_out")."""
     ctx = ctx or default_context()
-    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else seed_or_state
-    corr = np.concatenate([np.asarray(xI, np.float64).reshape(-1, 2), np.asarray(xJ, np.float64).reshape(-1, 2)], axis=1)
     K = np.concatenate([np.asarray(KI, np.float64).reshape(9), np.asarray(KJ, np.float64).reshape(9)])
-    return ctx.acransac_essential_pairs([corr], [tuple(sizeI) + tuple(sizeJ)], [K], st, maxIteration, precision)[0]
+    return ctx.acransac_essential_pairs(*_one_pair(xI, xJ, sizeI, sizeJ), [K], _start_state(seed_or_state), maxIteration, precision)[0]
 
 
 def _inverse3(M) -> np.ndarray:
@@ -704,39 +698,18 @@ def robustModelEstimation_E_AC(putatives: dict, regions_per_view: dict, image_si
     Returns (geometric matches {(I, J): {type: matches}} of the pairs with strong support, per-pair estimation
     {(I, J): {"valid", "strong_support", "E", "error_max"}, plus "mt_state_out" for the estimated pairs})."""
     ctx = ctx or default_context()
-    st = mt19937_state(int(seed_or_state)) if np.ndim(seed_or_state) == 0 else np.ascontiguousarray(seed_or_state, np.uint32)
-    pairs, common, est_all, corrs_all, whs_all = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
-    Ks = lambda p: [intrinsics.get(v) for v in p]  # noqa: E731
-    keep = [k for k, p in enumerate(est_all) if all(K is not None for K in Ks(p))]
-    est = [est_all[k] for k in keep]
-    corrs, whs = [corrs_all[k] for k in keep], [whs_all[k] for k in keep]
-    Kp = [np.concatenate([np.asarray(K, np.float64).reshape(9) for K in Ks(p)]) for p in est]
+    common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
+    Ks = {p: [intrinsics.get(v) for v in p] for p in est}
+    keep = [k for k, p in enumerate(est) if all(K is not None for K in Ks[p])]
+    est, corrs, whs = [est[k] for k in keep], [corrs[k] for k in keep], [whs[k] for k in keep]
+    Kp = [np.concatenate([np.asarray(K, np.float64).reshape(9) for K in Ks[p]]) for p in est]
     upper = precision * precision   # upperBoundPrecision = Square(m_dPrecision)
-    if not est:
-        res = []
-    elif chain:
-        res = []
-        for c, wh, K in zip(corrs, whs, Kp):
-            res.append(ctx.acransac_essential_pairs([c], [wh], [K], st, maxIteration, upper)[0])
-            st = res[-1]["mt_state_out"]
-    else:
-        res = ctx.acransac_essential_pairs(corrs, whs, Kp, st, maxIteration, upper)
-    info = {p: {"valid": False, "strong_support": False, "E": np.zeros((3, 3)), "error_max": np.inf} for p in pairs}
-    out = {}
-    for p, r in zip(est, res):
-        info[p].update(valid=r["valid"], E=r["E"], error_max=r["error_max"], mt_state_out=r["mt_state_out"])
-        if not r["valid"]:
-            continue
-        inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
-        info[p]["strong_support"] = hasStrongSupport(inl, 5)          # Essential5PSolver::getMinimumNbRequiredSamples
-        if info[p]["strong_support"]:
-            out[p] = inl
-    if guidedMatching and out:
-        _guided_stage(ctx, out, info, common, regions_per_view, guided_geometry,
-                      lambda vp, items: ctx.guided_match_pairs(vp, [fundamentalFromEssential(info[p]["E"], *Ks(p)) for p, _ in items],
-                                                               [info[p]["error_max"] * info[p]["error_max"] for p, _ in items],
-                                                               distanceRatio * distanceRatio))
-    return out, info
+    calls = [(lambda ks, st: ctx.acransac_essential_pairs([corrs[k] for k in ks], [whs[k] for k in ks], [Kp[k] for k in ks], st, maxIteration,
+                                                          upper), True)]
+    return _acransac_stage(ctx, putatives, regions_per_view, guided_geometry, common, est, [0] * len(est), calls, "E", 5, seed_or_state,
+                           chain, guidedMatching, distanceRatio,
+                           lambda vp, items, Es, th, ratio: ctx.guided_match_pairs(
+                               vp, [fundamentalFromEssential(E, *Ks[p]) for (p, _), E in zip(items, Es)], th, ratio))
 
 
 def removePoorlyOverlappingImagePairs(geometric: dict, putatives: dict, minimumRatio: float = 0.3, minimumGeometricCount: int = 50) -> dict:
