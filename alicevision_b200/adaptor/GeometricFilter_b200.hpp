@@ -9,6 +9,8 @@
 // b200m_guided_match_positions_pairs).
 // GeometricFilterMatrix_E_AC_Batch_b200 does the same for the `essential_matrix` filter (GeometricFilterMatrix_E_AC.hpp, pinhole pairs):
 // one b200m_acransac_essential_pairs call, then guided matching with F = K_J^-T E K_I^-1.
+// GeometricFilterMatrix_F_AC_Batch_b200 with estimateDistortion is the `fundamental_with_distortion` filter: its planar pairs go
+// through one b200m_acransac_fundamental_distortion_pairs call (Fundamental10PSolver, hasStrongSupport(.., 10)).
 // GeometricFilterMatrix_HGrowing_Batch_b200 does the same for the `homography_growing` filter (GeometricFilterMatrix_HGrowing.hpp:176-266,
 // filterMatchesByHGrowing): one b200m_hgrowing_pairs call for every (pair, common describer type) of the list.
 // Header-only; compiled inside an AliceVision build and linked against libb200match.so.  The caller gathers xI / xJ with the
@@ -174,18 +176,20 @@ protected:
         std::size_t offset;
     };
 
-    /// What one K10 call returned for its pairs (indices in addPair order, ascending), entry q for pairs[q].
+    /// What one K10 call returned for its pairs (indices in addPair order, ascending), entry q for pairs[q], and the minimum sample
+    /// count of its solver (getMinimumNbRequiredSamples, the pairs' hasStrongSupport threshold).
     struct K10Out
     {
         std::vector<int> pairs;
+        std::size_t minimumSamples;
         std::vector<int64_t> offsets;
         std::vector<uint8_t> valid;
         std::vector<int32_t> nInl, iters;
         std::vector<uint32_t> inl;
-        std::vector<double> M, errMax, nfa;
+        std::vector<double> M, L, errMax, nfa;
         /// nCorr: the size, in correspondences, of the buffer the pairs' offsets index
-        K10Out(const std::vector<PairIn>& added, std::vector<int> ks, std::size_t nCorr)
-          : pairs(std::move(ks))
+        K10Out(const std::vector<PairIn>& added, std::vector<int> ks, std::size_t nCorr, std::size_t minSamples)
+          : pairs(std::move(ks)), minimumSamples(minSamples)
         {
             const int n = (int)pairs.size();
             for (const int k : pairs)
@@ -196,6 +200,7 @@ protected:
             iters.resize(std::max(n, 1));
             inl.resize(std::max<std::size_t>(nCorr, 1));
             M.resize(9 * std::max(n, 1));
+            L.resize(2 * std::max(n, 1));
             errMax.resize(std::max(n, 1));
             nfa.resize(std::max(n, 1));
         }
@@ -217,12 +222,12 @@ protected:
 
     /// What every stage does after its engine call(s), each call's entries given with their pairs: fills estimates (the model into
     /// the field `model`; errorMax and support only for a pair ACRANSAC found valid), keeps the pairs whose copied inliers pass
-    /// hasStrongSupport(.., minimumSamples), minimumSamples the solver's getMinimumNbRequiredSamples, and with guidedMatching
+    /// hasStrongSupport(.., minimumSamples), minimumSamples the minimum sample count of the pair's call, and with guidedMatching
     /// replaces their lists by the guided ones (see guided) over pair k's model, or over modelOf(k) when the guided step needs
     /// another matrix.  Then moves the kept lists into out.
     template<class Estimate, class Call, class ModelOf = std::nullptr_t>
     bool finish(std::initializer_list<const K10Out*> calls, std::vector<Estimate>& estimates, double (Estimate::*model)[9],
-                std::size_t minimumSamples, bool guidedMatching, double distanceRatio, Call call, matching::PairwiseMatches& out,
+                bool guidedMatching, double distanceRatio, Call call, matching::PairwiseMatches& out,
                 ModelOf modelOf = nullptr) const
     {
         estimates.assign(_pairs.size(), Estimate());
@@ -241,7 +246,7 @@ protected:
                 const std::vector<std::size_t> inliers(r->inl.begin() + r->offsets[q], r->inl.begin() + r->offsets[q] + r->nInl[q]);
                 matching::MatchesPerDescType perType;
                 b200detail::copyInlierMatches(inliers, _pairs[k].putatives, _pairs[k].descTypes, perType);
-                e.strongSupport = b200detail::hasStrongSupport(perType, minimumSamples);
+                e.strongSupport = b200detail::hasStrongSupport(perType, r->minimumSamples);
                 if (e.strongSupport)
                 {
                     result[_pairs[k].pair] = std::move(perType);
@@ -325,17 +330,24 @@ protected:
 class GeometricFilterMatrix_F_AC_Batch_b200 : public GeometricFilterBatchBase_b200
 {
 public:
-    /// What the estimation of one pair gave (in addPair order): ACRANSAC's validity, F (row-major, x_J^T F x_I = 0), errorMax
-    /// (m_dPrecision_robust; infinite when not valid) and the support decision.
+    /// What the estimation of one pair gave (in addPair order): ACRANSAC's validity, F (row-major, x_J^T F x_I = 0; with
+    /// estimateDistortion a planar pair's F is Fundamental10PModel::getMatrix(), read the same way by the error and guided matching
+    /// while its solver's constraint is [x_I, y_I, 1 + l1 r_I^2] F [x_J, y_J, 1 + l2 r_J^2]^T = 0), L (that model's
+    /// getRadialDistortion(), in preconditioned units; 0 otherwise), errorMax (m_dPrecision_robust; infinite when not valid) and
+    /// the support decision.
     struct Estimate
     {
         bool valid = false, strongSupport = false;
         double F[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        double L[2] = {0, 0};
         double errorMax = std::numeric_limits<double>::infinity();
     };
 
-    explicit GeometricFilterMatrix_F_AC_Batch_b200(b200m_ctx* ctx = matching::b200detail::sharedContext())
-      : GeometricFilterBatchBase_b200(ctx)
+    /// estimateDistortion: GeometricFilterMatrix_F_AC's m_estimateDistortion (the `fundamental_with_distortion` filter): the planar
+    /// pairs are estimated by geometricEstimation_Mat_ACRANSAC<Fundamental10PSolver, Fundamental10PModel>.
+    explicit GeometricFilterMatrix_F_AC_Batch_b200(b200m_ctx* ctx = matching::b200detail::sharedContext(), bool estimateDistortion = false)
+      : GeometricFilterBatchBase_b200(ctx),
+        _estimateDistortion(estimateDistortion)
     {}
 
     /// addPair for a pair whose two cameras are camera::Equidistant (geometricEstimation_Spherical_Mat): bI / bJ are 3 x n, column c
@@ -364,8 +376,9 @@ public:
 
     /// robustModelEstimation over every pair added so far: each pair starts from `rng`.  geometricEstimation_Mat_ACRANSAC takes the
     /// generator by value; geometricEstimation_Spherical_Mat takes it by reference, so a single-threaded reference run hands it on
-    /// from a spherical pair to the next pair, which no batch reproduces.  The planar pairs go through one K10 call, the spherical
-    /// ones through another.  Pairs with strong support enter out; with guidedMatching their lists are the guided ones (errorTh =
+    /// from a spherical pair to the next pair, which no batch reproduces.  The planar pairs go through one K10 call (the 10-point
+    /// call with estimateDistortion), the spherical ones through another.  Pairs with strong support (hasStrongSupport(.., 10) for
+    /// the 10-point call, (.., 7) for the 7-point ones) enter out; with guidedMatching their lists are the guided ones (errorTh =
     /// errorMax^2, distRatio = distanceRatio^2, every common type, empty lists included; nothing when errorMax is infinite; a
     /// spherical F is applied to the guided positions, as the reference does).  Returns false (out untouched) when the engine is
     /// unavailable or fails.
@@ -384,21 +397,32 @@ public:
         std::vector<int32_t> wh;
         for (const int k : sub[0])
             wh.insert(wh.end(), _wh.begin() + 4 * k, _wh.begin() + 4 * k + 4);
-        K10Out r0(_pairs, sub[0], _corr.size() / 4), r1(_pairs, sub[1], _bear.size() / 6);
+        // minimum sample counts: Fundamental10PSolver 10, Fundamental7PSolver and Fundamental7PSphericalSolver 7
+        K10Out r0(_pairs, sub[0], _corr.size() / 4, _estimateDistortion ? 10 : 7), r1(_pairs, sub[1], _bear.size() / 6, 7);
         const int n0 = (int)sub[0].size(), n1 = (int)sub[1].size();
-        if (n0 > 0 && b200m_acransac_fundamental_pairs(_ctx, n0, r0.offsets.data(), corrData(), wh.data(), state, (int64_t)maxIteration,
-                                                       precision, r0.valid.data(), r0.nInl.data(), r0.inl.data(), r0.M.data(),
-                                                       r0.errMax.data(), r0.nfa.data(), r0.iters.data()) != B200M_OK)
+        if (n0 > 0 && !_estimateDistortion &&
+            b200m_acransac_fundamental_pairs(_ctx, n0, r0.offsets.data(), corrData(), wh.data(), state, (int64_t)maxIteration,
+                                             precision, r0.valid.data(), r0.nInl.data(), r0.inl.data(), r0.M.data(),
+                                             r0.errMax.data(), r0.nfa.data(), r0.iters.data()) != B200M_OK)
+            return false;
+        if (n0 > 0 && _estimateDistortion &&
+            b200m_acransac_fundamental_distortion_pairs(_ctx, n0, r0.offsets.data(), corrData(), wh.data(), state, (int64_t)maxIteration,
+                                                        precision, r0.valid.data(), r0.nInl.data(), r0.inl.data(), r0.M.data(),
+                                                        r0.L.data(), r0.errMax.data(), r0.nfa.data(), r0.iters.data()) != B200M_OK)
             return false;
         if (n1 > 0 && b200m_acransac_fundamental_spherical_pairs(_ctx, n1, r1.offsets.data(), _bear.data(), state, 0, (int64_t)maxIteration,
                                                                  precision, r1.valid.data(), r1.nInl.data(), r1.inl.data(), r1.M.data(),
                                                                  r1.errMax.data(), r1.nfa.data(), r1.iters.data(), nullptr) != B200M_OK)
             return false;
-        return finish({&r0, &r1}, _estimates, &Estimate::F, 7, guidedMatching, distanceRatio,   // 7: both 7-point solvers
-                      [&](const uint32_t* ids, int np, const double* M, const double* th, double distRatio, b200m_result** res) {
-                          return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distRatio, res);
-                      },
-                      out);
+        const bool ok = finish({&r0, &r1}, _estimates, &Estimate::F, guidedMatching, distanceRatio,
+                               [&](const uint32_t* ids, int np, const double* M, const double* th, double distRatio, b200m_result** res) {
+                                   return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distRatio, res);
+                               },
+                               out);
+        if (_estimateDistortion)
+            for (int q = 0; q < n0; ++q)
+                std::copy(r0.L.begin() + 2 * q, r0.L.begin() + 2 * q + 2, _estimates[sub[0][q]].L);
+        return ok;
     }
 
     /// The estimation of the k-th pair added, after run().
@@ -406,6 +430,7 @@ public:
 
 private:
     std::vector<Estimate> _estimates;
+    bool _estimateDistortion;
     std::vector<char> _spherical;   // per pair added: 1 = addPairSpherical (its offset indexes _bear)
     std::vector<double> _bear;      // 6 doubles per correspondence (xI, yI, zI, xJ, yJ, zJ)
 };
@@ -444,12 +469,12 @@ public:
         const int n = (int)_pairs.size();
         uint32_t state[625];
         b200detail::mtState(rng, state);
-        K10Out r(_pairs, allPairs(), _corr.size() / 4);
+        K10Out r(_pairs, allPairs(), _corr.size() / 4, 4);   // 4: Homography4PSolver
         if (n > 0 && b200m_acransac_homography_pairs(_ctx, n, r.offsets.data(), corrData(), _wh.data(), state, 0, (int64_t)maxIteration, precision,
                                                      r.valid.data(), r.nInl.data(), r.inl.data(), r.M.data(), r.errMax.data(), r.nfa.data(),
                                                      r.iters.data(), nullptr) != B200M_OK)
             return false;
-        return finish({&r}, _estimates, &Estimate::H, 4, guidedMatching, distanceRatio,   // 4: Homography4PSolver
+        return finish({&r}, _estimates, &Estimate::H, guidedMatching, distanceRatio,
                       [&](const uint32_t* ids, int np, const double* M, const double* th, double distRatio, b200m_result** res) {
                           if (distanceRatio < 0)
                               return b200m_guided_match_positions_pairs(_ctx, ids, np, B200M_MODEL_HOMOGRAPHY, M, th, 1, res);
@@ -516,13 +541,13 @@ public:
         const int n = (int)_pairs.size();
         uint32_t state[625];
         b200detail::mtState(rng, state);
-        K10Out r(_pairs, allPairs(), _corr.size() / 4);
+        K10Out r(_pairs, allPairs(), _corr.size() / 4, 5);   // 5: Essential5PSolver
         if (n > 0 && b200m_acransac_essential_pairs(_ctx, n, r.offsets.data(), corrData(), _wh.data(), _K.data(), state, 0, (int64_t)maxIteration,
                                                     precision * precision, r.valid.data(), r.nInl.data(), r.inl.data(), r.M.data(),
                                                     r.errMax.data(), r.nfa.data(), r.iters.data(), nullptr) != B200M_OK)
             return false;
         std::vector<double> F(9 * n);   // the guided step's F of each kept pair
-        return finish({&r}, _estimates, &Estimate::E, 5, guidedMatching, distanceRatio,   // 5: Essential5PSolver
+        return finish({&r}, _estimates, &Estimate::E, guidedMatching, distanceRatio,
                       [&](const uint32_t* ids, int np, const double* M, const double* th, double distRatio, b200m_result** res) {
                           return b200m_guided_match_pairs(_ctx, ids, np, B200M_MODEL_FUNDAMENTAL, M, th, distRatio, res);
                       },

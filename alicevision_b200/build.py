@@ -11,7 +11,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB = os.path.join(_HERE, "libb200match.so")
-SOURCES = ["engine.cu", "voctree.cu", "io.cpp"]
+SOURCES = ["engine.cu", "acransac_f10.cu", "voctree.cu", "io.cpp"]
 def _deps():
     """Every file the library is built from: all of csrc/ and the public headers (a forgotten header here once shipped a stale .so)."""
     import glob

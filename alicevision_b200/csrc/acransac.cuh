@@ -1,12 +1,13 @@
 // K10: a-contrario RANSAC estimation for a list of pairs, sm_90a: the fundamental matrix (b200m_acransac_fundamental_pairs,
 // FPolicy), the homography (b200m_acransac_homography_pairs, HPolicy) and the fundamental matrix of two equidistant cameras on
 // lifted unit vectors (b200m_acransac_fundamental_spherical_pairs, SPolicy) and the essential matrix of two pinhole cameras
-// (b200m_acransac_essential_pairs, EPolicy).  The kernel is one template over the model policy.
+// (b200m_acransac_essential_pairs, EPolicy) and the fundamental matrix with two radial distortion coefficients
+// (b200m_acransac_fundamental_distortion_pairs, F10Policy).  The kernel is one template over the model policy.
 //
 // One CTA runs one pair's robustEstimation::ACRANSAC loop (robustEstimation/ACRansac.hpp:186-272) iteration by iteration, with the
 // reference's control flow (10 % reserve, strict `<` on minNFA, the switch to sampling among the inliers, the "no model at all"
 // extension, the precision mode and its early exit).  Per iteration thread 0 draws the sample from the pair's own copy of the
-// caller's std::mt19937 (shared memory) and fits the models (7-point F, 4-point H or 5-point E, acransac_math.h); then the whole CTA scores
+// caller's std::mt19937 (shared memory) and fits the models (7-point F, 4-point H, 5-point E or 10-point F10, acransac_math.h); then the whole CTA scores
 // each model:
 //   * n residuals (F: point-to-line error, H: point-to-point transfer error, on normalised points; S: (F x_I . x_J)^2 on bearings);
 //   * certified skip: a shared-memory histogram of the residuals over quarter-binade bins gives, for every k, a lower bound of the
@@ -39,6 +40,7 @@ struct Out {
   long long evaluated, skipped, exact;
   int valid, n_inl, iterations, n_trace;
 };
+struct OutL { Out o; double L[2]; };   // F10Policy's result: the winner's radial distortion (l1, l2) beside it
 
 __device__ __forceinline__ int bin_of(double r) {
   const unsigned long long b = (unsigned long long)__double_as_longlong(r);
@@ -56,10 +58,11 @@ __device__ __forceinline__ double bin_low(int b) {
 // Model policies: sample size, maximum number of models, fit, residual, logalpha0, errorVectorDimension, unnormaliser, and the
 // correspondence layout: kPlanar = pixel pairs (xI, yI, xJ, yJ) preconditioned by the image sizes; kCalibrated = pixel pairs
 // followed by their K^-1-normalised copies (xI, yI, xJ, yJ, uI, vI, uJ, vJ), fitted on the copies, scored on the pixels; else
-// lifted unit vectors (xI, yI, zI, xJ, yJ, zJ) used as given; kWidth doubles per correspondence.
+// lifted unit vectors (xI, yI, zI, xJ, yJ, zJ) used as given; kWidth doubles per correspondence.  kDistortion: the model carries
+// (l1, l2) beside its matrix, the fit runs in a per-CTA shared-memory workspace and the result is an OutL.
 struct FPolicy {   // RelativePoseKernel<Fundamental7PSolver, FundamentalEpipolarDistanceError, UnnormalizerT>
   static constexpr int kSample = acr::kSample, kMaxModels = acr::kMaxModels, kErrDim = 1, kWidth = 4;
-  static constexpr bool kPlanar = true, kCalibrated = false;
+  static constexpr bool kPlanar = true, kCalibrated = false, kDistortion = false;
   __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) {
     return acr::fit7_solve<false>(a, b, c, d, m);   // = acr::fit7, one inlining level shallower
   }
@@ -71,7 +74,7 @@ struct FPolicy {   // RelativePoseKernel<Fundamental7PSolver, FundamentalEpipola
 };
 struct HPolicy {   // RelativePoseKernel<Homography4PSolver, HomographyAsymmetricError, UnnormalizerI>, point to point
   static constexpr int kSample = acr::kSampleH, kMaxModels = acr::kMaxModelsH, kErrDim = 2, kWidth = 4;
-  static constexpr bool kPlanar = true, kCalibrated = false;
+  static constexpr bool kPlanar = true, kCalibrated = false, kDistortion = false;
   __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m) { return acr::fit4(a, b, c, d, m); }
   __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::homography_error(m, x1, y1, x2, y2); }
   __device__ static double logalpha0(int w2, int h2, const acr::Norm& n2) { return acr::logalpha0_h(w2, h2, n2); }
@@ -79,7 +82,7 @@ struct HPolicy {   // RelativePoseKernel<Homography4PSolver, HomographyAsymmetri
 };
 struct SPolicy {   // RelativePoseSphericalKernel<Fundamental7PSphericalSolver, EpipolarSphericalDistanceError>
   static constexpr int kSample = acr::kSample, kMaxModels = acr::kMaxModels, kErrDim = 2, kWidth = 6;
-  static constexpr bool kPlanar = false, kCalibrated = false;
+  static constexpr bool kPlanar = false, kCalibrated = false, kDistortion = false;
   __device__ static int fit(const double* x1, const double* x2, double* m) { return acr::fit7s(x1, x2, m); }
   __device__ static double error(const double* m, const double* x1, const double* x2) { return acr::spherical_error(m, x1, x2); }
   __device__ static double logalpha0(int, int, const acr::Norm&) { return M_PI; }   // the value itself, not its log10
@@ -89,7 +92,7 @@ struct EPolicy {   // RelativePoseKernel_K<Essential5PSolver, FundamentalEpipola
   // models[] holds F = K_J^-T E K_I^-1 of each model for the residuals, then the Es.  errorVectorDimension is 0.5, which the int
   // kErrDim of the other policies cannot hold: nfa_of applies it under `if constexpr (P::kCalibrated)`, and kErrDim = 0 is unused.
   static constexpr int kSample = acr::kSampleE, kMaxModels = acr::kMaxModelsE, kErrDim = 0, kWidth = 8;
-  static constexpr bool kPlanar = false, kCalibrated = true;
+  static constexpr bool kPlanar = false, kCalibrated = true, kDistortion = false;
   __device__ static int fit(const double* a, const double* b, const double* c, const double* d, const double* kinv, double* m) {
     double* E = m + 9 * kMaxModels;
     const int nb = acr::fit5(a, b, c, d, E);
@@ -99,6 +102,18 @@ struct EPolicy {   // RelativePoseKernel_K<Essential5PSolver, FundamentalEpipola
   __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::epipolar_error(m, x1, y1, x2, y2); }
   __device__ static double logalpha0(int w2, int h2, const acr::Norm&) { return acr::logalpha0_e(w2, h2); }
   __device__ static void unnormalize(const acr::Norm&, const acr::Norm&, double*) {}
+};
+struct F10Policy {   // RelativePoseKernel<Fundamental10PSolver, FundamentalEpipolarDistanceError, UnnormalizerT, Fundamental10PModel>
+  // FPolicy's preconditioning, error, logalpha0 and unnormaliser (on the matrix only); models[] holds the 10 matrices, then their
+  // (l1, l2).  The error scores the matrix alone, transposed against the solver's constraint, as the reference does.
+  static constexpr int kSample = acr::kSampleF10, kMaxModels = acr::kMaxModelsF10, kErrDim = 1, kWidth = 4;
+  static constexpr bool kPlanar = true, kCalibrated = false, kDistortion = true;
+  __device__ static int fit(const double* a, const double* b, const double* c, const double* d, double* m, acr::F10Work& w) {
+    return acr::fit10(a, b, c, d, m, m + 9 * kMaxModels, w);
+  }
+  __device__ static double error(const double* m, double x1, double y1, double x2, double y2) { return acr::epipolar_error(m, x1, y1, x2, y2); }
+  __device__ static double logalpha0(int w2, int h2, const acr::Norm& n2) { return FPolicy::logalpha0(w2, h2, n2); }
+  __device__ static void unnormalize(const acr::Norm& n1, const acr::Norm& n2, double* m) { acr::unnormalize(n1, n2, m); }
 };
 
 // NFA(k) of bestNFA for the squared residual e of rank k: loge0 + (la0 + d log10(sqrt(e) + FLT_EPSILON)) (k - kSample) + logc_n[k]
@@ -175,7 +190,7 @@ __device__ __forceinline__ double residual(const double* M, const double* pts, i
 // Scratch at the pair's offset: pts (P::kWidth doubles), idx (the sampling list), logc (n + 1 floats each of logc_n and logc_k, at
 // 2 * (off + pair)), gkeys / gvals (pow2(n) at sort_off, pairs above kSmemSort only).  inliers: the result list at the offset.
 // mt_state: 625 words at p * mt_stride (mt_stride 0: one state for every pair); mt_out: NULL, or 625 words per pair receiving the
-// generator state after the pair's last draw.
+// generator state after the pair's last draw.  out_all: Out per pair, OutL for kDistortion.
 template <class P>
 __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __restrict__ pairs, const double* __restrict__ corr,
                                                              const float* __restrict__ l10, const uint32_t* __restrict__ mt_state,
@@ -184,7 +199,8 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
                                                              uint32_t* gvals, uint32_t* inliers_all, int* trace_all, double* trace_nfa_all,
                                                              Out* out_all, uint32_t* mt_out) {
   __shared__ acr::Mt19937 g;
-  __shared__ double models[9 * P::kMaxModels * (P::kCalibrated ? 2 : 1)], bestF[9];
+  __shared__ double models[9 * P::kMaxModels * (P::kCalibrated ? 2 : 1) + (P::kDistortion ? 2 * P::kMaxModels : 0)];
+  __shared__ double bestF[9 + (P::kDistortion ? 2 : 0)];   // F10: the winner's (l1, l2) at 9, 10
   __shared__ int hist[kBins];
   __shared__ unsigned long long skeys[kSmemSort];
   __shared__ uint32_t svals[kSmemSort];
@@ -197,7 +213,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
   const int p = blockIdx.x, tid = threadIdx.x;
   const Pair Q = P::kCalibrated ? reinterpret_cast<const PairE*>(pairs)[p].q : pairs[p];
   const int n = Q.n;
-  Out* out = out_all + p;
+  Out* out = P::kDistortion ? &reinterpret_cast<OutL*>(out_all)[p].o : out_all + p;
   const double inf = __longlong_as_double(0x7ff0000000000000ll);
   const uint32_t* st_in = mt_state + (long long)p * mt_stride;
   if (n <= P::kSample) {   // ACRANSAC returns (0, 0) at once, without a draw
@@ -205,6 +221,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
       for (int t = 0; t < 9; ++t) out->model[t] = 0;
       out->error_max = 0; out->min_nfa = 0; out->evaluated = out->skipped = out->exact = 0;
       out->valid = 0; out->n_inl = 0; out->iterations = 0; out->n_trace = 0;
+      if constexpr (P::kDistortion) reinterpret_cast<OutL*>(out)->L[0] = reinterpret_cast<OutL*>(out)->L[1] = 0;
     }
     if (mt_out)
       for (int i = tid; i <= acr::kMtN; i += kThreads) mt_out[(long long)p * (acr::kMtN + 1) + i] = st_in[i];
@@ -264,7 +281,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
     nReserve = max_iter / 10; nIter = max_iter - nReserve; iter = 0;
     evaluated = skipped = exact = 0;
     mode = precision == inf; minNFA = inf; errorMax = inf; n_inl = 0; n_idx = n; stop = 0; n_trace = 0;
-    for (int t = 0; t < 9; ++t) bestF[t] = 0;
+    for (int t = 0; t < 9 + (P::kDistortion ? 2 : 0); ++t) bestF[t] = 0;
   }
   __syncthreads();
 
@@ -281,7 +298,12 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
             const uint32_t j = mode ? idx[s[i]] : s[i];
             a[i] = pts[4 * j]; b[i] = pts[4 * j + 1]; cc[i] = pts[4 * j + 2]; d[i] = pts[4 * j + 3];
           }
-          nb = P::fit(a, b, cc, d, models);
+          if constexpr (P::kDistortion) {   // the 10-point solver's working arrays: thread 0's, in shared memory
+            __shared__ acr::F10Work work;
+            nb = P::fit(a, b, cc, d, models, work);
+          } else {
+            nb = P::fit(a, b, cc, d, models);
+          }
         } else if constexpr (P::kCalibrated) {
           double a[P::kSample], b[P::kSample], cc[P::kSample], d[P::kSample];
           for (int i = 0; i < P::kSample; ++i) {
@@ -368,6 +390,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
           errorMax = __longlong_as_double((long long)K[bk - 1]);
           const double* Mo = P::kCalibrated ? models + 9 * (P::kMaxModels + m) : F;   // E: the fitted model, not its F
           for (int t = 0; t < 9; ++t) bestF[t] = Mo[t];
+          if constexpr (P::kDistortion) { bestF[9] = models[9 * P::kMaxModels + 2 * m]; bestF[10] = models[9 * P::kMaxModels + 2 * m + 1]; }
           if (n_trace < kTraceCap) {
             trace_all[(long long)p * kTraceCap + n_trace] = (int)iter;
             trace_nfa_all[(long long)p * kTraceCap + n_trace] = bv;
@@ -409,6 +432,7 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
     out->error_max = em; out->min_nfa = minNFA;
     out->evaluated = evaluated; out->skipped = skipped; out->exact = exact;
     out->valid = valid; out->n_inl = valid ? n_inl : 0; out->iterations = (int)iter; out->n_trace = n_trace;
+    if constexpr (P::kDistortion) { reinterpret_cast<OutL*>(out)->L[0] = bestF[9]; reinterpret_cast<OutL*>(out)->L[1] = bestF[10]; }
   }
   if (mt_out) {   // thread 0's last draw is ordered before the loop's final __syncthreads
     uint32_t* so = mt_out + (long long)p * (acr::kMtN + 1);
@@ -416,5 +440,22 @@ __global__ void __launch_bounds__(kThreads, 4) acransac_kernel(const Pair* __res
     if (tid == 0) so[acr::kMtN] = (uint32_t)g.p;
   }
 }
+
+// One launch of acransac_kernel<P> over n_pairs CTAs on `st`, the kernel's arguments in order.
+template <class P>
+void launch(int n_pairs, cudaStream_t st, const Pair* pairs, const double* corr, const float* l10, const uint32_t* mt_state, int mt_stride,
+            long long max_iter, double precision, int skip_on, double* pts_all, uint32_t* idx_all, float* logc_all,
+            unsigned long long* gkeys, uint32_t* gvals, uint32_t* inliers_all, int* trace_all, double* trace_nfa_all, Out* out_all,
+            uint32_t* mt_out) {
+  acransac_kernel<P><<<n_pairs, kThreads, 0, st>>>(pairs, corr, l10, mt_state, mt_stride, max_iter, precision, skip_on, pts_all, idx_all,
+                                                   logc_all, gkeys, gvals, inliers_all, trace_all, trace_nfa_all, out_all, mt_out);
+}
+// F10Policy's kernel is compiled in its own translation unit (acransac_f10.cu), so that engine.cu's module, the other policies'
+// kernels among it, compiles exactly as it did before this policy.
+template <>
+void launch<F10Policy>(int n_pairs, cudaStream_t st, const Pair* pairs, const double* corr, const float* l10, const uint32_t* mt_state,
+                       int mt_stride, long long max_iter, double precision, int skip_on, double* pts_all, uint32_t* idx_all, float* logc_all,
+                       unsigned long long* gkeys, uint32_t* gvals, uint32_t* inliers_all, int* trace_all, double* trace_nfa_all, Out* out_all,
+                       uint32_t* mt_out);
 
 }  // namespace acrk

@@ -798,6 +798,49 @@ ACR_HD bool real_schur(const double A[N][N], double T[N][N], double U[N][N]) {
   return true;
 }
 
+// std::complex<double> division as GCC compiles it (libgcc's __divdc3): Smith's algorithm on the larger of |c|, |d|, with its
+// rescaling of extreme operands and its recovery of a zero divisor; (a + b i) / (c + d i) -> (x, y).  The recovery of infinite
+// operands is not restated (every operand here is finite or NaN).
+ACR_HD void cdiv(double a, double b, double c, double d, double& x, double& y) {
+  constexpr double kRbig = 1.7976931348623157e308 / 2, kRmin = kMin, kRmin2 = kEps, kRminscal = 1.0 / kEps, kRmax2 = kRbig * kRmin2;
+  double ratio, denom;
+  if (fabs(c) < fabs(d)) {
+    if (fabs(d) >= kRbig) { a = a / 2; b = b / 2; c = c / 2; d = d / 2; }
+    if (fabs(d) < kRmin2 || (fabs(a) < kRmin && fabs(b) < kRmax2 && fabs(d) < kRmax2) ||
+        (fabs(b) < kRmin && fabs(a) < kRmax2 && fabs(d) < kRmax2)) {
+      a = mul(a, kRminscal); b = mul(b, kRminscal); c = mul(c, kRminscal); d = mul(d, kRminscal);
+    }
+    ratio = c / d;
+    denom = add(mul(c, ratio), d);
+    if (fabs(ratio) > kRmin) {
+      x = add(mul(a, ratio), b) / denom;
+      y = sub(mul(b, ratio), a) / denom;
+    } else {
+      x = add(mul(c, a / d), b) / denom;
+      y = sub(mul(c, b / d), a) / denom;
+    }
+  } else {
+    if (fabs(c) >= kRbig) { a = a / 2; b = b / 2; c = c / 2; d = d / 2; }
+    if (fabs(c) < kRmin2 || (fabs(a) < kRmin && fabs(b) < kRmax2 && fabs(c) < kRmax2) ||
+        (fabs(b) < kRmin && fabs(a) < kRmax2 && fabs(c) < kRmax2)) {
+      a = mul(a, kRminscal); b = mul(b, kRminscal); c = mul(c, kRminscal); d = mul(d, kRminscal);
+    }
+    ratio = d / c;
+    denom = add(mul(d, ratio), c);
+    if (fabs(ratio) > kRmin) {
+      x = add(mul(b, ratio), a) / denom;
+      y = sub(b, mul(a, ratio)) / denom;
+    } else {
+      x = add(a, mul(d, b / c)) / denom;
+      y = sub(b, mul(d, a / c)) / denom;
+    }
+  }
+  if (x != x && y != y && c == 0 && d == 0 && (a == a || b == b)) {   // NaN + NaN i from a zero divisor: signed infinities
+    const double inf = copysign((double)INFINITY, c);
+    x = mul(inf, a); y = mul(inf, b);
+  }
+}
+
 // EigenSolver<Mat10>(A): the real Schur form, its eigenvalues (a 2 x 2 block gives (T(i+1, i+1) + p) +- z i, z computed without
 // overflow), and the normalised eigenvectors of the real ones (imag() exactly 0), by doComputeEigenvectors' back-substitution
 // and back-transformation.  re[i], im[i]: the eigenvalues in Schur order; V[i][*]: the eigenvector of eigenvalue i when im[i] == 0.
@@ -876,6 +919,140 @@ ACR_HD bool eigen_solve(const double A[N][N], double re[N], double im[N], double
   }
   return true;
 }
+// EigenSolver<Mat10>(A) as the F10 solver reads it: eigen_solve's Schur form, eigenvalues and real back-substitution, with in
+// addition doComputeEigenvectors' complex branch (the pair (j, j + 1), im[j] > 0, leaves its vector's real part in m_eivec's column j
+// and its imaginary part in column j + 1), every column back-transformed, and eigenvectors()' assembly: column j is real when
+// |im[j]| <= |re[j]| 2 eps or j + 1 == N, else the pair is (col j) +- i (col j + 1); each column normalised (squared norm summed in
+// index order, divided by its square root when positive).  V[j][*] + i Vi[j][*] is eigenvectors().col(j).  A function of its own:
+// E's eigen_solve, which it restates in part, keeps the code it compiles to.
+ACR_HD bool eigen_solve_complex(const double A[N][N], double re[N], double im[N], double V[N][N], double Vi[N][N]) {
+  double T[N][N], U[N][N];
+  if (!real_schur(A, T, U)) return false;
+  for (int i = 0; i < N;) {
+    if (i == N - 1 || T[i + 1][i] == 0) {
+      re[i] = T[i][i]; im[i] = 0;
+      if (!(fabs(re[i]) <= 1.7976931348623157e308)) return false;   // not finite
+      ++i;
+    } else {
+      const double p = mul(0.5, sub(T[i][i], T[i + 1][i + 1]));
+      double t0 = T[i + 1][i], t1 = T[i][i + 1];
+      const double mx = fmax(fabs(p), fmax(fabs(t0), fabs(t1)));
+      t0 = t0 / mx; t1 = t1 / mx;
+      const double p0 = p / mx;
+      const double z = mul(mx, sqrt(fabs(add(mul(p0, p0), mul(t0, t1)))));
+      re[i] = re[i + 1] = add(T[i + 1][i + 1], p);
+      im[i] = z; im[i + 1] = -z;
+      i += 2;
+    }
+  }
+  double norm = 0;
+  for (int j = 0; j < N; ++j)
+    for (int c = (j > 0 ? j - 1 : 0); c < N; ++c) norm = add(norm, fabs(T[j][c]));
+  if (norm != 0) {
+    for (int n = N - 1; n >= 0; --n) {   // back-substitution
+      {
+        if (im[n] < 0 && n > 0) {   // the complex branch: columns n - 1 (real part) and n (imaginary part)
+          const double p = re[n], q = im[n];
+          double lastra = 0, lastsa = 0, lastw = 0;
+          int l = n - 1;
+          if (fabs(T[n][n - 1]) > fabs(T[n - 1][n])) {   // last vector component imaginary: the matrix is triangular
+            T[n - 1][n - 1] = q / T[n][n - 1];
+            T[n - 1][n] = -sub(T[n][n], p) / T[n][n - 1];
+          } else {
+            cdiv(0.0, -T[n - 1][n], sub(T[n - 1][n - 1], p), q, T[n - 1][n - 1], T[n - 1][n]);
+          }
+          T[n][n - 1] = 0;
+          T[n][n] = 1.0;
+          for (int i = n - 2; i >= 0; --i) {
+            double ra = 0, sa = 0;
+            for (int k = l; k <= n; ++k) { ra = add(ra, mul(T[i][k], T[k][n - 1])); sa = add(sa, mul(T[i][k], T[k][n])); }
+            const double w = sub(T[i][i], p);
+            if (im[i] < 0) {
+              lastw = w; lastra = ra; lastsa = sa;
+            } else {
+              l = i;
+              if (im[i] == 0) {
+                cdiv(-ra, -sa, w, q, T[i][n - 1], T[i][n]);
+              } else {   // solve the complex equations
+                const double x = T[i][i + 1], y = T[i + 1][i];
+                const double dr = sub(re[i], p);
+                double vr = sub(add(mul(dr, dr), mul(im[i], im[i])), mul(q, q));
+                const double vi = mul(mul(dr, 2.0), q);
+                if (vr == 0 && vi == 0)
+                  vr = mul(mul(kEps, norm), add(add(add(add(fabs(w), fabs(q)), fabs(x)), fabs(y)), fabs(lastw)));
+                cdiv(add(sub(mul(x, lastra), mul(lastw, ra)), mul(q, sa)), sub(sub(mul(x, lastsa), mul(lastw, sa)), mul(q, ra)), vr, vi,
+                     T[i][n - 1], T[i][n]);
+                if (fabs(x) > add(fabs(lastw), fabs(q))) {
+                  T[i + 1][n - 1] = add(sub(-ra, mul(w, T[i][n - 1])), mul(q, T[i][n])) / x;
+                  T[i + 1][n] = sub(sub(-sa, mul(w, T[i][n])), mul(q, T[i][n - 1])) / x;
+                } else {
+                  cdiv(sub(-lastra, mul(y, T[i][n - 1])), sub(-lastsa, mul(y, T[i][n])), lastw, q, T[i + 1][n - 1], T[i + 1][n]);
+                }
+              }
+              const double t = fmax(fabs(T[i][n - 1]), fabs(T[i][n]));   // overflow control
+              if (mul(mul(kEps, t), t) > 1)
+                for (int k = i; k < N; ++k) { T[k][n - 1] = T[k][n - 1] / t; T[k][n] = T[k][n] / t; }
+            }
+          }
+          --n;   // the pair is done
+          continue;
+        }
+      }
+      if (im[n] != 0) continue;
+      const double p = re[n];
+      double lastr = 0, lastw = 0;
+      int l = n;
+      T[n][n] = 1.0;
+      for (int i = n - 1; i >= 0; --i) {
+        const double w = sub(T[i][i], p);
+        double r = 0;
+        for (int k = l; k <= n; ++k) r = add(r, mul(T[i][k], T[k][n]));
+        if (im[i] < 0) {
+          lastw = w; lastr = r;
+        } else {
+          l = i;
+          if (im[i] == 0) {
+            T[i][n] = w != 0 ? -r / w : -r / mul(kEps, norm);
+          } else {   // a complex pair above: solve the real 2 x 2 equations
+            const double x = T[i][i + 1], y = T[i + 1][i];
+            const double dr = sub(re[i], p);
+            const double denom = add(mul(dr, dr), mul(im[i], im[i]));
+            const double t = sub(mul(x, lastr), mul(lastw, r)) / denom;
+            T[i][n] = t;
+            T[i + 1][n] = fabs(x) > fabs(lastw) ? sub(-r, mul(w, t)) / x : sub(-lastr, mul(y, t)) / lastw;
+          }
+          const double t = fabs(T[i][n]);   // overflow control
+          if (mul(mul(kEps, t), t) > 1)
+            for (int k = i; k < N; ++k) T[k][n] = T[k][n] / t;
+        }
+      }
+    }
+    for (int j = N - 1; j >= 0; --j) {   // back-transformation: column j <- U[:, 0..j] T[0..j, j]
+      double col[N];
+      for (int r = 0; r < N; ++r) {
+        double s = mul(U[r][0], T[0][j]);
+        for (int k = 1; k <= j; ++k) s = add(s, mul(U[r][k], T[k][j]));
+        col[r] = s;
+      }
+      for (int r = 0; r < N; ++r) U[r][j] = col[r];
+    }
+  }
+  {   // eigenvectors()
+    for (int j = 0; j < N; ++j) {
+      const bool real = fabs(im[j]) <= mul(fabs(re[j]), 2 * kEps) || j + 1 == N;
+      double s = 0;
+      for (int r = 0; r < N; ++r) s = real ? add(s, mul(U[r][j], U[r][j])) : add(s, add(mul(U[r][j], U[r][j]), mul(U[r][j + 1], U[r][j + 1])));
+      const double nr = sqrt(s);
+      for (int r = 0; r < N; ++r) {
+        V[j][r] = s > 0 ? U[r][j] / nr : U[r][j];
+        Vi[j][r] = real ? 0.0 : (s > 0 ? U[r][j + 1] / nr : U[r][j + 1]);
+        if (!real) { V[j + 1][r] = V[j][r]; Vi[j + 1][r] = -Vi[j][r]; }
+      }
+      if (!real) ++j;
+    }
+  }
+  return true;
+}
 // Steps 1-4 of Essential5PSolver::solve on the 5 epipolar rows A: the null-space basis Eb (column c = N[c] of nullspace<5>), the
 // constraint matrix, its full-pivot LU solve and the action matrix At
 ACR_HD void action_matrix(const double A[5][9], double Eb[9][4], double At[N][N]) {
@@ -918,6 +1095,228 @@ ACR_HD int fit5(const double* x1, const double* y1, const double* x2, const doub
       E[nb * 9 + t] = add(add(add(mul(Eb[t][0], v[0]), mul(Eb[t][1], v[1])), mul(Eb[t][2], v[2])), mul(Eb[t][3], v[3]));
     ++nb;
   }
+  return nb;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- F10 kernel
+// RelativePoseKernel<Fundamental10PSolver, FundamentalEpipolarDistanceError, UnnormalizerT, Fundamental10PModel>: F's image-size
+// preconditioning, point-to-line error (on model.getMatrix() alone: the distortion L plays no part in the score), logalpha0,
+// errorVectorDimension 1 and N2^T F N1 (L stays in preconditioned units); only the sample size, the model count and the fit
+// differ.  F10RelativePose's F satisfies [x_I, y_I, 1 + l1 r_I^2] F [x_J, y_J, 1 + l2 r_J^2]^T = 0: the error reads it as
+// x_J^T F x_I, the transpose, as the reference does.
+//
+// Eigen 3.4 rules restated for it (the E solver's RealSchur / EigenSolver code is shared):
+//   * PartialPivLU<Mat10>: unblocked at this size; per column the first largest |entry| at or below the diagonal is the pivot
+//     (strict >), the rows swap (the right-hand side with them, as P b), the column below divides by the pivot unless it is
+//     exactly 0 (not caught: inf / NaN flow on), and the rank-1 update follows.  The solve is the TRSM of triangular_solve_matrix
+//     with its 4-wide panels: inside a panel x_i = b_i * (1 / u_ii) (unit lower: b_i) and the panel's rows update sequentially;
+//     the rows past a panel take the panel's products summed in index order (the GEBP accumulator) in one subtraction.
+//   * colEchelonForm(M, 1e-16) as written: p starts at DBL_MIN, `tp > p` (the first column wins a tie, a NaN never), a row below
+//     the tolerance is zeroed, column swap, scaling (division), elimination of every other column.
+//   * EigenSolver: eigen_solve_complex (doComputeEigenvectors with its complex branch, the complex divisions as cdiv, and
+//     eigenvectors()' assembly and normalisation).
+//   * esols = row(2) / row(0) and row(1) / row(0) of eigenvectors(): the rows are strided, so Eigen takes the scalar path, std::complex
+//     division, i.e. cdiv; a solution is kept when both imaginary parts are at most 100 eps in magnitude.
+//   * the dot products of the model step in Eigen's unrolled redux order: b(4:10) . m2 and b(0:4) . m1 on SSE2 packets of 2,
+//     m3 . mr.row(k) (a strided row) as the scalar unroller's halving tree.
+// Divergences (rounding level): every other summation runs in index order where Eigen's packet code may pair terms differently,
+// and where the Schur iteration does not converge or an eigenvalue is not finite the fit returns no model (Eigen then leaves
+// eigenvectors() unspecified).
+constexpr int kSampleF10 = 10;      // Fundamental10PSolver::getMinimumNbRequiredSamples
+constexpr int kMaxModelsF10 = 10;   // Fundamental10PSolver::getMaximumNbModels
+
+// fit10's working arrays (5960 bytes): the device keeps them in a per-CTA shared-memory workspace, the host on its stack (the Schur
+// form and its vectors, 1.6 KB, stay eigen_solve_complex's locals)
+struct F10Work {
+  double A[10][16];   // the monomial matrix; after the solve its last 6 columns hold mr
+  double M[20][10];   // f10e_gb's M, then its column echelon form
+  double At[10][10];  // the action matrix
+  double V[10][10], Vi[10][10];   // eigenvectors(): V[j] + i Vi[j] is column j
+  double P[29], c[36];
+  double re[10], im[10];
+};
+
+// A(:, 0:10) x = A(:, 10:16) by PartialPivLU, in place: x lands in A(:, 10:16)
+ACR_HD void partial_lu_solve(double A[10][16]) {
+  constexpr int n = 10, kPanel = 4;
+  for (int k = 0; k < n; ++k) {
+    int br = k;
+    double big = fabs(A[k][k]);
+    for (int r = k + 1; r < n; ++r)
+      if (fabs(A[r][k]) > big) { big = fabs(A[r][k]); br = r; }
+    if (big != 0) {
+      if (br != k)
+        for (int c = 0; c < 16; ++c) { const double t = A[k][c]; A[k][c] = A[br][c]; A[br][c] = t; }
+      for (int r = k + 1; r < n; ++r) A[r][k] = A[r][k] / A[k][k];
+    }
+    for (int c = k + 1; c < n; ++c)
+      for (int r = k + 1; r < n; ++r) A[r][c] = sub(A[r][c], mul(A[r][k], A[k][c]));
+  }
+  for (int j = 10; j < 16; ++j) {
+    for (int k1 = 0; k1 < n; k1 += kPanel) {   // unit lower, panels from the top
+      const int w = k1 + kPanel < n ? kPanel : n - k1;
+      for (int i = k1; i < k1 + w; ++i)
+        for (int r = i + 1; r < k1 + w; ++r) A[r][j] = sub(A[r][j], mul(A[i][j], A[r][i]));
+      for (int r = k1 + w; r < n; ++r) {
+        double acc = 0;
+        for (int i = k1; i < k1 + w; ++i) acc = add(acc, mul(A[r][i], A[i][j]));
+        A[r][j] = sub(A[r][j], acc);
+      }
+    }
+    for (int k1 = 0; k1 < n; k1 += kPanel) {   // upper, panels from the bottom
+      const int w = k1 + kPanel < n ? kPanel : n - k1, top = n - k1 - w;
+      for (int i = n - k1 - 1; i >= top; --i) {
+        A[i][j] = mul(A[i][j], 1.0 / A[i][i]);
+        for (int r = top; r < i; ++r) A[r][j] = sub(A[r][j], mul(A[i][j], A[r][i]));
+      }
+      for (int r = 0; r < top; ++r) {
+        double acc = 0;
+        for (int i = top; i < top + w; ++i) acc = add(acc, mul(A[r][i], A[i][j]));
+        A[r][j] = sub(A[r][j], acc);
+      }
+    }
+  }
+}
+
+// colEchelonForm(M, pivtol) on the 20 x 10 M
+ACR_HD void col_echelon(double M[20][10], double pivtol) {
+  constexpr int n = 20, m = 10;
+  int i = 0, j = 0;
+  while (i < m && j < n) {
+    double p = e5::kMin;
+    int col = i;
+    for (int k = i; k < m; ++k) {
+      const double tp = fabs(M[j][k]);
+      if (tp > p) { p = tp; col = k; }
+    }
+    if (p < pivtol) {
+      for (int k = i; k < m; ++k) M[j][k] = 0;
+      ++j;
+    } else {
+      if (col != i)
+        for (int r = j; r < n; ++r) { const double t = M[r][i]; M[r][i] = M[r][col]; M[r][col] = t; }
+      for (int r = j + 1; r < n; ++r) M[r][i] = M[r][i] / M[j][i];
+      M[j][i] = 1.0;
+      for (int k = 0; k < m; ++k) {
+        if (k == i) continue;
+        const double s = M[j][k];
+        for (int r = j; r < n; ++r) M[r][k] = sub(M[r][k], mul(s, M[r][i]));
+      }
+      ++i; ++j;
+    }
+  }
+}
+
+// Fundamental10PSolver::solve (F10RelativePose, f10e_gb) on 10 preconditioned correspondences (x1[i], y1[i]) <-> (x2[i], y2[i]):
+// returns the number of models (0..10), F row-major at F[9 m] (F(2, 2) = 1) and (l1, l2) at L[2 m].
+ACR_HD int fit10(const double* x1, const double* y1, const double* x2, const double* y2, double* F, double* L, F10Work& w) {
+  double(&A)[10][16] = w.A;
+  for (int i = 0; i < 10; ++i) {   // X = the I points, U = the J points
+    const double x = x1[i], y = y1[i], u = x2[i], v = y2[i];
+    const double z1 = add(mul(x, x), mul(y, y)), z2 = add(mul(u, u), mul(v, v));
+    double* a = A[i];
+    a[0] = mul(x, u); a[1] = mul(x, v); a[2] = mul(y, u); a[3] = mul(y, v); a[4] = mul(u, z1); a[5] = u; a[6] = mul(v, z1); a[7] = v;
+    a[8] = mul(x, z2); a[9] = x; a[10] = mul(y, z2); a[11] = y; a[12] = mul(z1, z2); a[13] = z1; a[14] = z2; a[15] = 1.0;
+  }
+  partial_lu_solve(A);
+#define MR(r, c) A[r][10 + (c)]
+  double* P = w.P;
+  {
+    const double p[29] = {MR(5, 0), MR(5, 1), -MR(4, 0), -MR(4, 1), MR(5, 2), MR(5, 3), sub(MR(5, 4), MR(4, 2)), sub(MR(5, 5), MR(4, 3)),
+                          -MR(4, 4), -MR(4, 5), MR(7, 0), MR(7, 1), -MR(6, 0), -MR(6, 1), MR(7, 2), MR(7, 3), sub(MR(7, 4), MR(6, 2)),
+                          sub(MR(7, 5), MR(6, 3)), -MR(6, 4), -MR(6, 5), MR(9, 0), sub(MR(9, 1), MR(8, 0)), -MR(8, 1), MR(9, 2), MR(9, 4),
+                          sub(MR(9, 3), MR(8, 2)), -MR(8, 3), sub(MR(9, 5), MR(8, 4)), -MR(8, 5)};
+    for (int t = 0; t < 29; ++t) P[t] = p[t];
+  }
+  double* c = w.c;
+  c[0] = sub(mul(P[0], P[14]), mul(P[4], P[10]));
+  c[1] = sub(sub(add(mul(P[0], P[16]), mul(P[2], P[14])), mul(P[4], P[12])), mul(P[6], P[10]));
+  c[2] = sub(mul(P[2], P[18]), mul(P[8], P[12]));
+  c[3] = sub(mul(P[1], P[15]), mul(P[5], P[11]));
+  c[4] = sub(sub(add(mul(P[1], P[17]), mul(P[3], P[15])), mul(P[5], P[13])), mul(P[7], P[11]));
+  c[5] = sub(sub(add(mul(P[0], P[15]), mul(P[1], P[14])), mul(P[4], P[11])), mul(P[5], P[10]));
+  c[6] = sub(sub(sub(sub(add(add(add(mul(P[0], P[17]), mul(P[1], P[16])), mul(P[2], P[15])), mul(P[3], P[14])), mul(P[4], P[13])), mul(P[5], P[12])), mul(P[6], P[11])), mul(P[7], P[10]));
+  c[7] = sub(sub(add(mul(P[0], P[18]), mul(P[2], P[16])), mul(P[6], P[12])), mul(P[8], P[10]));
+  c[8] = sub(sub(sub(sub(add(add(add(mul(P[0], P[19]), mul(P[1], P[18])), mul(P[2], P[17])), mul(P[3], P[16])), mul(P[6], P[13])), mul(P[7], P[12])), mul(P[8], P[11])), mul(P[9], P[10]));
+  c[9] = sub(sub(add(mul(P[2], P[19]), mul(P[3], P[18])), mul(P[8], P[13])), mul(P[9], P[12]));
+  c[10] = sub(sub(add(mul(P[1], P[19]), mul(P[3], P[17])), mul(P[7], P[13])), mul(P[9], P[11]));
+  c[11] = sub(mul(P[3], P[19]), mul(P[9], P[13]));
+  c[12] = sub(mul(P[0], P[23]), mul(P[4], P[20]));
+  c[13] = sub(sub(add(mul(P[1], P[23]), mul(P[0], P[25])), mul(P[4], P[21])), mul(P[5], P[20]));
+  c[14] = sub(mul(P[2], P[24]), mul(P[8], P[20]));
+  c[15] = sub(sub(add(mul(P[3], P[24]), mul(P[2], P[27])), mul(P[8], P[21])), mul(P[9], P[20]));
+  c[16] = sub(mul(P[1], P[26]), mul(P[5], P[22]));
+  c[17] = sub(add(mul(P[0], P[24]), mul(P[2], P[23])), mul(P[6], P[20]));
+  c[18] = sub(sub(add(mul(P[0], P[26]), mul(P[1], P[25])), mul(P[4], P[22])), mul(P[5], P[21]));
+  c[19] = sub(sub(add(add(add(mul(P[1], P[24]), mul(P[3], P[23])), mul(P[0], P[27])), mul(P[2], P[25])), mul(P[6], P[21])), mul(P[7], P[20]));
+  c[20] = sub(sub(add(add(add(mul(P[0], P[28]), mul(P[1], P[27])), mul(P[2], P[26])), mul(P[3], P[25])), mul(P[6], P[22])), mul(P[7], P[21]));
+  c[21] = sub(sub(add(mul(P[2], P[28]), mul(P[3], P[27])), mul(P[8], P[22])), mul(P[9], P[21]));
+  c[22] = sub(add(mul(P[1], P[28]), mul(P[3], P[26])), mul(P[7], P[22]));
+  c[23] = sub(mul(P[3], P[28]), mul(P[9], P[22]));
+  c[24] = sub(mul(P[10], P[23]), mul(P[14], P[20]));
+  c[25] = sub(sub(add(mul(P[11], P[23]), mul(P[10], P[25])), mul(P[14], P[21])), mul(P[15], P[20]));
+  c[26] = sub(mul(P[12], P[24]), mul(P[18], P[20]));
+  c[27] = sub(sub(add(mul(P[13], P[24]), mul(P[12], P[27])), mul(P[18], P[21])), mul(P[19], P[20]));
+  c[28] = sub(mul(P[11], P[26]), mul(P[15], P[22]));
+  c[29] = sub(add(mul(P[10], P[24]), mul(P[12], P[23])), mul(P[16], P[20]));
+  c[30] = sub(sub(add(mul(P[10], P[26]), mul(P[11], P[25])), mul(P[14], P[22])), mul(P[15], P[21]));
+  c[31] = sub(sub(add(add(add(mul(P[11], P[24]), mul(P[13], P[23])), mul(P[10], P[27])), mul(P[12], P[25])), mul(P[16], P[21])), mul(P[17], P[20]));
+  c[32] = sub(sub(add(add(add(mul(P[10], P[28]), mul(P[11], P[27])), mul(P[12], P[26])), mul(P[13], P[25])), mul(P[16], P[22])), mul(P[17], P[21]));
+  c[33] = sub(sub(add(mul(P[12], P[28]), mul(P[13], P[27])), mul(P[18], P[22])), mul(P[19], P[21]));
+  c[34] = sub(add(mul(P[11], P[28]), mul(P[13], P[26])), mul(P[17], P[22]));
+  c[35] = sub(mul(P[13], P[28]), mul(P[19], P[22]));
+  double(&M)[20][10] = w.M;   // M(k) of the column-major 20 x 10 matrix is M[k % 20][k / 20]
+  for (int r = 0; r < 20; ++r)
+    for (int q = 0; q < 10; ++q) M[r][q] = 0;
+#define ACR_F10_M3(k, i0, i1, i2) (M[(i0) % 20][(i0) / 20] = M[(i1) % 20][(i1) / 20] = M[(i2) % 20][(i2) / 20] = c[k])
+#define ACR_F10_M(k, i0, i1, i2, i3) (ACR_F10_M3(k, i0, i1, i2), M[(i3) % 20][(i3) / 20] = c[k])
+  ACR_F10_M(0, 0, 61, 82, 144); ACR_F10_M(1, 2, 64, 85, 148); ACR_F10_M(2, 9, 72, 93, 156); ACR_F10_M(3, 3, 66, 87, 150); ACR_F10_M(4, 7, 70, 91, 154); ACR_F10_M(5, 1, 63, 84, 147);
+  ACR_F10_M(6, 4, 67, 88, 151); ACR_F10_M(7, 5, 68, 89, 152); ACR_F10_M(8, 8, 71, 92, 155); ACR_F10_M(9, 12, 75, 96, 158); ACR_F10_M(10, 11, 74, 95, 157); ACR_F10_M(11, 15, 77, 98, 159);
+  ACR_F10_M3(12, 20, 102, 165); ACR_F10_M3(13, 21, 104, 168); ACR_F10_M3(14, 25, 109, 173); ACR_F10_M3(15, 28, 112, 176); ACR_F10_M3(16, 26, 110, 174); ACR_F10_M3(17, 22, 105, 169);
+  ACR_F10_M3(18, 23, 107, 171); ACR_F10_M3(19, 24, 108, 172); ACR_F10_M3(20, 27, 111, 175); ACR_F10_M3(21, 31, 115, 178); ACR_F10_M3(22, 30, 114, 177); ACR_F10_M3(23, 34, 117, 179);
+  ACR_F10_M3(24, 40, 122, 185); ACR_F10_M3(25, 41, 124, 188); ACR_F10_M3(26, 45, 129, 193); ACR_F10_M3(27, 48, 132, 196); ACR_F10_M3(28, 46, 130, 194); ACR_F10_M3(29, 42, 125, 189);
+  ACR_F10_M3(30, 43, 127, 191); ACR_F10_M3(31, 44, 128, 192); ACR_F10_M3(32, 47, 131, 195); ACR_F10_M3(33, 51, 135, 198); ACR_F10_M3(34, 50, 134, 197); ACR_F10_M3(35, 54, 137, 199);
+#undef ACR_F10_M
+#undef ACR_F10_M3
+  col_echelon(M, 1e-16);
+  double(&At)[10][10] = w.At;
+  for (int r = 0; r < 10; ++r)
+    for (int q = 0; q < 10; ++q) At[r][q] = 0;
+  At[0][2] = At[1][4] = At[2][5] = At[3][7] = At[4][8] = At[5][9] = 1.0;
+  for (int r = 6; r < 10; ++r)
+    for (int q = 0; q < 10; ++q) At[r][q] = -M[19 - q][15 - r];
+  if (!e5::eigen_solve_complex(At, w.re, w.im, w.V, w.Vi)) return 0;
+  int nb = 0;
+  for (int j = 0; j < 10; ++j) {   // esols = (row 2 / row 0, row 1 / row 0), kept when both imaginary parts are within 100 eps
+    const double *v = w.V[j], *vi = w.Vi[j];
+    double l1r, l1i, l2r, l2i;
+    e5::cdiv(v[2], vi[2], v[0], vi[0], l1r, l1i);
+    e5::cdiv(v[1], vi[1], v[0], vi[0], l2r, l2i);
+    if (fabs(l1i) <= 100 * e5::kEps && fabs(l2i) <= 100 * e5::kEps) { L[2 * nb] = l1r; L[2 * nb + 1] = l2r; ++nb; }
+  }
+  if (nb == 0) return 0;
+  for (int m = 0; m < nb; ++m) {
+    const double l1 = L[2 * m], l2 = L[2 * m + 1], l1l1 = mul(l1, l1), l1l2 = mul(l1, l2);
+    // b = P[0..9]; f23 = -b(4:10) . m2 / b(0:4) . m1, both in SSE2 packet order
+    const double m1[4] = {l1l2, l1, l2, 1.0}, m2[6] = {mul(l1l2, l1), l1l1, l1l2, l1, l2, 1.0};
+    double t2[6], t1[4];
+    for (int k = 0; k < 6; ++k) t2[k] = mul(P[4 + k], m2[k]);
+    for (int k = 0; k < 4; ++k) t1[k] = mul(P[k], m1[k]);
+    const double d2 = add(add(t2[0], add(t2[2], t2[4])), add(t2[1], add(t2[3], t2[5])));
+    const double d1 = add(add(t1[0], t1[2]), add(t1[1], t1[3]));
+    const double f23 = -d2 / d1;
+    const double m3[6] = {mul(l2, f23), f23, l1l2, l1, l2, 1.0};
+    auto dot = [&](int row) {   // m3 . -mr.row(row), the scalar unroller's (0 + (1 + 2)) + (3 + (4 + 5))
+      double t[6];
+      for (int k = 0; k < 6; ++k) t[k] = mul(m3[k], -MR(row, k));
+      return add(add(t[0], add(t[1], t[2])), add(t[3], add(t[4], t[5])));
+    };
+    double* f = F + 9 * m;
+    f[0] = dot(0); f[1] = dot(1); f[2] = dot(9);
+    f[3] = dot(2); f[4] = dot(3); f[5] = f23;
+    f[6] = dot(5); f[7] = dot(7); f[8] = 1.0;
+  }
+#undef MR
   return nb;
 }
 

@@ -2216,20 +2216,23 @@ int b200m_ctx_set_hgrowing_window(b200m_ctx* c, int window) {
 
 }  // extern "C"
 
-// ---- K10: a-contrario RANSAC for a pair list: fundamental matrix, homography, spherical fundamental matrix, essential matrix
-// (acransac.cuh) ----
+// ---- K10: a-contrario RANSAC for a pair list: fundamental matrix, homography, spherical fundamental matrix, essential matrix,
+// fundamental matrix with radial distortion (acransac.cuh) ----
 // One launch of acransac_kernel<Policy> over the list; the entry points differ in the model, the correspondence width
 // (Policy::kWidth doubles; 4 pixel doubles in for the calibrated policy) and the generator contract.  wh: image sizes of the planar
 // and calibrated policies (unused, may be NULL, for bearings).  K: n_pairs x 18 (K_I, K_J row-major) for the calibrated policy, else
 // unused.  mt_per_pair: 0 = mt_state is one 625-word state for every pair, 1 = n_pairs x 625.  mt_out: NULL or n_pairs x 625.
+// L: n_pairs x 2, the winners' radial distortion, for the distortion policy (required there), else unused.
 template <class Policy>
 static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh, const double* K,
                           const uint32_t* mt_state, int mt_per_pair, int64_t max_iteration, double precision, uint8_t* valid, int32_t* n_inliers,
-                          uint32_t* inliers, double* model, double* error_max, double* min_nfa, int32_t* iterations, uint32_t* mt_out) {
+                          uint32_t* inliers, double* model, double* error_max, double* min_nfa, int32_t* iterations, uint32_t* mt_out,
+                          double* L = nullptr) {
+  using OutT = std::conditional_t<Policy::kDistortion, acrk::OutL, acrk::Out>;
   constexpr bool kSized = Policy::kPlanar || Policy::kCalibrated;
   if (!c || n_pairs < 0 || max_iteration < 0 || max_iteration > INT32_MAX || !(precision > 0) || (mt_per_pair != 0 && mt_per_pair != 1) ||
       (n_pairs > 0 && (!offsets || (kSized && !wh) || (Policy::kCalibrated && !K) || !mt_state || !valid || !n_inliers || !model ||
-                       !error_max || !min_nfa || !iterations)))
+                       !error_max || !min_nfa || !iterations || (Policy::kDistortion && !L))))
     return fail(B200M_ERR_ARG, "bad arguments");
   if (n_pairs > 0 && offsets[0] != 0) return fail(B200M_ERR_ARG, "offsets[0] must be 0");
   std::vector<acrk::Pair> pairs((size_t)n_pairs);
@@ -2285,7 +2288,7 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
                o_logc = take(sizeof(float) * 2 * (N + n_pairs)), o_gk = take(sizeof(unsigned long long) * sort_total),
                o_gv = take(sizeof(uint32_t) * sort_total), o_inl = take(sizeof(uint32_t) * N),
                o_tr = take(sizeof(int32_t) * acrk::kTraceCap * n_pairs),
-               o_trn = take(sizeof(double) * acrk::kTraceCap * n_pairs), o_out = take(sizeof(acrk::Out) * n_pairs),
+               o_trn = take(sizeof(double) * acrk::kTraceCap * n_pairs), o_out = take(sizeof(OutT) * n_pairs),
                o_mto = take(mt_out ? sizeof(uint32_t) * 625 * n_pairs : 0);
   int rc;
   if ((rc = c->acr.d.reserve(at)) || (rc = c->acr.ev0.create()) || (rc = c->acr.ev1.create())) return rc;
@@ -2296,15 +2299,15 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
   CK(cudaMemcpyAsync(d + o_l10, l10.data(), sizeof(float) * l10.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d + o_mt, mt_state, sizeof(uint32_t) * 625 * n_states, cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(c->acr.ev0, st));
-  acrk::acransac_kernel<Policy><<<n_pairs, acrk::kThreads, 0, st>>>(
-      (const acrk::Pair*)(d + o_pairs), (const double*)(d + o_corr), (const float*)(d + o_l10), (const uint32_t*)(d + o_mt),
+  acrk::launch<Policy>(
+      n_pairs, st, (const acrk::Pair*)(d + o_pairs), (const double*)(d + o_corr), (const float*)(d + o_l10), (const uint32_t*)(d + o_mt),
       mt_per_pair ? 625 : 0, (long long)max_iteration, precision, c->acr.skip ? 1 : 0, (double*)(d + o_pts), (uint32_t*)(d + o_idx),
       (float*)(d + o_logc), (unsigned long long*)(d + o_gk), (uint32_t*)(d + o_gv), (uint32_t*)(d + o_inl), (int*)(d + o_tr),
       (double*)(d + o_trn), (acrk::Out*)(d + o_out), mt_out ? (uint32_t*)(d + o_mto) : nullptr);
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->acr.ev1, st));
-  std::vector<acrk::Out> outs((size_t)n_pairs);
-  CK(cudaMemcpyAsync(outs.data(), d + o_out, sizeof(acrk::Out) * n_pairs, cudaMemcpyDeviceToHost, st));
+  std::vector<OutT> outs((size_t)n_pairs);
+  CK(cudaMemcpyAsync(outs.data(), d + o_out, sizeof(OutT) * n_pairs, cudaMemcpyDeviceToHost, st));
   if (N) CK(cudaMemcpyAsync(inliers, d + o_inl, sizeof(uint32_t) * N, cudaMemcpyDeviceToHost, st));
   if (mt_out) CK(cudaMemcpyAsync(mt_out, d + o_mto, sizeof(uint32_t) * 625 * n_pairs, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(c->acr.trace.data(), d + o_tr, sizeof(int32_t) * acrk::kTraceCap * n_pairs, cudaMemcpyDeviceToHost, st));
@@ -2315,7 +2318,8 @@ static int acransac_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, con
   c->acr.last_ms = ms;
   c->acr.stats[3] = 1;
   for (int k = 0; k < n_pairs; ++k) {
-    const acrk::Out& o = outs[k];
+    const acrk::Out& o = reinterpret_cast<const acrk::Out&>(outs[k]);   // an OutL begins with its Out
+    if constexpr (Policy::kDistortion) { L[2 * k] = outs[k].L[0]; L[2 * k + 1] = outs[k].L[1]; }
     valid[k] = (uint8_t)o.valid; n_inliers[k] = o.n_inl;
     for (int t = 0; t < 9; ++t) model[9 * k + t] = o.model[t];
     error_max[k] = o.error_max; min_nfa[k] = o.min_nfa; iterations[k] = o.iterations;
@@ -2357,6 +2361,14 @@ int b200m_acransac_essential_pairs(b200m_ctx* c, int n_pairs, const int64_t* off
                                    uint32_t* mt_state_out) {
   return acransac_pairs<acrk::EPolicy>(c, n_pairs, offsets, corr, wh, K, mt_state, mt_state_per_pair, max_iteration, precision, valid,
                                        n_inliers, inliers, E, error_max, min_nfa, iterations, mt_state_out);
+}
+
+int b200m_acransac_fundamental_distortion_pairs(b200m_ctx* c, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh,
+                                                const uint32_t* mt_state, int64_t max_iteration, double precision, uint8_t* valid,
+                                                int32_t* n_inliers, uint32_t* inliers, double* F, double* L, double* error_max, double* min_nfa,
+                                                int32_t* iterations) {
+  return acransac_pairs<acrk::F10Policy>(c, n_pairs, offsets, corr, wh, nullptr, mt_state, 0, max_iteration, precision, valid, n_inliers, inliers,
+                                         F, error_max, min_nfa, iterations, nullptr, L);
 }
 
 double b200m_acransac_last_stats(const b200m_ctx* c, int64_t stats[4]) {

@@ -43,7 +43,7 @@ ABI_SYMBOLS = [
     "b200m_acransac_fundamental_pairs", "b200m_acransac_last_stats", "b200m_acransac_last_trace", "b200m_ctx_set_acransac_skip",
     "b200m_mt19937_seed", "b200m_debug_rand_sample", "b200m_acransac_homography_pairs", "b200m_debug_rand_sample_k", "b200m_guided_match_pairs",
     "b200m_guided_match_positions_pairs", "b200m_acransac_fundamental_spherical_pairs", "b200m_hgrowing_pairs", "b200m_hgrowing_last_stats",
-    "b200m_ctx_set_hgrowing_window", "b200m_acransac_essential_pairs",
+    "b200m_ctx_set_hgrowing_window", "b200m_acransac_essential_pairs", "b200m_acransac_fundamental_distortion_pairs",
 ]
 
 
@@ -266,6 +266,15 @@ class Context:
         Km = np.ascontiguousarray(K, np.float64).reshape(len(corr_list), 18)
         return self._acransac_pairs("E", corr_list, wh, _mt_states(mt_state_or_states, len(corr_list)), maxIteration, precision, Km)
 
+    def acransac_fundamental_distortion_pairs(self, corr_list, wh, mt_state, maxIteration: int = 50000, precision: float = np.inf) -> list[dict]:
+        """b200m_acransac_fundamental_distortion_pairs: GeometricFilterMatrix_F_AC::geometricEstimation_Mat_ACRANSAC<Fundamental10PSolver,
+        Fundamental10PModel> (the fundamental_with_distortion filter on a planar pair) for every pair.  Arguments as in
+        acransac_fundamental_pairs (every pair starts from mt_state).  Returns per pair its fields, with "F" the reference's model
+        matrix (the solver's constraint is [x_I, y_I, 1 + l1 r_I^2] F [x_J, y_J, 1 + l2 r_J^2]^T = 0 on preconditioned points; the
+        score reads F as x_J^T F x_I on undistorted pixels, as the reference does), and "L" = (l1, l2), the same model's radial
+        distortion in preconditioned units (0 without a model).  A pair with at most 10 correspondences returns (0, 0)."""
+        return self._acransac_pairs("F10", corr_list, wh, np.ascontiguousarray(mt_state, np.uint32).reshape(625), maxIteration, precision)
+
     def _acransac_pairs(self, kind: str, corr_list, wh, st, maxIteration, precision, K=None) -> list[dict]:
         width = 6 if kind == "S" else 4
         cs = [np.ascontiguousarray(c, np.float64).reshape(-1, width) for c in corr_list]
@@ -277,7 +286,8 @@ class Context:
         valid = np.zeros(max(n, 1), np.uint8); ninl = np.zeros(max(n, 1), np.int32); it = np.zeros(max(n, 1), np.int32)
         inl = np.zeros(max(int(offsets[-1]), 1), np.uint32); M = np.zeros((max(n, 1), 9)); em = np.zeros(max(n, 1)); nfa = np.zeros(max(n, 1))
         ptr = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-        sto = np.zeros((max(n, 1), 625), np.uint32) if kind != "F" else None
+        sto = np.zeros((max(n, 1), 625), np.uint32) if kind not in ("F", "F10") else None
+        Ls = np.zeros((max(n, 1), 2)) if kind == "F10" else None
         if kind == "H":
             _check(self.lib.b200m_acransac_homography_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st), C.c_int(int(st.ndim == 2)),
                                                             C.c_int64(maxIteration), C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(M),
@@ -293,6 +303,11 @@ class Context:
                                                                        C.c_int64(maxIteration), C.c_double(precision), ptr(valid), ptr(ninl),
                                                                        ptr(inl), ptr(M), ptr(em), ptr(nfa), ptr(it), ptr(sto)),
                    "b200m_acransac_fundamental_spherical_pairs")
+        elif kind == "F10":
+            _check(self.lib.b200m_acransac_fundamental_distortion_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st),
+                                                                        C.c_int64(maxIteration), C.c_double(precision), ptr(valid), ptr(ninl),
+                                                                        ptr(inl), ptr(M), ptr(Ls), ptr(em), ptr(nfa), ptr(it)),
+                   "b200m_acransac_fundamental_distortion_pairs")
         else:
             _check(self.lib.b200m_acransac_fundamental_pairs(self._h, C.c_int(n), ptr(offsets), ptr(corr), ptr(whm), ptr(st), C.c_int64(maxIteration),
                                                              C.c_double(precision), ptr(valid), ptr(ninl), ptr(inl), ptr(M), ptr(em), ptr(nfa), ptr(it)),
@@ -306,12 +321,14 @@ class Context:
                  "trace": tr[:min(nt, tr.size)].copy(), "trace_nfa": trn[:min(nt, trn.size)].copy()}
             if sto is not None:
                 r["mt_state_out"] = sto[k].copy()
+            if Ls is not None:
+                r["L"] = Ls[k].copy()
             out.append(r)
         return out
 
     def acransac_last_stats(self) -> dict:
-        """Instrumentation of the last acransac_fundamental_pairs, acransac_homography_pairs, acransac_fundamental_spherical_pairs or
-        acransac_essential_pairs call."""
+        """Instrumentation of the last acransac_fundamental_pairs, acransac_homography_pairs, acransac_fundamental_spherical_pairs,
+        acransac_essential_pairs or acransac_fundamental_distortion_pairs call."""
         st = np.zeros(4, np.int64)
         ms = self.lib.b200m_acransac_last_stats(self._h, st.ctypes.data_as(C.c_void_p))
         return {"gpu_ms": ms, "models_evaluated": int(st[0]), "models_skipped": int(st[1]), "models_exact": int(st[2]), "launches": int(st[3])}
@@ -395,6 +412,15 @@ def geometricEstimation_F_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: 
     return ctx.acransac_fundamental_pairs(*_one_pair(xI, xJ, sizeI, sizeJ), _start_state(seed_or_state), maxIteration, precision)[0]
 
 
+def geometricEstimation_F10_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: int = 50000, precision: float = np.inf,
+                               ctx: Context | None = None) -> dict:
+    """GeometricFilterMatrix_F_AC::geometricEstimation_Mat_ACRANSAC<Fundamental10PSolver, Fundamental10PModel> of one planar pair on the
+    GPU (the fundamental_with_distortion filter; arguments as geometricEstimation_F_AC).  Returns the dict of
+    Context.acransac_fundamental_distortion_pairs: "F" and "L"."""
+    ctx = ctx or default_context()
+    return ctx.acransac_fundamental_distortion_pairs(*_one_pair(xI, xJ, sizeI, sizeJ), _start_state(seed_or_state), maxIteration, precision)[0]
+
+
 def geometricEstimation_H_AC(xI, xJ, sizeI, sizeJ, seed_or_state, maxIteration: int = 50000, precision: float = np.inf,
                              ctx: Context | None = None) -> dict:
     """GeometricFilterMatrix_H_AC::geometricEstimation of one pair on the GPU (arguments as geometricEstimation_F_AC).  Returns the
@@ -449,7 +475,7 @@ def hasStrongSupport(matches_per_type: dict, minimumSamples: int = 7) -> bool:
 def robustModelEstimation_F_AC(putatives: dict, regions_per_view: dict, image_sizes: dict, seed_or_state, maxIteration: int = 50000,
                                precision: float = np.inf, guidedMatching: bool = False, distanceRatio: float = 0.6, geometry: dict | None = None,
                                guided_geometry: dict | None = None, desc_types=None, ctx: Context | None = None, bearings: dict | None = None,
-                               chain: bool = False):
+                               chain: bool = False, estimateDistortion: bool = False):
     """matchingImageCollection::robustModelEstimation with GeometricFilterMatrix_F_AC (ACRANSAC, Fundamental7PSolver; GeometricFilter.hpp:40-88),
     the default `fundamental_matrix` filter of featureMatching, for a whole putative list: one a-contrario RANSAC call for every pair
     (b200m_acransac_fundamental_pairs), then, with guidedMatching, one guided-matching call for every kept pair and common descriptor
@@ -476,22 +502,33 @@ def robustModelEstimation_F_AC(putatives: dict, regions_per_view: dict, image_si
                               generator and hands it on; each run of planar pairs between two of them is one planar call from the
                               current state.  Bit for bit the reference's run; meant for tests and short lists.
                      Without spherical pairs both give today's single planar call.
+    estimateDistortion  GeometricFilterMatrix_F_AC's m_estimateDistortion, the `fundamental_with_distortion` filter: the planar
+                     pairs are estimated by geometricEstimation_Mat_ACRANSAC<Fundamental10PSolver, Fundamental10PModel>
+                     (b200m_acransac_fundamental_distortion_pairs), whose minimum sample count 10 is their hasStrongSupport threshold;
+                     spherical pairs are estimated as without it (7).  Their "F" is the reference's model matrix, scored and
+                     guided-matched as x_J^T F x_I while the solver fits it transposed with distortion (see
+                     acransac_fundamental_distortion_pairs), and info gains "L" ((l1, l2) in preconditioned units, 0 for the
+                     other pairs).  The filter itself does not use L.
 
     Returns (geometric matches {(I, J): {type: matches}} of the pairs with strong support, per-pair estimation
-    {(I, J): {"valid", "strong_support", "F", "error_max", "spherical"}, plus "mt_state_out" for the spherical pairs estimated}).
+    {(I, J): {"valid", "strong_support", "F", "error_max", "spherical"}, plus "mt_state_out" for the spherical pairs estimated, and
+    "L" with estimateDistortion}).
     Without guided matching the kept lists are the inlier putatives (ratio and distance kept); with it, the guided lists of every
     common type (empty ones included) replace them, or nothing when error_max is infinite (GeometricFilterMatrix_F_AC.hpp:363).  A
     spherical pair's guided matching uses its F and error_max on the guided positions, as the reference does."""
     ctx = ctx or default_context()
     common, est, corrs, whs = _estimation_inputs(putatives, regions_per_view, image_sizes, geometry, desc_types)
     sph = _spherical_inputs(putatives, regions_per_view, bearings or {}, common, est)
-    calls = [(lambda ks, st: ctx.acransac_fundamental_pairs([corrs[k] for k in ks], [whs[k] for k in ks], st, maxIteration, precision), False),
+    planar = ctx.acransac_fundamental_distortion_pairs if estimateDistortion else ctx.acransac_fundamental_pairs
+    calls = [(lambda ks, st: planar([corrs[k] for k in ks], [whs[k] for k in ks], st, maxIteration, precision), False),
              (lambda ks, st: ctx.acransac_fundamental_spherical_pairs([sph[est[k]] for k in ks], st, maxIteration, precision), True)]
-    out, info = _acransac_stage(ctx, putatives, regions_per_view, guided_geometry, common, est, [int(p in sph) for p in est], calls, "F", 7,
-                                seed_or_state, chain, guidedMatching, distanceRatio,
+    out, info = _acransac_stage(ctx, putatives, regions_per_view, guided_geometry, common, est, [int(p in sph) for p in est], calls, "F",
+                                [10, 7] if estimateDistortion else 7, seed_or_state, chain, guidedMatching, distanceRatio,
                                 lambda vp, items, Fs, th, ratio: ctx.guided_match_pairs(vp, Fs, th, ratio))
     for p, d in info.items():
         d["spherical"] = p in sph
+        if estimateDistortion:
+            d.setdefault("L", np.zeros(2))
     return out, info
 
 
@@ -577,7 +614,8 @@ def _acransac_stage(ctx: Context, putatives: dict, regions_per_view: dict, guide
                      the generator contract of its geometricEstimation.  chain=False: one call per group from the caller's state, in
                      `calls` order.  chain=True: in list order, a by-reference pair alone, handing its mt_state_out to the next call,
                      and each run of by-value pairs of one group in one call from the current state.
-      key            the model's name in the results and in info; min_samples: the solver's getMinimumNbRequiredSamples
+      key            the model's name in the results and in info; min_samples: the solver's getMinimumNbRequiredSamples, one for
+                     every group or a list with one per group (the hasStrongSupport threshold of the group's pairs)
       guided         guided(view_pairs, items, models, errorTh, distRatio): the batched guided call over items = [(pair, type)],
                      with errorTh = error_max^2 and distRatio = distanceRatio^2
     ACRANSAC's validity comes before support.  Returns (out, info) as robustModelEstimation_H_AC describes them, "mt_state_out"
@@ -596,14 +634,15 @@ def _acransac_stage(ctx: Context, putatives: dict, regions_per_view: dict, guide
             st = res[ks[0]]["mt_state_out"]
     info = {p: {"valid": False, "strong_support": False, key: np.zeros((3, 3)), "error_max": np.inf} for p in putatives}
     out = {}
-    for p, r in zip(est, res):
+    for p, g, r in zip(est, groups, res):
         info[p].update({"valid": r["valid"], key: r[key], "error_max": r["error_max"]})
-        if "mt_state_out" in r:
-            info[p]["mt_state_out"] = r["mt_state_out"]
+        for extra in ("mt_state_out", "L"):
+            if extra in r:
+                info[p][extra] = r[extra]
         if not r["valid"]:
             continue
         inl = copyInlierMatches(r["inliers"], putatives[p], common[p])
-        info[p]["strong_support"] = hasStrongSupport(inl, min_samples)
+        info[p]["strong_support"] = hasStrongSupport(inl, min_samples[g] if isinstance(min_samples, (list, tuple)) else min_samples)
         if info[p]["strong_support"]:
             out[p] = inl
     if guidedMatching and out:

@@ -277,11 +277,25 @@ int b200m_acransac_essential_pairs(b200m_ctx* ctx, int n_pairs, const int64_t* o
                                    const uint32_t* mt_state, int mt_state_per_pair, int64_t max_iteration, double precision, uint8_t* valid,
                                    int32_t* n_inliers, uint32_t* inliers, double* E, double* error_max, double* min_nfa, int32_t* iterations,
                                    uint32_t* mt_state_out);
+/* GeometricFilterMatrix_F_AC::geometricEstimation_Mat_ACRANSAC<Fundamental10PSolver, Fundamental10PModel> (the
+ * fundamental_with_distortion filter on a planar pair) for every pair: ACRANSAC over RelativePoseKernel<Fundamental10PSolver,
+ * FundamentalEpipolarDistanceError, UnnormalizerT, Fundamental10PModel>, 10-point samples, at most 10 models a sample.
+ * Arguments as in b200m_acransac_fundamental_pairs (one generator state that every pair starts from: the filter takes it by value).
+ * F[9 * n_pairs]: the model's matrix (Fundamental10PModel::getMatrix(), row-major, unnormalised N2^T F N1 like the F call's).  It is
+ * the reference's model matrix: the solver fits [x_I, y_I, 1 + l1 r_I^2] F [x_J, y_J, 1 + l2 r_J^2]^T = 0 on preconditioned points,
+ * while the residual, errorMax and a guided step read it as the point-to-line error of F x_I on undistorted pixels.
+ * L[2 * n_pairs]: the same model's (l1, l2) (getRadialDistortion()), in preconditioned units: the unnormaliser leaves it as is; 0 for
+ * a pair without a model.  The filter does not use L.  A pair with at most 10 correspondences returns (0, 0) and no iteration. */
+int b200m_acransac_fundamental_distortion_pairs(b200m_ctx* ctx, int n_pairs, const int64_t* offsets, const double* corr, const int32_t* wh,
+                                                const uint32_t* mt_state, int64_t max_iteration, double precision, uint8_t* valid,
+                                                int32_t* n_inliers, uint32_t* inliers, double* F, double* L, double* error_max, double* min_nfa,
+                                                int32_t* iterations);
 /* instrumentation of the last a-contrario RANSAC call (b200m_acransac_fundamental_pairs, b200m_acransac_homography_pairs,
- * b200m_acransac_fundamental_spherical_pairs or b200m_acransac_essential_pairs): stats = {models evaluated in the a-contrario mode, of them skipped by the histogram
- * bound, scored exactly, kernel launches}; returns its GPU time in ms */
+ * b200m_acransac_fundamental_spherical_pairs, b200m_acransac_essential_pairs or b200m_acransac_fundamental_distortion_pairs): stats =
+ * {models evaluated in the a-contrario mode, of them skipped by the histogram bound, scored exactly, kernel launches}; returns its GPU
+ * time in ms */
 double b200m_acransac_last_stats(const b200m_ctx* ctx, int64_t stats[4]);
-/* the `better` events of the last a-contrario RANSAC call's pair `pair` (F, H, spherical F or E): the iterations at which a better model was found
+/* the `better` events of the last a-contrario RANSAC call's pair `pair` (F, H, spherical F, E or F10): the iterations at which a better model was found
  * and the new minNFA of each (the first `cap`, at most 256; either pointer may be NULL); returns their number.  The getters of the
  * last call take the context's lock, so a concurrent call on the same context cannot rewrite what they read. */
 int b200m_acransac_last_trace(const b200m_ctx* ctx, int pair, int32_t* iters, double* nfa, int cap);
