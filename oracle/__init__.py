@@ -40,22 +40,37 @@ def reference_src() -> str | None:
     return None
 
 
+# Entry points a library must define, by checker: make goes by modification times, and a library compiled from older sources can be
+# newer than a fresh checkout of the sources, so build() rebuilds a library that lacks one of these.
+ENTRY_POINTS = {
+    "acransac": ("acr_solve_cubic", "acr_nullspace7", "acr_epipolar_error", "acr_precondition", "acr_unnormalize", "acr_logalpha0",
+                 "acr_unnormalize_error"),
+    "acransac_h": ("acr_nullspace8", "acr_inverse3", "acr_unnormalize_h", "acr_logalpha0_h", "acr_unnormalize_error_h"),
+    "acransac_s": ("acrs_fit7s", "acrs_spherical_error", "acrs_estimate"),
+    "acransac_e": ("acre_fit5", "acre_action", "acre_eigen", "acre_estimate"),
+    "acransac_f10": ("acrf10_fit10", "acrf10_estimate", "acrf10_mt_seed"),
+    "hgrowing": ("hg_filter", "hg_grow_steps", "hg_refine", "hg_exp", "hg_log"),
+}
+
+
 def build(ref: bool | None = None) -> None:
-    """Compile the oracle libraries (port always; ref and the C++ adaptor test when reference_src() finds an AliceVision tree)."""
+    """Compile every checker library (oracle/Makefile): the ports always; with ref (by default when reference_src() finds an
+    AliceVision tree) also the "ref" libraries and, once alicevision_b200/libb200match.so is built, the C++ adaptor tests."""
     src = reference_src()
     if ref is None:
         ref = src is not None
     if ref and src is None:
         raise RuntimeError("the compiled reference needs an AliceVision source tree: set ALICEVISION_SRC to its src directory")
-    targets = ["all"] + (["ref", f"REF={src}"] if ref else [])
-    subprocess.run(["make", "-C", _HERE] + targets, check=True, stdout=subprocess.DEVNULL)
-    # the C++ adaptor test needs the reference's interface headers AND the built CUDA library
+    make = ["make", "-C", _HERE] + ([f"REF={src}"] if ref else [])
+    subprocess.run(make + ["all"] + (["ref"] if ref else []), check=True, stdout=subprocess.DEVNULL)
+    for name in ENTRY_POINTS:
+        for kind in ("port", "ref") if ref else ("port",):
+            if lib_available(name, kind) and not lib_current(name, kind):
+                subprocess.run(make + ["-B", os.path.relpath(lib_path(name, kind), _HERE)], check=True, stdout=subprocess.DEVNULL)
+                assert lib_current(name, kind), f"{lib_path(name, kind)} lacks {sorted(ENTRY_POINTS[name])} after a rebuild"
+    # the C++ adaptor tests need the reference's interface headers AND the built CUDA library
     if ref and os.path.exists(os.path.join(os.path.dirname(_HERE), "alicevision_b200", "libb200match.so")):
-        subprocess.run(["make", "-C", _HERE, "adaptor", f"REF={src}"], check=True, stdout=subprocess.DEVNULL)
-
-
-def available(kind: str) -> bool:
-    return os.path.exists(_lib_path(kind))
+        subprocess.run(make + ["adaptors"], check=True, stdout=subprocess.DEVNULL)
 
 
 def exports(path: str, names) -> bool:
@@ -65,20 +80,37 @@ def exports(path: str, names) -> bool:
     return r.returncode == 0 and set(names) <= {ln.split()[-1] for ln in r.stdout.splitlines() if ln.strip()}
 
 
-def make_current(makefile: str, targets: dict, make_args) -> None:
-    """make -f makefile <make_args>, then rebuild (make -B) every target of `targets` ({target: (library path, symbols)}) whose
-    library was not rebuilt but lacks symbols: make goes by modification times, and a library compiled from older sources can be
-    newer than a fresh checkout of the sources."""
-    subprocess.run(["make", "-C", _HERE, "-f", makefile] + list(make_args), check=True, stdout=subprocess.DEVNULL)
-    for target, (path, names) in targets.items():
-        if os.path.exists(path) and not exports(path, names):
-            extra = [a for a in make_args if "=" in a]
-            subprocess.run(["make", "-C", _HERE, "-f", makefile, "-B", target] + extra, check=True, stdout=subprocess.DEVNULL)
-            assert exports(path, names), f"{path} lacks {sorted(names)} after a rebuild"
+# ---------------------------------------------------------------------------------------------- checker libraries
+def lib_path(name: str, kind: str | None = "port") -> str:
+    """The library of checker `name`: oracle/libport_<name>.so, its "ref" build oracle/_ref/libref_<name>.so, or for a checker with
+    one build (kind None) oracle/lib<name>.so."""
+    if kind == "ref":
+        return os.path.join(_HERE, "_ref", f"libref_{name}.so")
+    return os.path.join(_HERE, f"libport_{name}.so" if kind == "port" else f"lib{name}.so")
 
 
-def _lib_path(kind: str) -> str:
-    return os.path.join(_HERE, "_ref", "libref_oracle.so") if kind == "ref" else os.path.join(_HERE, "libport_oracle.so")
+def lib_available(name: str, kind: str | None = "port") -> bool:
+    return os.path.exists(lib_path(name, kind))
+
+
+def lib_current(name: str, kind: str = "port") -> bool:
+    """The library is built and defines every entry point ENTRY_POINTS lists for it (a build from older sources may lack some)."""
+    return lib_available(name, kind) and exports(lib_path(name, kind), ENTRY_POINTS[name])
+
+
+def load_lib(name: str, kind: str | None = "port") -> C.CDLL:
+    path = lib_path(name, kind)
+    if not os.path.exists(path):
+        raise FileNotFoundError(f"{path} missing: run oracle.build()")
+    return C.CDLL(path)
+
+
+def _p(a: np.ndarray):
+    return a.ctypes.data_as(C.c_void_p)
+
+
+def available(kind: str) -> bool:
+    return lib_available("oracle", kind)
 
 
 def _dt(a: np.ndarray, hamming: bool) -> int:
@@ -89,18 +121,11 @@ def _dt(a: np.ndarray, hamming: bool) -> int:
     raise TypeError(f"unsupported descriptor dtype {a.dtype}")
 
 
-def _p(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 class Oracle:
     def __init__(self, kind: str = "port"):
         assert kind in ("ref", "port")
         self.kind = kind
-        path = _lib_path(kind)
-        if not os.path.exists(path):
-            raise FileNotFoundError(f"{path} missing: run oracle.build()")
-        self.lib = C.CDLL(path)
+        self.lib = load_lib("oracle", kind)
         self.pfx = "ref_" if kind == "ref" else "port_"
         f = self._f
         f("metric").restype = C.c_double
@@ -282,7 +307,7 @@ class Oracle:
 
     def save_matches_txt(self, path: str, blocks) -> None:
         """blocks: [((I, J), descTypeName, matches[MATCH_DTYPE])] in PairwiseMatches map order (restated: port library)."""
-        lib = C.CDLL(_lib_path("port"))
+        lib = load_lib("oracle")
         ids = np.array([[b[0][0], b[0][1]] for b in blocks], np.uint32).reshape(-1, 2)
         names = (C.c_char_p * max(len(blocks), 1))(*[b[1].encode() for b in blocks])
         offs = np.concatenate([[0], np.cumsum([len(b[2]) for b in blocks])]).astype(np.int64)
@@ -290,7 +315,7 @@ class Oracle:
         assert lib.port_save_matches_txt(path.encode(), C.c_int(len(blocks)), _p(ids), names, _p(offs), _p(data)) == 0
 
     def load_matches_txt(self, path: str, cap_blocks: int = 1 << 16, cap_matches: int = 1 << 22):
-        lib = C.CDLL(_lib_path("port"))
+        lib = load_lib("oracle")
         ids = np.zeros((cap_blocks, 2), np.uint32); names = np.zeros((cap_blocks, 32), np.uint8)
         offs = np.zeros(cap_blocks + 1, np.int64); data = np.zeros(cap_matches, MATCH_DTYPE)
         nb = lib.port_load_matches_txt(path.encode(), C.c_int(cap_blocks), _p(ids), _p(names), _p(offs), C.c_long(cap_matches), _p(data))
@@ -305,16 +330,13 @@ class VoctreeOracle:
     def __init__(self, kind: str = "port"):
         assert kind in ("ref", "port")
         self.kind = kind
-        path = os.path.join(_HERE, "_ref", "libref_voctree.so") if kind == "ref" else os.path.join(_HERE, "libport_voctree.so")
-        if not os.path.exists(path):
-            raise FileNotFoundError(f"{path} missing: run oracle.build()")
-        self.lib = C.CDLL(path)
+        self.lib = load_lib("voctree", kind)
         self.pfx = "refv_" if kind == "ref" else "portv_"
         getattr(self.lib, self.pfx + "image_matching").restype = C.c_long
 
     @staticmethod
     def available(kind: str) -> bool:
-        return os.path.exists(os.path.join(_HERE, "_ref", "libref_voctree.so") if kind == "ref" else os.path.join(_HERE, "libport_voctree.so"))
+        return lib_available("voctree", kind)
 
     def _tree_args(self, k, levels, centers, valid, tmp):
         c = np.ascontiguousarray(centers, np.float32); v = np.ascontiguousarray(valid, np.uint8)
@@ -358,7 +380,7 @@ def best(prefer_ref: bool = True) -> Oracle:
 
 # ---------------------------------------------------------------------------------------------- stored reference outputs
 REFERENCE_OUTPUTS = os.path.join(os.path.dirname(_HERE), "tests", "golden", "reference_outputs.npz")
-_stored: dict | None = None
+_stored: dict = {}      # {store path: {key: output}}, each file read once
 
 
 def _flatten(key, v, out):
@@ -420,31 +442,31 @@ def _load_flat(path):
     return out
 
 
-def reference_output(key: str, compute, live: bool):
-    """What the compiled reference returns for test case `key`.  live (the reference is built): compute() it and check it against
-    the stored copy - or, with ORACLE_RECORD_REFERENCE=1, store it (ORACLE_RECORD_REFERENCE=1 python -m pytest tests -m "not gpu"
-    with the reference built rewrites the file).  Otherwise the stored copy, so that the comparison with the reference runs without the
-    reference's sources."""
-    global _stored
-    if _stored is None:
-        _stored = {}
-        if os.path.exists(REFERENCE_OUTPUTS):
-            flat = _load_flat(REFERENCE_OUTPUTS)
+def reference_output(key: str, compute, live: bool, path: str = REFERENCE_OUTPUTS):
+    """What the compiled reference returns for test case `key`, stored in the file `path`.  live (the reference is built): compute()
+    it and check it against the stored copy - or, with ORACLE_RECORD_REFERENCE=1, store it (ORACLE_RECORD_REFERENCE=1 python -m pytest
+    tests -m "not gpu" with the reference built rewrites the files).  Otherwise the stored copy, so that the comparison with the
+    reference runs without the reference's sources.  Each checker module binds this to its own file as its reference_output."""
+    if path not in _stored:
+        _stored[path] = {}
+        if os.path.exists(path):
+            flat = _load_flat(path)
             tops = {k.split("/")[0].split("#")[0] for k in flat}
-            _stored = {t: _unflatten(t, flat) for t in tops}
+            _stored[path] = {t: _unflatten(t, flat) for t in tops}
+    stored = _stored[path]
     if not live:
-        if key not in _stored:
-            raise KeyError(f"no stored reference output for {key!r}: regenerate {REFERENCE_OUTPUTS} with the reference built")
-        return _stored[key]
+        if key not in stored:
+            raise KeyError(f"no stored reference output for {key!r}: regenerate {path} with the reference built")
+        return stored[key]
     v = compute()
     if os.environ.get("ORACLE_RECORD_REFERENCE") == "1":
-        _stored[key] = v
+        stored[key] = v
         out = {}
-        for k, x in _stored.items():
+        for k, x in stored.items():
             _flatten(k, x, out)
-        _save_flat(REFERENCE_OUTPUTS, out)
-    elif key in _stored:
-        assert _same(v, _stored[key]), f"the compiled reference no longer gives the stored output for {key!r}"
+        _save_flat(path, out)
+    elif key in stored:
+        assert _same(v, stored[key]), f"the compiled reference no longer gives the stored output for {key!r}"
     return v
 
 

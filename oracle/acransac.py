@@ -12,11 +12,13 @@ not built, like ``oracle.guided_fast.reference_output`` does.
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
 
 import numpy as np
 
 import oracle
+from oracle import _p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 STORED = os.path.join(os.path.dirname(_HERE), "tests", "golden", "reference_acransac.npz")
@@ -24,46 +26,15 @@ TRACE_CAP = 4096
 FIELDS = ("valid", "inliers", "F", "error_max", "min_nfa", "iterations", "trace")   # the stored fields of AcransacOracle.estimate
 
 
-def _lib_path(kind: str) -> str:
-    return os.path.join(_HERE, "_ref", "libref_acransac.so") if kind == "ref" else os.path.join(_HERE, "libport_acransac.so")
-
-
-def available(kind: str) -> bool:
-    return os.path.exists(_lib_path(kind))
-
-
-# the primitives the exact-arithmetic tests call (test_acransac_exact.py); the estimation entry points predate them
-PRIMITIVES = ("acr_solve_cubic", "acr_nullspace7", "acr_epipolar_error", "acr_precondition", "acr_unnormalize", "acr_logalpha0",
-                "acr_unnormalize_error")
-
-
-def current(kind: str) -> bool:
-    """The library is built and has every entry point of this source (an older build lacks PRIMITIVES)."""
-    return available(kind) and oracle.exports(_lib_path(kind), PRIMITIVES)
-
-
-def build(ref: bool | None = None) -> None:
-    """Compile the port always, the "ref" build when oracle.reference_src() finds an AliceVision tree; a library older than these
-    sources' entry points is rebuilt even when make finds it up to date."""
-    src = oracle.reference_src()
-    ref = (src is not None) if ref is None else ref
-    targets = {"libport_acransac.so": (_lib_path("port"), PRIMITIVES)}
-    if ref:
-        targets["_ref/libref_acransac.so"] = (_lib_path("ref"), PRIMITIVES)
-    oracle.make_current("acransac.mk", targets, ["all"] + (["ref", f"REF={src}"] if ref else []))
-
-
-def _p(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
+available = functools.partial(oracle.lib_available, "acransac")
+current = functools.partial(oracle.lib_current, "acransac")
 
 
 class AcransacOracle:
     def __init__(self, kind: str = "port"):
         assert kind in ("ref", "port")
         self.kind = kind
-        if not available(kind):
-            raise FileNotFoundError(f"{_lib_path(kind)} missing: run oracle.acransac.build()")
-        self.lib = C.CDLL(_lib_path(kind))
+        self.lib = oracle.load_lib("acransac", kind)
         self.lib.acr_estimate.restype = C.c_long
         self.lib.acr_fit7.restype = C.c_int
 
@@ -157,30 +128,4 @@ def best(prefer_ref: bool = True) -> AcransacOracle:
     return AcransacOracle("ref" if prefer_ref and available("ref") else "port")
 
 
-_stored: dict | None = None
-
-
-def reference_output(key: str, compute, live: bool):
-    """What the "ref" build returns for test case `key`: computed and checked against the stored copy when it is built (stored with
-    ORACLE_RECORD_REFERENCE=1), else the stored copy."""
-    global _stored
-    if _stored is None:
-        _stored = {}
-        if os.path.exists(STORED):
-            flat = oracle._load_flat(STORED)
-            tops = {k.split("/")[0].split("#")[0] for k in flat}
-            _stored = {t: oracle._unflatten(t, flat) for t in tops}
-    if not live:
-        if key not in _stored:
-            raise KeyError(f"no stored reference output for {key!r}: regenerate {STORED} with the reference built")
-        return _stored[key]
-    v = compute()
-    if os.environ.get("ORACLE_RECORD_REFERENCE") == "1":
-        _stored[key] = v
-        out = {}
-        for k, x in _stored.items():
-            oracle._flatten(k, x, out)
-        oracle._save_flat(STORED, out)
-    elif key in _stored:
-        assert oracle._same(v, _stored[key]), f"the compiled reference no longer gives the stored output for {key!r}"
-    return v
+reference_output = functools.partial(oracle.reference_output, path=STORED)

@@ -2,7 +2,7 @@
 //
 // A-contrario RANSAC essential-matrix estimation of one pair of pinhole cameras, as GeometricFilterMatrix_E_AC::geometricEstimation
 // runs it (matchingImageCollection/GeometricFilterMatrix_E_AC.hpp): ACRANSAC over RelativePoseKernel_K<Essential5PSolver,
-// FundamentalEpipolarDistanceError, Mat3Model>, the std::mt19937 passed by reference.  Built twice by oracle/acransac_e.mk, like
+// FundamentalEpipolarDistanceError, Mat3Model>, the std::mt19937 passed by reference.  Built twice by oracle/Makefile (`all`, `ref`), like
 // oracle/acransac_s_oracle.cpp:
 //   -DACR_USE_REFERENCE -> _ref/libref_acransac_e.so: robustEstimation::ACRANSAC, makelogcombi (robustEstimation/ACRansac.hpp) and
 //                          randSample (robustEstimation/randSampling.hpp) compiled verbatim from an AliceVision source tree through

@@ -13,48 +13,28 @@ not built, like ``oracle.acransac_e.reference_output`` does for the essential ma
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
 
 import numpy as np
 
 import oracle
+from oracle import _p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 STORED = os.path.join(os.path.dirname(_HERE), "tests", "golden", "reference_acransac_f10.npz")
 TRACE_CAP = 4096
 FIELDS = ("valid", "inliers", "F", "L", "error_max", "min_nfa", "iterations", "trace", "mt_state_out")   # stored fields of estimate()
-PRIMITIVES = ("acrf10_fit10", "acrf10_estimate", "acrf10_mt_seed")
 
 
-def _lib_path(kind: str) -> str:
-    return os.path.join(_HERE, "_ref", "libref_acransac_f10.so") if kind == "ref" else os.path.join(_HERE, "libport_acransac_f10.so")
-
-
-def available(kind: str) -> bool:
-    return os.path.exists(_lib_path(kind))
-
-
-def build(ref: bool | None = None) -> None:
-    """Compile the port always, the "ref" build when oracle.reference_src() finds an AliceVision tree."""
-    src = oracle.reference_src()
-    ref = (src is not None) if ref is None else ref
-    targets = {"libport_acransac_f10.so": (_lib_path("port"), PRIMITIVES)}
-    if ref:
-        targets["_ref/libref_acransac_f10.so"] = (_lib_path("ref"), PRIMITIVES)
-    oracle.make_current("acransac_f10.mk", targets, ["all"] + (["ref", f"REF={src}"] if ref else []))
-
-
-def _p(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
+available = functools.partial(oracle.lib_available, "acransac_f10")
 
 
 class AcransacF10Oracle:
     def __init__(self, kind: str = "port"):
         assert kind in ("ref", "port")
         self.kind = kind
-        if not available(kind):
-            raise FileNotFoundError(f"{_lib_path(kind)} missing: run oracle.acransac_f10.build()")
-        self.lib = C.CDLL(_lib_path(kind))
+        self.lib = oracle.load_lib("acransac_f10", kind)
         self.lib.acrf10_estimate.restype = C.c_long
         self.lib.acrf10_fit10.restype = C.c_int
 
@@ -91,30 +71,4 @@ class AcransacF10Oracle:
                 "mt_state_out": sto}
 
 
-_stored: dict | None = None
-
-
-def reference_output(key: str, compute, live: bool):
-    """What the "ref" build returns for test case `key`: computed and checked against the stored copy when it is built (stored with
-    ORACLE_RECORD_REFERENCE=1), else the stored copy."""
-    global _stored
-    if _stored is None:
-        _stored = {}
-        if os.path.exists(STORED):
-            flat = oracle._load_flat(STORED)
-            tops = {k.split("/")[0].split("#")[0] for k in flat}
-            _stored = {t: oracle._unflatten(t, flat) for t in tops}
-    if not live:
-        if key not in _stored:
-            raise KeyError(f"no stored reference output for {key!r}: regenerate {STORED} with the reference built")
-        return _stored[key]
-    v = compute()
-    if os.environ.get("ORACLE_RECORD_REFERENCE") == "1":
-        _stored[key] = v
-        out = {}
-        for k, x in _stored.items():
-            oracle._flatten(k, x, out)
-        oracle._save_flat(STORED, out)
-    elif key in _stored:
-        assert oracle._same(v, _stored[key]), f"the compiled reference no longer gives the stored output for {key!r}"
-    return v
+reference_output = functools.partial(oracle.reference_output, path=STORED)

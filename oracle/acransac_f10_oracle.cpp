@@ -3,7 +3,7 @@
 // A-contrario RANSAC fundamental-matrix estimation with radial distortion of one planar pair, as
 // GeometricFilterMatrix_F_AC::geometricEstimation_Mat_ACRANSAC<Fundamental10PSolver, Fundamental10PModel> runs it (the
 // `fundamental_with_distortion` filter): ACRANSAC over RelativePoseKernel<Fundamental10PSolver, FundamentalEpipolarDistanceError,
-// UnnormalizerT, Fundamental10PModel>, the std::mt19937 taken by value.  Built twice by oracle/acransac_f10.mk, like
+// UnnormalizerT, Fundamental10PModel>, the std::mt19937 taken by value.  Built twice by oracle/Makefile (`all`, `ref`), like
 // oracle/acransac_e_oracle.cpp:
 //   -DACR_USE_REFERENCE -> _ref/libref_acransac_f10.so: robustEstimation::ACRANSAC, makelogcombi (robustEstimation/ACRansac.hpp)
 //                          and randSample (robustEstimation/randSampling.hpp) compiled verbatim from an AliceVision source tree

@@ -3,7 +3,7 @@
 // A-contrario RANSAC homography estimation of one pair, as GeometricFilterMatrix_H_AC::geometricEstimation runs it
 // (matchingImageCollection/GeometricFilterMatrix_H_AC.hpp:40-100): ACRANSAC over RelativePoseKernel<Homography4PSolver,
 // HomographyAsymmetricError, UnnormalizerI, Mat3Model> with the point-to-point error, the std::mt19937 passed by reference.
-// Built twice by oracle/acransac_h.mk, like oracle/acransac_oracle.cpp (the fundamental-matrix oracle, a separate library):
+// Built twice by oracle/Makefile (`all`, `ref`), like oracle/acransac_oracle.cpp (the fundamental-matrix oracle, a separate library):
 //   -DACR_USE_REFERENCE -> _ref/libref_acransac_h.so: robustEstimation::ACRANSAC, makelogcombi (robustEstimation/ACRansac.hpp) and
 //                          randSample (robustEstimation/randSampling.hpp) compiled verbatim from an AliceVision source tree through
 //                          oracle/shim, around the restated H kernel below; the generator is the library's own std::mt19937.

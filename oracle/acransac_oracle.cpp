@@ -2,7 +2,7 @@
 //
 // A-contrario RANSAC fundamental-matrix estimation of one pair, as GeometricFilterMatrix_F_AC::geometricEstimation_Mat_ACRANSAC
 // <Fundamental7PSolver, Mat3Model> runs it (matchingImageCollection/GeometricFilterMatrix_F_AC.hpp:266-299).
-// Built twice by oracle/acransac.mk:
+// Built twice by oracle/Makefile (`all`, `ref`):
 //   -DACR_USE_REFERENCE -> _ref/libref_acransac.so: robustEstimation::ACRANSAC (robustEstimation/ACRansac.hpp: the loop, bestNFA,
 //                          makelogcombi), randSample / uniformSample (robustEstimation/randSampling.hpp) and SolveCubicPolynomial
 //                          (numeric/polynomial.hpp) compiled verbatim from an AliceVision source tree through oracle/shim, around

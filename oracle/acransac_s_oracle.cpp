@@ -3,7 +3,7 @@
 // A-contrario RANSAC fundamental-matrix estimation of one pair of equidistant cameras, as
 // GeometricFilterMatrix_F_AC::geometricEstimation_Spherical_Mat runs it (matchingImageCollection/GeometricFilterMatrix_F_AC.hpp:186-253):
 // ACRANSAC over RelativePoseSphericalKernel<Fundamental7PSphericalSolver, EpipolarSphericalDistanceError, Mat3Model> on the lifted
-// unit vectors, the std::mt19937 passed by reference.  Built twice by oracle/acransac_s.mk, like oracle/acransac_oracle.cpp:
+// unit vectors, the std::mt19937 passed by reference.  Built twice by oracle/Makefile (`all`, `ref`), like oracle/acransac_oracle.cpp:
 //   -DACR_USE_REFERENCE -> _ref/libref_acransac_s.so: robustEstimation::ACRANSAC, makelogcombi (robustEstimation/ACRansac.hpp),
 //                          randSample (robustEstimation/randSampling.hpp) and SolveCubicPolynomial (numeric/polynomial.hpp) compiled
 //                          verbatim from an AliceVision source tree through oracle/shim, around the restated spherical kernel below;

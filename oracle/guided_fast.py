@@ -12,37 +12,19 @@ reference is not built, like ``oracle.reference_output`` does for the other comp
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
-import subprocess
 
 import numpy as np
 
 import oracle
+from oracle import _p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 STORED = os.path.join(os.path.dirname(_HERE), "tests", "golden", "reference_guided_fast.npz")
 
 
-def _lib_path(kind: str) -> str:
-    return os.path.join(_HERE, "_ref", "libref_guided_fast.so") if kind == "ref" else os.path.join(_HERE, "libport_guided_fast.so")
-
-
-def available(kind: str) -> bool:
-    return os.path.exists(_lib_path(kind))
-
-
-def build(ref: bool | None = None) -> None:
-    """Compile the port always, the "ref" build and the C++ adaptor test when oracle.reference_src() finds an AliceVision tree."""
-    src = oracle.reference_src()
-    ref = (src is not None) if ref is None else ref
-    mk = ["make", "-C", _HERE, "-f", "guided_fast.mk"]
-    subprocess.run(mk + ["all"] + (["ref", f"REF={src}"] if ref else []), check=True, stdout=subprocess.DEVNULL)
-    if ref and os.path.exists(os.path.join(os.path.dirname(_HERE), "alicevision_b200", "libb200match.so")):
-        subprocess.run(mk + ["adaptor", f"REF={src}"], check=True, stdout=subprocess.DEVNULL)
-
-
-def _p(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
+available = functools.partial(oracle.lib_available, "guided_fast")
 
 
 def _dt(a: np.ndarray, binary: bool) -> int:
@@ -55,9 +37,7 @@ class GuidedFastOracle:
     def __init__(self, kind: str = "port"):
         assert kind in ("ref", "port")
         self.kind = kind
-        if not available(kind):
-            raise FileNotFoundError(f"{_lib_path(kind)} missing: run oracle.guided_fast.build()")
-        self.lib = C.CDLL(_lib_path(kind))
+        self.lib = oracle.load_lib("guided_fast", kind)
         self.lib.gf_guided_fast.restype = C.c_int
         self.lib.gf_guided_match.restype = C.c_int
 
@@ -93,30 +73,4 @@ def best(prefer_ref: bool = True) -> GuidedFastOracle:
     return GuidedFastOracle("ref" if prefer_ref and available("ref") else "port")
 
 
-_stored: dict | None = None
-
-
-def reference_output(key: str, compute, live: bool):
-    """What the "ref" build returns for test case `key`: computed and checked against the stored copy when it is built (stored with
-    ORACLE_RECORD_REFERENCE=1), else the stored copy."""
-    global _stored
-    if _stored is None:
-        _stored = {}
-        if os.path.exists(STORED):
-            flat = oracle._load_flat(STORED)
-            tops = {k.split("/")[0].split("#")[0] for k in flat}
-            _stored = {t: oracle._unflatten(t, flat) for t in tops}
-    if not live:
-        if key not in _stored:
-            raise KeyError(f"no stored reference output for {key!r}: regenerate {STORED} with the reference built")
-        return _stored[key]
-    v = compute()
-    if os.environ.get("ORACLE_RECORD_REFERENCE") == "1":
-        _stored[key] = v
-        out = {}
-        for k, x in _stored.items():
-            oracle._flatten(k, x, out)
-        oracle._save_flat(STORED, out)
-    elif key in _stored:
-        assert oracle._same(v, _stored[key]), f"the compiled reference no longer gives the stored output for {key!r}"
-    return v
+reference_output = functools.partial(oracle.reference_output, path=STORED)

@@ -5,7 +5,7 @@
 //                    with pixToBucket / lineToEndPoints (matching/guidedMatching.cpp:13-70)
 //   gf_guided_match  matching::guidedMatching<Mat3Model, FundamentalEpipolarDistanceError | HomographyAsymmetricError>
 //                    (matching/guidedMatching.hpp:206-268), the loop of ref_oracle.cpp / port_oracle.cpp on double positions
-// Built twice by oracle/guided_fast.mk:
+// Built twice by oracle/Makefile (`all`, `ref`):
 //   -DGF_USE_REFERENCE  -> _ref/libref_guided_fast.so: descriptor distances from the reference's own Regions::SquaredDescriptorDistance
 //                          (feature/Regions.hpp:198-207 -> SquaredMetric), compiled from an AliceVision source tree through oracle/shim
 //   (none)              -> libport_guided_fast.so: the restated metrics (L2_Vectorized, squared Hamming)

@@ -8,40 +8,19 @@ reference's own when it is built).
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
+import functools
 
 import numpy as np
 
 import oracle
+from oracle import _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB = os.path.join(_HERE, "libguided_positions.so")
-
-
-def available() -> bool:
-    return os.path.exists(LIB)
-
-
-def build() -> None:
-    """Compile the oracle; with an AliceVision tree (oracle.reference_src()) and the CUDA library built, also the C++ test of the
-    homography-filter adaptor."""
-    mk = ["make", "-C", _HERE, "-f", "homography_filter.mk"]
-    subprocess.run(mk + ["all"], check=True, stdout=subprocess.DEVNULL)
-    src = oracle.reference_src()
-    if src is not None and os.path.exists(os.path.join(os.path.dirname(_HERE), "alicevision_b200", "libb200match.so")):
-        subprocess.run(mk + ["adaptor", f"REF={src}"], check=True, stdout=subprocess.DEVNULL)
-
-
-def _p(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
+available = functools.partial(oracle.lib_available, "guided_positions", None)
 
 
 class GuidedPositionsOracle:
     def __init__(self):
-        if not available():
-            raise FileNotFoundError(f"{LIB} missing: run oracle.guided_positions.build()")
-        self.lib = C.CDLL(LIB)
+        self.lib = oracle.load_lib("guided_positions", None)
         self.lib.gf_guided_match_positions.restype = C.c_int
 
     def guided_match_positions(self, xy_l, xy_r, M, errorTh: float, model: int = 1) -> np.ndarray:

@@ -5,7 +5,7 @@
 //                              (model, xLeft, xRight, errorTh, matches) (matching/guidedMatching.hpp:37-70), then
 //                              IndMatch::getDeduplicated (IndMatch.hpp:52-58)
 // No descriptor is read, so there is nothing of the reference to compile in: the "ref" and "port" builds of the other guided oracles
-// would be the same code, and oracle/homography_filter.mk builds this file once.  The geometry is RESTATED, as in
+// would be the same code, and oracle/Makefile (target `all`) builds this file once.  The geometry is RESTATED, as in
 // guided_fast_oracle.cpp: the association a coefficient-wise Eigen evaluation gives (H x)(r) = (H(r,0)*x + H(r,1)*y) + H(r,2)*1,
 // separate multiply / add (-ffp-contract=off).  Eigen is not in this image, so this part of the parity is not pinned by compiled
 // reference code.  The decorator that follows in GeometricFilterMatrix_H_AC is the compiled reference's own (ref_decorator_dedup,

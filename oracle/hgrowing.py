@@ -7,31 +7,20 @@ math header, ``oracle/libport_hgrowing.so``, and the stage around it (``stage``)
 from __future__ import annotations
 
 import ctypes as C
-import os
+import functools
 
 import numpy as np
 
 import oracle
+from oracle import _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB = os.path.join(_HERE, "libport_hgrowing.so")
-SYMBOLS = ("hg_filter", "hg_grow_steps", "hg_refine", "hg_exp", "hg_log")
 
 # GrowParameters / HGrowingFilteringParam defaults (GeometricFilterMatrix_HGrowing.hpp)
 DEFAULT_PARAM = dict(similarityTolerance=20.0, affinityTolerance=10.0, homographyTolerance=5.0, minInliersToRefine=6,
                      nbRefiningIterations=8, maxNbHomographies=10, minNbMatchesPerH=20)
 
 
-def available() -> bool:
-    return os.path.exists(LIB)
-
-
-def build() -> None:
-    oracle.make_current("hgrowing.mk", {"libport_hgrowing.so": (LIB, SYMBOLS)}, ["all"])
-
-
-def _p(a: np.ndarray):
-    return a.ctypes.data_as(C.c_void_p)
+available = functools.partial(oracle.lib_available, "hgrowing")
 
 
 def param_arrays(param: dict | None):
@@ -43,9 +32,7 @@ def param_arrays(param: dict | None):
 
 class HGrowingOracle:
     def __init__(self):
-        if not available():
-            raise FileNotFoundError(f"{LIB} missing: run oracle.hgrowing.build()")
-        self.lib = C.CDLL(LIB)
+        self.lib = oracle.load_lib("hgrowing")
         self.lib.hg_exp.restype = C.c_double
         self.lib.hg_exp.argtypes = [C.c_double]
         self.lib.hg_log.restype = C.c_double

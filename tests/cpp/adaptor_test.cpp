@@ -1,6 +1,6 @@
 // Compiles the C++ adaptors against the REFERENCE's own interface headers (through oracle/shim) and checks, on a GPU,
 // that ArrayMatcher_b200 / ImageCollectionMatcher_b200 return exactly what the reference classes return on the same
-// Regions.  Built by oracle/Makefile target `adaptor` into oracle/_ref/adaptor_test (needs /root/reference at build time).
+// Regions.  Built by oracle/Makefile target `adaptors` into oracle/_ref/adaptor_test (needs an AliceVision source tree at build time).
 #include <aliceVision/matching/ArrayMatcher_bruteForce.hpp>
 #include <aliceVision/matching/RegionsMatcher.hpp>
 #include <aliceVision/feature/regionsFactory.hpp>

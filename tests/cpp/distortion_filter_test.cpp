@@ -3,7 +3,7 @@
 // the "ref" oracles: the reference's ACRANSAC loop around the restated F10 kernel (acrf10_estimate) from the same generator state,
 // the inlier copy and hasStrongSupport(.., 10), and with guided matching the reference's guidedMatching loop (gf_guided_match,
 // fundamental model) on the adaptor's own F and errorMax^2.
-// Built by oracle/distortion_filter.mk into oracle/_ref/distortion_filter_test.
+// Built by oracle/Makefile target `adaptors` into oracle/_ref/distortion_filter_test.
 #include <aliceVision/feature/regionsFactory.hpp>
 
 #include <GeometricFilter_b200.hpp>

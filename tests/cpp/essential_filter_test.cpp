@@ -3,7 +3,7 @@
 // essential-matrix kernel (acre_estimate) from the same generator state and with the filter's Square(precision), the inlier copy and
 // hasStrongSupport(.., 5), and with guided matching the reference's guidedMatching loop (gf_guided_match, fundamental model) on the
 // adaptor's own F = K_J^-T E K_I^-1 and errorMax^2.
-// Built by oracle/essential_filter.mk into oracle/_ref/essential_filter_test.
+// Built by oracle/Makefile target `adaptors` into oracle/_ref/essential_filter_test.
 #include <aliceVision/feature/regionsFactory.hpp>
 
 #include <GeometricFilter_b200.hpp>

@@ -2,7 +2,7 @@
 // checks, on a GPU, GeometricFilterMatrix_F_AC_Batch_b200 against the "ref" oracles: the reference's ACRANSAC loop around the restated F
 // kernel (acr_estimate) from the same generator state, the inlier copy and support rules, and guidedMatching on the reference's
 // Regions distances (gf_guided_match) with the adaptor's own F and errorMax^2.
-// Built by oracle/geometric_filter.mk into oracle/_ref/geometric_filter_test.
+// Built by oracle/Makefile target `adaptors` into oracle/_ref/geometric_filter_test.
 #include <aliceVision/feature/regionsFactory.hpp>
 
 #include <GeometricFilter_b200.hpp>

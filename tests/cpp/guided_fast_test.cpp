@@ -1,7 +1,7 @@
 // Compiles alicevision_b200/adaptor/guidedMatchingFast_b200.hpp against the REFERENCE's own interface headers (through oracle/shim)
 // and checks, on a GPU, that GuidedMatchingFastBatch_b200 and guidedMatchingFundamentalFast_b200 return exactly what the "ref"
 // oracle (guidedMatchingFundamentalFast restated around the reference's Regions::SquaredDescriptorDistance) returns.
-// Built by oracle/guided_fast.mk target `adaptor` into oracle/_ref/guided_fast_adaptor_test.
+// Built by oracle/Makefile target `adaptors` into oracle/_ref/guided_fast_adaptor_test.
 #include <aliceVision/feature/regionsFactory.hpp>
 
 #include <guidedMatchingFast_b200.hpp>

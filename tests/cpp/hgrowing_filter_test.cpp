@@ -3,7 +3,7 @@
 // (oracle/libport_hgrowing.so, hg_filter) on the same putatives: every (pair, type)'s homographies bit for bit, their matches, the
 // kept lists, and the stage rules (an empty filtered list is kept, a type without putatives is skipped, a pair without a common type
 // gets nothing, guidedMatching gives an empty map).
-// Built by oracle/hgrowing.mk (target `adaptor`) into oracle/_ref/hgrowing_filter_test.
+// Built by oracle/Makefile target `adaptors` into oracle/_ref/hgrowing_filter_test.
 #include <aliceVision/feature/regionsFactory.hpp>
 
 #include <GeometricFilter_b200.hpp>

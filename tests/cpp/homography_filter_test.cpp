@@ -3,7 +3,7 @@
 // homography kernel (acr_estimate_h) from the same generator state, the inlier copy and hasStrongSupport(.., 4), and with
 // distanceRatio = -1 the position-only guidedMatching loop (gf_guided_match_positions) followed by the reference's own
 // IndMatchDecorator, on the adaptor's own H and errorMax^2.
-// Built by oracle/homography_filter.mk into oracle/_ref/homography_filter_test.
+// Built by oracle/Makefile target `adaptors` into oracle/_ref/homography_filter_test.
 #include <aliceVision/feature/regionsFactory.hpp>
 #include <aliceVision/matching/IndMatchDecorator.hpp>
 

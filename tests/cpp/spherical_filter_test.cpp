@@ -5,7 +5,7 @@
 // reference's Regions distances (gf_guided_match) with the adaptor's own F and errorMax^2.  Every pair's estimate is also checked bit
 // for bit against a one-pair engine call of its own kind from the same state, which pins how run() splits the list into its planar and
 // spherical calls and merges them back in addPair order.
-// Built by oracle/spherical_filter.mk into oracle/_ref/spherical_filter_test.
+// Built by oracle/Makefile target `adaptors` into oracle/_ref/spherical_filter_test.
 #include <aliceVision/feature/regionsFactory.hpp>
 
 #include <GeometricFilter_b200.hpp>

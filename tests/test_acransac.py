@@ -83,7 +83,6 @@ def reference(name):
 
 @pytest.fixture(scope="module")
 def port():
-    acr_oracle.build(ref=False) if not acr_oracle.available("port") else None
     return acr_oracle.AcransacOracle("port")
 
 

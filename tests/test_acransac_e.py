@@ -86,7 +86,6 @@ def _params(name):
 
 @pytest.fixture(scope="module")
 def port():
-    acransac_e.build(ref=False) if not acransac_e.available("port") else None
     return acransac_e.AcransacEOracle("port")
 
 

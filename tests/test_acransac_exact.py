@@ -58,13 +58,11 @@ def fro(A) -> mp.mpf:
 
 @pytest.fixture(scope="module")
 def pf():
-    acr_oracle.build(ref=False) if not acr_oracle.current("port") else None
     return acr_oracle.AcransacOracle("port")
 
 
 @pytest.fixture(scope="module")
 def ph():
-    acrh.build(ref=False) if not acrh.current("port") else None
     return acrh.AcransacHOracle("port")
 
 

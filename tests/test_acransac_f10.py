@@ -98,7 +98,6 @@ def params(name):
 
 @pytest.fixture(scope="module")
 def port():
-    acransac_f10.build(ref=False) if not acransac_f10.available("port") else None
     return acransac_f10.AcransacF10Oracle("port")
 
 

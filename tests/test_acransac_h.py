@@ -117,7 +117,6 @@ def reference(name):
 
 @pytest.fixture(scope="module")
 def port():
-    acrh.build(ref=False) if not acrh.available("port") else None
     return acrh.AcransacHOracle("port")
 
 

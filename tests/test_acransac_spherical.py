@@ -115,7 +115,6 @@ def reference(name):
 
 @pytest.fixture(scope="module")
 def port():
-    acrs.build(ref=False) if not acrs.available("port") else None
     return acrs.AcransacSOracle("port")
 
 

@@ -13,8 +13,6 @@ DEF = hgrowing.DEFAULT_PARAM
 
 
 def _port():
-    if not hgrowing.available():
-        hgrowing.build()
     return hgrowing.HGrowingOracle()
 
 

@@ -91,8 +91,9 @@ def main():
     k10 = ctx.acransac_last_stats()
     kept = [p for p in out if np.isfinite(info[p]["error_max"])]
 
+    import oracle
     from oracle import acransac_s as acrs
-    acrs.build(ref=False) if not acrs.available("port") else None
+    oracle.build(ref=False) if not acrs.available("port") else None
     O = acrs.AcransacSOracle("port")
     st = O.mt_seed(42)
     cpu = []
