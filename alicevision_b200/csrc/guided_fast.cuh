@@ -22,8 +22,10 @@
 // A NaN distance never passes `dist < bd` nor `dist < sbd` in the reference: it is skipped.
 //
 // Arithmetic.  All double arithmetic that decides a bucket is uncontracted (__dmul_rn / __dadd_rn / __dsub_rn / __ddiv_rn /
-// __dsqrt_rn) with the reference's association: when neither end point is clamped, r1 and r2 are rounding noise and the choice
-// of x0 depends on the exact operations.  r1 and r2 are floats, as in lineToEndPoints.
+// __dsqrt_rn): when neither end point is clamped, r1 and r2 are rounding noise and the choice of x0 depends on the exact operations.
+// Each row of F x is summed as (F(r,0) x + F(r,1) y) + F(r,2); Eigen's own association for that product is not compiled here, and
+// DESIGN.md (K9) gives the reading of it, why this order is kept and what the difference changes.  r1 and r2 are floats, as in
+// lineToEndPoints.
 //
 // Divergence (documented in include/b200match.h and DESIGN.md): where the reference is undefined - an epipole at infinity
 // (ep2(2) == 0: division by 0) or a right feature exactly at the epipole (n = 0 * inf = NaN) - it casts NaN to int and indexes
